@@ -66,6 +66,11 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
                   long long ldo, int out_f32, int act, float alpha, int bn, int ksplit, void* workspace,
                   size_t ws_bytes, void* stream);
 
+/* The tiling the last vdb_gemm_bf16 / vdb_gemm_ln_bf16 / vdb_conv3x3_bf16 call on this thread launched (host-side record, no
+ * device work): out[0..n) receives {BN, STAGES, epilogue MODE, ksplit, grid, M tiles, N tiles, nfast, chunked} (as many as n
+ * allows).  Returns the number of fields (9).  For tests and tools that need to know which kernel instantiation ran. */
+int vdb_igemm_last_plan(int* out, int n);
+
 /* ---- the same GEMM with a LayerNorm folded in — BasicTransformerBlock norm1/2/3, attention.py:206-208,214-218 -------------
  * CONSUMER (ln_stats != NULL):  out = act( LN(x) W0^T + b0 )  computed from the RAW x without ever forming LN(x):
  *     out[m,n] = act( rstd[m] * (x W^T - mean[m] * ln_colsum[n]) + bias[n] )

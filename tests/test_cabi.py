@@ -1,5 +1,6 @@
 """C-ABI surface (no GPU needed): the library loads and exports every symbol include/vdb200.h declares,
 and the ctypes signature table covers exactly that set."""
+import ctypes
 import os
 import re
 
@@ -33,6 +34,31 @@ def test_host_side_argument_checks_without_gpu():
     assert lib.vdb_attention_dk_pad(40) == 64 and lib.vdb_attention_dv_pad(40) == 48
     assert lib.vdb_attention_dk_pad(160) == 192 and lib.vdb_attention_dv_pad(160) == 160
     assert lib.vdb_attention_dk_pad(512) == -1
+
+
+def test_misaligned_output_or_residual_is_rejected_before_launch():
+    """A bf16 `out` or `resid` that is not 16-byte aligned fails the TMA-store tensor map, and the launch would fall back to the
+    epilogues that store and load 16-byte vectors there: the entry points refuse such pointers up front (the fake addresses
+    below are never dereferenced)."""
+    from vdb200._lib import lib
+    A, W, ok, bad = 0x10000, 0x20000, 0x30000, 0x30008
+    gemm = lambda out, resid: lib.vdb_gemm_bf16(A, 256, 64, 64, None, 0, 0, W, 64, 64, None, 0, 1, resid, 64 if resid else 0, out, 64,
+                                                0, 0, 1.0, 0, 1, None, 0, None)
+    for out, resid in ((bad, None), (ok, bad)):
+        assert gemm(out, resid) == 1 and b"16-byte aligned" in lib.vdb_last_error()
+    assert lib.vdb_conv3x3_bf16(A, 1, 8, 8, 64, 0, W, 64, 576, None, 0, None, 0, None, 0, None, 0, bad, 64, 0, 0, 0, 1, None, 0,
+                                None) == 1 and b"16-byte aligned" in lib.vdb_last_error()
+    assert lib.vdb_conv3x3_bf16(A, 1, 8, 8, 64, 0, W, 64, 576, None, 0, None, 0, None, 0, bad, 64, ok, 64, 0, 0, 0, 1, None, 0,
+                                None) == 1 and b"16-byte aligned" in lib.vdb_last_error()
+    parts = ctypes.c_int(0)
+    assert lib.vdb_gemm_ln_bf16(A, 256, 64, 64, W, 64, 64, None, None, 0, bad, 64, 0, None, 0, 0, 0, 0.0, None, 0, None, ok,
+                                ctypes.byref(parts), 0, None) == 1 and b"16-byte aligned" in lib.vdb_last_error()
+
+
+def test_igemm_last_plan_reports_nine_fields():
+    from vdb200._lib import lib
+    buf = (ctypes.c_int * 9)()
+    assert lib.vdb_igemm_last_plan(buf, 9) == 9 and lib.vdb_igemm_last_plan(None, 0) == 9
 
 
 def test_product_path_refuses_cpu_tensors():

@@ -1,8 +1,9 @@
 """Per-kernel numerics: every vdb200 kernel against a plain torch fp32 restatement of the same op
 (the reference's own arithmetic for that call site), on bf16-rounded inputs.
 
-Tolerances: bf16 tensor-core kernels  max|err| <= 2e-2 * max|ref| and cosine >= 0.999 (SURVEY §8c);
-fp32 elementwise kernels bit-exact or <= 1e-6 relative as stated per test.
+Tolerances: bf16 tensor-core kernels  max|err| <= 2e-2 * max|ref| and cosine >= 0.999;
+fp32 elementwise kernels bit-exact or <= 1e-6 relative as stated per test.  test_igemm_coverage_gpu.py checks every
+implicit-GEMM instantiation per element against fp64.
 """
 import math
 
@@ -79,7 +80,7 @@ GEMM_CASES = [
     (4096, 1280, 640, True, True, 0, 0, 1, False),
     (77, 768, 768, True, False, 3, 0, 1, False),
     (300, 256, 128, True, False, 1, 128, 1, False),
-    (512, 1280, 2880, True, True, 0, 0, 0, False),     # auto split-K
+    (512, 1280, 2880, True, True, 0, 0, 0, False),     # auto BN and split-K (132 SMs: the tile-width model picks BN 64, no split)
     (512, 1280, 11520, True, True, 0, 0, 8, False),    # forced split-K
     (640, 200, 192, True, False, 2, 0, 1, True),       # fp32 out, N tail
     (8192, 320, 1280, False, True, 0, 160, 1, False),
@@ -428,7 +429,7 @@ ATT_CASES = [
     (2, 12, 77, 77, 64, True),
     (2, 16, 257, 257, 64, False),
     (3, 8, 4096, 77, 40, False),
-    # shapes served by the two-tile kernel (attention_fa_kernel: d_head <= 64, >= 512 keys, Nq % 256 == 0)
+    # longer key ranges, ragged tails and the d_head <= 64 instantiations (attention_kernel<DK 64, DVP 48 / 64>)
     (2, 8, 1024, 1024, 40, False),
     (2, 4, 512, 640, 64, False),       # d 64: all four K16 steps, DVP 64
     (1, 3, 256, 1000, 40, False),      # masked tail tile (1000 = 7 * 128 + 104)
@@ -437,7 +438,7 @@ ATT_CASES = [
     (2, 3, 512, 900, 56, False),       # d 56 in DVP 64: row sums through the ones row of V^T, masked tail
     (1, 2, 256, 512, 32, False),       # d 32 in DVP 48: two padding swizzle groups behind the data rows
     (1, 8, 1024, 1028, 40, False),     # four token-concatenated image contexts (4 x 257 keys, app.py mcg tab): 8 full tiles + 4 keys
-    (2, 8, 256, 514, 80, False),       # two images at d_head 80 (round-1 kernel, masked tail tile)
+    (2, 8, 256, 514, 80, False),       # two images at d_head 80 (attention_kernel<DK 128, DVP 80>, masked tail tile)
 ]
 
 

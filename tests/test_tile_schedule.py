@@ -85,8 +85,29 @@ def test_chunked_order_covers_every_tile_once_and_rarely_changes_the_n_tile(sms,
 
 
 def test_strided_walk_changes_the_n_tile_every_other_tile_on_the_geglu_shape():
-    tiles = list(walk(148, 256, 10, 1, nfast=False))
+    tiles = list(walk(132, 256, 10, 1, nfast=False))
     seq = [n for cta, _, n, _ in tiles if cta == 0]
-    assert sum(1 for a, b in zip(seq, seq[1:]) if a != b) >= len(seq) // 2 - 1          # 18 tiles, ~9 table reloads
-    seq_c = [n for cta, _, n, _ in walk(148, 256, 10, 1, nfast=False, chunked=True) if cta == 0]
+    assert sum(1 for a, b in zip(seq, seq[1:]) if a != b) >= len(seq) // 2 - 1          # 20 tiles, ~10 table reloads
+    seq_c = [n for cta, _, n, _ in walk(132, 256, 10, 1, nfast=False, chunked=True) if cta == 0]
     assert sum(1 for a, b in zip(seq_c, seq_c[1:]) if a != b) == 0
+
+
+# the instantiations run_igemm can launch: (BN, epilogue MODE)
+IGEMM_INSTANTIATIONS = [(bn, mode) for bn in (64, 128, 160, 256) for mode in (0, 1, 3, 5, 7)] + [(256, 2), (256, 4), (256, 6)]
+
+
+def test_igemm_coverage_table_reaches_every_instantiation_with_a_multi_tile_walk():
+    """test_igemm_coverage_gpu.CASES: every instantiation has a row in which, on 132 SMs, some CTA runs two or more tiles on
+    different N tiles, with an M tail, a K tail and (except GEGLU, whose N is a multiple of 256) a partial last N tile.  A new
+    instantiation without such a row fails here."""
+    from test_igemm_coverage_gpu import CASES, multi_tile_n_change, tile_geometry
+    assert len(IGEMM_INSTANTIATIONS) == 23
+    for bn, mode in IGEMM_INSTANTIATIONS:
+        rows = [c for c in CASES if (c["bn"], c["mode"]) == (bn, mode) and c["walk"]]
+        assert rows, f"no multi-tile case for BN {bn} mode {mode}"
+        for c in rows:
+            tm, tn, ks, _ = tile_geometry(c)
+            assert multi_tile_n_change(min(tm * tn * ks, 132), tm, tn, ks), f"{c['id']}: no CTA changes its N tile on 132 SMs"
+        assert any(c["kind"] != "conv" and c["M"] % 128 and c["K"] % 64 and (c["N"] % bn or mode in (2, 4, 6)) for c in rows), \
+            f"BN {bn} mode {mode}: no multi-tile case with M, K and N tails"
+    assert {(c["bn"], c["mode"]) for c in CASES if c["bn"]} <= set(IGEMM_INSTANTIATIONS)

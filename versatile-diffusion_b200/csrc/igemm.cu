@@ -899,6 +899,21 @@ static int pick_bn(int N, int act, int forced) {
 
 static unsigned long long* g_timeline = nullptr;
 
+// The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN, nfast, chunked
+constexpr int kPlanFields = 9;
+static thread_local int g_last_plan[kPlanFields] = {0};
+
+// The non-TMA epilogues store bf16 output rows and load residual rows as 16-byte vectors, and the split-K reduction stores fp32
+// rows as float4, so out / resid must be 16-byte aligned.  Checked before any tensor map is built: a misaligned `out` fails the
+// TMA-store map, and the launch would otherwise fall back to exactly those vector stores.
+static int check_epilogue_pointers(const void* out, long long ldo, int out_f32, const void* resid, long long ldr, const char* who) {
+  if ((reinterpret_cast<uintptr_t>(out) & 15) || (resid && (reinterpret_cast<uintptr_t>(resid) & 15)))
+    return set_error(VDB_ERR_INVALID, "%s: out and resid must be 16-byte aligned", who);
+  if (!out_f32 && (ldo % 8)) return set_error(VDB_ERR_INVALID, "%s: ldo must be a multiple of 8 for bf16 out", who);
+  if (resid && (ldr % 8)) return set_error(VDB_ERR_INVALID, "%s: ldr must be a multiple of 8", who);
+  return VDB_OK;
+}
+
 struct IgemmEpilogue {
   const float* bias = nullptr;
   long long bias_bstride = 0;
@@ -970,8 +985,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   p.bias = e.bias; p.bias_bstride = e.bias_bstride; p.rows_per_batch = e.rows_per_batch > 0 ? e.rows_per_batch : 1;
   p.resid = reinterpret_cast<const __nv_bfloat16*>(e.resid); p.ldr = e.ldr;
   p.out = e.out; p.ldo = e.ldo; p.out_f32 = e.out_f32; p.act = e.act; p.alpha = e.alpha;
-  if (!e.out_f32 && (e.ldo % 8)) return set_error(VDB_ERR_INVALID, "igemm: ldo must be a multiple of 8 for bf16 out");
-  if (e.resid && (e.ldr % 8)) return set_error(VDB_ERR_INVALID, "igemm: ldr must be a multiple of 8");
   const long long M = static_cast<long long>(p.Bo) * p.Ho * p.Wo;
   if (M >= (1LL << 30)) return set_error(VDB_ERR_UNSUPPORTED, "igemm: more than 2^30 output rows");
   const int tilesM = p.tilesW * p.tilesH * p.tilesB;
@@ -986,7 +999,8 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   }
   if (ksplit > 1) {
     const size_t need = static_cast<size_t>(ksplit) * M * N * sizeof(float);
-    if (workspace == nullptr || ws_bytes < need || e.act == ACT_GEGLU || (N % 4)) ksplit = 1;
+    // (the reduction stores fp32 rows as float4: an fp32 row stride must keep them 16-byte aligned)
+    if (workspace == nullptr || ws_bytes < need || e.act == ACT_GEGLU || (N % 4) || (e.out_f32 && (e.ldo % 4))) ksplit = 1;
   }
   p.ksplit = ksplit;
   p.kb_per_split = (p.kb_total + ksplit - 1) / ksplit;
@@ -1065,6 +1079,11 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     if (ln_in && e.resid) return set_error(VDB_ERR_UNSUPPORTED, "igemm: a folded-LayerNorm GEMM takes no residual");
     if (ln_in && mode == 4 && e.ln_on_cols) return set_error(VDB_ERR_UNSUPPORTED, "igemm: GEGLU with column statistics");
     mode = st_out ? 7 : mode + 2;
+  }
+  {
+    const int stages = BN == 64 ? 8 : BN == 128 ? 6 : BN == 160 ? 5 : 4;   // (as instantiated below)
+    const int plan[kPlanFields] = {BN, stages, mode, p.ksplit, std::min(num_tiles, num_sms()), tilesM, p.tilesN, p.nfast, p.chunked};
+    for (int i = 0; i < kPlanFields; ++i) g_last_plan[i] = plan[i];
   }
   if (mode == 7) {
     switch (BN) {
@@ -1149,6 +1168,12 @@ extern "C" {
 // debug aid (not part of the product ABI): device buffer of 16*8 u64 receiving CTA 0's per-tile role timestamps
 void vdb_debug_igemm_timeline(void* buf) { g_timeline = reinterpret_cast<unsigned long long*>(buf); }
 
+// see include/vdb200.h
+int vdb_igemm_last_plan(int* out, int n) {
+  for (int i = 0; out && i < n && i < kPlanFields; ++i) out[i] = g_last_plan[i];
+  return kPlanFields;
+}
+
 // out[M,N] = act(alpha * ([A | A2] @ W^T + bias)) + resid     (see include/vdb200.h)
 int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const void* A2, long long K2,
                   long long lda2, const void* W, long long N, long long ldw, const float* bias,
@@ -1160,13 +1185,15 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
   if (A2 && ((K % kBlockK) || (K2 % 8) || (lda2 % 8)))
     return set_error(VDB_ERR_INVALID, "gemm: two-source A needs K % 64 == 0 and K2, lda2 % 8 == 0");
   if (M > 0x7fffffffLL || N > 0x7fffffffLL) return set_error(VDB_ERR_INVALID, "gemm: dimension too large");
+  int rc = check_epilogue_pointers(out, ldo, out_f32, resid, ldr, "gemm");
+  if (rc) return rc;
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   // GEMM view of the pixel grid: one row of M "pixels"; the box is always 128 rows (TMA zero-fills past M)
   p.Wo = static_cast<int>(M); p.Ho = 1; p.Bo = 1;
   p.TW = kBlockM; p.TH = 1; p.TB = 1;
   p.tilesW = static_cast<int>((M + kBlockM - 1) / kBlockM); p.tilesH = 1; p.tilesB = 1;
-  int rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
+  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
   if (rc) return rc;
   p.seg[0] = ASeg{0, 0, 0, static_cast<int16_t>((K + kBlockK - 1) / kBlockK), 0};
   p.nseg = 1;
@@ -1201,12 +1228,14 @@ int vdb_gemm_ln_bf16(const void* A, long long M, long long K, long long lda, con
     if (ln_rows < (ln_on_cols ? N : M)) return set_error(VDB_ERR_INVALID, "gemm_ln: statistics table has too few rows");
   }
   if (stats_out && ((N % 32) || !stats_parts)) return set_error(VDB_ERR_INVALID, "gemm_ln: stats_out needs N %% 32 == 0 and stats_parts");
+  int rc = check_epilogue_pointers(out, ldo, 0, resid, ldr, "gemm_ln");
+  if (rc) return rc;
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   p.Wo = static_cast<int>(M); p.Ho = 1; p.Bo = 1;
   p.TW = kBlockM; p.TH = 1; p.TB = 1;
   p.tilesW = static_cast<int>((M + kBlockM - 1) / kBlockM); p.tilesH = 1; p.tilesB = 1;
-  int rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
+  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
   if (rc) return rc;
   p.seg[0] = ASeg{0, 0, 0, static_cast<int16_t>((K + kBlockK - 1) / kBlockK), 0};
   p.nseg = 1;
@@ -1247,13 +1276,14 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int Wd, int C, int mode, const
   const bool strided = (mode == 1 || mode == 2), folded = mode >= 3;
   if (strided && ((H & 1) || (Wd & 1))) return set_error(VDB_ERR_UNSUPPORTED, "conv3x3: stride 2 needs even H, W");
   if (folded && (skip1 || skip2)) return set_error(VDB_ERR_INVALID, "conv3x3: the folded-upsample modes take no skip inputs");
+  int rc = check_epilogue_pointers(out, ldo, out_f32, resid, ldr, "conv3x3");
+  if (rc) return rc;
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   const int Ho = strided ? H / 2 : H, Wo = strided ? Wd / 2 : Wd;
   set_tile_shape(p, Wo, Ho, B);
   const uint64_t eb = 2;
   const int nkb = C / kBlockK;
-  int rc;
   int nmaps = 0;
   int ntaps = 9;
   if (mode == 0 || folded) {

@@ -30,7 +30,8 @@ SIGNATURES = {
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),
     "vdb_gemm_bf16": (i, [p, ll, ll, ll, p, ll, ll, p, ll, ll, p, ll, ll, p, ll, p, ll, i, i, f, i, i, p, sz, p]),
-    "vdb_gemm_ln_bf16": (i, [p, ll, ll, ll, p, ll, ll, p, p, ll, p, ll, i, p, ll, i, i, f, p, i, p, p, p, i, p]),
+    "vdb_igemm_last_plan": (i, [C.POINTER(i), i]),
+    "vdb_gemm_ln_bf16":(i, [p, ll, ll, ll, p, ll, ll, p, p, ll, p, ll, i, p, ll, i, i, f, p, i, p, p, p, i, p]),
     "vdb_gemm_skinny_fits": (i, [i, ll]),
     "vdb_gemm_skinny_bf16": (i, [p, i, ll, ll, p, ll, ll, p, ll, ll, p, ll, p, ll, p, ll, i, p]),
     "vdb_conv3x3_bf16": (i, [p, i, i, i, i, i, p, i, ll, p, i, p, i, p, ll, p, ll, p, ll, i, i, i, i, p, sz, p]),

@@ -257,6 +257,18 @@ def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype
     return out
 
 
+IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n", "nfast", "chunked")
+
+
+def igemm_last_plan():
+    """The tiling of the last gemm / gemm_ln / conv3x3 launch on this thread (vdb_igemm_last_plan): which kernel instantiation
+    (BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile walk."""
+    buf = (ctypes.c_int * len(IGEMM_PLAN_FIELDS))()
+    n = lib.vdb_igemm_last_plan(buf, len(buf))
+    assert n == len(IGEMM_PLAN_FIELDS), n
+    return dict(zip(IGEMM_PLAN_FIELDS, buf))
+
+
 class LnFold(object):
     """What a GEMM needs to consume a LayerNorm it never sees (vdb_gemm_ln_bf16): the producer's partial sums `stats`
     [>= parts, rows, 2] fp32 (`parts` of them valid), the LayerNorm's width and epsilon; the weights' column sums ride with the
