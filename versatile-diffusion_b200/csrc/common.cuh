@@ -29,6 +29,18 @@ VDB_DEVINL float4 lds_f4(uint32_t addr) {
   return v;
 }
 
+VDB_DEVINL float2 lds_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
+}
+// stmatrix: four 8x8 b16 matrices from the mma accumulator-fragment layout to shared memory.  Register i of lane l holds
+// row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1 of matrix i; lanes 8i .. 8i + 7 give the 16-byte row addresses of matrix i.
+VDB_DEVINL void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+
 VDB_DEVINL uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

@@ -84,7 +84,7 @@ int make_tmap_4d(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint
   return encode(m, ptr, 4, dims, strides, box);
 }
 
-// store-side map of an epilogue staging tile: 32 bf16 columns (64 B) x 32 rows, SWIZZLE_64B
+// store-side map of an epilogue staging box: 32 bf16 columns (64 B) x 16 rows, SWIZZLE_64B
 int make_tmap_4d_sw64(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t d3,
                       uint64_t stride1, uint64_t stride2, uint64_t stride3, uint32_t box0, uint32_t box1, uint32_t box2,
                       uint32_t box3) {

@@ -11,7 +11,8 @@
 //
 // Structure: grid = #SMs (persistent, static round-robin over output tiles), 288 threads:
 //   warps 0-7: two consumer warpgroups (wgmma m64 x BN x 16 each, fp32 accumulators in registers), then the epilogue
-//              (accumulator parked in shared memory -> bias/act/residual -> coalesced bf16 or TMA stores)
+//              (TMA-store modes: straight from the registers -> bias / LayerNorm / GEGLU / residual -> bf16 TMA stores;
+//              other modes: accumulator parked in shared memory -> bias/act/residual -> coalesced bf16 / fp32 stores)
 //   warp 8   : TMA producer  (cp.async.bulk.tensor 4D box loads of A, 2D box loads of W)
 // smem ring of STAGES x (A 128x64 bf16 | W BNx64 bf16), both 128B-swizzled K-major.
 #include "common.cuh"
@@ -38,7 +39,7 @@ struct ASeg {
 struct alignas(64) IgemmParams {
   CUtensorMap tmA[kMaxA];  // 4D (C, W, H, B) bf16, box (64, TW, TH, TB), SWIZZLE_128B
   CUtensorMap tmB;         // 2D (Ktot, N) bf16, box (64, BN), SWIZZLE_128B
-  CUtensorMap tmO;         // TMA-store epilogues: 4D (N, Wo, Ho, Bo) bf16 output, box (32, bw, bh, bb) = one warp's 32 x 32 chunk, SWIZZLE_64B
+  CUtensorMap tmO;         // TMA-store epilogues: 4D (N, Wo, Ho, Bo) bf16 output, box (32, bw, bh, bb) = one warp's 16-row x 32-column chunk, SWIZZLE_64B
   ASeg seg[kMaxSeg];
   int nseg;
   int kb_total;      // total k-blocks over all segments
@@ -68,8 +69,8 @@ struct alignas(64) IgemmParams {
   float ln_inv_dim, ln_eps;   // 1 / normalised width, epsilon
   const float* ln_colsum;     // on_cols 0: [N] sum_k W'[n, k];  on_cols 1: [M] (per output row)
   const float* ln_rowbias;    // on_cols 1: [M] beta-term of the output row (null = 0); on_cols 0 the beta term lives in `bias`
-  float* stats_out;           // mode 7: [2 * tilesN][M][2] fp32: (sum, sum of squares) of the columns each of the two epilogue
-                              // warps of a 32-row quarter handled in each N tile, for every OUTPUT row
+  float* stats_out;           // mode 7: [2 * tilesN][M][2] fp32: (sum, sum of squares) over the even (slot 2n) and the odd
+                              // (slot 2n + 1) 32-column chunks of N tile n, for every OUTPUT row
   int epi_alt;                // 1: the two warps of a 32-row quarter swap chunk parity every tile (odd chunk counts)
   int nfast;                  // 1: N is the fast tile index (tile t -> n = t % tilesN, m = t / tilesN); needs ksplit == 1
   unsigned long long* timeline; // debug: per-tile role timestamps of CTA 0 (null = off)
@@ -108,10 +109,15 @@ VDB_DEVINL float apply_act(float v, int act) {
 // the B operand (the transposed V^T projection) the statistics belong to the output columns instead (ln_on_cols).
 //
 // Roles: warps 0-7 are two consumer warpgroups (warpgroup g computes output rows [64 g, 64 g + 64) of the tile with wgmma, fp32
-// accumulators in registers), warp 8 is the TMA producer.  After the mainloop of a tile both warpgroups park the accumulator in
-// shared memory (sacc, [128][BN + 4] fp32, aliasing the operand ring) and run the epilogue on it: each warp reads 32-column chunks
-// of one ROW per thread (acc_ld32), the layout the epilogue paths below are written for.  The producer starts the next tile's
-// loads once every consumer warp is done with sacc (acc_free).
+// accumulators in registers), warp 8 is the TMA producer.
+// Modes 3-7 run the epilogue from the registers, in the wgmma fragment layout: warp w owns 16 rows of the tile and walks their
+// 32-column chunks, staging each as a 16 x 32 bf16 box (stmatrix) for a TMA store.  The warpgroups do not wait for each other
+// after the mainloop, and the producer is gated by the empty barriers alone: it loads the next tile's first STAGES k-blocks while
+// the epilogue runs, so the next mainloop starts on a full ring.  tests/test_igemm_protocol_tma_epi.py models this protocol.
+// Modes 0-2 park the accumulator in shared memory (sacc, [128][BN + 4] fp32, aliasing the operand ring) after the mainloop and
+// run the epilogue on it: each warp reads 32-column chunks of one ROW per thread (acc_ld32), the layout those paths are written
+// for.  The producer starts the next tile's loads once every consumer warp is done with sacc (acc_free;
+// tests/test_igemm_protocol.py).
 template <int BN, int STAGES, int EW, int MODE>
 __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
   constexpr bool kTmaEpi = MODE >= 3;                 // TMA-store epilogues
@@ -213,7 +219,9 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         const int kb_begin = ks * p.kb_per_split;
         const int kb_end = min(p.kb_total, kb_begin + p.kb_per_split);
         int kb = 0;
-        if (it > 0) mbar_wait(acc_free, (it - 1) & 1);   // the ring holds the previous tile's accumulator until its epilogue ends
+        // modes 0-2: the ring holds the previous tile's accumulator until its epilogue ends.  The TMA-store modes keep it in
+        // registers, so only the empty barriers gate the ring and the next tile's first STAGES k-blocks load during the epilogue.
+        if (!kTmaEpi && it > 0) mbar_wait(acc_free, (it - 1) & 1);
         VDB_TL(0, it);   // producer: starts issuing this tile
         for (int s = 0; s < p.nseg; ++s) {
           const ASeg sg = p.seg[s];
@@ -253,12 +261,12 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         v[4 * i + 2] = __float_as_uint(x.z); v[4 * i + 3] = __float_as_uint(x.w);
       }
     };
-    // mainloop of one tile: warpgroup g multiplies its 64 rows of A by the BN x 64 B tile of every k-block, then both
-    // warpgroups park the accumulator in sacc
+    // mainloop of one tile: warpgroup g multiplies its 64 rows of A by the BN x 64 B tile of every k-block, then (modes 0-2)
+    // both warpgroups park the accumulator in sacc
     uint32_t ml_stage = 0, ml_phase = 0;
+    float acc[BN / 2];
     auto mainloop = [&](int kb_begin, int kb_end) {
       const int g = warp >> 2;
-      float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       uint32_t prev = 0;
@@ -282,14 +290,16 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       wgmma_fence_regs(acc);
       __syncwarp();
       if (lane == 0 && kb_end > kb_begin) mbar_arrive(&empty_bar[prev]);
-      epi_bar_sync();                   // sacc aliases the ring: both warpgroups' MMAs have finished reading it
-      float* srow = sacc + (g * 64 + (warp & 3) * 16 + (lane >> 2)) * kAccStride + 2 * (lane & 3);
+      if constexpr (!kTmaEpi) {
+        epi_bar_sync();                 // sacc aliases the ring: both warpgroups' MMAs have finished reading it
+        float* srow = sacc + (g * 64 + (warp & 3) * 16 + (lane >> 2)) * kAccStride + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(srow + 8 * kAccStride + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(srow + 8 * kAccStride + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        epi_bar_sync();
       }
-      epi_bar_sync();
     };
     auto stage_write = [&](const uint32_t (&v)[32]) {
       float* srow = stage + lane * 32;
@@ -305,7 +315,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       o[0] = x0.x; o[1] = x0.y; o[2] = x0.z; o[3] = x0.w; o[4] = x1.x; o[5] = x1.y; o[6] = x1.z; o[7] = x1.w;
     };
     int it = 0;
-    int st_buf = 0;                     // TMA-store epilogues: which of this warp's two staging tiles is written next
+    int st_buf = 0;                     // TMA-store epilogues: which of this warp's four staging boxes is written next
     (void)st_buf;
     const float* sbias_src = nullptr;   // which bias row/offset currently sits in sbias
     // The per-tile bookkeeping sits on the critical path of epilogue-bound GEMMs (it was ~0.75 us of every ~3.6 us
@@ -319,20 +329,33 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
     int unit_m = t_first % unitsM, rest = t_first / unitsM;
     const int nf_step_n = p.nfast ? t_step % p.tilesN : 0, nf_step_m = p.nfast ? t_step / p.tilesN : 0;   // (see the producer)
     int nf_n = p.nfast ? t_first % p.tilesN : 0, nf_m = p.nfast ? t_first / p.tilesN : 0;
-    // folded LayerNorm, row statistics: partial sums of the row this thread owns in the NEXT tile, requested a tile ahead
-    constexpr int kLnPre = 16;
+    // TMA-store epilogues: the accumulator stays in the wgmma fragment layout, so warp w owns the 16 tile rows from e_row0 on
+    // (warpgroup w / 4, quarter w % 4) and this thread rows e_row0 + lane / 4 and e_row0 + lane / 4 + 8, at columns
+    // 8 j + 2 (lane % 4) + {0, 1}
+    const int e_row0 = (warp >> 2) * 64 + (warp & 3) * 16;
+    int e_tw[2], e_th[2], e_tb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int er = e_row0 + (lane >> 2) + 8 * h;
+      e_tw[h] = er % p.TW; e_th[h] = (er / p.TW) % p.TH; e_tb[h] = er / (p.TW * p.TH);
+    }
+    // folded LayerNorm, row statistics: partial sums of the warp's rows in the NEXT tile, requested a tile ahead.  Lane l serves
+    // row e_row0 + l % 16: lanes 0-15 load partials 0-7, lanes 16-31 partials 8-15 of the same rows (kLnPre each)
+    constexpr int kLnPre = 8;
     float2 ln_pre[kLnIn ? kLnPre : 1];
     auto ln_prefetch = [&](int row) {
       if constexpr (kLnIn) {
         const bool ok = row < p.Wo;
+        const int i0 = (lane >> 4) * kLnPre;
 #pragma unroll
         for (int i = 0; i < kLnPre; ++i)
-          ln_pre[i] = (ok && i < p.ln_parts) ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + static_cast<long long>(i) * p.ln_mstat + row)
-                                              : make_float2(0.f, 0.f);
+          ln_pre[i] = (ok && i0 + i < p.ln_parts)
+                          ? __ldg(reinterpret_cast<const float2*>(p.ln_stats) + static_cast<long long>(i0 + i) * p.ln_mstat + row)
+                          : make_float2(0.f, 0.f);
       }
     };
     if constexpr (kLnIn) {
-      if (!p.ln_on_cols && p.ln_parts <= kLnPre && t_first < t_end) ln_prefetch((t_first % unitsM) * kBlockM + r);
+      if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t_first < t_end) ln_prefetch((t_first % unitsM) * kBlockM + e_row0 + (lane & 15));
     }
     for (int t = t_first; t < t_end; t += t_step, ++it) {
       const int m_idx = p.nfast ? nf_m : unit_m;
@@ -358,7 +381,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       // per-tile row bookkeeping for the transposed role (independent of the accumulator: done before the wait)
       int gp_k[4];
       bool ok_k[4];
-      {
+      if constexpr (!kTmaEpi) {
         const unsigned okmask = __ballot_sync(0xffffffffu, row_ok);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -432,33 +455,60 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         if (has_resid && f_first < f_nchunks) load_resid_fast(f_first, rr_first);
       }
 
-      // folded LayerNorm: this thread's row scalars (requested before the accumulator wait)
-      float ln_a0 = 0.f, ln_a1 = 1.f;     // on_cols 0: (mean, rstd) of the row;  on_cols 1: (s[m], c[m]) of the output row
-      if constexpr (kLnIn) {
-        if (row_ok) {
-          if (p.ln_on_cols) {
-            ln_a0 = __ldg(p.ln_colsum + gp);
-            ln_a1 = p.ln_rowbias ? __ldg(p.ln_rowbias + gp) : 0.f;
-          } else {
-            float su = 0.f, sq = 0.f;
-            if (p.ln_parts <= kLnPre) {
-              // the partials of THIS tile's row were requested one tile ago (ln_pre): a tile's own request would sit on the
-              // critical path of every epilogue-bound tile (first version: +75 % on the K = 320 GEMMs)
+      // TMA-store epilogues: output pixels (GEMM rows) of this thread's two accumulator rows
+      int e_gp[2];
+      bool e_ok[2];
 #pragma unroll
-              for (int i = 0; i < kLnPre; ++i) { su += ln_pre[i].x; sq += ln_pre[i].y; }
-            } else {
+      for (int h = 0; h < 2; ++h) {
+        const int ew = wt * p.TW + e_tw[h], eh = ht * p.TH + e_th[h], eb = bt * p.TB + e_tb[h];
+        e_ok[h] = (ew < p.Wo) && (eh < p.Ho) && (eb < p.Bo);
+        e_gp[h] = (eb * p.Ho + eh) * p.Wo + ew;
+      }
+      // folded LayerNorm: the scalars of this thread's two rows (requested before the accumulator wait)
+      float ln_a0[2] = {0.f, 0.f}, ln_a1[2] = {1.f, 1.f};   // on_cols 0: (mean, rstd) of the row;  on_cols 1: (s[m], c[m]) of the output row
+      if constexpr (kLnIn) {
+        if (p.ln_on_cols) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (e_ok[h]) {
+              ln_a0[h] = __ldg(p.ln_colsum + e_gp[h]);
+              ln_a1[h] = p.ln_rowbias ? __ldg(p.ln_rowbias + e_gp[h]) : 0.f;
+            }
+          }
+        } else {
+          // lane l sums the partials of row e_row0 + l % 16 in the order 0, 1, 2, ... and hands mean and rstd to the two lanes that
+          // hold the row (lanes 16-31 compute nothing useful)
+          float su = 0.f, sq = 0.f;
+          if (p.ln_parts <= 2 * kLnPre) {
+            // the partials of THIS tile's rows were requested one tile ago (ln_pre): a tile's own request would sit on the
+            // critical path of every epilogue-bound tile (first version: +75 % on the K = 320 GEMMs)
+#pragma unroll
+            for (int i = 0; i < kLnPre; ++i) { su += ln_pre[i].x; sq += ln_pre[i].y; }
+#pragma unroll
+            for (int i = 0; i < kLnPre; ++i) {
+              su += __shfl_sync(0xffffffffu, ln_pre[i].x, lane | 16);
+              sq += __shfl_sync(0xffffffffu, ln_pre[i].y, lane | 16);
+            }
+          } else {
+            const int row = m_idx * kBlockM + e_row0 + (lane & 15);
+            if (row < p.Wo) {
 #pragma unroll 8
               for (int ch = 0; ch < p.ln_parts; ++ch) {
-                const float2 v = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + static_cast<long long>(ch) * p.ln_mstat + gp);
+                const float2 v = __ldg(reinterpret_cast<const float2*>(p.ln_stats) + static_cast<long long>(ch) * p.ln_mstat + row);
                 su += v.x; sq += v.y;
               }
             }
-            ln_a0 = su * p.ln_inv_dim;
-            ln_a1 = rsqrtf(fmaxf(sq * p.ln_inv_dim - ln_a0 * ln_a0, 0.f) + p.ln_eps);
+          }
+          const float mu = su * p.ln_inv_dim;
+          const float rs = rsqrtf(fmaxf(sq * p.ln_inv_dim - mu * mu, 0.f) + p.ln_eps);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            ln_a0[h] = __shfl_sync(0xffffffffu, mu, (lane >> 2) + 8 * h);
+            ln_a1[h] = __shfl_sync(0xffffffffu, rs, (lane >> 2) + 8 * h);
           }
         }
         // request the next tile's row partials (GEMM view, M-fast order: unit_m already points at the next tile)
-        if (!p.ln_on_cols && p.ln_parts <= kLnPre && t + t_step < t_end) ln_prefetch(unit_m * kBlockM + r);
+        if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t + t_step < t_end) ln_prefetch(unit_m * kBlockM + e_row0 + (lane & 15));
       }
       VDB_TLE(4, it);   // consumers: mainloop starts
       mainloop(ks * p.kb_per_split, min(p.kb_total, ks * p.kb_per_split + p.kb_per_split));
@@ -504,148 +554,161 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         }
       };
       if constexpr (kTmaEpi) {
-        // ---- TMA-store epilogues (round 2).  Everything stays in the acc_ld32 layout (one ROW of 32 columns per thread):
-        // bias from shared memory (broadcast reads), residual as this row's own 64 contiguous bytes, bf16 pack, four 16-byte
-        // shared-memory stores into this warp's 32 x 32 staging tile (64-byte rows, SWIZZLE_64B pattern: conflict-free),
-        // then ONE thread hands the tile to the TMA unit (cp.async.bulk.tensor store; out-of-range rows / columns are clipped by
-        // the tensor map).  Against the fp32 transposition above this halves the shared-memory traffic of the epilogue
-        // (2 x 64 B instead of 2 x 128 B per row and chunk) and removes the 8 global-store instructions per thread and chunk —
-        // the K <= 640 GEMMs were bound by exactly that.  Two staging tiles per warp:
-        // the store of chunk i is read out while chunk i+1 is built.
-        uint8_t* stg = reinterpret_cast<uint8_t*>(sstage) + warp * 4096;
-        const int qrow = quarter * 32;                                   // first tile row of this warp's 32-row quarter
-        const int ow = wt * p.TW + (qrow % p.TW), oh = ht * p.TH + ((qrow / p.TW) % p.TH), ob = bt * p.TB + qrow / (p.TW * p.TH);
+        // ---- TMA-store epilogues, straight from the wgmma registers (no park, no barrier between the warpgroups).  Each warp
+        // walks the 32-column chunks of its 16 rows: per-element fp32 arithmetic on the thread's 2 rows x 8 columns of the chunk,
+        // bf16 pack, two stmatrix into one 1 KB staging box of this warp (16 rows of 64 B, SWIZZLE_64B pattern), then lane 0
+        // hands the box to the TMA unit (cp.async.bulk.tensor store; out-of-range rows / columns are clipped by the tensor
+        // map).  Four boxes per warp rotate: a box is rewritten once the store issued from it three chunks ago has read it.
+        // Bias / LayerNorm tables are read from shared memory as 8-byte broadcasts (columns 2 (lane % 4) + {0, 1}).
+        const uint32_t stg_s = smem_u32(sstage) + warp * 4096;
+        const int ow = wt * p.TW + (e_row0 % p.TW), oh = ht * p.TH + ((e_row0 / p.TW) % p.TH), ob = bt * p.TB + e_row0 / (p.TW * p.TH);
         constexpr int OUTC = kGegluEpi ? BN / 2 : BN;                    // output columns per tile
         const int ochunks = kGegluEpi ? OUTC / 32 : f_nchunks;
         const int ocol0 = n_idx * OUTC;
-        const int o_first = (((OUTC / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half;
-        auto load_resid_row = [&](int c, uint4 (&rr)[4]) {
-          const uint4* src = reinterpret_cast<const uint4*>(p.resid + static_cast<long long>(gp) * p.ldr + ocol0 + c * 32);
+        const int tq2 = 2 * (lane & 3);                                  // this thread's first column of every 8-column group
+        // residual (modes 3 / 7): the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each,
+        // requested a chunk ahead
+        const bool do_resid = (MODE == 3 || MODE == 7) && has_resid;
+        const uint32_t* rrow[2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) rr[k] = __ldg(src + k);
+        for (int h = 0; h < 2; ++h)
+          rrow[h] = (do_resid && e_ok[h]) ? reinterpret_cast<const uint32_t*>(p.resid + static_cast<long long>(e_gp[h]) * p.ldr + ocol0 + tq2)
+                                          : nullptr;
+        auto load_resid = [&](int c, uint32_t (&rr)[2][4]) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rrow[h] ? __ldg(rrow[h] + (c * 32 + 8 * jj) / 2) : 0u;
         };
-        uint4 rr[4];
-        float st_su = 0.f, st_sq = 0.f;                                  // mode 7: partial LayerNorm sums of this thread's columns
+        uint32_t rr[2][4];
+        if (do_resid) load_resid(0, rr);
+        float st_su[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // mode 7: [row][chunk parity]
         (void)st_su; (void)st_sq;
-        const bool do_resid = (MODE == 3 || MODE == 7) && has_resid && row_ok;
-        if (do_resid && o_first < ochunks) load_resid_row(o_first, rr);
-#pragma unroll 1
-        for (int c = o_first; c < ochunks; c += kWPQ) {
-          float o[32];
-          if constexpr (MODE == 6) {
-            // GEGLU over a folded LayerNorm (row statistics only): value and gate both get the rank-1 correction
-            uint32_t va[32], vg[32];
-            acc_ld32(c * 32, va);
-            acc_ld32(OUTC + c * 32, vg);
-            // r * (acc - mu * s) + c  ==  fma(r, acc, fma(-r mu, s, c)); the tables are read as 16-byte broadcasts
-            const float nrm = -ln_a1 * ln_a0;
+        float nrm[2];                                                    // LN rows: -rstd * mean of the row
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 sa = lds_f4(slnx_s + 4 * (c * 32 + j)), ca = lds_f4(sbias_s + 4 * (c * 32 + j));
-              const float4 sg = lds_f4(slnx_s + 4 * (OUTC + c * 32 + j)), cg = lds_f4(sbias_s + 4 * (OUTC + c * 32 + j));
-              o[j] = fmaf(ln_a1, __uint_as_float(va[j]), fmaf(nrm, sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1, __uint_as_float(vg[j]), fmaf(nrm, sg.x, cg.x)));
-              o[j + 1] = fmaf(ln_a1, __uint_as_float(va[j + 1]), fmaf(nrm, sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1, __uint_as_float(vg[j + 1]), fmaf(nrm, sg.y, cg.y)));
-              o[j + 2] = fmaf(ln_a1, __uint_as_float(va[j + 2]), fmaf(nrm, sa.z, ca.z)) * gelu_fast_f(fmaf(ln_a1, __uint_as_float(vg[j + 2]), fmaf(nrm, sg.z, cg.z)));
-              o[j + 3] = fmaf(ln_a1, __uint_as_float(va[j + 3]), fmaf(nrm, sa.w, ca.w)) * gelu_fast_f(fmaf(ln_a1, __uint_as_float(vg[j + 3]), fmaf(nrm, sg.w, cg.w)));
-            }
-          } else if constexpr (MODE == 5) {
-            uint32_t v[32];
-            acc_ld32(c * 32, v);
-            if (p.ln_on_cols) {          // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
-              const float ns = -ln_a0;
+        for (int h = 0; h < 2; ++h) nrm[h] = -ln_a1[h] * ln_a0[h];
+        (void)nrm;
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 mu = lds_f4(slnx_s + 4 * (c * 32 + j)), rs = lds_f4(sbias_s + 4 * (c * 32 + j));
-                o[j] = fmaf(rs.x, fmaf(mu.x, ns, __uint_as_float(v[j])), ln_a1);
-                o[j + 1] = fmaf(rs.y, fmaf(mu.y, ns, __uint_as_float(v[j + 1])), ln_a1);
-                o[j + 2] = fmaf(rs.z, fmaf(mu.z, ns, __uint_as_float(v[j + 2])), ln_a1);
-                o[j + 3] = fmaf(rs.w, fmaf(mu.w, ns, __uint_as_float(v[j + 3])), ln_a1);
-              }
-            } else {                     // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
-              const float nrm = -ln_a1 * ln_a0;
+        for (int c = 0; c < OUTC / 32; ++c) {
+          if (c >= ochunks) break;
+          float o[4][2][2];                                              // [8-column group][row][column]
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 sx = lds_f4(slnx_s + 4 * (c * 32 + j)), cx = lds_f4(sbias_s + 4 * (c * 32 + j));
-                o[j] = fmaf(ln_a1, __uint_as_float(v[j]), fmaf(nrm, sx.x, cx.x));
-                o[j + 1] = fmaf(ln_a1, __uint_as_float(v[j + 1]), fmaf(nrm, sx.y, cx.y));
-                o[j + 2] = fmaf(ln_a1, __uint_as_float(v[j + 2]), fmaf(nrm, sx.z, cx.z));
-                o[j + 3] = fmaf(ln_a1, __uint_as_float(v[j + 3]), fmaf(nrm, sx.w, cx.w));
-              }
-            }
-          } else if constexpr (MODE == 4) {
-            uint32_t va[32], vg[32];
-            acc_ld32(c * 32, va);
-            acc_ld32(OUTC + c * 32, vg);
+          for (int jj = 0; jj < 4; ++jj) {
+            const int n = c * 32 + 8 * jj + tq2;                         // tile column of o[jj][.][0]
+            const float* va = acc + 4 * (4 * c + jj);                    // {row 0: n, n + 1; row 8: n, n + 1}
+            if constexpr (kGegluEpi) {
+              const float* vg = acc + 4 * (BN / 16 + 4 * c + jj);        // gate columns OUTC + n
+              if constexpr (kLnIn) {   // GEGLU over a folded LayerNorm: r * (acc - mu * s) + c == fma(r, acc, fma(-r mu, s, c))
+                const float2 sa = lds_f2(slnx_s + 4 * n), ca = lds_f2(sbias_s + 4 * n);
+                const float2 sg = lds_f2(slnx_s + 4 * (OUTC + n)), cg = lds_f2(sbias_s + 4 * (OUTC + n));
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 ba = p.bias ? lds_f4(sbias_s + 4 * (c * 32 + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              const float4 bg = p.bias ? lds_f4(sbias_s + 4 * (OUTC + c * 32 + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              o[j] = (__uint_as_float(va[j]) + ba.x) * gelu_fast_f(__uint_as_float(vg[j]) + bg.x);
-              o[j + 1] = (__uint_as_float(va[j + 1]) + ba.y) * gelu_fast_f(__uint_as_float(vg[j + 1]) + bg.y);
-              o[j + 2] = (__uint_as_float(va[j + 2]) + ba.z) * gelu_fast_f(__uint_as_float(vg[j + 2]) + bg.z);
-              o[j + 3] = (__uint_as_float(va[j + 3]) + ba.w) * gelu_fast_f(__uint_as_float(vg[j + 3]) + bg.w);
-            }
-          } else {
-            uint32_t v[32];
-            acc_ld32(c * 32, v);
-            uint4 rn[4];
-            const bool more = c + kWPQ < ochunks;
-            if (do_resid && more) load_resid_row(c + kWPQ, rn);
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h], fmaf(nrm[h], sg.x, cg.x)));
+                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h + 1], fmaf(nrm[h], sg.y, cg.y)));
+                }
+              } else {
+                const float2 ba = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
+                const float2 bg = p.bias ? lds_f2(sbias_s + 4 * (OUTC + n)) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 bb = p.bias ? lds_f4(sbias_s + 4 * (c * 32 + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              o[j] = __uint_as_float(v[j]) + bb.x; o[j + 1] = __uint_as_float(v[j + 1]) + bb.y;
-              o[j + 2] = __uint_as_float(v[j + 2]) + bb.z; o[j + 3] = __uint_as_float(v[j + 3]) + bb.w;
-            }
-            if (do_resid) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const uint32_t w4[4] = {rr[k].x, rr[k].y, rr[k].z, rr[k].w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 x = unpack_bf16x2(w4[q]);
-                  o[k * 8 + 2 * q] += x.x;
-                  o[k * 8 + 2 * q + 1] += x.y;
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = (va[2 * h] + ba.x) * gelu_fast_f(vg[2 * h] + bg.x);
+                  o[jj][h][1] = (va[2 * h + 1] + ba.y) * gelu_fast_f(vg[2 * h + 1] + bg.y);
                 }
               }
-              if (more) {
+            } else if constexpr (kLnIn) {
+              if (p.ln_on_cols) {      // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
+                const float2 mu = lds_f2(slnx_s + 4 * n), rs = lds_f2(sbias_s + 4 * n);
 #pragma unroll
-                for (int k = 0; k < 4; ++k) rr[k] = rn[k];
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(rs.x, fmaf(mu.x, -ln_a0[h], va[2 * h]), ln_a1[h]);
+                  o[jj][h][1] = fmaf(rs.y, fmaf(mu.y, -ln_a0[h], va[2 * h + 1]), ln_a1[h]);
+                }
+              } else {                 // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
+                const float2 sx = lds_f2(slnx_s + 4 * n), cx = lds_f2(sbias_s + 4 * n);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sx.x, cx.x));
+                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sx.y, cx.y));
+                }
               }
+            } else {                   // modes 3 / 7: acc + bias, then + residual
+              const float2 bb = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                o[jj][h][0] = va[2 * h] + bb.x;
+                o[jj][h][1] = va[2 * h + 1] + bb.y;
+              }
+            }
+          }
+          if (do_resid) {
+            uint32_t rn[2][4];
+            const bool more = c + 1 < ochunks;
+            if (more) load_resid(c + 1, rn);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const float2 x = unpack_bf16x2(rr[h][jj]);
+                o[jj][h][0] += x.x;
+                o[jj][h][1] += x.y;
+              }
+            if (more) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rn[h][jj];
             }
           }
           if constexpr (kStatsOut) {
-            // LayerNorm statistics of the rows this GEMM produces: this thread's columns of the tile (fp32, before the rounding)
-            float su = 0.f, sq = 0.f;
+            // LayerNorm statistics of the rows this GEMM produces (fp32, before the rounding), split by chunk parity
 #pragma unroll
-            for (int j = 0; j < 32; ++j) { su += o[j]; sq = fmaf(o[j], o[j], sq); }
-            st_su += su; st_sq += sq;
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  st_su[h][c & 1] += o[jj][h][e];
+                  st_sq[h][c & 1] = fmaf(o[jj][h][e], o[jj][h][e], st_sq[h][c & 1]);
+                }
           }
-          // the staging tile about to be rewritten was handed to the TMA unit two chunks ago: wait until it has been read
-          if (lane == 0) bulk_wait_read<1>();
+          // the box about to be rewritten was handed to the TMA unit three chunks ago: wait until it has been read
+          if (lane == 0) bulk_wait_read<3>();
           __syncwarp();
-          uint8_t* tile = stg + st_buf * 2048;
-          const uint32_t trow_s = smem_u32(tile) + lane * 64;
+          const uint32_t box = stg_s + st_buf * 1024;
+          {
+            // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
+            // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
+            const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(trow_s + ((q ^ ((lane >> 1) & 3)) << 4)),
-                         "r"(pack_bf16x2(o[q * 8], o[q * 8 + 1])), "r"(pack_bf16x2(o[q * 8 + 2], o[q * 8 + 3])),
-                         "r"(pack_bf16x2(o[q * 8 + 4], o[q * 8 + 5])), "r"(pack_bf16x2(o[q * 8 + 6], o[q * 8 + 7]))
-                         : "memory");
+            for (int u = 0; u < 2; ++u) {
+              const int unit = 2 * u + (mi >> 1);
+              stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
+                          pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
+                          pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
+            }
           }
           fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
           __syncwarp();
           if (lane == 0) {
-            tma_store_4d(&p.tmO, tile, ocol0 + c * 32, ow, oh, ob);
+            tma_store_4d(&p.tmO, reinterpret_cast<const uint8_t*>(sstage) + warp * 4096 + st_buf * 1024, ocol0 + c * 32, ow, oh, ob);
             bulk_commit();
           }
-          st_buf ^= 1;
+          st_buf = (st_buf + 1) & 3;
         }
         if constexpr (kStatsOut) {
-          // one partial per (N tile, warp of the lane quarter): the two warps own disjoint chunk sets (o_first = 0 / 1)
-          if (row_ok)
-            reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * kWPQ + o_first) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + gp] =
-                make_float2(st_su, st_sq);
+          // one (sum, sum of squares) per row, N tile and chunk parity: slot 2 n_idx + parity of [2 tilesN][M][2].  The four lanes
+          // of a row reduce over the quad; a parity without chunks writes zeros
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int par = 0; par < 2; ++par) {
+              float su = st_su[h][par], sq = st_sq[h][par];
+              su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+              su += __shfl_xor_sync(0xffffffffu, su, 2); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+              if ((lane & 3) == 0 && e_ok[h])
+                reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * 2 + par) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + e_gp[h]] =
+                    make_float2(su, sq);
+            }
         }
       } else if constexpr (MODE == 1) {
         // lean fast path: every chunk is a full 32-column bf16 chunk with one bias row; the residual rows of the
@@ -808,10 +871,12 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
           chunk(c, v, rr, is_fast(c));
         }
       }
-      fence_proxy_async_smem();        // this warp's sacc reads are ordered before the producer's next TMA writes
-      __syncwarp();
-      VDB_TLE(6, it);   // epilogue: tile stored (this warp)
-      if (lane == 0) mbar_arrive(acc_free);
+      if constexpr (!kTmaEpi) {
+        fence_proxy_async_smem();      // this warp's sacc reads are ordered before the producer's next TMA writes
+        __syncwarp();
+        VDB_TLE(6, it);   // epilogue: tile stored (this warp)
+        if (lane == 0) mbar_arrive(acc_free);
+      }
     }
     if constexpr (MODE >= 3) {
       if (lane == 0) bulk_wait<0>();     // every TMA store of this thread has completed before the CTA may exit
@@ -1049,11 +1114,11 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     else if (e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0) mode = 1;
   }
   // TMA-store epilogues (modes 3 / 4 = modes 1 / 2 with the output tile leaving through shared memory + cp.async.bulk.tensor;
-  // VDB_EPI_TMA=0 keeps the transposing epilogues): the warp's 32 rows x 32 columns must be one box of the output tensor map
+  // VDB_EPI_TMA=0 keeps the transposing epilogues): a warp's 16 rows x 32 columns must be one box of the output tensor map
   static const int epi_tma = [] { const char* ev = getenv("VDB_EPI_TMA"); return (ev && ev[0] == '0') ? 0 : 1; }();
   if (epi_tma && (mode == 1 || mode == 2) && (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 &&
       (!e.resid || (reinterpret_cast<uintptr_t>(e.resid) & 15) == 0)) {
-    const int bw = std::min(p.TW, 32), bh = std::min(p.TH, 32 / bw), bb = 32 / (bw * bh);
+    const int bw = std::min(p.TW, 16), bh = std::min(p.TH, 16 / bw), bb = 16 / (bw * bh);
     const long long ncols = (mode == 2) ? N / 2 : N;
     // out_parity >= 0: the same tile, written into every second pixel of every second row of the [B, 2Ho, 2Wo, N] tensor —
     // only the strides and the base of the output tensor map change, the kernel does not know
