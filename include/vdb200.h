@@ -24,7 +24,8 @@ extern "C" {
 #endif
 
 enum { VDB_OK = 0, VDB_ERR_INVALID = 1, VDB_ERR_CUDA = 2, VDB_ERR_UNSUPPORTED = 3 };
-enum { VDB_ACT_NONE = 0, VDB_ACT_SILU = 1, VDB_ACT_GELU = 2, VDB_ACT_QUICK_GELU = 3, VDB_ACT_GEGLU = 4 };
+enum { VDB_ACT_NONE = 0, VDB_ACT_SILU = 1, VDB_ACT_GELU = 2, VDB_ACT_QUICK_GELU = 3, VDB_ACT_GEGLU = 4,
+       VDB_ACT_GELU_TANH = 5 /* GPT-2's tanh approximation; vdb_textdec_gemv only */ };
 
 /* ---- library state ------------------------------------------------------------------------- */
 const char* vdb_version(void);
@@ -233,6 +234,37 @@ int vdb_pack_geglu(const float* w, const float* b, int n2, int K, void* w_out, f
 /* CrossAttention.to_q / to_k / to_v weight [H*d, K] (attention.py:152-168) -> [H*dpad, K] with zero rows after each head's d
  * rows; dpad = vdb_attention_dk_pad(d) for q / k, vdb_attention_dv_pad(d) for v. */
 int vdb_pad_heads(const float* w, int H, int d, int dpad, int K, void* out, void* stream);
+
+/* ---- Optimus GPT-2 text decoder, one token step for R <= 16 rows — optimus_vae_next.decode / sample_single_sequence_conditional
+ *      (optimus.py:662-688, 746-763) over GPT2ForLatentConnector_XX (optimus_gpt2.py:870-994, 1025-1082).  The step index is a
+ *      device int (`step` = the input token's index s, advanced with vdb_add_int), so one captured graph serves every step.
+ *      Residual stream, activations, logits and the KV cache are fp32; weights bf16 [N, K] (Conv1D's [in, out] transposed). ---- */
+/* out[r, n] = act( LN(x)[r, :] . W[n, :] + bias[n] ), or out += that (accumulate != 0: the in-place residual add of Block.forward,
+ * optimus_gpt2.py:236-240).  LN = LayerNorm(gamma, beta, eps) of the fp32 row when ln_gamma != NULL (ln_1 / ln_2 / ln_f fused into
+ * c_attn / c_fc / lm_head), else the identity.  act VDB_ACT_NONE or VDB_ACT_GELU_TANH (MLP.act).  Replaces Conv1D.forward
+ * (modeling_utils.py:420-424) for attn.c_attn / attn.c_proj / mlp.c_fc / mlp.c_proj, transformer.linear / linear_emb and
+ * lm_head.  1 <= R <= 16, K % 32 == 0, K <= 3072, W 16-byte aligned with ldw % 8 == 0, x != out.  Reads every weight once. */
+int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const float* ln_gamma, const float* ln_beta, float ln_eps,
+                     const void* W, long long N, long long ldw, const float* bias, int act, int accumulate, float* out, long long ldo,
+                     void* stream);
+/* Attention.forward for the one new query of each row (optimus_gpt2.py:205-227, _attn :152-175), d_head 64.  qkv [R, ldq] holds
+ * c_attn's q | k | v (H*64 each); this step's k / v are appended at slot *step of kcache / vcache ([R][H][T][64] fp32, this
+ * layer); the keys are the layer's latent slice mem[r, h*64 ..] (key == value, position 0) then slots 0 .. *step.  out [R, H*64]. */
+int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache, int R,
+                          int H, int T, const int* step, float scale, float* out, long long ldo, void* stream);
+/* h[r, :] = wte[tokens[r, s]] + wpe[s + pos_offset] + emb[r, :], s = *step: the embedding sum of GPT2Model_XX.forward
+ * (optimus_gpt2.py:941-948) with emb = linear_emb(z); pos_offset 1 (the latent is position 0).  fp32 wte [V, D], wpe [P, D]. */
+int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* wte, int V, const float* wpe, int P, int pos_offset,
+                      const float* emb, int R, int D, float* h, void* stream);
+/* torch.multinomial(softmax(logits / temperature)) of sample_single_sequence_conditional (top_k 0, top_p 1: no filtering), by
+ * inverse CDF of u in [0, 1): u = uniforms[r * ldu + s] when uniforms != NULL, else a Philox4x32-10 draw keyed by *seed (device
+ * u64) at counter (r, s).  forced != NULL takes token s+1 from forced[r * ldf + s + 1] instead (teacher forcing).  Writes
+ * tokens[r * ldt + s + 1]; == eos sets done[r] = 1 and lengths[r] = s + 2; when s + 1 == max_len - 2 a non-eos row also gets eos at
+ * s + 2 (the reference overwrites the max_len-th token, so its last draw is skipped).  Rows with done[r] != 0 are left frozen.
+ * record (may be NULL) receives the step's logits at record[(s * R + r) * V ..]. */
+int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
+                       const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
+                       const int* step, int eos, int max_len, float* record, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,111 @@
+"""Optimus text decoding on one GPU at full size (12 layers, vocabulary 50260), synthetic weights, 4 rows (app.py's n_sample_text),
+<EOS> never drawn so every row runs all 28 token steps.  Reports, from CUDA events after warm-up: ms per token step (replays of the
+captured step graph), launches per step, and the bytes a step must read over its time against 3.35 TB/s (H100 SXM data sheet);
+then one complete i2t call: 50 DDIM steps on the text latent, then the decode.  Prints the card name and power limit.
+    python tools/text_decode_bench.py [--no-i2t]"""
+import json
+import os
+import subprocess
+import sys
+import time
+
+os.environ["VDB_TEXT_FLOWS"] = "1"
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "versatile-diffusion_b200"))
+import torch  # noqa: E402
+from lib.cfg_helper import model_cfg_bank  # noqa: E402
+from lib.model_zoo import get_model  # noqa: E402
+from lib.model_zoo.ddim import DDIMSampler  # noqa: E402
+from lib.model_zoo.optimus import STEPS_PER_CHECK  # noqa: E402
+from vdb200 import ops  # noqa: E402
+
+HBM = 3.35e12
+dev = torch.device("cuda", 0)
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                      text=True).stdout.strip()
+print("card:", card)
+cfg = model_cfg_bank()('vd_four_flow_v1-0')
+cfg.args.ctx_cfg_list = []
+cfg.args.vae_cfg_list = [v for v in cfg.args.vae_cfg_list if v[0] == "text"]
+t0 = time.time()
+torch.manual_seed(0)
+with torch.device(dev):
+    net = get_model()(cfg, verbose=False)
+g = torch.Generator(device=dev).manual_seed(1)
+with torch.no_grad():
+    for _, p in net.named_parameters():
+        if p.ndim == 1 or not bool(p.any()):
+            if p.ndim == 1 and p.shape[0] > 0 and bool((p == 1).all()):
+                continue
+            p.normal_(0.0, 0.02, generator=g)
+net.eval()
+net.to(dev)
+vae = net.vae["text"]
+print(f"built in {time.time() - t0:.1f} s")
+
+R = 4
+z = torch.randn(R, 768, generator=torch.Generator().manual_seed(3)).to(dev) * 3.0
+with torch.no_grad():
+    for _ in range(2):
+        vae.decode_ids(z, eos_token=-1)                      # warm-up: packs weights, captures the step-chunk graph
+    p = vae.packed()
+    st = vae._state(R, dev)
+    graph = st.graphs[(1.0, -1, 30, "seed", False)]
+    n0 = ops.launch_count()
+    vae._step(st, p, 1.0, -1, 30, "seed", False)
+    launches = ops.launch_count() - n0
+    torch.cuda.synchronize()
+    reps = 20
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    st.step.zero_()
+    e0.record()
+    for i in range(reps):
+        st.step.zero_()                                       # keep the step index inside the 28-step window
+        graph.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    ms_step = e0.elapsed_time(e1) / (reps * STEPS_PER_CHECK)
+    wbytes = sum(t.numel() * t.element_size() for L in p["layers"] for t in L.values() if torch.is_tensor(t))
+    wbytes += sum(t.numel() * t.element_size() for L in p["layers"] for pair in (L["ln1"], L["ln2"]) for t in pair[:2])
+    wbytes += p["lm_head"].numel() * 2 + R * 50260 * 4 * 2       # LM head weights, logits written then read by the sampler
+    # one full decode call (28 steps, host checks every STEPS_PER_CHECK steps)
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(5):
+        vae.decode_ids(z, eos_token=-1)
+    e1.record()
+    torch.cuda.synchronize()
+    ms_decode = e0.elapsed_time(e1) / 5
+res = dict(card=card, rows=R, ms_per_token_step=round(ms_step, 4), launches_per_step=launches,
+           bytes_per_step=wbytes, achieved_TBps=round(wbytes / (ms_step * 1e-3) / 1e12, 3),
+           share_of_3_35_TBps=round(wbytes / (ms_step * 1e-3) / HBM, 3), ms_per_decode_28_steps=round(ms_decode, 3))
+print(json.dumps(res))
+
+if "--no-i2t" not in sys.argv:
+    bs = 4
+    gq = torch.Generator().manual_seed(3)
+    xT = torch.randn(bs, 768, generator=gq).to(dev)
+    c = (torch.randn(bs, 257, 768, generator=gq) * 0.5).to(dev)
+    u = torch.zeros(bs, 257, 768, device=dev)
+    S = DDIMSampler(net)
+    kw = dict(steps=50, shape=[bs, 768], x_info={"type": "text", "xt": xT},
+              c_info={"type": "image", "conditioning": c, "unconditional_conditioning": u, "unconditional_guidance_scale": 7.5},
+              verbose=False, eta=0.)
+    with torch.no_grad():
+        for _ in range(2):
+            x, _ = S.sample(**{**kw, "x_info": {"type": "text", "xt": xT.clone()}})
+            vae.decode_ids(x)                                 # the ids: no vocabulary file is needed to time the decode
+        t_diff, t_dec = [], []
+        for _ in range(3):
+            torch.cuda.synchronize()
+            t1 = time.perf_counter()
+            x, _ = S.sample(**{**kw, "x_info": {"type": "text", "xt": xT.clone()}})
+            torch.cuda.synchronize()
+            t2 = time.perf_counter()
+            rows = vae.decode_ids(x)
+            torch.cuda.synchronize()
+            t3 = time.perf_counter()
+            t_diff.append((t2 - t1) * 1e3); t_dec.append((t3 - t2) * 1e3)
+    print(json.dumps(dict(card=card, i2t_ms_diffusion_50_steps=round(min(t_diff), 2), i2t_ms_decode=round(min(t_dec), 2),
+                          i2t_decode_tokens=[len(r) for r in rows])))

@@ -2,8 +2,9 @@
 
 The reference resolves YAML with `super_cfg` inheritance and MODEL(name) indirection; the values below
 are the resolved results for the shipped configs (configs/model/{vd,openai_unet,autokl,clip}.yaml).
-Text-latent flows (Optimus VAE, 0D data blocks) are outside the hot path: 'vd_four_flow_v1-0' here
-carries the image VAE, both CLIP context encoders, the 2D diffuser and the 0D diffuser's context blocks.
+By default 'vd_four_flow_v1-0' carries the image VAE, both CLIP context encoders, the 2D diffuser and the 0D diffuser's context
+blocks.  VDB_TEXT_FLOWS=1 adds what the i2t / t2t flows need: the 0D diffuser's data blocks and the Optimus text VAE's GPT-2
+decoder (vae.text).
 """
 import copy
 import os
@@ -82,17 +83,30 @@ for _sfx, _parts in _PARTS.items():
     _BANK["openai_unet_0d_v1" + _sfx] = _unet0d(_parts)
 
 
+def _optimus_text_vae():
+    """configs/model/optimus.yaml 'optimus_v1', decoder side only (the BERT encoder is not built).  The GPT-2 vocabulary is read
+    from the reference's relative path, where app.py runs; no public bank name (the default build has no text VAE)."""
+    return dict(symbol="optimus", find_unused_parameters=False, type="optimus_vae_next", args=dict(
+        decoder=dict(type="optimus_gpt2_connector", args=dict(config=dict(
+            vocab_size=50260, n_positions=1024, n_ctx=1024, n_embd=768, n_layer=12, n_head=12, layer_norm_epsilon=1e-5,
+            latent_size=768), latent_size=768)),
+        tokenizer_decoder=dict(type="optimus_gpt2_tokenizer", args=dict(
+            vocab_file="lib/model_zoo/optimus_models/vocab/gpt2-vocab.json")),
+        args=dict(latent_size=768)))
+
+
 class model_cfg_bank(object):
     def __call__(self, name):
         if name == "vd_four_flow_v1-0":
             cfg = CfgDict(copy.deepcopy(_BANK["vd_base"]))
+            text_flows = os.environ.get("VDB_TEXT_FLOWS") == "1"
             cfg.args.update(dict(
-                vae_cfg_list=[["image", self("autokl_v1")]],
+                vae_cfg_list=[["image", self("autokl_v1")]] + ([["text", CfgDict(_optimus_text_vae())]] if text_flows else []),
                 ctx_cfg_list=[["image", self("clip_image_context_encoder")], ["text", self("clip_text_context_encoder")]],
                 # the 0D (text-latent) diffuser contributes only its context blocks to image sampling; VDB_TEXT_FLOWS=1 builds its
                 # data blocks too (the reference's 'openai_unet_0d_v1_dc': +1.7 G parameters) for the i2t / t2t diffusion
                 diffuser_cfg_list=[["image", self("openai_unet_2d_v1")],
-                                   ["text", self("openai_unet_0d_v1_dc" if os.environ.get("VDB_TEXT_FLOWS") == "1" else "openai_unet_0d_v1_c")]],
+                                   ["text", self("openai_unet_0d_v1_dc" if text_flows else "openai_unet_0d_v1_c")]],
                 global_layer_ptr="image", latent_scale_factor={"image": 0.18215}))
             return cfg
         if name not in _BANK:

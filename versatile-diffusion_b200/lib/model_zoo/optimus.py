@@ -1,0 +1,359 @@
+"""Optimus text VAE, decoder side, on vdb200 kernels — reference lib/model_zoo/optimus.py:662-688, 746-763 (optimus_vae_next.decode)
+over GPT2ForLatentConnector_XX (optimus_models/optimus_gpt2.py:813-994, 1025-1082), configs/model/optimus.yaml.
+
+decode(z) turns text latents [n, 768] into strings, the last call of app.py's i2t / t2t flows (`net.vae_decode(x, which='text')`).
+GPT-2 (LayerNorm eps 1e-5, tanh GELU, Conv1D weights [in, out], attention scale 1/8) runs one token at a time for all n rows as one
+batch, with the latent injected twice: `transformer.linear` maps z to one slice per layer that is both key and value of position 0,
+and `transformer.linear_emb` is added to every token embedding (positions start at 1).  The LM head is tied to `wte`.
+
+Differences from the reference, all deliberate:
+  - the reference decodes each latent alone and re-runs the whole prefix at every token; here every row advances one token per step
+    over a KV cache, and a row that has finished keeps its tokens frozen while the others continue;
+  - the draw of token s+1 of row r is an inverse-CDF pick of softmax(logits / temperature) with a Philox4x32-10 uniform at counter
+    (r, s), keyed by one 64-bit seed taken from torch's default CPU generator per decode() call: `torch.manual_seed` fixes the text,
+    but the tokens are not those torch.multinomial would draw;
+  - the full softmax is sampled.  The reference's top_k_top_p_filtering(top_p=1.0) removes nothing in exact arithmetic but, in fp32,
+    can cut a tail whose sorted cumulative sum rounds above 1.0 (probability mass of order 1e-6);
+  - the reference's 29th forward pass, whose draw is always overwritten with <EOS>, is skipped;
+  - weights are bf16 (packed at load); the residual stream, attention, logits and the sampler's sums are fp32 / fp64.
+encode (the BERT encoder) is not part of this build.
+"""
+import json
+import os
+
+import torch
+import torch.nn as nn
+
+from lib.model_zoo.common.get_model import register
+from .diffusion_utils import PackedModule, bf16, f32, require_cuda
+
+symbol = 'optimus'
+
+PAD_ID, BOS_ID, EOS_ID = 50257, 50258, 50259     # added in the order <PAD>, <BOS>, <EOS> after GPT-2's 50257 tokens (optimus.py:30-34)
+MAX_LENGTH = 30                                   # optimus.py:756 (max_length=30)
+CACHE_SLOTS = 32                                  # token slots of the KV cache (a sequence holds at most MAX_LENGTH - 1 inputs)
+# Steps per captured graph between two host reads of the all-done flags.  A step of the full-size decoder streams ~247 MB of weights
+# (>= 74 us at 3.35 TB/s); a host read of the flags costs one device sync plus a graph launch, a few tens of us.  A chunk of 4
+# caps the steps that run after every row has finished at 3 and the syncs of a full-length decode (28 steps) at 7.
+STEPS_PER_CHECK = 4
+DEFAULT_VOCAB_FILE = 'lib/model_zoo/optimus_models/vocab/gpt2-vocab.json'   # relative to the reference's tree, where app.py runs
+
+
+def _ops():
+    from vdb200 import ops
+    return ops
+
+
+class VocabularyMissingError(RuntimeError):
+    pass
+
+
+# ---------------------------------------------------------------------------------------------------------- detokenizer
+def _byte_to_char():
+    """GPT-2's reversible byte <-> printable-character table: printable Latin-1 bytes stand for themselves, every other byte b is
+    the character 256 + (its rank among the non-printable bytes)."""
+    keep = list(range(ord('!'), ord('~') + 1)) + list(range(0xA1, 0xAC + 1)) + list(range(0xAE, 0xFF + 1))
+    table, extra = {}, 0
+    for b in range(256):
+        if b in keep:
+            table[b] = chr(b)
+        else:
+            table[b] = chr(256 + extra)
+            extra += 1
+    return table
+
+
+_CLEANUP = ((' .', '.'), (' ?', '?'), (' !', '!'), (' ,', ','), (" ' ", "'"), (" n't", "n't"), (" 'm", "'m"), (" do not", " don't"),
+            (" 's", "'s"), (" 've", "'ve"), (" 're", "'re"))
+
+
+class GPT2Detokenizer(object):
+    """ids -> text as the reference's GPT2Tokenizer.decode(ids, clean_up_tokenization_spaces=True) with <PAD> / <BOS> / <EOS> added:
+    byte-level tokens are joined and decoded as UTF-8 with errors='replace', each added token contributes " " + its text, then the
+    tokenizer's clean-up replacements run.  The vocabulary (gpt2-vocab.json) is read on first use."""
+    ADDED = {PAD_ID: '<PAD>', BOS_ID: '<BOS>', EOS_ID: '<EOS>'}
+
+    def __init__(self, vocab_file=DEFAULT_VOCAB_FILE):
+        self.vocab_file = vocab_file
+        self._id_to_bytes = None
+
+    def _load(self):
+        if self._id_to_bytes is None:
+            if not os.path.isfile(self.vocab_file):
+                raise VocabularyMissingError(
+                    f"GPT-2 vocabulary '{self.vocab_file}' not found (cwd {os.getcwd()}): the text decoder needs the Optimus "
+                    "gpt2-vocab.json to turn token ids into text; set the text VAE's vocab_file, or call decode_ids() for the ids")
+            with open(self.vocab_file, encoding='utf-8') as fh:
+                enc = json.load(fh)
+            char_to_byte = {c: b for b, c in _byte_to_char().items()}
+            self._id_to_bytes = {i: bytes(char_to_byte[c] for c in tok) for tok, i in enc.items()}
+        return self._id_to_bytes
+
+    def decode(self, ids):
+        table = self._load()
+        parts, run = [], bytearray()
+        for i in ids:
+            i = int(i)
+            if i in self.ADDED:
+                if run:
+                    parts.append(run.decode('utf-8', errors='replace'))
+                    run = bytearray()
+                parts.append(' ' + self.ADDED[i])
+            else:
+                run += table[i]
+        if run:
+            parts.append(run.decode('utf-8', errors='replace'))
+        text = ''.join(parts)
+        for a, b in _CLEANUP:
+            text = text.replace(a, b)
+        return text
+
+    def sentence(self, ids):
+        """optimus.py:759-762: decode, drop the first and last words (<BOS>, <EOS>), join with single spaces."""
+        return ' '.join(self.decode(ids).split()[1:-1])
+
+
+# ---------------------------------------------------------------------------------------------------------- modules (key layout)
+class _Conv1D(nn.Module):
+    def __init__(self, nf, nx):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(nx, nf).normal_(std=0.02))   # [in, out]
+        self.bias = nn.Parameter(torch.zeros(nf))
+
+
+class _Attention(nn.Module):
+    def __init__(self, nx, n_ctx):
+        super().__init__()
+        self.register_buffer("bias", torch.tril(torch.ones(n_ctx, n_ctx)).view(1, 1, n_ctx, n_ctx))   # kept so checkpoints load
+        self.c_attn = _Conv1D(3 * nx, nx)
+        self.c_proj = _Conv1D(nx, nx)
+
+
+class _MLP(nn.Module):
+    def __init__(self, n_state, nx):
+        super().__init__()
+        self.c_fc = _Conv1D(n_state, nx)
+        self.c_proj = _Conv1D(nx, n_state)
+
+
+class _Block(nn.Module):
+    def __init__(self, n_ctx, nx, eps):
+        super().__init__()
+        self.ln_1 = nn.LayerNorm(nx, eps=eps)
+        self.attn = _Attention(nx, n_ctx)
+        self.ln_2 = nn.LayerNorm(nx, eps=eps)
+        self.mlp = _MLP(4 * nx, nx)
+
+
+class _GPT2Model(nn.Module):
+    def __init__(self, vocab_size, n_positions, n_ctx, n_embd, n_layer, eps, latent_size):
+        super().__init__()
+        self.wte = nn.Embedding(vocab_size, n_embd)
+        self.wpe = nn.Embedding(n_positions, n_embd)
+        self.h = nn.ModuleList([_Block(n_ctx, n_embd, eps) for _ in range(n_layer)])
+        self.ln_f = nn.LayerNorm(n_embd, eps=eps)
+        self.linear = nn.Linear(latent_size, n_embd * n_layer, bias=False)
+        self.linear_emb = nn.Linear(latent_size, n_embd, bias=False)
+        for m in self.modules():      # GPT2PreTrainedModel._init_weights (optimus_gpt2.py:845-857)
+            if isinstance(m, (nn.Linear, nn.Embedding)):
+                m.weight.data.normal_(mean=0.0, std=0.02)
+
+
+class GPT2LatentDecoder(nn.Module):
+    """GPT2ForLatentConnector_XX with latent_as_gpt_emb = latent_as_gpt_memory = True: `transformer.*` and the tied `lm_head`."""
+
+    def __init__(self, config, latent_size=768):
+        super().__init__()
+        c = dict(config)
+        self.n_layer, self.n_embd, self.n_head = int(c['n_layer']), int(c['n_embd']), int(c['n_head'])
+        self.vocab_size, self.eps = int(c['vocab_size']), float(c.get('layer_norm_epsilon', 1e-5))
+        if self.n_embd != 64 * self.n_head:
+            raise NotImplementedError("the decode attention kernel needs d_head == 64")
+        self.transformer = _GPT2Model(self.vocab_size, int(c['n_positions']), int(c['n_ctx']), self.n_embd, self.n_layer, self.eps,
+                                      int(c.get('latent_size', latent_size)))
+        self.lm_head = nn.Linear(self.n_embd, self.vocab_size, bias=False)
+        self.lm_head.weight = self.transformer.wte.weight                # tie_weights (optimus_gpt2.py:1063-1068)
+
+
+OPTIMUS_GPT2_CONFIG = dict(      # configs/model/optimus.yaml: optimus_gpt2_decoder (inference-relevant fields)
+    vocab_size=50260, n_positions=1024, n_ctx=1024, n_embd=768, n_layer=12, n_head=12, layer_norm_epsilon=1e-5, latent_size=768)
+
+
+class _State(object):
+    """Device buffers of one batch size: fixed addresses, so captured step graphs can be replayed on later decode() calls."""
+
+    def __init__(self, dec, R, device):
+        D, L, V = dec.n_embd, dec.n_layer, dec.vocab_size
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        self.R = R
+        self.h, self.emb, self.a = z(R, D), z(R, D), z(R, D)
+        self.qkv, self.m, self.mem = z(R, 3 * D), z(R, 4 * D), z(R, L * D)
+        self.logits = z(R, V)
+        self.kc = z(L, R, dec.n_head, CACHE_SLOTS, 64)
+        self.vc = z(L, R, dec.n_head, CACHE_SLOTS, 64)
+        self.tokens = z(R, CACHE_SLOTS + 1, dt=torch.int32)
+        self.forced = z(R, CACHE_SLOTS + 1, dt=torch.int32)
+        self.uniforms = z(R, CACHE_SLOTS, dt=torch.float64)
+        self.done, self.lengths = z(R, dt=torch.int32), z(R, dt=torch.int32)
+        self.step, self.seed = z(1, dt=torch.int32), z(1, dt=torch.int64)
+        self.record = z(CACHE_SLOTS, R, V)
+        self.graphs = {}
+
+
+@register('optimus_vae_next')
+class optimus_vae_next(PackedModule):
+    """Same state-dict layout as the reference's optimus_vae_next for the decoder (`decoder.transformer.*`, `decoder.lm_head.weight`
+    tied to `wte`, the persistent `h.i.attn.bias` masks); a checkpoint's `encoder.*` keys are absorbed by strict=False."""
+
+    def __init__(self, decoder=None, tokenizer_decoder=None, encoder=None, tokenizer_encoder=None, args=None, vocab_file=None):
+        super().__init__()
+        dcfg = dict(decoder.get('args', decoder)) if decoder is not None else {}
+        config = dict(OPTIMUS_GPT2_CONFIG)
+        config.update(dict(dcfg.get('config', {})))
+        self.decoder = GPT2LatentDecoder(config, latent_size=dcfg.get('latent_size', 768))
+        if vocab_file is None and tokenizer_decoder is not None:
+            vocab_file = dict(tokenizer_decoder.get('args', tokenizer_decoder)).get('vocab_file')
+        self.tokenizer_decoder = GPT2Detokenizer(vocab_file or DEFAULT_VOCAB_FILE)
+        self.nz = int(config['latent_size'])
+        self.eos_token_id, self.pad_token_id = EOS_ID, PAD_ID
+
+    def get_device(self):
+        return self.decoder.transformer.wte.weight.device
+
+    def encode(self, text, max_length=77):
+        raise NotImplementedError("optimus_vae_next.encode needs the Optimus BERT encoder and its tokenizer (optimus_bert.py, "
+                                  "bert-base-cased-vocab.txt), which this build does not include; only decode() is implemented")
+
+    def _pack(self):
+        t = self.decoder.transformer
+        layers = []
+        for blk in t.h:
+            layers.append(dict(
+                ln1=(f32(blk.ln_1.weight), f32(blk.ln_1.bias), blk.ln_1.eps),
+                w_attn=bf16(blk.attn.c_attn.weight.t()), b_attn=f32(blk.attn.c_attn.bias),
+                w_aproj=bf16(blk.attn.c_proj.weight.t()), b_aproj=f32(blk.attn.c_proj.bias),
+                ln2=(f32(blk.ln_2.weight), f32(blk.ln_2.bias), blk.ln_2.eps),
+                w_fc=bf16(blk.mlp.c_fc.weight.t()), b_fc=f32(blk.mlp.c_fc.bias),
+                w_mproj=bf16(blk.mlp.c_proj.weight.t()), b_mproj=f32(blk.mlp.c_proj.bias)))
+        return dict(layers=layers, lnf=(f32(t.ln_f.weight), f32(t.ln_f.bias), t.ln_f.eps),
+                    wte32=f32(t.wte.weight), wpe32=f32(t.wpe.weight), lm_head=bf16(self.decoder.lm_head.weight),
+                    w_lin=bf16(t.linear.weight), w_emb=bf16(t.linear_emb.weight))
+
+    def _state(self, R, device):
+        states = self.__dict__.setdefault('_states', {})
+        key = (str(device), R)
+        if key not in states:
+            states[key] = _State(self.decoder, R, device)
+        return states[key]
+
+    def invalidate_packed(self):
+        super().invalidate_packed()
+        self.__dict__['_states'] = {}        # captured graphs hold the old weight addresses
+
+    # ------------------------------------------------------------------ one token step (5 launches per layer + 4)
+    def _step(self, st, p, temperature, eos, max_len, mode, record):
+        ops = _ops()
+        dec = self.decoder
+        D = dec.n_embd
+        ops.textdec_embed(st.tokens, st.step, p["wte32"], p["wpe32"], st.emb, st.h, pos_offset=1)
+        for i, L in enumerate(p["layers"]):
+            ops.textdec_gemv(st.h, L["w_attn"], st.qkv, bias=L["b_attn"], ln=L["ln1"])
+            ops.textdec_attention(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.step, st.a, scale=0.125)
+            ops.textdec_gemv(st.a, L["w_aproj"], st.h, bias=L["b_aproj"], accumulate=True)
+            ops.textdec_gemv(st.h, L["w_fc"], st.m, bias=L["b_fc"], ln=L["ln2"], act=ops.ACT_GELU_TANH)
+            ops.textdec_gemv(st.m, L["w_mproj"], st.h, bias=L["b_mproj"], accumulate=True)
+        ops.textdec_gemv(st.h, p["lm_head"], st.logits, ln=p["lnf"])
+        ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=temperature,
+                           seed=st.seed if mode == "seed" else None, uniforms=st.uniforms if mode == "uniforms" else None,
+                           forced=st.forced if mode == "forced" else None, eos=eos, max_len=max_len,
+                           record=st.record if record else None)
+        ops.add_int(st.step, 1)
+
+    @torch.no_grad()
+    def _run(self, z, temperature, eos, pre_scale=1.0, max_len=MAX_LENGTH, nsteps=None, mode="seed", uniforms=None, forced=None,
+             record=False, graph=True):
+        require_cuda(z, "optimus_vae_next.decode")
+        if z.dim() != 2 or z.shape[1] != self.nz:
+            raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
+        R = z.shape[0]
+        if not 1 <= R <= 16:
+            raise ValueError(f"optimus_vae_next: decodes 1 to 16 latents per call, got {R}")
+        ops = _ops()
+        p = self.packed()
+        st = self._state(R, z.device)
+        nsteps = max_len - 2 if nsteps is None else nsteps
+        if nsteps > CACHE_SLOTS:
+            raise ValueError(f"optimus_vae_next: at most {CACHE_SLOTS} steps")
+        # per-call state: latent projections (the memory slices and the embedding offset), tokens, flags, seed
+        zs = (z.float() * float(pre_scale)).contiguous()
+        ops.textdec_gemv(zs, p["w_emb"], st.emb)
+        ops.textdec_gemv(zs, p["w_lin"], st.mem)
+        init = torch.full((R, CACHE_SLOTS + 1), eos, dtype=torch.int32)
+        init[:, 0] = BOS_ID
+        if mode == "forced":
+            init[:, :forced.shape[1]] = forced.cpu()
+        st.tokens.copy_(init)
+        st.done.zero_()
+        st.lengths.fill_(nsteps + 1)
+        st.step.zero_()
+        if mode == "seed":
+            st.seed.copy_(torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64))
+        elif mode == "uniforms":
+            st.uniforms.zero_()
+            st.uniforms[:, :uniforms.shape[1]].copy_(uniforms)
+        else:
+            st.forced.zero_()
+            st.forced[:, :forced.shape[1]].copy_(forced)
+        key = (float(temperature), int(eos), int(max_len), mode, bool(record))
+        s = 0
+        while s < nsteps:
+            n = min(STEPS_PER_CHECK, nsteps - s)
+            g = st.graphs.get(key) if graph and n == STEPS_PER_CHECK else None
+            if g is not None:
+                g.replay()
+            else:
+                for _ in range(n):
+                    self._step(st, p, temperature, eos, max_len, mode, record)
+                if graph and n == STEPS_PER_CHECK and key not in st.graphs:
+                    # the chunk just ran eagerly (kernels configured, caches warm); capture one for the later chunks
+                    torch.cuda.current_stream().synchronize()
+                    step_before = st.step.clone()
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        for _ in range(n):
+                            self._step(st, p, temperature, eos, max_len, mode, record)
+                    st.step.copy_(step_before)        # capture does not execute, but keep the counter exactly as the eager chunk left it
+                    st.graphs[key] = g
+            s += n
+            if mode != "forced" and bool(st.done.cpu().all()):
+                break
+        return st, s
+
+    @torch.no_grad()
+    def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True):
+        """Sampled token rows, each an int64 CPU tensor starting with <BOS> and (unless eos_token never occurs and is never forced)
+        ending with eos_token, length <= 30.  uniforms (fp64 [n, >=28]) replaces the Philox draws; return_logits also returns the
+        fp32 logits of every step that ran, [steps, n, 50260] on the device."""
+        st, ran = self._run(z, temperature, int(eos_token), pre_scale=pre_scale, mode="uniforms" if uniforms is not None else "seed",
+                            uniforms=uniforms, record=return_logits, graph=graph)
+        tokens, lengths = st.tokens.cpu(), st.lengths.cpu()
+        rows = [tokens[r, :int(lengths[r])].long() for r in range(st.R)]
+        if return_logits:
+            return rows, st.record[:ran].clone()
+        return rows
+
+    @torch.no_grad()
+    def teacher_forced_logits(self, z, ids, graph=False):
+        """fp32 logits [n, L, vocab] of every position of the given token rows (int64 [n, L], L <= 32), the product's kernels run
+        step by step over the KV cache with the tokens forced instead of sampled."""
+        ids = torch.as_tensor(ids)
+        R, L = ids.shape
+        st, ran = self._run(z, 1.0, -1, max_len=1 << 30, nsteps=L, mode="forced", forced=ids.to(torch.int32).to(z.device),
+                            record=True, graph=graph)
+        return st.record[:L].permute(1, 0, 2).contiguous()
+
+    @torch.no_grad()
+    def decode(self, z, temperature=1.0, pre_scale=1.0):
+        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row."""
+        rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale)
+        return [self.tokenizer_decoder.sentence(r.tolist()) for r in rows]

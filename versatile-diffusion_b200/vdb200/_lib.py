@@ -64,6 +64,10 @@ SIGNATURES = {
     "vdb_pack_conv_weight": (i, [p, i, i, i, i, p, ll, ll, p]),
     "vdb_pack_geglu": (i, [p, p, i, i, p, p, p]),
     "vdb_pad_heads": (i, [p, i, i, i, i, p, p]),
+    "vdb_textdec_gemv": (i, [p, i, ll, ll, p, p, f, p, ll, ll, p, i, i, p, ll, p]),
+    "vdb_textdec_attention": (i, [p, ll, p, ll, p, p, i, i, i, p, f, p, ll, p]),
+    "vdb_textdec_embed": (i, [p, i, p, p, i, p, i, i, p, i, i, p, p]),
+    "vdb_textdec_sample": (i, [p, i, i, ll, f, p, p, i, p, i, p, i, p, p, p, i, i, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

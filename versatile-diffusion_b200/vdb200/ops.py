@@ -654,3 +654,59 @@ def scale_by_row_norm(z, L, idx=None, row_scale=None):
     out = torch.empty((B, L, C), dtype=torch.float32, device=z.device)
     check(lib.vdb_scale_by_row_norm(_ptr(z), _ptr(idx), _ptr(row_scale), B, L, Lp, C, _ptr(out), _stream()), "scale_by_row_norm")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Optimus GPT-2 text decoder (optimus.py:662-688, 746-763): one token step for R <= 16 rows
+# ------------------------------------------------------------------------------------------------
+ACT_GELU_TANH = 5
+
+
+def textdec_gemv(x, w, out, bias=None, ln=None, act=ACT_NONE, accumulate=False):
+    """out[R,N] (=|+=) act(LN(x) @ w^T + bias); x fp32 [R<=16, K] (row-strided ok), w bf16 [N, K], ln = (gamma, beta, eps) or None."""
+    _need(x, torch.float32, "x", rows_ok=True); _need(w, BF16, "w", rows_ok=True); _need(out, torch.float32, "out", rows_ok=True)
+    _need(bias, torch.float32, "bias")
+    g, b, eps = ln if ln is not None else (None, None, 0.0)
+    _need(g, torch.float32, "ln_gamma"); _need(b, torch.float32, "ln_beta")
+    R, K = x.shape
+    N = w.shape[0]
+    check(lib.vdb_textdec_gemv(_ptr(x), R, K, x.stride(0), _ptr(g), _ptr(b), float(eps), _ptr(w), N, w.stride(0), _ptr(bias),
+                               int(act), int(bool(accumulate)), _ptr(out), out.stride(0), _stream()), "textdec_gemv")
+    return out
+
+
+def textdec_attention(qkv, mem, kcache, vcache, step, out, scale=0.125):
+    """qkv fp32 [R, 3*H*64], mem fp32 [R, >=H*64] (this layer's latent slice), caches fp32 [R, H, T, 64], step int32 [1]."""
+    for n, t in (("qkv", qkv), ("mem", mem), ("out", out)):
+        _need(t, torch.float32, n, rows_ok=True)
+    _need(kcache, torch.float32, "kcache"); _need(vcache, torch.float32, "vcache"); _need(step, torch.int32, "step")
+    R, H, T, _ = kcache.shape
+    check(lib.vdb_textdec_attention(_ptr(qkv), qkv.stride(0), _ptr(mem), mem.stride(0), _ptr(kcache), _ptr(vcache), R, H, T,
+                                    _ptr(step), float(scale), _ptr(out), out.stride(0), _stream()), "textdec_attention")
+    return out
+
+
+def textdec_embed(tokens, step, wte, wpe, emb, out, pos_offset=1):
+    """out[r] = wte[tokens[r, *step]] + wpe[*step + pos_offset] + emb[r]; tokens int32 [R, L], tables / emb / out fp32."""
+    _need(tokens, torch.int32, "tokens"); _need(step, torch.int32, "step")
+    for n, t in (("wte", wte), ("wpe", wpe), ("emb", emb), ("out", out)):
+        _need(t, torch.float32, n)
+    R, D = out.shape
+    check(lib.vdb_textdec_embed(_ptr(tokens), tokens.stride(0), _ptr(step), _ptr(wte), wte.shape[0], _ptr(wpe), wpe.shape[0],
+                                int(pos_offset), _ptr(emb), R, D, _ptr(out), _stream()), "textdec_embed")
+    return out
+
+
+def textdec_sample(logits, tokens, done, lengths, step, temperature=1.0, seed=None, uniforms=None, forced=None, eos=50259,
+                   max_len=30, record=None):
+    """Token *step+1 of every unfinished row ~ softmax(logits / temperature) (see vdb_textdec_sample).  seed: device uint64 [1]
+    (as int64), uniforms: fp64 [R, >=steps] given draws, forced: int32 [R, L] teacher-forced tokens, record: fp32 [steps, R, V]."""
+    _need(logits, torch.float32, "logits", rows_ok=True)
+    _need(tokens, torch.int32, "tokens"); _need(done, torch.int32, "done"); _need(lengths, torch.int32, "lengths")
+    _need(step, torch.int32, "step"); _need(seed, torch.int64, "seed"); _need(uniforms, torch.float64, "uniforms")
+    _need(forced, torch.int32, "forced"); _need(record, torch.float32, "record")
+    R, V = logits.shape
+    check(lib.vdb_textdec_sample(_ptr(logits), R, V, logits.stride(0), float(temperature), _ptr(seed), _ptr(uniforms),
+                                 uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
+                                 forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done),
+                                 _ptr(lengths), _ptr(step), int(eos), int(max_len), _ptr(record), _stream()), "textdec_sample")
