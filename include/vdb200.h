@@ -150,6 +150,14 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
 int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, const float* beta, float eps, void* y,
                   void* stream);
 
+/* The kernel the last vdb_groupnorm_nhwc / vdb_layernorm call on this thread launched (host-side record, no device work):
+ * out[0..n) receives {family, T0, T1, G, S, nsplit, grid x, grid y, grid z} (as many as n allows).  family 1: gn_bundle_kernel
+ * <T0 = NVMAX, T1 = THREADS>, G groups per CTA, cluster size S; 2: gn_fused_kernel<T0 = NV>, nsplit CTAs per image; 3:
+ * gn_stats_kernel + gn_apply_kernel, nsplit statistics CTAs per image (grid: the statistics kernel's); 4: layernorm_rg_kernel
+ * <T0 = VPL, T1 = LPR>; 5: layernorm_kernel<T0 = MAXV, T1 = R>; 0: none yet.  Returns the number of fields (9).  For tests
+ * and tools that need to know which kernel instantiation ran. */
+int vdb_norm_last_plan(int* out, int n);
+
 /* ---- nearest 2x upsample NHWC — Upsample.forward openaimodel.py:114, autokl_modules.py:54 -------- */
 int vdb_upsample2x_nhwc(const void* x, int B, int H, int W, int C, void* y, void* stream);
 

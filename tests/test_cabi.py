@@ -61,6 +61,36 @@ def test_igemm_last_plan_reports_nine_fields():
     assert lib.vdb_igemm_last_plan(buf, 9) == 9 and lib.vdb_igemm_last_plan(None, 0) == 9
 
 
+def test_norm_last_plan_reports_nine_fields_and_refused_calls_leave_it():
+    """vdb_norm_last_plan copies at most n fields and returns 9; GroupNorm / LayerNorm / affine calls refused by their
+    argument checks launch nothing and leave the record as it was (the fake addresses below are never dereferenced)."""
+    from vdb200._lib import lib
+    assert lib.vdb_norm_last_plan(None, 0) == 9
+    buf = (ctypes.c_int * 9)(*([-7] * 9))
+    assert lib.vdb_norm_last_plan(buf, 3) == 9 and list(buf)[3:] == [-7] * 6
+    before = (ctypes.c_int * 9)()
+    lib.vdb_norm_last_plan(before, 9)
+    x, g, b, s, y = 0x10000, 0x20000, 0x30000, 0x40000, 0x50000
+    assert lib.vdb_groupnorm_nhwc(None, 320, None, 0, 2, 64, 32, g, b, 1e-5, 1, s, y, None) == 1
+    assert b"groupnorm" in lib.vdb_last_error()
+    assert lib.vdb_groupnorm_nhwc(x, 320, None, 0, 2, 64, 32, g, b, 1e-5, 1, None, y, None) == 1
+    assert lib.vdb_groupnorm_nhwc(x, 320, None, 0, 1025, 64, 32, g, b, 1e-5, 1, s, y, None) == 3      # batch > 1024
+    assert lib.vdb_groupnorm_nhwc(x, 320, None, 0, 2, 64, 16, g, b, 1e-5, 1, s, y, None) == 3         # groups != 32
+    assert lib.vdb_groupnorm_nhwc(x, 324, None, 0, 2, 64, 32, g, b, 1e-5, 1, s, y, None) == 3         # C1 % 8
+    assert lib.vdb_groupnorm_nhwc(x, 320, x, 12, 2, 64, 32, g, b, 1e-5, 1, s, y, None) == 3           # C2 % 8
+    assert lib.vdb_groupnorm_nhwc(x, 4096, x, 32, 2, 64, 32, g, b, 1e-5, 1, s, y, None) == 3          # C / 8 > 512
+    assert b"32 groups" in lib.vdb_last_error()
+    assert lib.vdb_layernorm(x, 0, 320, g, b, 1e-5, y, None) == 1
+    assert lib.vdb_layernorm(None, 4, 320, g, b, 1e-5, y, None) == 1
+    assert lib.vdb_layernorm(x, 4, 324, g, b, 1e-5, y, None) == 3
+    assert lib.vdb_layernorm(x, 4, 2056, g, b, 1e-5, y, None) == 3 and b"layernorm" in lib.vdb_last_error()
+    assert lib.vdb_affine_act_rows(x, 4, 12, g, b, 1, y, None) == 1 and b"affine_act_rows" in lib.vdb_last_error()
+    assert lib.vdb_affine_act_rows(x, 0, 16, g, b, 1, y, None) == 1
+    after = (ctypes.c_int * 9)()
+    lib.vdb_norm_last_plan(after, 9)
+    assert list(after) == list(before)
+
+
 def test_product_path_refuses_cpu_tensors():
     import pytest
     import torch

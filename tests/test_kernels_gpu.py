@@ -458,6 +458,29 @@ def test_attention(B, H, Nq, Nk, d, causal):
     assert_close(out, ref, what=f"attention B{B} H{H} {Nq}x{Nk} d{d}")
 
 
+def _switched_off(name):
+    """an opt-in kernel switch as the library reads it (test_variants_gpu runs this file under them)"""
+    return os.environ.get(name, "")[:1] == "0"
+
+
+def _forced_norm_kernel(kind):
+    """(family, template parameter or None) the kernel switches force on every case below, None under the default switches"""
+    if kind == "layernorm":
+        return ("ln_warp", None) if _switched_off("VDB_LN_RG") else None
+    if not _switched_off("VDB_GN_BUNDLE"):
+        return None
+    if _switched_off("VDB_GN_FUSED"):
+        return ("gn_stats_apply", None)
+    return ("gn_fused", 0) if _switched_off("VDB_GN_REG") else ("gn_fused", None)
+
+
+def check_forced_plan(kind, plan):
+    forced = _forced_norm_kernel(kind)
+    if forced is not None:
+        family, t0 = forced
+        assert plan["family"] == family and (t0 is None or plan["t0"] == t0), f"{kind}: launched {plan}, switches force {forced}"
+
+
 @pytest.mark.parametrize("B,HW,C1,C2,act,eps", [(2, 4096, 320, 0, 1, 1e-5), (2, 1024, 640, 320, 1, 1e-5),
                                               (3, 64, 1280, 1280, 1, 1e-5), (2, 256, 1280, 640, 0, 1e-6),
                                               (1, 65536, 128, 0, 1, 1e-6), (2, 4096, 512, 0, 0, 1e-6),
@@ -479,6 +502,7 @@ def test_groupnorm(B, HW, C1, C2, act, eps):
     C = C1 + C2
     g, b = rnd(C, seed=3, dtype=torch.float32), rnd(C, seed=4, dtype=torch.float32)
     out = ops.groupnorm(x1, g, b, eps, act=act, x2=x2)
+    check_forced_plan("groupnorm", ops.norm_last_plan())
     x = torch.cat([x1, x2], -1) if C2 else x1
     ref = F.group_norm(x.float().permute(0, 2, 1), 32, g, b, eps)
     if act:
@@ -495,6 +519,7 @@ def test_layernorm(rows, C):
     x = rnd(rows, C, seed=1) * 3 + 1
     g, b = rnd(C, seed=3, dtype=torch.float32), rnd(C, seed=4, dtype=torch.float32)
     out = ops.layernorm(x, g, b, 1e-5)
+    check_forced_plan("layernorm", ops.norm_last_plan())
     ref = F.layer_norm(x.float(), (C,), g, b, 1e-5)
     assert_close(out, ref, tol=1.5e-2, what="layernorm")
 

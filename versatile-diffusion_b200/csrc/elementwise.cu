@@ -1491,6 +1491,17 @@ __global__ void pad_heads_kernel(const float* __restrict__ w, int H, int d, int 
   }
 }
 
+// The last vdb_groupnorm_nhwc / vdb_layernorm launch on this thread (vdb_norm_last_plan): family, two template parameters,
+// G, S, nsplit, grid x / y / z.  Families: 1 gn_bundle <NVMAX, THREADS>, 2 gn_fused <NV, 0>, 3 gn_stats_apply (the statistics
+// kernel's grid), 4 ln_rg <VPL, LPR>, 5 ln_warp <MAXV, R>.
+constexpr int kNormPlanFields = 9;
+static thread_local int g_norm_plan[kNormPlanFields] = {0};
+static void set_norm_plan(int family, int t0, int t1, int G, int S, int nsplit, dim3 grid) {
+  const int plan[kNormPlanFields] = {family, t0, t1, G, S, nsplit, static_cast<int>(grid.x), static_cast<int>(grid.y),
+                                     static_cast<int>(grid.z)};
+  for (int i = 0; i < kNormPlanFields; ++i) g_norm_plan[i] = plan[i];
+}
+
 static int ew_blocks(long long work_items, int threads) {
   long long b = (work_items + threads - 1) / threads;
   const long long cap = static_cast<long long>(num_sms()) * 16;
@@ -1578,6 +1589,12 @@ void vdb_debug_gn_timeline(void* buf) {
   cudaMemcpyToSymbol(vdb::g_gn_timeline_dev, &p, sizeof(p));
 }
 
+// see include/vdb200.h
+int vdb_norm_last_plan(int* out, int n) {
+  for (int i = 0; out && i < n && i < kNormPlanFields; ++i) out[i] = g_norm_plan[i];
+  return kNormPlanFields;
+}
+
 // scratch: ZERO-INITIALISED device buffer of vdb_groupnorm_scratch_floats(B, HW) floats (reusable across calls on
 // one stream: the kernels leave its counters at zero)
 int vdb_groupnorm_nsplit(int B, int HW) {
@@ -1613,9 +1630,10 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       const __nv_bfloat16* x1b = reinterpret_cast<const __nv_bfloat16*>(x1);
       const __nv_bfloat16* x2b = reinterpret_cast<const __nv_bfloat16*>(x2);
       __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(y);
-      auto launch = [&](auto kernel, int threads, int S, size_t smem = 0) -> int {
+      auto launch = [&](auto kernel, int nvmax, int threads, int S, size_t smem = 0) -> int {
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(groups / G, S, B); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+        set_norm_plan(1, nvmax, threads, G, S, 0, cfg.gridDim);
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeClusterDimension;
         attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = S; attr[0].val.clusterDim.z = 1;
@@ -1642,7 +1660,7 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
               VDB_CUDA_CHECK(cudaFuncSetAttribute(gn_bundle_kernel<11, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
               configured = true;
             }
-            return launch(gn_bundle_kernel<11, 1024>, 1024, S, smem);
+            return launch(gn_bundle_kernel<11, 1024>, 11, 1024, S, smem);
           }
         }
       }
@@ -1653,9 +1671,9 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       // small grids: more CTAs per image while every thread still keeps >= 2 pixels
       while (S < 8 && static_cast<long long>(groups / G) * S * B < num_sms() && nper(S * 2) >= 2) S *= 2;
       const int n = nper(S);
-      if (n <= 2) return launch(gn_bundle_kernel<2, 512>, 512, S);
-      if (n <= 6) return launch(gn_bundle_kernel<6, 512>, 512, S);
-      if (n <= 12) return launch(gn_bundle_kernel<12, 512>, 512, S);
+      if (n <= 2) return launch(gn_bundle_kernel<2, 512>, 2, 512, S);
+      if (n <= 6) return launch(gn_bundle_kernel<6, 512>, 6, 512, S);
+      if (n <= 12) return launch(gn_bundle_kernel<12, 512>, 12, 512, S);
     }
   }
   static const bool fused_ok = [] { const char* ev = getenv("VDB_GN_FUSED"); return !(ev && ev[0] == '0'); }();
@@ -1674,10 +1692,12 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
     __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(y);
     if (reg_ok && ns4 <= max_ns) {
       const int ns = std::max(1, std::min(max_ns, std::max(ns4, (HW + 7) / 8)));
+      set_norm_plan(2, 4, 0, 0, 0, ns, dim3(ns, B));
       VDB_CUDA_CHECK(launch_pdl(gn_fused_kernel<4>, dim3(ns, B), dim3(kGnThreads), 0, st, x1b, C1, x2b, C2, HW, groups, eps,
                                 act, gamma, beta, scratch, yb));
     } else {
       const int ns = std::max(1, std::min(max_ns, (HW + 31) / 32));
+      set_norm_plan(2, 0, 0, 0, 0, ns, dim3(ns, B));
       VDB_CUDA_CHECK(launch_pdl(gn_fused_kernel<0>, dim3(ns, B), dim3(kGnThreads), 0, st, x1b, C1, x2b, C2, HW, groups, eps,
                                 act, gamma, beta, scratch, yb));
     }
@@ -1687,6 +1707,7 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
   const int nsplit = vdb_groupnorm_nsplit(B, HW);
   VDB_PREFER_MAX_SMEM(gn_stats_kernel);
   VDB_PREFER_MAX_SMEM(gn_apply_kernel);
+  set_norm_plan(3, 0, 0, 0, 0, nsplit, dim3(nsplit, B));
   VDB_CUDA_CHECK(launch_pdl(gn_stats_kernel, dim3(nsplit, B), dim3(kGnThreads), 0, st,
                             reinterpret_cast<const __nv_bfloat16*>(x1), C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2,
                             HW, groups, eps, scratch));
@@ -1715,31 +1736,33 @@ int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, cons
   // row-group kernel (default; VDB_LN_RG=0 falls back to the warp-per-row kernels): C = 8 * VPL * LPR
   static const bool ln_rg = [] { const char* ev = getenv("VDB_LN_RG"); return !(ev && ev[0] == '0'); }();
   if (ln_rg) {
-    auto launch_rg = [&](auto kernel, int rpw) -> int {
+    auto launch_rg = [&](auto kernel, int vpl, int rpw) -> int {
       int occ = 0;
       const size_t smem = 2 * static_cast<size_t>(C) * sizeof(float);
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1) occ = 1;
       const long long steps = (rows + rpw - 1) / rpw;                         // warp steps
       const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>((steps + 7) / 8, static_cast<long long>(occ) * num_sms())));
+      set_norm_plan(4, vpl, 32 / rpw, 0, 0, 0, dim3(grid));
       VDB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(threads), smem, st, xp, rows, C, gamma, beta, eps, yp));
       count_launch();
       return VDB_OK;
     };
     switch (V) {
-      case 40: return launch_rg(layernorm_rg_kernel<5, 8>, 4);      // C 320
-      case 80: return launch_rg(layernorm_rg_kernel<5, 16>, 2);     // C 640
-      case 160: return launch_rg(layernorm_rg_kernel<5, 32>, 1);    // C 1280
-      case 96: return launch_rg(layernorm_rg_kernel<3, 32>, 1);     // C 768  (CLIP text)
-      case 128: return launch_rg(layernorm_rg_kernel<4, 32>, 1);    // C 1024 (CLIP vision)
-      case 8: return launch_rg(layernorm_rg_kernel<1, 8>, 4);       // C 64   (reduced-width test nets)
-      case 16: return launch_rg(layernorm_rg_kernel<2, 8>, 4);      // C 128
-      case 32: return launch_rg(layernorm_rg_kernel<4, 8>, 4);      // C 256
+      case 40: return launch_rg(layernorm_rg_kernel<5, 8>, 5, 4);      // C 320
+      case 80: return launch_rg(layernorm_rg_kernel<5, 16>, 5, 2);     // C 640
+      case 160: return launch_rg(layernorm_rg_kernel<5, 32>, 5, 1);    // C 1280
+      case 96: return launch_rg(layernorm_rg_kernel<3, 32>, 3, 1);     // C 768  (CLIP text)
+      case 128: return launch_rg(layernorm_rg_kernel<4, 32>, 4, 1);    // C 1024 (CLIP vision)
+      case 8: return launch_rg(layernorm_rg_kernel<1, 8>, 1, 4);       // C 64   (reduced-width test nets)
+      case 16: return launch_rg(layernorm_rg_kernel<2, 8>, 2, 4);      // C 128
+      case 32: return launch_rg(layernorm_rg_kernel<4, 8>, 4, 4);      // C 256
       default: break;
     }
   }
   VDB_PREFER_MAX_SMEM((layernorm_kernel<2, 4>));
   VDB_PREFER_MAX_SMEM((layernorm_kernel<5, 2>));
   VDB_PREFER_MAX_SMEM((layernorm_kernel<8, 1>));
+  set_norm_plan(5, V <= 64 ? 2 : (V <= 160 ? 5 : 8), R, 0, 0, 0, dim3(blocks));
   if (V <= 64)
     VDB_CUDA_CHECK(launch_pdl(layernorm_kernel<2, 4>, dim3(blocks), dim3(threads), 0, st, xp, rows, C, gamma, beta, eps, yp));
   else if (V <= 160)

@@ -42,6 +42,7 @@ SIGNATURES = {
     "vdb_groupnorm_scratch_floats": (ll, [i, i]),
     "vdb_groupnorm_nhwc": (i, [p, i, p, i, i, i, i, p, p, f, i, p, p, p]),
     "vdb_layernorm": (i, [p, ll, i, p, p, f, p, p]),
+    "vdb_norm_last_plan": (i, [C.POINTER(i), i]),
     "vdb_upsample2x_nhwc": (i, [p, i, i, i, i, p, p]),
     "vdb_interleave2x2_nhwc": (i, [p, i, i, i, i, p, p]),
     "vdb_clip_to_u8_hwc": (i, [p, i, i, i, p, p]),

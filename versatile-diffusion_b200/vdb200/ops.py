@@ -397,6 +397,22 @@ def layernorm(x, gamma, beta, eps=1e-5, out=None):
     return out
 
 
+NORM_PLAN_FIELDS = ("family", "t0", "t1", "G", "S", "nsplit", "grid_x", "grid_y", "grid_z")
+NORM_FAMILIES = {0: None, 1: "gn_bundle", 2: "gn_fused", 3: "gn_stats_apply", 4: "ln_rg", 5: "ln_warp"}
+
+
+def norm_last_plan():
+    """The kernel the last groupnorm / layernorm call on this thread launched (vdb_norm_last_plan): family (gn_bundle,
+    gn_fused, gn_stats_apply, ln_rg, ln_warp), template parameters t0 / t1 (NVMAX / THREADS, NV, VPL / LPR, MAXV / R),
+    GroupNorm's groups per CTA G, cluster size S and pixel splits nsplit, and the grid."""
+    buf = (ctypes.c_int * len(NORM_PLAN_FIELDS))()
+    n = lib.vdb_norm_last_plan(buf, len(buf))
+    assert n == len(NORM_PLAN_FIELDS), n
+    plan = dict(zip(NORM_PLAN_FIELDS, buf))
+    plan["family"] = NORM_FAMILIES[plan["family"]]
+    return plan
+
+
 def affine_silu_rows(x, gamma, beta, act=ACT_SILU, out=None):
     """y[r, i] = act(x[r, i] * gamma[i] + beta[i]); x bf16 [rows, n], gamma / beta fp32 [n] (FCBlock's per-position GroupNorm affine)."""
     _need(x, BF16, "x"); _need(gamma, torch.float32, "gamma"); _need(beta, torch.float32, "beta")
