@@ -25,7 +25,8 @@ extern "C" {
 
 enum { VDB_OK = 0, VDB_ERR_INVALID = 1, VDB_ERR_CUDA = 2, VDB_ERR_UNSUPPORTED = 3 };
 enum { VDB_ACT_NONE = 0, VDB_ACT_SILU = 1, VDB_ACT_GELU = 2, VDB_ACT_QUICK_GELU = 3, VDB_ACT_GEGLU = 4,
-       VDB_ACT_GELU_TANH = 5 /* GPT-2's tanh approximation; vdb_textdec_gemv only */ };
+       VDB_ACT_GELU_TANH = 5 /* GPT-2's tanh approximation; vdb_textdec_gemv only */,
+       VDB_ACT_TANH = 6 /* BertPooler's tanh; vdb_textdec_gemv only */ };
 
 /* ---- library state ------------------------------------------------------------------------- */
 const char* vdb_version(void);
@@ -135,6 +136,16 @@ int vdb_attention_dv_pad(int d_head);
 int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
                        const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
                        int q_bstride, int kv_bstride, int d_head, float scale, int causal, void* stream);
+/* The same attention with a key count per batch item — BertSelfAttention.forward, optimus_bert.py:200-233, under the padding mask
+ * of BertForLatentConnector_XX.forward (:1404-1412): key j of item b is visible iff j < kv_len[b] (kv_len: device int32 [B],
+ * clamped to [0, Nk]).  The reference adds -10000 to the masked scores; exp of that underflows to exactly 0 in fp32 next to any
+ * visible key, so the hard mask computes the same function.  An item with kv_len[b] <= 0 gets zero output rows.  Masked K / V
+ * rows are never weighted (they may hold any finite values).  d_head 64 only (VDB_ERR_UNSUPPORTED otherwise); causal != 0 and a
+ * NULL or misaligned kv_len return VDB_ERR_INVALID.  The other arguments are those of vdb_attention_bf16. */
+int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                              const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                              int q_bstride, int kv_bstride, int d_head, float scale, int causal, const int* kv_len,
+                              void* stream);
 
 /* ---- GroupNorm(32) [+SiLU] [+channel concat] on NHWC — normalization()/Normalize():
  *      diffusion_utils.py:168-191 (eps 1e-5), attention.py:76-77 & autokl_modules.py:38-39 (1e-6) ----
@@ -249,9 +260,10 @@ int vdb_pad_heads(const float* w, int H, int d, int dpad, int K, void* out, void
  *      Residual stream, activations, logits and the KV cache are fp32; weights bf16 [N, K] (Conv1D's [in, out] transposed). ---- */
 /* out[r, n] = act( LN(x)[r, :] . W[n, :] + bias[n] ), or out += that (accumulate != 0: the in-place residual add of Block.forward,
  * optimus_gpt2.py:236-240).  LN = LayerNorm(gamma, beta, eps) of the fp32 row when ln_gamma != NULL (ln_1 / ln_2 / ln_f fused into
- * c_attn / c_fc / lm_head), else the identity.  act VDB_ACT_NONE or VDB_ACT_GELU_TANH (MLP.act).  Replaces Conv1D.forward
- * (modeling_utils.py:420-424) for attn.c_attn / attn.c_proj / mlp.c_fc / mlp.c_proj, transformer.linear / linear_emb and
- * lm_head.  1 <= R <= 16, K % 32 == 0, K <= 3072, W 16-byte aligned with ldw % 8 == 0, x != out.  Reads every weight once. */
+ * c_attn / c_fc / lm_head), else the identity.  act VDB_ACT_NONE, VDB_ACT_GELU_TANH (MLP.act) or VDB_ACT_TANH.  Replaces
+ * Conv1D.forward (modeling_utils.py:420-424) for attn.c_attn / attn.c_proj / mlp.c_fc / mlp.c_proj, transformer.linear / linear_emb
+ * and lm_head; on the encoder side, BertPooler.forward (optimus_bert.py:364-376, VDB_ACT_TANH on the [CLS] rows: ldx = the token
+ * stream's batch stride) and the z_mu half of BertForLatentConnector_XX.linear (optimus.py:741).  1 <= R <= 16, K % 32 == 0, K <= 3072, W 16-byte aligned with ldw % 8 == 0, x != out.  Reads every weight once. */
 int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const float* ln_gamma, const float* ln_beta, float ln_eps,
                      const void* W, long long N, long long ldw, const float* bias, int act, int accumulate, float* out, long long ldo,
                      void* stream);

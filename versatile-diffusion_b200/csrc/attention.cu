@@ -36,6 +36,7 @@ struct alignas(64) AttnParams {
   float scale_log2;  // d^-1/2 * log2(e)
   __nv_bfloat16* out;
   long long ldo;
+  const int* kv_len; // [B] valid keys per batch item (VARLEN instantiations only; key j of item b is visible iff j < kv_len[b])
 };
 
 template <int DK, int DVP, int BKV, int KV_STAGES>
@@ -44,8 +45,9 @@ constexpr size_t attention_smem_bytes() {
 }
 
 // DK = padded q/k head width (64-channel swizzle atoms), DVP = padded v head width (the N of the PV product),
-// BKV = keys per tile (the N of the QK^T product).
-template <int DK, int DVP, int BKV, int KV_STAGES>
+// BKV = keys per tile (the N of the QK^T product).  VARLEN: batch item b sees only its first min(kv_len[b], Nk) keys (BERT's
+// padding mask); an item with no key writes zero rows.
+template <int DK, int DVP, int BKV, int KV_STAGES, bool VARLEN = false>
 __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant__ AttnParams p) {
   constexpr int KA = DK / 64;                      // 64-wide K atoms of the QK^T reduction
   constexpr int KVA = BKV / 64;                    // 64-kv atoms per tile (K dimension of the PV product)
@@ -74,6 +76,7 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
   const int head = blockIdx.y;
   const int b = blockIdx.z;
 
+  int nk = 0;                                      // VARLEN: this item's key count
   int ntiles = (p.Nk + BKV - 1) / BKV;
   if (p.causal) ntiles = min(ntiles, (q0 + kBQ + BKV - 1) / BKV);
 
@@ -93,6 +96,10 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();
+  if constexpr (VARLEN) {   // kv_len may be written by the kernel this launch overlaps: read it only after pdl_wait
+    nk = max(0, min(p.kv_len[b], p.Nk));
+    ntiles = (nk + BKV - 1) / BKV;
+  }
 
   if (warp == 8) {
     if (lane == 0) {
@@ -152,10 +159,10 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
     if (lane == 0) mbar_arrive(&k_empty[st]);
 
     const int kv0 = j * BKV;
-    if (kv0 + BKV > p.Nk || p.causal) {
+    if (kv0 + BKV > (VARLEN ? nk : p.Nk) || p.causal) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int lim = p.causal ? min(p.Nk, q_idx[i] + 1) : p.Nk;   // valid kv indices are < lim
+        const int lim = p.causal ? min(p.Nk, q_idx[i] + 1) : (VARLEN ? nk : p.Nk);   // valid kv indices are < lim
 #pragma unroll
         for (int jj = 0; jj < BKV / 8; ++jj)
 #pragma unroll
@@ -220,7 +227,7 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
     float l = l_sum[i];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv_l = 1.f / l;
+    const float inv_l = (VARLEN && !(l > 0.f)) ? 0.f : 1.f / l;   // VARLEN, no visible key: o == 0, write zeros, not 0 / 0
     if (q_idx[i] >= p.Nq) continue;
     __nv_bfloat16* orow = p.out + (static_cast<long long>(b) * p.q_bs + q_idx[i]) * p.ldo + head * p.dv;
 #pragma unroll
@@ -238,11 +245,11 @@ struct AttnArgs {   // what the C ABI received; the tensor maps depend on the ke
   int B, H, q_bstride, kv_bstride;
 };
 
-template <int DK, int DVP, int BKV, int KV_STAGES>
+template <int DK, int DVP, int BKV, int KV_STAGES, bool VARLEN = false>
 static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t stream) {
   constexpr size_t smem = attention_smem_bytes<DK, DVP, BKV, KV_STAGES>();
   static_assert(smem <= 227 * 1024, "attention smem budget");
-  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES>;
+  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES, VARLEN>;
   static bool configured = false;
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -277,9 +284,10 @@ int vdb_attention_dv_pad(int d_head) {
   return -1;
 }
 
-int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                       const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                       int q_bstride, int kv_bstride, int d_head, float scale, int causal, void* stream) {
+// Argument checks and parameter block shared by both entry points; returns VDB_OK or the error status.
+static int attention_prepare(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0, const void* Vt,
+                             long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk, int q_bstride, int kv_bstride,
+                             int d_head, float scale, int causal, AttnParams& p, AttnArgs& a) {
   if (!Q || !K || !Vt || !out || B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0)
     return set_error(VDB_ERR_INVALID, "attention: null/empty argument");
   const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
@@ -292,13 +300,24 @@ int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, 
   if (q_bstride < Nq || kv_bstride < Nk || (kv_bstride % 8))
     return set_error(VDB_ERR_INVALID, "attention: need q_bstride >= Nq, kv_bstride >= Nk and kv_bstride %% 8 == 0 (got %d, %d)",
                      q_bstride, kv_bstride);
-  AttnParams p;
   memset(&p, 0, sizeof(p));
-  const AttnArgs a{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride};
+  a = AttnArgs{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride};
   p.Nq = Nq; p.Nk = Nk; p.q_bs = q_bstride; p.kv_bs = kv_bstride; p.q_col0 = q_col0; p.k_col0 = k_col0; p.dv = d_head; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.ldo = ldo;
+  return VDB_OK;
+}
+
+int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                       const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                       int q_bstride, int kv_bstride, int d_head, float scale, int causal, void* stream) {
+  AttnParams p;
+  AttnArgs a{};
+  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
+                                   scale, causal, p, a);
+  if (rc) return rc;
+  const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // 128-key tiles up to d_head 80; 64-key tiles at d_head 160 keep S + O + P within the register budget
   if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 2>(p, a, st);
@@ -306,6 +325,24 @@ int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, 
   if (DK == 128 && DVP == 80) return launch_attention<128, 80, 128, 2>(p, a, st);
   if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2>(p, a, st);
   return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel for d_head %d", d_head);
+}
+
+int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                              const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                              int q_bstride, int kv_bstride, int d_head, float scale, int causal, const int* kv_len,
+                              void* stream) {
+  if (!kv_len || (reinterpret_cast<uintptr_t>(kv_len) & 3))
+    return set_error(VDB_ERR_INVALID, "attention_varlen: kv_len must be a non-null, 4-byte aligned device int32 [B]");
+  if (causal) return set_error(VDB_ERR_INVALID, "attention_varlen: causal masking together with kv_len is not supported");
+  if (vdb_attention_dk_pad(d_head) != 64 || vdb_attention_dv_pad(d_head) != 64)
+    return set_error(VDB_ERR_UNSUPPORTED, "attention_varlen: only d_head 64 (BERT) is instantiated, got %d", d_head);
+  AttnParams p;
+  AttnArgs a{};
+  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
+                                   scale, causal, p, a);
+  if (rc) return rc;
+  p.kv_len = kv_len;
+  return launch_attention<64, 64, 128, 2, true>(p, a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -19,6 +19,7 @@ constexpr int kGvWarps = 8;                   // warps per GEMV CTA
 constexpr int kGvMaxRows = 16;                // the mma M dimension: rows beyond R are zero in shared memory
 constexpr int kGvMaxK = 3072;                 // mlp.c_proj's input width
 constexpr int kActGeluTanh = 5;               // VDB_ACT_GELU_TANH
+constexpr int kActTanh = 6;                   // VDB_ACT_TANH (the BERT encoder's pooler)
 constexpr int kHeadDim = 64;
 constexpr int kSampleThreads = 1024;
 
@@ -135,6 +136,7 @@ textdec_gemv_kernel(const float* __restrict__ x, int R, int K, long long ldx, co
       if (r >= R || n >= N) return;
       if (bias) v += bias[n];
       if (act == kActGeluTanh) v = gelu_tanh(v);
+      else if (act == kActTanh) v = tanhf(v);
       float* o = out + static_cast<size_t>(r) * ldo + n;
       *o = accumulate ? *o + v : v;
     };
@@ -345,7 +347,8 @@ int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const fl
   if (ldx < K || ldw < K || ldo < N) return set_error(VDB_ERR_INVALID, "textdec_gemv: leading dimensions smaller than the rows");
   if (!aligned16(W) || ldw % 8) return set_error(VDB_ERR_INVALID, "textdec_gemv: W must be 16-byte aligned with ldw %% 8 == 0");
   if (!ln_gamma != !ln_beta) return set_error(VDB_ERR_INVALID, "textdec_gemv: LayerNorm needs both gamma and beta");
-  if (act != 0 && act != kActGeluTanh) return set_error(VDB_ERR_INVALID, "textdec_gemv: act must be VDB_ACT_NONE or VDB_ACT_GELU_TANH");
+  if (act != 0 && act != kActGeluTanh && act != kActTanh)
+    return set_error(VDB_ERR_INVALID, "textdec_gemv: act must be VDB_ACT_NONE, VDB_ACT_GELU_TANH or VDB_ACT_TANH");
   if (static_cast<const void*>(x) == static_cast<const void*>(out)) return set_error(VDB_ERR_INVALID, "textdec_gemv: x must not alias out");
   const int k = static_cast<int>(K), n = static_cast<int>(N);
   const int ldxs = k + (k % 64 == 0 ? 32 : 0);   // row stride = 64 mod 128 bytes

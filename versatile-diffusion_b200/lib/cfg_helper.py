@@ -3,8 +3,8 @@
 The reference resolves YAML with `super_cfg` inheritance and MODEL(name) indirection; the values below
 are the resolved results for the shipped configs (configs/model/{vd,openai_unet,autokl,clip}.yaml).
 By default 'vd_four_flow_v1-0' carries the image VAE, both CLIP context encoders, the 2D diffuser and the 0D diffuser's context
-blocks.  VDB_TEXT_FLOWS=1 adds what the i2t / t2t flows need: the 0D diffuser's data blocks and the Optimus text VAE's GPT-2
-decoder (vae.text).
+blocks.  VDB_TEXT_FLOWS=1 adds what the text flows need: the 0D diffuser's data blocks and the Optimus text VAE (vae.text) with
+its BERT encoder and GPT-2 decoder.
 """
 import copy
 import os
@@ -84,12 +84,17 @@ for _sfx, _parts in _PARTS.items():
 
 
 def _optimus_text_vae():
-    """configs/model/optimus.yaml 'optimus_v1', decoder side only (the BERT encoder is not built).  The GPT-2 vocabulary is read
-    from the reference's relative path, where app.py runs; no public bank name (the default build has no text VAE)."""
+    """configs/model/optimus.yaml 'optimus_v1': the BERT encoder and the GPT-2 decoder.  Both vocabularies are read from the
+    reference's relative paths, where app.py runs; no public bank name (the default build has no text VAE)."""
     return dict(symbol="optimus", find_unused_parameters=False, type="optimus_vae_next", args=dict(
+        encoder=dict(type="optimus_bert_connector", args=dict(config=dict(
+            vocab_size=28996, hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
+            max_position_embeddings=512, type_vocab_size=2, layer_norm_eps=1e-12, hidden_act="gelu"), latent_size=768)),
         decoder=dict(type="optimus_gpt2_connector", args=dict(config=dict(
             vocab_size=50260, n_positions=1024, n_ctx=1024, n_embd=768, n_layer=12, n_head=12, layer_norm_epsilon=1e-5,
             latent_size=768), latent_size=768)),
+        tokenizer_encoder=dict(type="optimus_bert_tokenizer", args=dict(
+            vocab_file="lib/model_zoo/optimus_models/vocab/bert-base-cased-vocab.txt")),
         tokenizer_decoder=dict(type="optimus_gpt2_tokenizer", args=dict(
             vocab_file="lib/model_zoo/optimus_models/vocab/gpt2-vocab.json")),
         args=dict(latent_size=768)))

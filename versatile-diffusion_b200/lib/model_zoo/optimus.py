@@ -1,5 +1,22 @@
-"""Optimus text VAE, decoder side, on vdb200 kernels — reference lib/model_zoo/optimus.py:662-688, 746-763 (optimus_vae_next.decode)
-over GPT2ForLatentConnector_XX (optimus_models/optimus_gpt2.py:813-994, 1025-1082), configs/model/optimus.yaml.
+"""Optimus text VAE on vdb200 kernels — reference lib/model_zoo/optimus.py:662-688, 729-763 (optimus_vae_next.encode / decode)
+over BertForLatentConnector_XX (optimus_models/optimus_bert.py:1348-1437) and GPT2ForLatentConnector_XX
+(optimus_models/optimus_gpt2.py:813-994, 1025-1082), configs/model/optimus.yaml.
+
+encode(texts) turns sentences into text latents z_mu [n, 768] (`net.vae_encode(texts, which='text')`, `net.ctx_encode(texts,
+which='vae_text')`).  The BERT encoder is built only when the module is given an `encoder` config.  Its 12 post-LN layers (LayerNorm
+eps 1e-12, erf GELU) run on the same kernels as the CLIP towers: ops.gemm, ops.layernorm and the flash attention, here with one key
+count per sentence (vdb_attention_varlen_bf16) in place of the reference's -10000 padding mask.  The pooler (tanh of a dense layer on
+the [CLS] row) and the z_mu half of `linear` run as two weight-streaming GEMVs on the [CLS] rows, 16 sentences at a time.
+The WordPiece tokenizer is written from the behaviour of the reference's: the sentence is lowercased first (optimus.py:731, although
+the vocabulary is cased and do_lower_case is false, so accents are kept), BERT's basic tokenizer drops control characters, spaces out
+CJK characters, splits on whitespace and splits off every punctuation character, then greedy longest-match WordPiece with `##`
+continuations gives the pieces ([UNK] for a word over 100 characters or with no match); they are cut to max_length and framed by
+[CLS] ... [SEP].  Differences from the reference's encode, all deliberate:
+  - bf16 weights and activations with fp32 accumulation and fp32 LayerNorm statistics (the pooler and head read fp32 rows);
+  - the padding mask is a hard mask (exactly what -10000 gives in fp32);
+  - a bare `str` raises TypeError: the reference would iterate over its characters and encode each one as a sentence;
+  - a sentence of whitespace only encodes as [CLS] [SEP], like the empty one.  The reference's tokenizer turns it into one of its
+    special tokens, picked by the iteration order of a Python set of strings, which changes with the process's hash seed.
 
 decode(z) turns text latents [n, 768] into strings, the last call of app.py's i2t / t2t flows (`net.vae_decode(x, which='text')`).
 GPT-2 (LayerNorm eps 1e-5, tanh GELU, Conv1D weights [in, out], attention scale 1/8) runs one token at a time for all n rows as one
@@ -16,10 +33,10 @@ Differences from the reference, all deliberate:
     can cut a tail whose sorted cumulative sum rounds above 1.0 (probability mass of order 1e-6);
   - the reference's 29th forward pass, whose draw is always overwritten with <EOS>, is skipped;
   - weights are bf16 (packed at load); the residual stream, attention, logits and the sampler's sums are fp32 / fp64.
-encode (the BERT encoder) is not part of this build.
 """
 import json
 import os
+import unicodedata
 
 import torch
 import torch.nn as nn
@@ -37,6 +54,9 @@ CACHE_SLOTS = 32                                  # token slots of the KV cache 
 # caps the steps that run after every row has finished at 3 and the syncs of a full-length decode (28 steps) at 7.
 STEPS_PER_CHECK = 4
 DEFAULT_VOCAB_FILE = 'lib/model_zoo/optimus_models/vocab/gpt2-vocab.json'   # relative to the reference's tree, where app.py runs
+DEFAULT_BERT_VOCAB_FILE = 'lib/model_zoo/optimus_models/vocab/bert-base-cased-vocab.txt'
+ENC_MAX_POSITIONS = 512                           # BERT's position table; [CLS] and [SEP] take two of them
+ENC_HEAD_ROWS = 16                                # [CLS] rows per pooler / z_mu GEMV launch (vdb_textdec_gemv's row limit)
 
 
 def _ops():
@@ -113,6 +133,111 @@ class GPT2Detokenizer(object):
         return ' '.join(self.decode(ids).split()[1:-1])
 
 
+# ---------------------------------------------------------------------------------------------------------- WordPiece tokenizer
+def _bert_whitespace(ch):
+    return ch in ' \t\n\r' or unicodedata.category(ch) == 'Zs'
+
+
+def _bert_control(ch):
+    return ch not in '\t\n\r' and unicodedata.category(ch).startswith('C')
+
+
+def _bert_punctuation(ch):
+    cp = ord(ch)   # every non-alphanumeric ASCII symbol counts, as well as Unicode's P* categories
+    return 33 <= cp <= 47 or 58 <= cp <= 64 or 91 <= cp <= 96 or 123 <= cp <= 126 or unicodedata.category(ch).startswith('P')
+
+
+_CJK_RANGES = ((0x4E00, 0x9FFF), (0x3400, 0x4DBF), (0x20000, 0x2A6DF), (0x2A700, 0x2B73F), (0x2B740, 0x2B81F), (0x2B820, 0x2CEAF),
+               (0xF900, 0xFAFF), (0x2F800, 0x2FA1F))    # the CJK Unified Ideographs blocks BERT isolates (not kana / hangul)
+
+
+def _bert_cjk(ch):
+    cp = ord(ch)
+    return any(lo <= cp <= hi for lo, hi in _CJK_RANGES)
+
+
+class BertWordPieceTokenizer(object):
+    """sentence -> BERT ids as optimus_vae_next.encode tokenizes (optimus.py:731-737): lowercase, basic tokenization, greedy
+    longest-match WordPiece, [CLS] ... [SEP].  The vocabulary (one piece per line, id = line number) is read on first use."""
+    CLS, SEP, UNK = '[CLS]', '[SEP]', '[UNK]'
+    MAX_WORD_CHARS = 100
+
+    def __init__(self, vocab_file=DEFAULT_BERT_VOCAB_FILE):
+        self.vocab_file = vocab_file
+        self._vocab = None
+
+    def _load(self):
+        if self._vocab is None:
+            if not os.path.isfile(self.vocab_file):
+                raise VocabularyMissingError(
+                    f"BERT vocabulary '{self.vocab_file}' not found (cwd {os.getcwd()}): the text encoder needs the Optimus "
+                    "bert-base-cased-vocab.txt to turn text into token ids; set the text VAE's tokenizer_encoder vocab_file, or "
+                    "call encode_ids() with ids")
+            vocab = {}
+            with open(self.vocab_file, encoding='utf-8') as fh:
+                for i, line in enumerate(fh):
+                    vocab[line.rstrip('\n')] = i
+            self._vocab = vocab
+        return self._vocab
+
+    @staticmethod
+    def basic_tokens(text):
+        """BERT's basic tokenizer without case folding: drop NUL / U+FFFD / control characters, whitespace -> ' ', spaces around
+        CJK ideographs, split on whitespace, then every punctuation character becomes a token of its own."""
+        chars = []
+        for ch in text:
+            if ch in '\x00\ufffd' or _bert_control(ch):
+                continue
+            if _bert_whitespace(ch):
+                chars.append(' ')
+            elif _bert_cjk(ch):
+                chars += [' ', ch, ' ']
+            else:
+                chars.append(ch)
+        out = []
+        for word in ''.join(chars).split():
+            run = ''
+            for ch in word:
+                if _bert_punctuation(ch):
+                    if run:
+                        out.append(run)
+                    out.append(ch)
+                    run = ''
+                else:
+                    run += ch
+            if run:
+                out.append(run)
+        return out
+
+    def wordpieces(self, word):
+        vocab = self._load()
+        if len(word) > self.MAX_WORD_CHARS:
+            return [self.UNK]
+        pieces, start = [], 0
+        while start < len(word):
+            end = len(word)
+            while end > start:
+                piece = word[start:end] if start == 0 else '##' + word[start:end]
+                if piece in vocab:
+                    break
+                end -= 1
+            if end == start:                 # no piece of the vocabulary starts here: the whole word is unknown
+                return [self.UNK]
+            pieces.append(piece)
+            start = end
+        return pieces
+
+    def tokenize(self, sentence):
+        return [p for w in self.basic_tokens(sentence.lower()) for p in self.wordpieces(w)]
+
+    def encode(self, sentence, max_length=77):
+        """-> [CLS] id, the ids of the first max_length pieces, [SEP] id."""
+        vocab = self._load()
+        unk = vocab.get(self.UNK)
+        ids = [vocab.get(p, unk) for p in self.tokenize(sentence)[:max_length]]
+        return [vocab[self.CLS]] + ids + [vocab[self.SEP]]
+
+
 # ---------------------------------------------------------------------------------------------------------- modules (key layout)
 class _Conv1D(nn.Module):
     def __init__(self, nf, nx):
@@ -178,6 +303,96 @@ class GPT2LatentDecoder(nn.Module):
 OPTIMUS_GPT2_CONFIG = dict(      # configs/model/optimus.yaml: optimus_gpt2_decoder (inference-relevant fields)
     vocab_size=50260, n_positions=1024, n_ctx=1024, n_embd=768, n_layer=12, n_head=12, layer_norm_epsilon=1e-5, latent_size=768)
 
+OPTIMUS_BERT_CONFIG = dict(      # configs/model/optimus.yaml: optimus_bert_encoder (inference-relevant fields)
+    vocab_size=28996, hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
+    max_position_embeddings=512, type_vocab_size=2, layer_norm_eps=1e-12, hidden_act='gelu')
+
+
+class _Dense(nn.Module):
+    """nn.Linear's parameters with BERT's init (normal 0.02, zero bias)"""
+
+    def __init__(self, nin, nout, bias=True):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(nout, nin).normal_(std=0.02))
+        self.bias = nn.Parameter(torch.zeros(nout)) if bias else None
+
+
+class _BertEmbeddings(nn.Module):
+    def __init__(self, c):
+        super().__init__()
+        D = c['hidden_size']
+        self.word_embeddings = nn.Embedding(c['vocab_size'], D)
+        self.position_embeddings = nn.Embedding(c['max_position_embeddings'], D)
+        self.token_type_embeddings = nn.Embedding(c['type_vocab_size'], D)
+        self.LayerNorm = nn.LayerNorm(D, eps=c['layer_norm_eps'])
+        for e in (self.word_embeddings, self.position_embeddings, self.token_type_embeddings):
+            e.weight.data.normal_(std=0.02)
+
+
+class _BertSelfAttention(nn.Module):
+    def __init__(self, D):
+        super().__init__()
+        self.query, self.key, self.value = _Dense(D, D), _Dense(D, D), _Dense(D, D)
+
+
+class _BertAddNorm(nn.Module):   # BertSelfOutput / BertOutput: LayerNorm(dense(x) + residual)
+    def __init__(self, nin, D, eps):
+        super().__init__()
+        self.dense = _Dense(nin, D)
+        self.LayerNorm = nn.LayerNorm(D, eps=eps)
+
+
+class _BertAttention(nn.Module):
+    def __init__(self, D, eps):
+        super().__init__()
+        self.self = _BertSelfAttention(D)
+        self.output = _BertAddNorm(D, D, eps)
+
+
+class _BertIntermediate(nn.Module):
+    def __init__(self, D, F):
+        super().__init__()
+        self.dense = _Dense(D, F)
+
+
+class _BertLayer(nn.Module):
+    def __init__(self, c):
+        super().__init__()
+        D, F, eps = c['hidden_size'], c['intermediate_size'], c['layer_norm_eps']
+        self.attention = _BertAttention(D, eps)
+        self.intermediate = _BertIntermediate(D, F)
+        self.output = _BertAddNorm(F, D, eps)
+
+
+class _BertLayers(nn.Module):
+    def __init__(self, c):
+        super().__init__()
+        self.layer = nn.ModuleList([_BertLayer(c) for _ in range(c['num_hidden_layers'])])
+
+
+class _BertPooler(nn.Module):
+    def __init__(self, D):
+        super().__init__()
+        self.dense = _Dense(D, D)
+
+
+class BertLatentEncoder(nn.Module):
+    """BertForLatentConnector_XX's parameters (`embeddings.*`, `encoder.layer.i.*`, `pooler.dense`, `linear` [2 * latent, 768])."""
+
+    def __init__(self, config, latent_size=768):
+        super().__init__()
+        c = dict(config)
+        self.hidden, self.n_head = int(c['hidden_size']), int(c['num_attention_heads'])
+        self.eps = float(c['layer_norm_eps'])
+        if self.hidden != 64 * self.n_head:
+            raise NotImplementedError("the encoder's varlen attention kernel needs d_head == 64")
+        if c.get('hidden_act', 'gelu') != 'gelu':
+            raise NotImplementedError(f"BERT hidden_act '{c['hidden_act']}': only the erf GELU is built")
+        self.embeddings = _BertEmbeddings(c)
+        self.encoder = _BertLayers(c)
+        self.pooler = _BertPooler(self.hidden)
+        self.linear = _Dense(self.hidden, 2 * latent_size, bias=False)
+
 
 class _State(object):
     """Device buffers of one batch size: fixed addresses, so captured step graphs can be replayed on later decode() calls."""
@@ -202,8 +417,9 @@ class _State(object):
 
 @register('optimus_vae_next')
 class optimus_vae_next(PackedModule):
-    """Same state-dict layout as the reference's optimus_vae_next for the decoder (`decoder.transformer.*`, `decoder.lm_head.weight`
-    tied to `wte`, the persistent `h.i.attn.bias` masks); a checkpoint's `encoder.*` keys are absorbed by strict=False."""
+    """Same state-dict layout as the reference's optimus_vae_next: the decoder (`decoder.transformer.*`, `decoder.lm_head.weight`
+    tied to `wte`, the persistent `h.i.attn.bias` masks) and, when an `encoder` config is given, the BERT encoder (`encoder.*`).
+    Without one, a checkpoint's `encoder.*` keys are absorbed by strict=False and encode() raises NotImplementedError."""
 
     def __init__(self, decoder=None, tokenizer_decoder=None, encoder=None, tokenizer_encoder=None, args=None, vocab_file=None):
         super().__init__()
@@ -216,15 +432,124 @@ class optimus_vae_next(PackedModule):
         self.tokenizer_decoder = GPT2Detokenizer(vocab_file or DEFAULT_VOCAB_FILE)
         self.nz = int(config['latent_size'])
         self.eos_token_id, self.pad_token_id = EOS_ID, PAD_ID
+        self.tokenizer_encoder = None
+        if encoder is not None:
+            ecfg = dict(encoder.get('args', encoder))
+            bert = dict(OPTIMUS_BERT_CONFIG)
+            bert.update(dict(ecfg.get('config', {})))
+            self.encoder = BertLatentEncoder(bert, latent_size=ecfg.get('latent_size', self.nz))
+            bert_vocab = None
+            if tokenizer_encoder is not None:
+                bert_vocab = dict(tokenizer_encoder.get('args', tokenizer_encoder)).get('vocab_file')
+            self.tokenizer_encoder = BertWordPieceTokenizer(bert_vocab or DEFAULT_BERT_VOCAB_FILE)
 
     def get_device(self):
         return self.decoder.transformer.wte.weight.device
 
-    def encode(self, text, max_length=77):
-        raise NotImplementedError("optimus_vae_next.encode needs the Optimus BERT encoder and its tokenizer (optimus_bert.py, "
-                                  "bert-base-cased-vocab.txt), which this build does not include; only decode() is implemented")
+    # ------------------------------------------------------------------ encoder
+    def _pack_encoder(self):
+        e = self.encoder
+        D = e.hidden
+        emb = e.embeddings
+        layers = []
+        for lyr in e.encoder.layer:
+            a, ao, io, oo = lyr.attention.self, lyr.attention.output, lyr.intermediate, lyr.output
+            wo = ao.dense.weight.detach().float()
+            layers.append(dict(
+                wqk=bf16(torch.cat([a.query.weight.detach(), a.key.weight.detach()], 0)),
+                bqk=f32(torch.cat([a.query.bias.detach(), a.key.bias.detach()], 0)),
+                wv=bf16(a.value.weight),
+                # the rows of P sum to 1 over the visible keys, so P (V + 1 b_v^T) = P V + b_v: the V bias moves through dense
+                wo=bf16(wo), bo=(ao.dense.bias.detach().float() + wo @ a.value.bias.detach().float()).contiguous(),
+                ln1=(f32(ao.LayerNorm.weight), f32(ao.LayerNorm.bias)),
+                w1=bf16(io.dense.weight), b1=f32(io.dense.bias),
+                w2=bf16(oo.dense.weight), b2=f32(oo.dense.bias),
+                ln2=(f32(oo.LayerNorm.weight), f32(oo.LayerNorm.bias))))
+        # token type ids are always 0 here: token_type_embeddings[0] rides in the position table
+        pos = (emb.position_embeddings.weight.detach().float() + emb.token_type_embeddings.weight.detach().float()[0]).contiguous()
+        return dict(layers=layers, word=f32(emb.word_embeddings.weight), pos=pos,
+                    ln_emb=(f32(emb.LayerNorm.weight), f32(emb.LayerNorm.bias)),
+                    w_pool=bf16(e.pooler.dense.weight), b_pool=f32(e.pooler.dense.bias),
+                    w_mu=bf16(e.linear.weight[:e.linear.weight.shape[0] // 2]), heads=e.n_head, D=D, eps=e.eps)
 
+    def _require_encoder(self):
+        if getattr(self, 'encoder', None) is None:
+            raise NotImplementedError("optimus_vae_next.encode needs the Optimus BERT encoder: build the text VAE with an `encoder` "
+                                      "config (configs/model/optimus.yaml optimus_bert_encoder; VDB_TEXT_FLOWS=1 does)")
+
+    @torch.no_grad()
+    def encode_ids(self, ids, lengths):
+        """BertForLatentConnector_XX.forward + linear(.).chunk(2)[0] on token rows: ids int64 [n, L] ([CLS] first, zero padded),
+        lengths [n] = the ids of each row that are not padding.  -> z_mu fp32 [n, latent] on the module's device."""
+        self._require_encoder()
+        ops = _ops()
+        dev = self.encoder.linear.weight.device
+        ids = torch.as_tensor(ids).long()
+        V = self.encoder.embeddings.word_embeddings.num_embeddings
+        if ids.dim() != 2 or ids.numel() == 0 or int(ids.min()) < 0 or int(ids.max()) >= V:
+            raise ValueError(f"optimus_vae_next.encode: need token ids [n, L] in [0, {V})")
+        ids = ids.to(dev).contiguous()
+        require_cuda(ids, "optimus_vae_next.encode")
+        n, L = ids.shape
+        lengths = [int(v) for v in lengths]
+        if len(lengths) != n or not all(1 <= v <= L for v in lengths):
+            raise ValueError(f"optimus_vae_next.encode: need 1 <= lengths[i] <= {L} for each of the {n} rows, got {lengths}")
+        if L > ENC_MAX_POSITIONS:
+            raise ValueError(f"optimus_vae_next.encode: at most {ENC_MAX_POSITIONS} tokens per row, got {L}")
+        p = self.packed()["enc"]
+        D, H = p["D"], p["heads"]
+        Lp = (L + 7) // 8 * 8
+        kv_len = torch.tensor(lengths, dtype=torch.int32).to(dev)      # one copy per call, shared by every layer
+        x = ops.clip_text_embed(ids, p["word"], p["pos"], Lp).view(n * Lp, D)    # word + position (+ type 0); pad rows zero
+        x = ops.layernorm(x, *p["ln_emb"], eps=p["eps"])
+        o = torch.zeros(n * Lp, D, dtype=torch.bfloat16, device=dev)
+        for lp in p["layers"]:
+            qk = ops.gemm(x, lp["wqk"], bias=lp["bqk"])                                   # [n*Lp, 2D]: q | k
+            vt = ops.gemm(lp["wv"], x)                                                    # [D, n*Lp] = V^T (bias folded into bo)
+            ops.attention(qk, qk, vt, o, n, H, Lp, Lp, D // H, scale=(D // H) ** -0.5, q_col0=0, k_col0=D,
+                          q_bstride=Lp, kv_bstride=Lp, kv_len=kv_len)
+            x = ops.layernorm(ops.gemm(o, lp["wo"], bias=lp["bo"], resid=x), *lp["ln1"], eps=p["eps"])
+            h = ops.gemm(x, lp["w1"], bias=lp["b1"], act=ops.ACT_GELU)
+            x = ops.layernorm(ops.gemm(h, lp["w2"], bias=lp["b2"], resid=x), *lp["ln2"], eps=p["eps"])
+        cls = ops.to_f32(x).view(n, Lp * D)[:, :D]                                       # the [CLS] rows, row stride Lp * D
+        pooled = torch.empty(n, D, dtype=torch.float32, device=dev)
+        z = torch.empty(n, p["w_mu"].shape[0], dtype=torch.float32, device=dev)
+        for r0 in range(0, n, ENC_HEAD_ROWS):
+            r1 = min(n, r0 + ENC_HEAD_ROWS)
+            ops.textdec_gemv(cls[r0:r1], p["w_pool"], pooled[r0:r1], bias=p["b_pool"], act=ops.ACT_TANH)
+            ops.textdec_gemv(pooled[r0:r1], p["w_mu"], z[r0:r1])
+        return z
+
+    def tokenize(self, text, max_length=77):
+        """-> (ids int64 [n, 2 + longest], lengths): the rows optimus_vae_next.encode feeds BERT (optimus.py:730-738)."""
+        self._require_encoder()
+        if isinstance(text, str):
+            raise TypeError("optimus_vae_next.encode takes a list of sentences, not a str (the reference would encode every "
+                            "character of it as a sentence of its own)")
+        if not 0 <= int(max_length) <= ENC_MAX_POSITIONS - 2:
+            raise ValueError(f"optimus_vae_next.encode: max_length must be in [0, {ENC_MAX_POSITIONS - 2}], got {max_length}")
+        rows = [self.tokenizer_encoder.encode(s, max_length=int(max_length)) for s in text]
+        if not rows:
+            raise ValueError("optimus_vae_next.encode: no sentences")
+        ids = torch.zeros(len(rows), max(len(r) for r in rows), dtype=torch.long)
+        for i, r in enumerate(rows):
+            ids[i, :len(r)] = torch.tensor(r, dtype=torch.long)
+        return ids, [len(r) for r in rows]
+
+    @torch.no_grad()
+    def encode(self, text, max_length=77):
+        """optimus_vae_next.encode (optimus.py:729-743): z_mu [n, latent] of a list of sentences, in the parameters' dtype."""
+        ids, lengths = self.tokenize(text, max_length=max_length)
+        return self.encode_ids(ids, lengths).to(self.encoder.linear.weight.dtype)
+
+    # ------------------------------------------------------------------ decoder
     def _pack(self):
+        packed = self._pack_decoder()
+        if getattr(self, 'encoder', None) is not None:
+            packed["enc"] = self._pack_encoder()
+        return packed
+
+    def _pack_decoder(self):
         t = self.decoder.transformer
         layers = []
         for blk in t.h:

@@ -38,6 +38,7 @@ SIGNATURES = {
     "vdb_attention_dk_pad": (i, [i]),
     "vdb_attention_dv_pad": (i, [i]),
     "vdb_attention_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p]),
+    "vdb_attention_varlen_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p, p]),
     "vdb_groupnorm_nsplit": (i, [i, i]),
     "vdb_groupnorm_scratch_floats": (ll, [i, i]),
     "vdb_groupnorm_nhwc": (i, [p, i, p, i, i, i, i, p, p, f, i, p, p, p]),

@@ -356,17 +356,21 @@ def attention_pads(d_head):
 
 
 def attention(q, k, vt, out, B, H, Nq, Nk, d_head, scale=None, q_col0=0, k_col0=0, causal=False,
-              q_bstride=0, kv_bstride=0):
+              q_bstride=0, kv_bstride=0, kv_len=None):
     """Flash attention. q [B*q_bstride, ldq], k [B*kv_bstride, ldk], vt [H*DVP, B*kv_bstride], out [B*q_bstride, H*d_head].
-    kv_bstride (default Nk) must be a multiple of 8: pad ragged contexts per batch item."""
+    kv_bstride (default Nk) must be a multiple of 8: pad ragged contexts per batch item.  kv_len (int32 device [B], d_head 64,
+    not causal): item b attends to its first kv_len[b] keys only (vdb_attention_varlen_bf16)."""
     _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(vt, BF16, "vt", True); _need(out, BF16, "out", True)
+    _need(kv_len, torch.int32, "kv_len")
     if scale is None:
         scale = d_head ** -0.5
+    args = (_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt), vt.stride(0), _ptr(out), out.stride(0),
+            B, H, Nq, Nk, int(q_bstride), int(kv_bstride), d_head, float(scale), 1 if causal else 0)
     with _Span("attention", 4.0 * B * H * Nq * Nk * d_head, 2.0 * B * H * d_head * (2 * Nq + 2 * Nk)):
-        check(lib.vdb_attention_bf16(_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt),
-                                     vt.stride(0), _ptr(out), out.stride(0), B, H, Nq, Nk, int(q_bstride),
-                                     int(kv_bstride), d_head, float(scale), 1 if causal else 0, _stream()),
-              "attention_bf16")
+        if kv_len is None:
+            check(lib.vdb_attention_bf16(*args, _stream()), "attention_bf16")
+        else:
+            check(lib.vdb_attention_varlen_bf16(*args, _ptr(kv_len), _stream()), "attention_varlen_bf16")
     return out
 
 
@@ -676,6 +680,7 @@ def scale_by_row_norm(z, L, idx=None, row_scale=None):
 # Optimus GPT-2 text decoder (optimus.py:662-688, 746-763): one token step for R <= 16 rows
 # ------------------------------------------------------------------------------------------------
 ACT_GELU_TANH = 5
+ACT_TANH = 6            # BertPooler (textdec_gemv only)
 
 
 def textdec_gemv(x, w, out, bias=None, ln=None, act=ACT_NONE, accumulate=False):
