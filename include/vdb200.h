@@ -286,6 +286,19 @@ int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float t
                        const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
                        const int* step, int eos, int max_len, float* record, void* stream);
 
+/* ---- semantic/style disentanglement of the image context — decompose / adjust_rank of the reference app.py:48-127 -----------
+ * For each item b < n_items of x [n_items, m, n] (fp32, contiguous):  X = x - rowmean(x);  the randomized PCA of torch.pca_lowrank
+ * (X, q, center=False, niter) with the Gaussian start R [m, q] (fp32, shared by all items; the reference's torch.randn(m, q)) gives
+ * X ~= U diag(S) V^T;  x_new = U diag(S * factors) V^T + rowmean(x) [+ X - U diag(S) V^T when keep_remainder != 0];
+ * out = x_new / std(x_new) * std(x) (unbiased, over all m * n elements of the item).  factors: device fp32 [q].  s_out (may be NULL):
+ * device fp32 [n_items, q], the unscaled S, descending; u_out [n_items, m, q] and v_out [n_items, n, q] (may be NULL): U and V.
+ * One launch (one 8-CTA cluster per item, X resident in shared memory); the QRs are CholeskyQR2 in fp64, so U and V differ from
+ * torch's by column signs only.  Deterministic for a given R.
+ * NULL x / R / factors / out, n_items < 1, niter < 0 or a misaligned x / out return VDB_ERR_INVALID; shapes other than n = 768,
+ * q = 20, 40 <= m <= 320 (n_items <= 65535) return VDB_ERR_UNSUPPORTED.  out must not alias x. */
+int vdb_rank_adjust_f32(const float* x, int n_items, int m, int n, const float* R, int q, int niter, const float* factors,
+                        int keep_remainder, float* out, float* s_out, float* u_out, float* v_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

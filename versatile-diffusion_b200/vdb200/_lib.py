@@ -70,6 +70,7 @@ SIGNATURES = {
     "vdb_textdec_attention": (i, [p, ll, p, ll, p, p, i, i, i, p, f, p, ll, p]),
     "vdb_textdec_embed": (i, [p, i, p, p, i, p, i, i, p, i, i, p, p]),
     "vdb_textdec_sample": (i, [p, i, i, ll, f, p, p, i, p, i, p, i, p, p, p, i, i, p, p]),
+    "vdb_rank_adjust_f32": (i, [p, i, i, i, p, i, i, p, i, p, p, p, p, p]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

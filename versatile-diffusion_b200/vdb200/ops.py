@@ -731,3 +731,27 @@ def textdec_sample(logits, tokens, done, lengths, step, temperature=1.0, seed=No
                                  uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
                                  forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done),
                                  _ptr(lengths), _ptr(step), int(eos), int(max_len), _ptr(record), _stream()), "textdec_sample")
+
+
+# ------------------------------------------------------------------------------------------------
+# Semantic/style disentanglement (app.py:48-127): the rank adjustment of the image context, one launch
+# ------------------------------------------------------------------------------------------------
+def rank_adjust(x, factors, keep_remainder, R, niter=100, out=None, s_out=None, u_out=None, v_out=None):
+    """x fp32 [n, m, 768] -> x_new (see vdb_rank_adjust_f32): the rank-q PCA of each item's row-centred x, started from R fp32
+    [m, q] (shared by all items), with S scaled by factors fp32 [q]; keep_remainder adds back what the rank-q part misses.
+    Optional outputs: s_out fp32 [n, q] the unscaled S, u_out [n, m, q] and v_out [n, 768, q] the factors U and V."""
+    for name, t in (("x", x), ("factors", factors), ("R", R), ("s_out", s_out), ("u_out", u_out), ("v_out", v_out)):
+        _need(t, torch.float32, name)
+    if x.dim() != 3 or R.dim() != 2 or R.shape[0] != x.shape[1] or factors.numel() != R.shape[1]:
+        raise ValueError(f"rank_adjust: x {tuple(x.shape)}, R {tuple(R.shape)} and factors {tuple(factors.shape)} disagree")
+    n, m, d = x.shape
+    q = R.shape[1]
+    if out is None:
+        out = torch.empty_like(x)
+    _need(out, torch.float32, "out")
+    for name, t, shape in (("s_out", s_out, (n, q)), ("u_out", u_out, (n, m, q)), ("v_out", v_out, (n, d, q))):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError(f"rank_adjust: {name} must be {list(shape)}, got {list(t.shape)}")
+    check(lib.vdb_rank_adjust_f32(_ptr(x), n, m, d, _ptr(R), q, int(niter), _ptr(factors), int(bool(keep_remainder)), _ptr(out),
+                                  _ptr(s_out), _ptr(u_out), _ptr(v_out), _stream()), "rank_adjust")
+    return out
