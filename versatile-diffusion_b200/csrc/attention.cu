@@ -5,11 +5,16 @@
 // {4096,1024,256,64}, d_head in {40,80,160}; cross-attention M = 77 (text) / 257 (image) /
 // n*257 (multi-image) — and the CLIP encoder attention (d_head 64, optional causal mask).
 //
-// One CTA = one (q-tile of 128 rows, head, batch).  288 threads:
+// One CTA = one (q-tile of 128 rows, head, batch).
 //   warps 0-7 : two consumer warpgroups; warpgroup g owns query rows [64 g, 64 g + 64) of the tile.  Per kv tile:
 //               S = Q K_j^T (wgmma, both operands from shared memory, fp32 in registers), online softmax in registers
 //               (lazy rescale of O), P -> bf16 register fragments, O += P V_j (wgmma with A from registers).
-//   warp 8    : TMA producer (Q once; K and V^T tiles through two independent rings)
+//   TMA loads (Q once; K and V^T tiles through two independent rings) come from one of two places:
+//   * TMA_WARP (d_head 160): a ninth warp issues them; 288 threads, one CTA per SM.
+//   * otherwise (d_head <= 80): lane 0 of warp 0 refills the K ring and lane 0 of warp 4 the V^T ring, each for tile
+//     j + KV_STAGES - 1 while its warpgroup's S_j product runs.  256 threads fit 128 registers at two CTAs per SM, so one
+//     CTA's softmax (bound by MUFU ex2) can run under the other's wgmma; with a ninth warp, two CTAs would put five warps on
+//     some SM sub-partitions and cap registers at 96, which serialises the wgmmas.
 // Operand layouts (all K-major, 128B swizzle, written by the projection GEMMs):
 // Batch b occupies rows [b*q_bs, b*q_bs+Nq) of Q/O, rows [b*kv_bs, +Nk) of K, columns [b*kv_bs, +Nk) of Vt.
 //   Q  [B*Nq, ldq]  head h at columns q_col0 + h*DK .. (+DK, zero padded beyond d_head)
@@ -23,6 +28,8 @@ namespace vdb {
 
 constexpr int kBQ = 128;   // query rows per CTA
 constexpr float kRescaleThreshold = 8.0f;  // in log2 units (P stays <= 2^8)
+
+constexpr int attention_threads(bool tma_warp) { return tma_warp ? 288 : 256; }
 
 struct alignas(64) AttnParams {
   CUtensorMap tmQ;   // 2D (cols, rows) box (64, 128)
@@ -45,16 +52,21 @@ constexpr size_t attention_smem_bytes() {
 }
 
 // DK = padded q/k head width (64-channel swizzle atoms), DVP = padded v head width (the N of the PV product),
-// BKV = keys per tile (the N of the QK^T product).  VARLEN: batch item b sees only its first min(kv_len[b], Nk) keys (BERT's
-// padding mask); an item with no key writes zero rows.
-template <int DK, int DVP, int BKV, int KV_STAGES, bool VARLEN = false>
-__global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant__ AttnParams p) {
+// BKV = keys per tile (the N of the QK^T product), TMA_WARP = a ninth warp issues the loads (see the top of the file).
+// VARLEN: batch item b sees only its first min(kv_len[b], Nk) keys (BERT's padding mask); an item with no key writes zero rows.
+template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false>
+__global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
+    attention_kernel(const __grid_constant__ AttnParams p) {
   constexpr int KA = DK / 64;                      // 64-wide K atoms of the QK^T reduction
   constexpr int KVA = BKV / 64;                    // 64-kv atoms per tile (K dimension of the PV product)
   constexpr uint32_t kQBytes = KA * kBQ * 128;     // Q tile
   constexpr uint32_t kKBytes = KA * BKV * 128;     // one K stage
   constexpr uint32_t kVAtom = DVP * 128;           // one 64-kv atom of V^T
   constexpr uint32_t kVBytes = KVA * kVAtom;       // one V stage (BKV kv)
+  // K16 steps of QK^T: Q is zero past d_head <= DVP, so the steps past DVP add nothing (d 40: 3 of 4, d 80 in DK 128: 5 of 8).
+  // A fixed count issues the steps as one wgmma chain; with a count read at run time each step sat behind its own branch, and
+  // the registers ptxas kept around the conditional wgmmas (159 at d 40, 168 at d 80) ruled out two CTAs per SM.
+  constexpr int kQKSteps = (DVP < DK ? DVP : DK) / 16;
   static_assert(BKV == 64 || BKV == 128, "kv tile");
   static_assert(kVAtom % 1024 == 0, "V atom must keep 1024B alignment");
   static_assert(DVP % 16 == 0 && DVP <= 256, "invalid wgmma N for PV");
@@ -80,7 +92,7 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
   int ntiles = (p.Nk + BKV - 1) / BKV;
   if (p.causal) ntiles = min(ntiles, (q0 + kBQ + BKV - 1) / BKV);
 
-  if (warp == 8 && lane == 0) {
+  if (warp == (TMA_WARP ? 8 : 0) && lane == 0) {
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
@@ -101,26 +113,47 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
     ntiles = (nk + BKV - 1) / BKV;
   }
 
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, kQBytes);
-      for (int a = 0; a < KA; ++a)
-        tma_load_2d(sQ + a * kBQ * 128, &p.tmQ, q_full, p.q_col0 + head * DK + a * 64, b * p.q_bs + q0);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j % KV_STAGES;
-        const uint32_t ph = (j / KV_STAGES) & 1;
-        mbar_wait(&k_empty[st], ph ^ 1);
-        mbar_arrive_expect_tx(&k_full[st], kKBytes);
-        for (int a = 0; a < KA; ++a)
-          tma_load_2d(sK + st * kKBytes + a * BKV * 128, &p.tmK, &k_full[st], p.k_col0 + head * DK + a * 64,
-                      b * p.kv_bs + j * BKV);
-        mbar_wait(&v_empty[st], ph ^ 1);
-        mbar_arrive_expect_tx(&v_full[st], kVBytes);
-        for (int a = 0; a < KVA; ++a)
-          tma_load_2d(sV + st * kVBytes + a * kVAtom, &p.tmV, &v_full[st], b * p.kv_bs + j * BKV + a * 64, head * DVP);
+  // One thread each: the tile's Q, and K / V^T tile t into its stage once all eight consumer warps released the stage's
+  // previous tile (t - KV_STAGES).
+  auto load_q = [&] {
+    mbar_arrive_expect_tx(q_full, kQBytes);
+    for (int a = 0; a < KA; ++a)
+      tma_load_2d(sQ + a * kBQ * 128, &p.tmQ, q_full, p.q_col0 + head * DK + a * 64, b * p.q_bs + q0);
+  };
+  auto load_k = [&](int t) {
+    const int st = t % KV_STAGES;
+    mbar_wait(&k_empty[st], ((t / KV_STAGES) & 1) ^ 1);
+    mbar_arrive_expect_tx(&k_full[st], kKBytes);
+    for (int a = 0; a < KA; ++a)
+      tma_load_2d(sK + st * kKBytes + a * BKV * 128, &p.tmK, &k_full[st], p.k_col0 + head * DK + a * 64, b * p.kv_bs + t * BKV);
+  };
+  auto load_v = [&](int t) {
+    const int st = t % KV_STAGES;
+    mbar_wait(&v_empty[st], ((t / KV_STAGES) & 1) ^ 1);
+    mbar_arrive_expect_tx(&v_full[st], kVBytes);
+    for (int a = 0; a < KVA; ++a)
+      tma_load_2d(sV + st * kVBytes + a * kVAtom, &p.tmV, &v_full[st], b * p.kv_bs + t * BKV + a * 64, head * DVP);
+  };
+
+  if constexpr (TMA_WARP) {
+    if (warp == 8) {
+      if (lane == 0) {
+        load_q();
+        for (int j = 0; j < ntiles; ++j) {
+          load_k(j);
+          load_v(j);
+        }
       }
+      return;
     }
-    return;
+  } else {   // the first KV_STAGES - 1 tiles; iteration j of the loop below loads tile j + KV_STAGES - 1
+    if (lane == 0 && warp == 0) {
+      load_q();
+      for (int t = 0; t < min(KV_STAGES - 1, ntiles); ++t) load_k(t);
+    }
+    if (lane == 0 && warp == 4)
+      for (int t = 0; t < min(KV_STAGES - 1, ntiles); ++t) load_v(t);
+    __syncwarp();
   }
 
   // ------------------------------ consumer warpgroup g ------------------------------
@@ -129,7 +162,6 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
   const int row0 = g * 64 + (warp & 3) * 16 + (lane >> 2);
   const int c2 = 2 * (lane & 3);
   const int q_idx[2] = {q0 + row0, q0 + row0 + 8};
-  const int ksteps = (p.dv + 15) / 16;           // K16 steps of QK^T that can hold non-zero channels
   float o[DVP / 2];
 #pragma unroll
   for (int i = 0; i < DVP / 2; ++i) o[i] = 0.f;
@@ -144,15 +176,22 @@ __global__ void __launch_bounds__(288, 1) attention_kernel(const __grid_constant
     mbar_wait(&k_full[st], ph);
     wgmma_fence();
 #pragma unroll
-    for (int a = 0; a < KA; ++a) {
-      const uint64_t qd = make_desc_sw128(smem_u32(sQ + a * kBQ * 128 + g * 64 * 128));
-      const uint64_t kd = make_desc_sw128(smem_u32(sK + st * kKBytes + a * BKV * 128));
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (a * 4 + k < ksteps)      // the K16 steps past d_head multiply zero padding (d 80 in DK 128: 5 of 8 steps, d 40: 3 of 4)
-          wgmma_ss<BKV>(s, qd + 2 * k, kd + 2 * k, (a > 0 || k > 0) ? 1u : 0u);
+    for (int k = 0; k < kQKSteps; ++k) {
+      const uint64_t qd = make_desc_sw128(smem_u32(sQ + (k / 4) * kBQ * 128 + g * 64 * 128));
+      const uint64_t kd = make_desc_sw128(smem_u32(sK + st * kKBytes + (k / 4) * BKV * 128));
+      wgmma_ss<BKV>(s, qd + 2 * (k % 4), kd + 2 * (k % 4), k > 0 ? 1u : 0u);
     }
     wgmma_commit();
+    if constexpr (!TMA_WARP) {   // refill the stage of tile j - 1 (K by warpgroup 0, V^T by warpgroup 1) under the S product
+      const int t = j + KV_STAGES - 1;
+      if ((warp & 3) == 0 && lane == 0 && t < ntiles) {
+        if (g == 0)
+          load_k(t);
+        else
+          load_v(t);
+      }
+      __syncwarp();
+    }
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     __syncwarp();
@@ -245,15 +284,19 @@ struct AttnArgs {   // what the C ABI received; the tensor maps depend on the ke
   int B, H, q_bstride, kv_bstride;
 };
 
-template <int DK, int DVP, int BKV, int KV_STAGES, bool VARLEN = false>
+template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false>
 static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t stream) {
   constexpr size_t smem = attention_smem_bytes<DK, DVP, BKV, KV_STAGES>();
-  static_assert(smem <= 227 * 1024, "attention smem budget");
-  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES, VARLEN>;
+  // two CTAs per SM need twice the dynamic window plus 1 KB each reserved by the system, within 228 KB
+  static_assert(smem <= (TMA_WARP ? 227 * 1024 : 113 * 1024), "attention smem budget");
+  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES, TMA_WARP, VARLEN>;
   static bool configured = false;
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    prefer_max_smem(kernel);
+    if (TMA_WARP)
+      prefer_max_smem(kernel);
+    else   // the second CTA per SM is the point of this form: ask for the whole carveout, not the driver's pick
+      VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
   int rc = make_tmap_2d(&p.tmQ, a.Q, static_cast<uint64_t>(a.ldq), static_cast<uint64_t>(a.B) * a.q_bstride, a.ldq * 2, 64, kBQ);
@@ -263,7 +306,7 @@ static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t strea
   rc = make_tmap_2d(&p.tmV, a.Vt, static_cast<uint64_t>(a.B) * a.kv_bstride, static_cast<uint64_t>(a.H) * DVP, a.ldv * 2, 64, DVP);
   if (rc) return rc;
   dim3 grid((p.Nq + kBQ - 1) / kBQ, a.H, a.B);
-  VDB_CUDA_CHECK(launch_pdl(kernel, grid, dim3(288), smem, stream, p));
+  VDB_CUDA_CHECK(launch_pdl(kernel, grid, dim3(attention_threads(TMA_WARP)), smem, stream, p));
   count_launch();
   return VDB_OK;
 }
@@ -319,11 +362,13 @@ int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, 
   if (rc) return rc;
   const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // 128-key tiles up to d_head 80; 64-key tiles at d_head 160 keep S + O + P within the register budget
-  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 2>(p, a, st);
-  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2>(p, a, st);
-  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 128, 2>(p, a, st);
-  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2>(p, a, st);
+  // d_head <= 80: two CTAs per SM, each within 128 registers and half the shared memory (d_head <= 64: 128-key tiles,
+  // 3 / 2 stages; d_head 80: 64-key tiles, 3 stages).  d_head 160 keeps the TMA warp and one CTA per SM: two CTAs' Q and
+  // K / V^T stages do not fit; 64-key tiles keep its S + O + P within the register budget.
+  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false>(p, a, st);
+  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false>(p, a, st);
+  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false>(p, a, st);
+  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true>(p, a, st);
   return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel for d_head %d", d_head);
 }
 
@@ -342,7 +387,7 @@ int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const vo
                                    scale, causal, p, a);
   if (rc) return rc;
   p.kv_len = kv_len;
-  return launch_attention<64, 64, 128, 2, true>(p, a, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention<64, 64, 128, 2, false, true>(p, a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
