@@ -285,6 +285,25 @@ int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* 
 int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
                        const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
                        const int* step, int eos, int max_len, float* record, void* stream);
+/* vdb_textdec_sample with the top-k / nucleus cuts of top_k_top_p_filtering (reference optimus.py:690-719), as
+ * sample_single_sequence_conditional applies them (optimus.py:662-688).  Per row, l = logits / temperature (fp32):
+ *   top_k > 0: k = min(top_k, V); every token with l < (the k-th largest l) is removed.  Ties with the k-th value are kept, so
+ *     more than k tokens can survive.
+ *   then, when 0 < top_p < 1: the survivors' softmax, ordered by descending l; a survivor is kept when the probability mass
+ *     before it in that order is <= top_p (the first one always is).  Tied tokens are taken in ascending vocabulary index, as a
+ *     stable descending sort orders them: with boundary value v, M(>v) the mass above it and q the mass of one tied token, the
+ *     first min(#ties, 1 + floor((top_p - M(>v)) / q)) ties are kept.  (The reference's torch.sort is not stable, so this is the
+ *     one case its order leaves open.)  Masses are exp(l - max) / Z with Z the survivors' fp64 sum, compared as 64-bit fixed-point
+ *     integers (units of 2^-62), so the cut is exact and repeatable.
+ * top_k == 0 (or >= V) turns the top-k cut off, top_p == 0 or 1 the nucleus cut; with both off (or with forced tokens) this is
+ * vdb_textdec_sample exactly.  top_k = 1 is greedy decoding.  The draw is vdb_textdec_sample's inverse CDF over the kept tokens
+ * only, in vocabulary order, their mass renormalised, with the same u.  The filter stages the row in shared memory: with a cut on,
+ * V <= 53248.  top_k < 0 or top_p NaN or outside [0, 1] return VDB_ERR_INVALID before any launch, as do vdb_textdec_sample's
+ * argument errors. */
+int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
+                                const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
+                                int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
+                                void* stream);
 
 /* ---- semantic/style disentanglement of the image context — decompose / adjust_rank of the reference app.py:48-127 -----------
  * For each item b < n_items of x [n_items, m, n] (fp32, contiguous):  X = x - rowmean(x);  the randomized PCA of torch.pca_lowrank

@@ -2,7 +2,10 @@
 <EOS> never drawn so every row runs all 28 token steps.  Reports, from CUDA events after warm-up: ms per token step (replays of the
 captured step graph), launches per step, and the bytes a step must read over its time against 3.35 TB/s (H100 SXM data sheet);
 then one complete i2t call: 50 DDIM steps on the text latent, then the decode.  Prints the card name and power limit.
-    python tools/text_decode_bench.py [--no-i2t]"""
+With --top-k / --top-p: ms per token step at 4 and 16 rows with the sampler's cuts off and on, the two graphs replayed
+alternately in one session, and the launches per step of each.
+    python tools/text_decode_bench.py [--no-i2t] [--top-k K] [--top-p P]"""
+import argparse
 import json
 import os
 import subprocess
@@ -20,6 +23,11 @@ from lib.model_zoo.ddim import DDIMSampler  # noqa: E402
 from lib.model_zoo.optimus import STEPS_PER_CHECK  # noqa: E402
 from vdb200 import ops  # noqa: E402
 
+ap = argparse.ArgumentParser()
+ap.add_argument("--no-i2t", action="store_true")
+ap.add_argument("--top-k", type=int, default=0)
+ap.add_argument("--top-p", type=float, default=0.0)
+args = ap.parse_args()
 HBM = 3.35e12
 dev = torch.device("cuda", 0)
 card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
@@ -51,7 +59,7 @@ with torch.no_grad():
         vae.decode_ids(z, eos_token=-1)                      # warm-up: packs weights, captures the step-chunk graph
     p = vae.packed()
     st = vae._state(R, dev)
-    graph = st.graphs[(1.0, -1, 30, "seed", False)]
+    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0)]
     n0 = ops.launch_count()
     vae._step(st, p, 1.0, -1, 30, "seed", False)
     launches = ops.launch_count() - n0
@@ -82,7 +90,47 @@ res = dict(card=card, rows=R, ms_per_token_step=round(ms_step, 4), launches_per_
            share_of_3_35_TBps=round(wbytes / (ms_step * 1e-3) / HBM, 3), ms_per_decode_28_steps=round(ms_decode, 3))
 print(json.dumps(res))
 
-if "--no-i2t" not in sys.argv:
+
+
+def step_ms_off_and_on(R, top_k, top_p, rounds=5, reps=10):
+    """ms per token step of the captured chunk with the cuts off and on, alternated over rounds; launches per step of each."""
+    zr = torch.randn(R, 768, generator=torch.Generator().manual_seed(5)).to(dev) * 3.0
+    cuts = {"off": (0, 0.0), "on": (top_k, top_p)}
+    out = {}
+    with torch.no_grad():
+        st = vae._state(R, dev)
+        for name, (k, p) in cuts.items():
+            for _ in range(2):
+                vae.decode_ids(zr, eos_token=-1, top_k=k, top_p=p)
+            n0 = ops.launch_count()
+            vae._step(st, vae.packed(), 1.0, -1, 30, "seed", False, k, p)
+            out[name] = dict(launches_per_step=ops.launch_count() - n0, ms=[])
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for _ in range(rounds):
+            for name, (k, p) in cuts.items():
+                g = st.graphs[(1.0, -1, 30, "seed", False, k, p)]
+                e0.record()
+                for _ in range(reps):
+                    st.step.zero_()
+                    g.replay()
+                e1.record()
+                torch.cuda.synchronize()
+                out[name]["ms"].append(e0.elapsed_time(e1) / (reps * STEPS_PER_CHECK))
+    res = dict(card=card, rows=R, top_k=top_k, top_p=top_p)
+    for name in cuts:
+        res[f"ms_per_step_cuts_{name}"] = round(min(out[name]["ms"]), 4)
+        res[f"ms_per_step_cuts_{name}_all"] = [round(v, 4) for v in out[name]["ms"]]
+        res[f"launches_per_step_cuts_{name}"] = out[name]["launches_per_step"]
+    res["filter_cost_share_of_step"] = round(res["ms_per_step_cuts_on"] / res["ms_per_step_cuts_off"] - 1.0, 4)
+    return res
+
+
+if args.top_k or 0.0 < args.top_p < 1.0:
+    for rows_ in (4, 16):
+        print(json.dumps(step_ms_off_and_on(rows_, args.top_k, args.top_p)))
+
+if not args.no_i2t:
     bs = 4
     gq = torch.Generator().manual_seed(3)
     xT = torch.randn(bs, 768, generator=gq).to(dev)

@@ -224,6 +224,97 @@ __global__ void textdec_embed_kernel(const int* __restrict__ tokens, int ldt, co
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
+// top-k / nucleus filter of the sampler (kFilter instantiation).  The row's scaled logits l are staged once in shared memory
+// as order-preserving uint32 keys; both cuts are MSD radix selects over them, 8 bits per pass, with 256-bin histograms
+// privatised per group of 4 warps.  top-k counts tokens; the nucleus weighs each survivor by its probability as a 64-bit
+// fixed-point integer (exp(l - max) / Z scaled by 2^62, Z the survivors' fp64 sum in a fixed order): integer atomics are exact
+// and order-free, so graph replays stay bitwise repeatable.
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int kFilterHists = 8;                 // privatised histograms (kSampleThreads / 32 warps share them 4 to 1)
+constexpr int kFilterMaxV = 53248;              // staged keys (4 B each) + the histograms fit in the 227 KiB opt-in
+constexpr size_t kFilterHistBytes = kFilterHists * 256 * sizeof(unsigned long long);
+constexpr double kMassOne = 0x1.0p62;           // fixed-point unit of probability mass
+
+VDB_DEVINL uint32_t order_key(float f) {         // a < b  <=>  order_key(a) < order_key(b)  (non-NaN)
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+VDB_DEVINL float key_value(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+VDB_DEVINL unsigned long long key_mass(uint32_t k, float mx, double scale) {
+  return __double2ull_rn(static_cast<double>(expf(key_value(k) - mx)) * scale);
+}
+
+struct FilterShared {
+  unsigned long long above;
+  double red[32];
+  int bin, found;
+  int ties[32];
+};
+
+struct Selected {
+  bool found;
+  uint32_t key;
+  unsigned long long above;
+};
+
+// The largest key v among the staged keys >= lo with W(>= v) > T, where W sums 1 per key (kMass false) or key_mass (kMass
+// true) over the keys >= lo.  found is false when all of them together weigh <= T; else key = v and above = W(> v).
+template <bool kMass>
+VDB_DEVINL Selected radix_select(const uint32_t* keys, int V, uint32_t lo, unsigned long long T, float mx, double scale,
+                                 unsigned long long* hist, FilterShared& sh) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  unsigned long long* mine = hist + (warp % kFilterHists) * 256;
+  uint32_t prefix = 0;
+  unsigned long long ab = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < kFilterHists * 256; i += blockDim.x) hist[i] = 0ull;
+    __syncthreads();
+    const uint32_t hi = shift == 24 ? 0u : 0xffffffffu << (shift + 8);
+    for (int i = tid; i < V; i += blockDim.x) {
+      const uint32_t k = keys[i];
+      if (k >= lo && (k & hi) == prefix) atomicAdd(mine + ((k >> shift) & 255u), kMass ? key_mass(k, mx, scale) : 1ull);
+    }
+    __syncthreads();
+    if (tid < 256) {
+      unsigned long long t = hist[tid];
+      for (int h = 1; h < kFilterHists; ++h) t += hist[h * 256 + tid];
+      hist[tid] = t;
+    }
+    __syncthreads();
+    if (warp == 0) {                               // lane L holds bins 255 - 8L - j, j < 8: the bins in descending order
+      unsigned long long own = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) own += hist[255 - 8 * lane - j];
+      unsigned long long inc = own;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long n = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += n;
+      }
+      const unsigned hit = __ballot_sync(0xffffffffu, ab + inc > T);
+      if (lane == 0) sh.found = hit != 0u;
+      if (hit && lane == __ffs(hit) - 1) {
+        unsigned long long c = ab + inc - own;
+        int b = 255 - 8 * lane;
+        for (int j = 0; j < 8; ++j, --b) {
+          if (c + hist[b] > T) break;
+          c += hist[b];
+        }
+        sh.bin = b;
+        sh.above = c;
+      }
+    }
+    __syncthreads();
+    if (!sh.found) return Selected{false, 0u, 0ull};   // only the first pass can miss: later ones refine a bin that crossed T
+    prefix |= static_cast<uint32_t>(sh.bin) << shift;
+    ab = sh.above;
+  }
+  return Selected{true, prefix, ab};
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
 // Sampler, one CTA per row: token s+1 ~ softmax(logits / temperature) by inverse CDF of a uniform u in [0, 1).
 // Each thread owns a contiguous slice of the vocabulary; exp(x - max) is summed in fp64 per slice, the slice sums are
 // scanned across the block in a fixed order, and the thread whose [prefix, next prefix) holds u * total walks its slice.
@@ -231,12 +322,17 @@ __global__ void textdec_embed_kernel(const int* __restrict__ tokens, int ldt, co
 // forced (teacher forcing) replaces the draw.  A finished row (done[r] != 0) is left untouched.  After writing token s+1:
 // == eos ends the row; otherwise when s+1 == max_len - 2 the row gets eos at s+2 (optimus.py:682-688 overwrites the 30th
 // token, so that last draw is skipped).  record (may be NULL) receives this step's raw logits at [s][r][:].
+// kFilter: the same pick over the tokens the top-k / nucleus cuts keep (vdb_textdec_sample_filtered), removed tokens weigh 0.
+// The kept set is every key > bound plus the first `cap` keys == bound in vocabulary order.
 // ---------------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kSampleThreads)
+template <bool kFilter>
+__global__ void __launch_bounds__(kSampleThreads, 1)   // one CTA per SM: without the 1, ptxas caps it at 32 registers and spills
 textdec_sample_kernel(const float* __restrict__ logits, int R, int V, long long ldl, float temperature,
                       const unsigned long long* __restrict__ seed, const double* __restrict__ uniforms, int ldu,
                       const int* __restrict__ forced, int ldf, int* __restrict__ tokens, int ldt, int* __restrict__ done,
-                      int* __restrict__ lengths, const int* __restrict__ step, int eos, int max_len, float* __restrict__ record) {
+                      int* __restrict__ lengths, const int* __restrict__ step, int eos, int max_len, float* __restrict__ record,
+                      int top_k, float top_p) {
+  extern __shared__ __align__(16) unsigned char s_filter[];   // kFilter: histograms, then the V staged keys
   __shared__ float s_max[32];
   __shared__ double s_scan[32];
   __shared__ int s_tok, s_last;
@@ -255,8 +351,18 @@ textdec_sample_kernel(const float* __restrict__ logits, int R, int V, long long 
   } else {
     const int per = (V + blockDim.x - 1) / blockDim.x;
     const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
+    unsigned long long* hist = reinterpret_cast<unsigned long long*>(s_filter);
+    uint32_t* keys = reinterpret_cast<uint32_t*>(s_filter + kFilterHistBytes);
     float mx = -INFINITY;
-    for (int i = i0; i < i1; ++i) mx = fmaxf(mx, lr[i] / temperature);
+    if constexpr (kFilter) {
+      for (int i = tid; i < V; i += blockDim.x) {
+        const float l = lr[i] / temperature;
+        keys[i] = order_key(l);
+        mx = fmaxf(mx, l);
+      }
+    } else {
+      for (int i = i0; i < i1; ++i) mx = fmaxf(mx, lr[i] / temperature);
+    }
 #pragma unroll
     for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     if (lane == 0) s_max[warp] = mx;
@@ -265,10 +371,64 @@ textdec_sample_kernel(const float* __restrict__ logits, int R, int V, long long 
     mx = s_max[0];
     for (int i = 1; i < (int)(blockDim.x >> 5); ++i) mx = fmaxf(mx, s_max[i]);
 
+    uint32_t bound = 0u;
+    int cap = INT_MAX, rank0 = 0;
+    if constexpr (kFilter) {
+      __shared__ FilterShared sh;
+      if (top_k > 0 && top_k < V)        // the k-th largest key: W(>= v) > k - 1 counted
+        bound = radix_select<false>(keys, V, 0u, static_cast<unsigned long long>(top_k - 1), mx, 0.0, hist, sh).key;
+      if (top_p > 0.0f && top_p < 1.0f) {
+        double z = 0.0;                  // Z over the top-k survivors: per-thread strided sums, then a fixed tree
+        for (int i = tid; i < V; i += blockDim.x)
+          if (keys[i] >= bound) z += static_cast<double>(expf(key_value(keys[i]) - mx));
+#pragma unroll
+        for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+        if (lane == 0) sh.red[warp] = z;
+        __syncthreads();
+        z = sh.red[0];
+        for (int i = 1; i < (int)(blockDim.x >> 5); ++i) z += sh.red[i];
+        const double scale = kMassOne / z;
+        const unsigned long long P = __double2ull_rn(static_cast<double>(top_p) * kMassOne);
+        // boundary b: the largest value whose survivors at or above it weigh > top_p.  Everything above b is kept; the ties
+        // at b, taken in vocabulary order, each have exclusive mass above + t q, kept while that is <= top_p.
+        const Selected b = radix_select<true>(keys, V, bound, P, mx, scale, hist, sh);
+        if (b.found) {
+          const unsigned long long q = key_mass(b.key, mx, scale), n = 1ull + (P - b.above) / q;
+          bound = b.key;
+          cap = n < static_cast<unsigned long long>(INT_MAX) ? static_cast<int>(n) : INT_MAX;
+        }
+      }
+      if (cap != INT_MAX) {              // rank0: the ties at the bound in the slices before this thread's
+        int t = 0;
+        for (int i = i0; i < i1; ++i) t += keys[i] == bound;
+        int inc = t;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int n = __shfl_up_sync(0xffffffffu, inc, o);
+          if (lane >= o) inc += n;
+        }
+        if (lane == 31) sh.ties[warp] = inc;
+        __syncthreads();
+        int off = 0;
+        for (int w = 0; w < warp; ++w) off += sh.ties[w];
+        rank0 = off + inc - t;
+      }
+    }
+    // exp(l - max) of token i, or 0 for a token the cuts remove; rank counts the ties at the bound met so far
+    auto weight = [&](int i, int& rank) -> float {
+      if constexpr (kFilter) {
+        const uint32_t k = keys[i];
+        if (k < bound || (k == bound && rank++ >= cap)) return 0.0f;
+        return expf(key_value(k) - mx);
+      } else {
+        return expf(lr[i] / temperature - mx);
+      }
+    };
+
     double sum = 0.0;
-    int last = -1;
+    int last = -1, rank = rank0;
     for (int i = i0; i < i1; ++i) {
-      const float e = expf(lr[i] / temperature - mx);
+      const float e = weight(i, rank);
       sum += static_cast<double>(e);
       if (e > 0.0f) last = i;
     }
@@ -310,8 +470,9 @@ textdec_sample_kernel(const float* __restrict__ logits, int R, int V, long long 
     if (target >= pre && target < hi) {
       double c = pre;
       int pick = last;
+      rank = rank0;
       for (int i = i0; i < i1; ++i) {
-        c += static_cast<double>(expf(lr[i] / temperature - mx));
+        c += static_cast<double>(weight(i, rank));       // a removed token adds 0: it can never be the pick
         if (target < c) { pick = i; break; }
       }
       s_tok = pick;
@@ -402,9 +563,10 @@ int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* 
   return VDB_OK;
 }
 
-int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
-                       const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
-                       const int* step, int eos, int max_len, float* record, void* stream) {
+static int textdec_sample_launch(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
+                                 const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
+                                 int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
+                                 void* stream) {
   if (!logits || !tokens || !done || !lengths || !step) return set_error(VDB_ERR_INVALID, "textdec_sample: null pointer");
   if (!forced && !uniforms && !seed) return set_error(VDB_ERR_INVALID, "textdec_sample: need a seed, uniforms or forced tokens");
   if (R < 1 || R > kGvMaxRows || V < 1 || ldl < V) return set_error(VDB_ERR_INVALID, "textdec_sample: need 1 <= R <= 16, ldl >= V >= 1");
@@ -413,11 +575,48 @@ int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float t
     return set_error(VDB_ERR_INVALID, "textdec_sample: bad token / uniform row strides");
   if ((reinterpret_cast<uintptr_t>(seed) & 7) || (reinterpret_cast<uintptr_t>(uniforms) & 7))
     return set_error(VDB_ERR_INVALID, "textdec_sample: seed / uniforms must be 8-byte aligned");
-  textdec_sample_kernel<<<R, kSampleThreads, 0, as_stream(stream)>>>(logits, R, V, ldl, temperature, seed, uniforms, ldu, forced, ldf,
-                                                                     tokens, ldt, done, lengths, step, eos, max_len, record);
+  // forced tokens replace the draw, so the cuts have nothing to act on
+  const bool filter = !forced && ((top_k > 0 && top_k < V) || (top_p > 0.0f && top_p < 1.0f));
+  if (!filter) {
+    textdec_sample_kernel<false><<<R, kSampleThreads, 0, as_stream(stream)>>>(
+        logits, R, V, ldl, temperature, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record,
+        0, 0.0f);
+  } else {
+    if (V > kFilterMaxV)
+      return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top-k / top-p stage at most %d logits per row, got V = %d",
+                       kFilterMaxV, V);
+    const size_t smem = kFilterHistBytes + static_cast<size_t>(V) * sizeof(uint32_t);
+    static bool configured = false;
+    if (!configured) {
+      VDB_CUDA_CHECK(cudaFuncSetAttribute(textdec_sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          static_cast<int>(kFilterHistBytes + kFilterMaxV * sizeof(uint32_t))));
+      configured = true;
+    }
+    textdec_sample_kernel<true><<<R, kSampleThreads, smem, as_stream(stream)>>>(
+        logits, R, V, ldl, temperature, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record,
+        top_k, top_p);
+  }
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;
+}
+
+int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
+                       const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
+                       const int* step, int eos, int max_len, float* record, void* stream) {
+  return textdec_sample_launch(logits, R, V, ldl, temperature, 0, 0.0f, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths,
+                               step, eos, max_len, record, stream);
+}
+
+int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
+                                const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
+                                int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
+                                void* stream) {
+  if (top_k < 0) return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top_k must be >= 0, got %d", top_k);
+  if (!(top_p >= 0.0f && top_p <= 1.0f))
+    return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top_p must be in [0, 1], got %g", static_cast<double>(top_p));
+  return textdec_sample_launch(logits, R, V, ldl, temperature, top_k, top_p, seed, uniforms, ldu, forced, ldf, tokens, ldt, done,
+                               lengths, step, eos, max_len, record, stream);
 }
 
 }  // extern "C"

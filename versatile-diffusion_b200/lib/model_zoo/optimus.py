@@ -29,12 +29,19 @@ Differences from the reference, all deliberate:
   - the draw of token s+1 of row r is an inverse-CDF pick of softmax(logits / temperature) with a Philox4x32-10 uniform at counter
     (r, s), keyed by one 64-bit seed taken from torch's default CPU generator per decode() call: `torch.manual_seed` fixes the text,
     but the tokens are not those torch.multinomial would draw;
-  - the full softmax is sampled.  The reference's top_k_top_p_filtering(top_p=1.0) removes nothing in exact arithmetic but, in fp32,
-    can cut a tail whose sorted cumulative sum rounds above 1.0 (probability mass of order 1e-6);
+  - by default (top_k=0, top_p=0.0) the full softmax is sampled.  The reference's top_k_top_p_filtering(top_p=1.0) removes nothing
+    in exact arithmetic but, in fp32, can cut a tail whose sorted cumulative sum rounds above 1.0 (probability mass of order 1e-6);
+    top_p=1.0 here samples the full softmax too;
+  - decode(z, top_k=..., top_p=...) applies the reference's top-k and nucleus cuts (optimus.py:690-719) in the sampling kernel,
+    inside the captured step graph; top_k=1 is greedy decoding.  The probabilities the nucleus cut sums are fp64-exact fixed-point
+    integers rather than an fp32 cumsum, and tied tokens at the nucleus boundary are taken in vocabulary order (the reference's
+    unstable sort leaves their order open); see vdb_textdec_sample_filtered;
   - the reference's 29th forward pass, whose draw is always overwritten with <EOS>, is skipped;
   - weights are bf16 (packed at load); the residual stream, attention, logits and the sampler's sums are fp32 / fp64.
 """
 import json
+import math
+import numbers
 import os
 import unicodedata
 
@@ -62,6 +69,15 @@ ENC_HEAD_ROWS = 16                                # [CLS] rows per pooler / z_mu
 def _ops():
     from vdb200 import ops
     return ops
+
+
+def _check_cuts(top_k, top_p):
+    """-> (int top_k, float top_p) of the sampler's top-k / nucleus cuts, or ValueError."""
+    if isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral) or top_k < 0:
+        raise ValueError(f"optimus_vae_next: top_k must be an int >= 0 (0: no top-k cut), got {top_k!r}")
+    if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real) or not math.isfinite(top_p) or not 0.0 <= top_p <= 1.0:
+        raise ValueError(f"optimus_vae_next: top_p must be a finite float in [0, 1] (0 or 1: no nucleus cut), got {top_p!r}")
+    return int(top_k), float(top_p)
 
 
 class VocabularyMissingError(RuntimeError):
@@ -576,7 +592,7 @@ class optimus_vae_next(PackedModule):
         self.__dict__['_states'] = {}        # captured graphs hold the old weight addresses
 
     # ------------------------------------------------------------------ one token step (5 launches per layer + 4)
-    def _step(self, st, p, temperature, eos, max_len, mode, record):
+    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0):
         ops = _ops()
         dec = self.decoder
         D = dec.n_embd
@@ -591,12 +607,13 @@ class optimus_vae_next(PackedModule):
         ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=temperature,
                            seed=st.seed if mode == "seed" else None, uniforms=st.uniforms if mode == "uniforms" else None,
                            forced=st.forced if mode == "forced" else None, eos=eos, max_len=max_len,
-                           record=st.record if record else None)
+                           record=st.record if record else None, top_k=top_k, top_p=top_p)
         ops.add_int(st.step, 1)
 
     @torch.no_grad()
     def _run(self, z, temperature, eos, pre_scale=1.0, max_len=MAX_LENGTH, nsteps=None, mode="seed", uniforms=None, forced=None,
-             record=False, graph=True):
+             record=False, graph=True, top_k=0, top_p=0.0):
+        top_k, top_p = _check_cuts(top_k, top_p)
         require_cuda(z, "optimus_vae_next.decode")
         if z.dim() != 2 or z.shape[1] != self.nz:
             raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
@@ -629,7 +646,7 @@ class optimus_vae_next(PackedModule):
         else:
             st.forced.zero_()
             st.forced[:, :forced.shape[1]].copy_(forced)
-        key = (float(temperature), int(eos), int(max_len), mode, bool(record))
+        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p)
         s = 0
         while s < nsteps:
             n = min(STEPS_PER_CHECK, nsteps - s)
@@ -638,7 +655,7 @@ class optimus_vae_next(PackedModule):
                 g.replay()
             else:
                 for _ in range(n):
-                    self._step(st, p, temperature, eos, max_len, mode, record)
+                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p)
                 if graph and n == STEPS_PER_CHECK and key not in st.graphs:
                     # the chunk just ran eagerly (kernels configured, caches warm); capture one for the later chunks
                     torch.cuda.current_stream().synchronize()
@@ -646,7 +663,7 @@ class optimus_vae_next(PackedModule):
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
                         for _ in range(n):
-                            self._step(st, p, temperature, eos, max_len, mode, record)
+                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p)
                     st.step.copy_(step_before)        # capture does not execute, but keep the counter exactly as the eager chunk left it
                     st.graphs[key] = g
             s += n
@@ -655,12 +672,14 @@ class optimus_vae_next(PackedModule):
         return st, s
 
     @torch.no_grad()
-    def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True):
+    def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True,
+                   top_k=0, top_p=0.0):
         """Sampled token rows, each an int64 CPU tensor starting with <BOS> and (unless eos_token never occurs and is never forced)
         ending with eos_token, length <= 30.  uniforms (fp64 [n, >=28]) replaces the Philox draws; return_logits also returns the
-        fp32 logits of every step that ran, [steps, n, 50260] on the device."""
+        fp32 logits of every step that ran, [steps, n, 50260] on the device.  top_k > 0 keeps the top_k most likely tokens (ties
+        included), 0 < top_p < 1 the nucleus of mass top_p (optimus.py:690-719); the defaults sample the full softmax."""
         st, ran = self._run(z, temperature, int(eos_token), pre_scale=pre_scale, mode="uniforms" if uniforms is not None else "seed",
-                            uniforms=uniforms, record=return_logits, graph=graph)
+                            uniforms=uniforms, record=return_logits, graph=graph, top_k=top_k, top_p=top_p)
         tokens, lengths = st.tokens.cpu(), st.lengths.cpu()
         rows = [tokens[r, :int(lengths[r])].long() for r in range(st.R)]
         if return_logits:
@@ -678,7 +697,7 @@ class optimus_vae_next(PackedModule):
         return st.record[:L].permute(1, 0, 2).contiguous()
 
     @torch.no_grad()
-    def decode(self, z, temperature=1.0, pre_scale=1.0):
-        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row."""
-        rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale)
+    def decode(self, z, temperature=1.0, pre_scale=1.0, top_k=0, top_p=0.0):
+        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row; top_k / top_p as in decode_ids."""
+        rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale, top_k=top_k, top_p=top_p)
         return [self.tokenizer_decoder.sentence(r.tolist()) for r in rows]

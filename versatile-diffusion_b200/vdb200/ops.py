@@ -719,18 +719,23 @@ def textdec_embed(tokens, step, wte, wpe, emb, out, pos_offset=1):
 
 
 def textdec_sample(logits, tokens, done, lengths, step, temperature=1.0, seed=None, uniforms=None, forced=None, eos=50259,
-                   max_len=30, record=None):
+                   max_len=30, record=None, top_k=0, top_p=0.0):
     """Token *step+1 of every unfinished row ~ softmax(logits / temperature) (see vdb_textdec_sample).  seed: device uint64 [1]
-    (as int64), uniforms: fp64 [R, >=steps] given draws, forced: int32 [R, L] teacher-forced tokens, record: fp32 [steps, R, V]."""
+    (as int64), uniforms: fp64 [R, >=steps] given draws, forced: int32 [R, L] teacher-forced tokens, record: fp32 [steps, R, V].
+    top_k > 0 or 0 < top_p < 1 draw from the tokens those cuts keep instead (vdb_textdec_sample_filtered)."""
     _need(logits, torch.float32, "logits", rows_ok=True)
     _need(tokens, torch.int32, "tokens"); _need(done, torch.int32, "done"); _need(lengths, torch.int32, "lengths")
     _need(step, torch.int32, "step"); _need(seed, torch.int64, "seed"); _need(uniforms, torch.float64, "uniforms")
     _need(forced, torch.int32, "forced"); _need(record, torch.float32, "record")
     R, V = logits.shape
-    check(lib.vdb_textdec_sample(_ptr(logits), R, V, logits.stride(0), float(temperature), _ptr(seed), _ptr(uniforms),
-                                 uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
-                                 forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done),
-                                 _ptr(lengths), _ptr(step), int(eos), int(max_len), _ptr(record), _stream()), "textdec_sample")
+    args = (_ptr(seed), _ptr(uniforms), uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
+            forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done), _ptr(lengths), _ptr(step),
+            int(eos), int(max_len), _ptr(record), _stream())
+    if top_k == 0 and top_p in (0.0, 1.0):
+        check(lib.vdb_textdec_sample(_ptr(logits), R, V, logits.stride(0), float(temperature), *args), "textdec_sample")
+    else:
+        check(lib.vdb_textdec_sample_filtered(_ptr(logits), R, V, logits.stride(0), float(temperature), int(top_k), float(top_p),
+                                              *args), "textdec_sample_filtered")
 
 
 # ------------------------------------------------------------------------------------------------
