@@ -125,12 +125,17 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int W, int C, int mode, const 
 /* ---- wgmma flash attention — CrossAttention.forward, attention.py:178-192 -----------------
  * O = softmax(Q K^T * scale) V per (batch, head), fp32 online softmax, nothing materialised.
  * Q [B*Nq, ldq] head h at columns q_col0 + h*DK; K [B*Nk, ldk] at k_col0 + h*DK;
- * Vt [H*DVP, ldv] row h*DVP + c, column b*Nk + j; out [B*Nq, ldo] head h at columns h*d_head.
- * DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head); pad columns/rows must be
- * zero (the projection weights are zero-padded at pack time). causal != 0: CLIP text mask.
+ * Vt [H*DVP, ldv] row h*DVP + c, column b*kv_bstride + j; out [B*Nq, ldo] head h at columns h*d_head.
+ * DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head); the head pads must be
+ * zero: Q / K columns d_head .. DK-1 of each head and Vt rows h*DVP + d_head .. h*DVP + DVP-1 (the
+ * projection weights are zero-padded at pack time). causal != 0: CLIP text mask.
  * Batch b starts at row b*q_bstride of Q/out and at row (K) / column (Vt) b*kv_bstride; kv_bstride must be a
  * multiple of 8 (TMA: 16-byte aligned innermost coordinate), so ragged contexts (77, 257 tokens) are stored
- * padded to 80 / 264 per batch item; the pad keys are masked by Nk. 0 = dense (stride = count). */
+ * padded to 80 / 264 per batch item; the pad keys are masked by Nk. 0 = dense (stride = count).
+ * May hold any finite values: the pad keys (K rows / Vt columns b*kv_bstride + [Nk, kv_bstride)), the pad
+ * query rows b*q_bstride + [Nq, q_bstride) of Q, and everything outside the given slices (other columns of
+ * Q / K / Vt, Vt columns past B*kv_bstride).  Only rows b*q_bstride + [0, Nq), columns [0, H*d_head) of out
+ * are written. */
 int vdb_attention_dk_pad(int d_head);
 int vdb_attention_dv_pad(int d_head);
 int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,

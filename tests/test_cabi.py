@@ -55,6 +55,24 @@ def test_misaligned_output_or_residual_is_rejected_before_launch():
                                 ctypes.byref(parts), 0, None) == 1 and b"16-byte aligned" in lib.vdb_last_error()
 
 
+def test_attention_dispatch_edges():
+    """The instantiation table test_attention_coverage_gpu restates: the pads at each band's edges, and the d_head values
+    between and above the bands refused with VDB_ERR_UNSUPPORTED by both entry points before any launch (the fake
+    addresses below are never dereferenced)."""
+    from vdb200._lib import lib
+    pads = {8: (64, 48), 48: (64, 48), 56: (64, 64), 64: (64, 64), 72: (128, 80), 80: (128, 80), 136: (192, 160), 160: (192, 160)}
+    for d, want in pads.items():
+        assert (lib.vdb_attention_dk_pad(d), lib.vdb_attention_dv_pad(d)) == want, d
+    Q, K, Vt, out, kv_len = 0x10000, 0x20000, 0x30000, 0x40000, 0x50000
+    before = lib.vdb_launch_count()
+    for d in (88, 96, 128, 168, 200):
+        assert lib.vdb_attention_bf16(Q, 2048, 0, K, 2048, 0, Vt, 1024, out, 1024, 2, 2, 128, 128, 0, 0, d, 0.125, 0, None) == 3, d
+        assert b"d_head" in lib.vdb_last_error()
+        assert lib.vdb_attention_varlen_bf16(Q, 2048, 0, K, 2048, 0, Vt, 1024, out, 1024, 2, 2, 128, 128, 0, 0, d, 0.125, 0,
+                                             kv_len, None) == 3, d
+    assert lib.vdb_launch_count() == before
+
+
 def test_igemm_last_plan_reports_nine_fields():
     from vdb200._lib import lib
     buf = (ctypes.c_int * 9)()
