@@ -309,6 +309,40 @@ int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl
                                 const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
                                 int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
                                 void* stream);
+/* vdb_textdec_attention for beam search: cache slot j < *step of row r is read from physical row src[r * T + j] (int32 [R, T],
+ * every entry in [0, R)) instead of row r; this step's k / v are still written at row r, slot *step.  A physical (row, slot) is
+ * written once, at step == slot, so permuting beams permutes src rows and never moves the cache.  Same argument checks as
+ * vdb_textdec_attention, plus a non-null, 4-byte aligned src.  With src[r, j] = r the output equals vdb_textdec_attention's bitwise. */
+int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
+                                  const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo,
+                                  void* stream);
+/* One beam-search step, s = *step.  It stands in for the reference's optimus_vae.decode(z, strategy='beam', K)
+ * (optimus.py:196-213), whose beam_search_decode does not exist in the reference's GPT-2, so this definition is the specification.
+ * Rows r = latent * K + beam, R = n * K <= 16, 1 <= K <= 16.  Per beam: tokens [R, ldt] (token 0 = <BOS>), src [R, lds] (the
+ * slot-to-row table of vdb_textdec_attention_indexed), scores fp64 [R], done [R], lengths [R].  Before step 0 the caller sets
+ * every score to -inf except beam 0's (0), so the first step does not produce K copies of one hypothesis.
+ *   logp_r(v) = log softmax(logits[r] / temperature)(v), all in fp64 from the fp32 logits (the division, max, exp, sum and log).
+ *   Candidates: each live beam b crossed with each token v, score S_b + logp_b(v); each finished beam b as itself, score S_b.
+ *   The K best become beams 0 .. K-1 in rank order; ties go to the lower parent beam, then the lower token id.
+ *   New beam j with parent p: tokens[j, 0 .. s+1] = tokens[p, 0 .. s+1], src[j, 0 .. s-1] = src[p, 0 .. s-1], src[j, s] = p's row,
+ *   and for a live parent tokens[j, s+1] = v.  v == eos finishes it (lengths = s + 2); otherwise, when s + 1 == max_len - 2, <eos>
+ *   is appended at s + 2 unscored and it finishes (lengths = s + 3).  A finished beam keeps its score and length.
+ * A latent is finished when all K beams are; live scores only decrease, so no live beam could have beaten them.  A beam's
+ * scored-token count is min(lengths - 1, max_len - 2) (a chosen <eos> counts, a forced one does not).  Two launches: one CTA per
+ * row (K best tokens via the top-k radix select of vdb_textdec_sample_filtered, ties in vocabulary order; at most K of one
+ * row's tokens can enter the K best), then one CTA per latent.  The per-row pick orders a row's tokens by their fp32 logit
+ * (ties to the lower token id), which is the order of S_b + logp_b(v) except where the fp64 rounding of l / temperature - lse or
+ * of S_b + logp makes two different logits score equal: there the larger logit is kept, where the rule above would keep the
+ * lower token id.  cand_tok int32 [R * K] and cand_logp fp64 [R * K] are scratch.
+ * record (may be NULL): this step's logits per physical row, before the permutation, at record[(s * R + r) * V ..].
+ * trace (may be NULL): fp64 [steps][R][3], the new beam's (parent beam index, token or -1 for a finished beam, score).
+ * Deterministic.  Returns VDB_ERR_INVALID before any launch unless R = n * K <= 16, 1 <= K <= 16, K <= V <= 53248, ldl >= V,
+ * temperature > 0, max_len >= 2, ldt >= max_len, lds >= 1, the pointers are non-null, the fp32 / int32 buffers 4-byte aligned and
+ * the fp64 buffers 8-byte aligned.
+ * A step with s >= lds or s + 1 >= ldt does nothing. */
+int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, float temperature, int K, int* tokens, int ldt, int* src,
+                          int lds, double* scores, int* done, int* lengths, const int* step, int eos, int max_len, int* cand_tok,
+                          double* cand_logp, float* record, double* trace, void* stream);
 
 /* ---- semantic/style disentanglement of the image context — decompose / adjust_rank of the reference app.py:48-127 -----------
  * For each item b < n_items of x [n_items, m, n] (fp32, contiguous):  X = x - rowmean(x);  the randomized PCA of torch.pca_lowrank

@@ -4,7 +4,9 @@ captured step graph), launches per step, and the bytes a step must read over its
 then one complete i2t call: 50 DDIM steps on the text latent, then the decode.  Prints the card name and power limit.
 With --top-k / --top-p: ms per token step at 4 and 16 rows with the sampler's cuts off and on, the two graphs replayed
 alternately in one session, and the launches per step of each.
-    python tools/text_decode_bench.py [--no-i2t] [--top-k K] [--top-p P]"""
+With --num-beams K: 4 latents sampled (4 rows) against the same 4 latents under beam search (4 K rows, groups of 16 // K latents),
+the two step graphs replayed alternately: ms per token step, launches per step and the time of a whole decode call of each.
+    python tools/text_decode_bench.py [--no-i2t] [--top-k K] [--top-p P] [--num-beams K]"""
 import argparse
 import json
 import os
@@ -27,6 +29,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--no-i2t", action="store_true")
 ap.add_argument("--top-k", type=int, default=0)
 ap.add_argument("--top-p", type=float, default=0.0)
+ap.add_argument("--num-beams", type=int, default=0)
 args = ap.parse_args()
 HBM = 3.35e12
 dev = torch.device("cuda", 0)
@@ -59,7 +62,7 @@ with torch.no_grad():
         vae.decode_ids(z, eos_token=-1)                      # warm-up: packs weights, captures the step-chunk graph
     p = vae.packed()
     st = vae._state(R, dev)
-    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0)]
+    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0, 0)]
     n0 = ops.launch_count()
     vae._step(st, p, 1.0, -1, 30, "seed", False)
     launches = ops.launch_count() - n0
@@ -70,6 +73,7 @@ with torch.no_grad():
     e0.record()
     for i in range(reps):
         st.step.zero_()                                       # keep the step index inside the 28-step window
+        st.done.zero_()                                       # the warm-up decodes left every row finished
         graph.replay()
     e1.record()
     torch.cuda.synchronize()
@@ -109,10 +113,11 @@ def step_ms_off_and_on(R, top_k, top_p, rounds=5, reps=10):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
             for name, (k, p) in cuts.items():
-                g = st.graphs[(1.0, -1, 30, "seed", False, k, p)]
+                g = st.graphs[(1.0, -1, 30, "seed", False, k, p, 0)]
                 e0.record()
                 for _ in range(reps):
                     st.step.zero_()
+                    st.done.zero_()
                     g.replay()
                 e1.record()
                 torch.cuda.synchronize()
@@ -129,6 +134,58 @@ def step_ms_off_and_on(R, top_k, top_p, rounds=5, reps=10):
 if args.top_k or 0.0 < args.top_p < 1.0:
     for rows_ in (4, 16):
         print(json.dumps(step_ms_off_and_on(rows_, args.top_k, args.top_p)))
+
+def sampling_and_beams(K, n=4, rounds=5, reps=10):
+    """ms per token step of sampling n latents (n rows) and of beam search over them (n K rows per group), the captured chunks
+    replayed alternately; launches per step; one whole decode call of each (EOS never drawn: every step runs).  Before each timed chunk
+    every row is re-armed (done = 0): a decode leaves all rows finished, and a finished row skips the sampler / beam-step work."""
+    zr = torch.randn(n, 768, generator=torch.Generator().manual_seed(6)).to(dev) * 3.0
+    per = 16 // K
+    cases = {"sample": (n, "seed", 0, lambda: vae.decode_ids(zr, eos_token=-1)),
+             "beam": (min(n, per) * K, "beam", K, lambda: vae.decode_beams(zr, K, eos_token=-1))}
+    out = {}
+    with torch.no_grad():
+        for name, (rows, mode, k, call) in cases.items():
+            for _ in range(2):
+                call()
+            st = vae._state(rows, dev)
+            n0 = ops.launch_count()
+            vae._step(st, vae.packed(), 1.0, -1, 30, mode, False, 0, 0.0, k)
+            out[name] = dict(rows=rows, graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, k)], st=st,
+                             launches_per_step=ops.launch_count() - n0, ms=[], ms_decode=[])
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for _ in range(rounds):
+            for name, (rows, mode, k, call) in cases.items():
+                o = out[name]
+                torch.cuda.synchronize()
+                e0.record()
+                for _ in range(reps):
+                    o["st"].step.zero_()
+                    o["st"].done.zero_()          # a finished row would skip the sampler / beam work
+                    o["graph"].replay()
+                e1.record()
+                torch.cuda.synchronize()
+                o["ms"].append(e0.elapsed_time(e1) / (reps * STEPS_PER_CHECK))
+                assert not bool(o["st"].done.any()), "a timed step ran on finished rows"
+                e0.record()
+                call()
+                e1.record()
+                torch.cuda.synchronize()
+                o["ms_decode"].append(e0.elapsed_time(e1))
+    res = dict(card=card, latents=n, num_beams=K, groups=-(-n // per))
+    for name in cases:
+        o = out[name]
+        res[f"{name}_rows_per_step"] = o["rows"]
+        res[f"{name}_ms_per_step"] = round(min(o["ms"]), 4)
+        res[f"{name}_ms_per_step_all"] = [round(v, 4) for v in o["ms"]]
+        res[f"{name}_launches_per_step"] = o["launches_per_step"]
+        res[f"{name}_ms_per_decode"] = round(min(o["ms_decode"]), 3)
+        res[f"{name}_ms_per_decode_all"] = [round(v, 3) for v in o["ms_decode"]]
+    return res
+
+
+if args.num_beams:
+    print(json.dumps(sampling_and_beams(args.num_beams)))
 
 if not args.no_i2t:
     bs = 4

@@ -167,10 +167,14 @@ textdec_gemv_kernel(const float* __restrict__ x, int R, int K, long long ldx, co
 // Position 0 is the layer's latent slice (key == value, raw: GPT2Model_XX.forward, optimus_gpt2.py:882-895); positions
 // 1 .. s+1 are tokens 0 .. s, s = *step.  This step's k / v (from c_attn) are appended at cache slot s and used from registers.
 // fp32 online softmax, scale 1/sqrt(64); the causal mask admits every cached position.
+// kIndexed (beam search): cache slot j < s of row r is read from physical row src[r * T + j]; this step's k / v still go to row
+// r, slot s.  src is the last parameter, so the kIndexed = false instantiation keeps the parameter layout it had without it.
 // ---------------------------------------------------------------------------------------------------------------------------
+template <bool kIndexed>
 __global__ void textdec_attention_kernel(const float* __restrict__ qkv, long long ldq, const float* __restrict__ mem,
                                          long long ldm, float* __restrict__ kc, float* __restrict__ vc, int R, int H, int T,
-                                         const int* __restrict__ step, float scale, float* __restrict__ out, long long ldo) {
+                                         const int* __restrict__ step, float scale, float* __restrict__ out, long long ldo,
+                                         const int* __restrict__ src) {
   const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (w >= R * H) return;
   const int s = *step;
@@ -193,7 +197,11 @@ __global__ void textdec_attention_kernel(const float* __restrict__ qkv, long lon
     float2 kj, vj;
     if (j == 0) { kj = lat; vj = lat; }
     else if (j == s + 1) { kj = kn; vj = vn; }
-    else {
+    else if constexpr (kIndexed) {
+      const int pr = src[static_cast<size_t>(r) * T + j - 1];
+      const size_t o = (static_cast<size_t>(pr * H + h) * T + j - 1) * kHeadDim + d;
+      kj = make_float2(kc[o], kc[o + 1]); vj = make_float2(vc[o], vc[o + 1]);
+    } else {
       const size_t o = static_cast<size_t>(j - 1) * kHeadDim;
       kj = make_float2(kb[o], kb[o + 1]); vj = make_float2(vb[o], vb[o + 1]);
     }
@@ -491,6 +499,184 @@ textdec_sample_kernel(const float* __restrict__ logits, int R, int V, long long 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Beam search step (vdb_textdec_beam_step), two launches.  Row r = latent * K + beam.
+// (a) textdec_beam_topk_kernel, one CTA per row: the fp64 log-softmax logp(v) = l_v - lse, l_v = logit_v / temperature,
+//     lse = max + log(sum exp(l - max)) (per-thread slice sums, then a fixed tree), and the row's K best tokens: the filter's
+//     radix select with top_k = K over the raw logits' keys (dividing by temperature > 0 keeps their order), every key > bound
+//     plus the first K - #(> bound) keys == bound in vocabulary order.  Writes the K (token, logp) candidates in vocabulary
+//     order.  A finished row only records its logits.
+// (b) textdec_beam_select_kernel, one CTA per latent: candidates are (parent b, token v, S_b + logp_b(v)) for each live beam's
+//     K tokens and (b, -1, S_b) for each finished beam; rank = the number of candidates that beat it (higher score, then lower
+//     parent, then lower token): at most K x K of them, so the O(n^2) count is cheap and exact.  Candidate of rank j becomes
+//     beam j: its token and src rows are staged through shared memory from the parent's.
+// No floating-point atomics: replays are bitwise repeatable.
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int kBeamMax = 16;
+constexpr int kSelectThreads = 256;
+constexpr int kStageCols = 64;                    // token / src columns staged per pass of the permutation
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+textdec_beam_topk_kernel(const float* __restrict__ logits, int R, int V, long long ldl, float temperature, int K,
+                         const int* __restrict__ done, const int* __restrict__ step, int* __restrict__ cand_tok,
+                         double* __restrict__ cand_logp, float* __restrict__ record) {
+  extern __shared__ __align__(16) unsigned char s_filter[];   // histograms, then the V staged keys
+  __shared__ FilterShared sh;
+  __shared__ float s_max[32];
+  __shared__ int s_n, s_tok[kBeamMax];
+  const int r = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, nw = blockDim.x >> 5;
+  const int s = *step;
+  const float* lr = logits + static_cast<size_t>(r) * ldl;
+  if (record) {
+    float* dst = record + (static_cast<size_t>(s) * R + r) * V;
+    for (int i = tid; i < V; i += blockDim.x) dst[i] = lr[i];
+  }
+  if (done[r]) return;
+  unsigned long long* hist = reinterpret_cast<unsigned long long*>(s_filter);
+  uint32_t* keys = reinterpret_cast<uint32_t*>(s_filter + kFilterHistBytes);
+  float mx = -INFINITY;
+  for (int i = tid; i < V; i += blockDim.x) {
+    const float l = lr[i];
+    keys[i] = order_key(l == 0.0f ? 0.0f : l);    // -0 and +0 are one value: one key
+    mx = fmaxf(mx, l);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if (lane == 0) s_max[warp] = mx;
+  if (tid == 0) s_n = 0;
+  __syncthreads();
+  mx = s_max[0];
+  for (int i = 1; i < nw; ++i) mx = fmaxf(mx, s_max[i]);
+
+  const double t = static_cast<double>(temperature), m = static_cast<double>(mx) / t;
+  const int per = (V + blockDim.x - 1) / blockDim.x;
+  const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
+  double z = 0.0;
+  for (int i = i0; i < i1; ++i) z += exp(static_cast<double>(key_value(keys[i])) / t - m);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+  if (lane == 0) sh.red[warp] = z;
+  __syncthreads();
+  z = sh.red[0];
+  for (int i = 1; i < nw; ++i) z += sh.red[i];
+  const double lse = m + log(z);
+
+  // the K-th largest key; K <= V, so it always exists
+  const Selected b = radix_select<false>(keys, V, 0u, static_cast<unsigned long long>(K - 1), 0.0f, 0.0, hist, sh);
+  const uint32_t bound = b.key;
+  const int cap = K - static_cast<int>(b.above);
+  int nt = 0;                                       // rank0: the ties at the bound in the slices before this thread's
+  for (int i = i0; i < i1; ++i) nt += keys[i] == bound;
+  int inc = nt;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int n = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += n;
+  }
+  if (lane == 31) sh.ties[warp] = inc;
+  __syncthreads();
+  int rank = inc - nt;
+  for (int w = 0; w < warp; ++w) rank += sh.ties[w];
+  for (int i = i0; i < i1; ++i) {
+    const uint32_t k = keys[i];
+    if (k > bound || (k == bound && rank++ < cap)) s_tok[atomicAdd(&s_n, 1)] = i;
+  }
+  __syncthreads();
+  if (tid == 0) {                                   // exactly K picks; put them in vocabulary order
+    for (int i = 1; i < K; ++i)
+      for (int j = i; j > 0 && s_tok[j - 1] > s_tok[j]; --j) { const int x = s_tok[j]; s_tok[j] = s_tok[j - 1]; s_tok[j - 1] = x; }
+  }
+  __syncthreads();
+  if (tid < K) {
+    const int v = s_tok[tid];
+    cand_tok[r * K + tid] = v;
+    cand_logp[r * K + tid] = static_cast<double>(lr[v]) / t - lse;
+  }
+}
+
+__global__ void __launch_bounds__(kSelectThreads)
+textdec_beam_select_kernel(int R, int K, const int* __restrict__ cand_tok, const double* __restrict__ cand_logp,
+                           int* __restrict__ tokens, int ldt, int* __restrict__ src, int lds, double* __restrict__ scores,
+                           int* __restrict__ done, int* __restrict__ lengths, const int* __restrict__ step, int eos, int max_len,
+                           double* __restrict__ trace) {
+  __shared__ double c_score[kBeamMax * kBeamMax];
+  __shared__ int c_tok[kBeamMax * kBeamMax];       // -1: a finished beam carried over as itself; -2: no candidate
+  __shared__ double b_score[kBeamMax];
+  __shared__ int b_done[kBeamMax], b_len[kBeamMax], sel[kBeamMax];
+  __shared__ int stage[kBeamMax * kStageCols];
+  const int tid = threadIdx.x, row0 = blockIdx.x * K, nc = K * K;
+  const int s = *step;
+  if (s < 0 || s >= lds || s + 1 >= ldt) return;
+  if (tid < K) {
+    b_done[tid] = done[row0 + tid]; b_len[tid] = lengths[row0 + tid]; b_score[tid] = scores[row0 + tid];
+  }
+  __syncthreads();
+  for (int i = tid; i < nc; i += blockDim.x) {
+    const int p = i / K, j = i % K;
+    if (b_done[p]) {
+      c_tok[i] = j == 0 ? -1 : -2;
+      c_score[i] = b_score[p];
+    } else {
+      c_tok[i] = cand_tok[(row0 + p) * K + j];
+      c_score[i] = b_score[p] + cand_logp[(row0 + p) * K + j];
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < nc; i += blockDim.x) {
+    const int t = c_tok[i], p = i / K;
+    if (t == -2) continue;
+    const double sc = c_score[i];
+    int rank = 0;
+    for (int c = 0; c < nc; ++c) {
+      const int tc = c_tok[c], pc = c / K;
+      if (tc == -2) continue;
+      rank += c_score[c] > sc || (c_score[c] == sc && (pc < p || (pc == p && tc < t)));
+    }
+    if (rank < K) sel[rank] = i;
+  }
+  __syncthreads();
+  // beam j <- its parent's tokens 0 .. s+1 and src slots 0 .. s-1; src slot s <- the parent's row (its k / v of this step)
+  for (int pass = 0; pass < 2; ++pass) {
+    int* base = pass ? src : tokens;
+    const int ld = pass ? lds : ldt, ncol = pass ? s : s + 2;
+    for (int c0 = 0; c0 < ncol; c0 += kStageCols) {
+      const int w = min(kStageCols, ncol - c0);
+      for (int i = tid; i < K * w; i += blockDim.x) {
+        const int j = i / w, c = c0 + i % w;
+        stage[i] = base[static_cast<size_t>(row0 + sel[j] / K) * ld + c];
+      }
+      __syncthreads();
+      for (int i = tid; i < K * w; i += blockDim.x) {
+        const int j = i / w, c = c0 + i % w;
+        base[static_cast<size_t>(row0 + j) * ld + c] = stage[i];
+      }
+      __syncthreads();
+    }
+  }
+  if (tid < K) {
+    const int i = sel[tid], p = i / K, t = c_tok[i], row = row0 + tid;
+    int* tr = tokens + static_cast<size_t>(row) * ldt;
+    src[static_cast<size_t>(row) * lds + s] = row0 + p;
+    int d = 1, len = b_len[p];
+    if (t >= 0) {                                   // a live parent's child
+      tr[s + 1] = t;
+      if (t == eos) {
+        len = s + 2;
+      } else if (s + 1 >= max_len - 2) {           // the forced, unscored <eos>
+        if (s + 2 < ldt) tr[s + 2] = eos;
+        len = s + 3;
+      } else {
+        d = 0;
+      }
+    }
+    scores[row] = c_score[i]; done[row] = d; lengths[row] = len;
+    if (trace) {
+      double* tp = trace + (static_cast<size_t>(s) * R + row) * 3;
+      tp[0] = p; tp[1] = t; tp[2] = c_score[i];
+    }
+  }
+}
+
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
@@ -545,8 +731,29 @@ int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, lon
        reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache)) & 3)
     return set_error(VDB_ERR_INVALID, "textdec_attention: fp32 buffers must be 4-byte aligned");
   const int warps = R * H;
-  textdec_attention_kernel<<<(warps + 3) / 4, 128, 0, as_stream(stream)>>>(qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step, scale,
-                                                                         out, ldo);
+  textdec_attention_kernel<false><<<(warps + 3) / 4, 128, 0, as_stream(stream)>>>(qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step,
+                                                                                scale, out, ldo, nullptr);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
+                                  const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo,
+                                  void* stream) {
+  if (!qkv || !mem || !kcache || !vcache || !src || !step || !out)
+    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: null pointer");
+  if (R < 1 || R > kGvMaxRows || H < 1 || H > 64 || T < 1 || T > 1024)
+    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: need 1 <= R <= 16, 1 <= H <= 64, 1 <= T <= 1024");
+  const long long D = static_cast<long long>(H) * kHeadDim;
+  if (ldq < 3 * D || ldm < D || ldo < D)
+    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: leading dimensions smaller than the rows");
+  if ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(mem) | reinterpret_cast<uintptr_t>(out) |
+       reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache) | reinterpret_cast<uintptr_t>(src)) & 3)
+    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: buffers must be 4-byte aligned");
+  const int warps = R * H;
+  textdec_attention_kernel<true><<<(warps + 3) / 4, 128, 0, as_stream(stream)>>>(qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step,
+                                                                               scale, out, ldo, src);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;
@@ -617,6 +824,43 @@ int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl
     return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top_p must be in [0, 1], got %g", static_cast<double>(top_p));
   return textdec_sample_launch(logits, R, V, ldl, temperature, top_k, top_p, seed, uniforms, ldu, forced, ldf, tokens, ldt, done,
                                lengths, step, eos, max_len, record, stream);
+}
+
+int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, float temperature, int K, int* tokens, int ldt, int* src,
+                          int lds, double* scores, int* done, int* lengths, const int* step, int eos, int max_len, int* cand_tok,
+                          double* cand_logp, float* record, double* trace, void* stream) {
+  if (!logits || !tokens || !src || !scores || !done || !lengths || !step || !cand_tok || !cand_logp)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: null pointer");
+  if (K < 1 || K > kBeamMax) return set_error(VDB_ERR_INVALID, "textdec_beam_step: need 1 <= K <= %d beams, got %d", kBeamMax, K);
+  if (R < 1 || R > kGvMaxRows || R % K)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: need R = n * K <= %d rows, got R = %d, K = %d", kGvMaxRows, R, K);
+  if (V < K || V > kFilterMaxV || ldl < V)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: need K <= V <= %d (staged keys) and ldl >= V, got V = %d", kFilterMaxV, V);
+  if (!(temperature > 0.0f)) return set_error(VDB_ERR_INVALID, "textdec_beam_step: temperature must be > 0");
+  if (max_len < 2 || ldt < max_len || lds < 1)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: need max_len >= 2, ldt >= max_len and lds >= 1");
+  if ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(tokens) | reinterpret_cast<uintptr_t>(src) |
+       reinterpret_cast<uintptr_t>(done) | reinterpret_cast<uintptr_t>(lengths) | reinterpret_cast<uintptr_t>(step) |
+       reinterpret_cast<uintptr_t>(cand_tok) | reinterpret_cast<uintptr_t>(record)) & 3)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: fp32 / int32 buffers must be 4-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(scores) | reinterpret_cast<uintptr_t>(cand_logp) | reinterpret_cast<uintptr_t>(trace)) & 7)
+    return set_error(VDB_ERR_INVALID, "textdec_beam_step: scores / cand_logp / trace must be 8-byte aligned");
+  const size_t smem = kFilterHistBytes + static_cast<size_t>(V) * sizeof(uint32_t);
+  static bool configured = false;
+  if (!configured) {
+    VDB_CUDA_CHECK(cudaFuncSetAttribute(textdec_beam_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        static_cast<int>(kFilterHistBytes + kFilterMaxV * sizeof(uint32_t))));
+    configured = true;
+  }
+  textdec_beam_topk_kernel<<<R, kSampleThreads, smem, as_stream(stream)>>>(logits, R, V, ldl, temperature, K, done, step, cand_tok,
+                                                                           cand_logp, record);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  textdec_beam_select_kernel<<<R / K, kSelectThreads, 0, as_stream(stream)>>>(R, K, cand_tok, cand_logp, tokens, ldt, src, lds, scores,
+                                                                              done, lengths, step, eos, max_len, trace);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
 }
 
 }  // extern "C"

@@ -38,6 +38,26 @@ Differences from the reference, all deliberate:
     unstable sort leaves their order open); see vdb_textdec_sample_filtered;
   - the reference's 29th forward pass, whose draw is always overwritten with <EOS>, is skipped;
   - weights are bf16 (packed at load); the residual stream, attention, logits and the sampler's sums are fp32 / fp64.
+
+Beam search: decode(z, num_beams=K) (and decode_ids, decode_beams) stands in for the reference's optimus_vae.decode(z, 'beam', K)
+(optimus.py:196-213), whose beam_search_decode does not exist in its GPT-2, so the definition here is the specification
+(vdb_textdec_beam_step; oracle/text_beam_oracle.py implements the same):
+  - each latent gets K beams, rows latent * K + beam of one batch; each starts as <BOS> with the latent's memory and embedding
+    offset; at step 0 only beam 0 is live (the others start at score -inf), so the first step does not make K copies of one
+    hypothesis;
+  - a hypothesis' score is the sum over its chosen tokens of log softmax(logits / temperature), computed in fp64 from the fp32
+    logits (the division, max, exp, sum and log);
+  - candidates at step s: every live beam b crossed with every token v, scored S_b + logp_b(v), and every finished beam as itself
+    with its score unchanged; the K best become the new beams, ties to the lower parent beam, then the lower token id;
+  - a candidate whose token is <EOS> is finished; a live beam whose token s+1 lands on max_len - 2 without <EOS> gets <EOS>
+    appended unscored (the sampler's rule above) and is finished; a latent is done when all K beams are (live scores only fall);
+  - final ranking by S / n ** length_penalty, n the scored tokens (a chosen <EOS> counts, a forced one does not; length_penalty 0
+    ranks by the raw sum), ties to the lower beam index.  K = 1 picks the argmax, the lowest token id among equal maxima: the
+    tokens of greedy decoding (top_k=1), which differs only at an exact tie for the maximum, where it draws among the tied tokens.
+The KV cache is not moved when beams are reordered: each physical (row, slot) is written once, and the indexed attention reads
+slot j of beam r from row src[r, j], a table the beam step permutes with the token rows.  A step streams the weights once for all
+n * K rows (the GEMV is one 16-row tile), so n * K <= 16 rows run together; more latents are split into groups of 16 // K,
+decoded one after the other, each group re-streaming the weights.
 """
 import json
 import math
@@ -78,6 +98,20 @@ def _check_cuts(top_k, top_p):
     if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real) or not math.isfinite(top_p) or not 0.0 <= top_p <= 1.0:
         raise ValueError(f"optimus_vae_next: top_p must be a finite float in [0, 1] (0 or 1: no nucleus cut), got {top_p!r}")
     return int(top_k), float(top_p)
+
+
+MAX_BEAMS = 16                                    # the rows of one token step (vdb_textdec_beam_step's K limit)
+
+
+def _check_beams(num_beams, length_penalty, top_k, top_p):
+    """-> (int num_beams, float length_penalty), or ValueError; beam search takes no top-k / nucleus cut."""
+    if isinstance(num_beams, bool) or not isinstance(num_beams, numbers.Integral) or not 0 <= num_beams <= MAX_BEAMS:
+        raise ValueError(f"optimus_vae_next: num_beams must be an int in [0, {MAX_BEAMS}] (0: sampling), got {num_beams!r}")
+    if isinstance(length_penalty, bool) or not isinstance(length_penalty, numbers.Real) or not math.isfinite(length_penalty):
+        raise ValueError(f"optimus_vae_next: length_penalty must be a finite float, got {length_penalty!r}")
+    if num_beams and (top_k != 0 or top_p != 0.0):
+        raise ValueError("optimus_vae_next: beam search (num_beams >= 1) takes no top_k / top_p cut")
+    return int(num_beams), float(length_penalty)
 
 
 class VocabularyMissingError(RuntimeError):
@@ -428,6 +462,11 @@ class _State(object):
         self.done, self.lengths = z(R, dt=torch.int32), z(R, dt=torch.int32)
         self.step, self.seed = z(1, dt=torch.int32), z(1, dt=torch.int64)
         self.record = z(CACHE_SLOTS, R, V)
+        # beam search: slot-to-row table of the KV cache, fp64 scores, the per-row candidates, the per-step (parent, token, score)
+        self.src = z(R, CACHE_SLOTS, dt=torch.int32)
+        self.scores = z(R, dt=torch.float64)
+        self.cand_tok, self.cand_logp = z(R * MAX_BEAMS, dt=torch.int32), z(R * MAX_BEAMS, dt=torch.float64)
+        self.trace = z(CACHE_SLOTS, R, 3, dt=torch.float64)
         self.graphs = {}
 
 
@@ -592,34 +631,46 @@ class optimus_vae_next(PackedModule):
         self.__dict__['_states'] = {}        # captured graphs hold the old weight addresses
 
     # ------------------------------------------------------------------ one token step (5 launches per layer + 4)
-    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0):
+    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0, num_beams=0):
         ops = _ops()
         dec = self.decoder
         D = dec.n_embd
         ops.textdec_embed(st.tokens, st.step, p["wte32"], p["wpe32"], st.emb, st.h, pos_offset=1)
         for i, L in enumerate(p["layers"]):
             ops.textdec_gemv(st.h, L["w_attn"], st.qkv, bias=L["b_attn"], ln=L["ln1"])
-            ops.textdec_attention(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.step, st.a, scale=0.125)
+            if num_beams:
+                ops.textdec_attention_indexed(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.src, st.step, st.a,
+                                              scale=0.125)
+            else:
+                ops.textdec_attention(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.step, st.a, scale=0.125)
             ops.textdec_gemv(st.a, L["w_aproj"], st.h, bias=L["b_aproj"], accumulate=True)
             ops.textdec_gemv(st.h, L["w_fc"], st.m, bias=L["b_fc"], ln=L["ln2"], act=ops.ACT_GELU_TANH)
             ops.textdec_gemv(st.m, L["w_mproj"], st.h, bias=L["b_mproj"], accumulate=True)
         ops.textdec_gemv(st.h, p["lm_head"], st.logits, ln=p["lnf"])
-        ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=temperature,
-                           seed=st.seed if mode == "seed" else None, uniforms=st.uniforms if mode == "uniforms" else None,
-                           forced=st.forced if mode == "forced" else None, eos=eos, max_len=max_len,
-                           record=st.record if record else None, top_k=top_k, top_p=top_p)
+        if num_beams:
+            ops.textdec_beam_step(st.logits, num_beams, st.tokens, st.src, st.scores, st.done, st.lengths, st.step, st.cand_tok,
+                                  st.cand_logp, temperature=temperature, eos=eos, max_len=max_len,
+                                  record=st.record if record else None, trace=st.trace if record else None)
+        else:
+            ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=temperature,
+                               seed=st.seed if mode == "seed" else None, uniforms=st.uniforms if mode == "uniforms" else None,
+                               forced=st.forced if mode == "forced" else None, eos=eos, max_len=max_len,
+                               record=st.record if record else None, top_k=top_k, top_p=top_p)
         ops.add_int(st.step, 1)
 
     @torch.no_grad()
     def _run(self, z, temperature, eos, pre_scale=1.0, max_len=MAX_LENGTH, nsteps=None, mode="seed", uniforms=None, forced=None,
-             record=False, graph=True, top_k=0, top_p=0.0):
+             record=False, graph=True, top_k=0, top_p=0.0, num_beams=0):
+        """mode "beam" (num_beams >= 1) decodes the n latents of z as rows latent * num_beams + beam, n * num_beams <= 16."""
         top_k, top_p = _check_cuts(top_k, top_p)
         require_cuda(z, "optimus_vae_next.decode")
         if z.dim() != 2 or z.shape[1] != self.nz:
             raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
-        R = z.shape[0]
+        K = int(num_beams) if mode == "beam" else 0
+        R = z.shape[0] * max(K, 1)
         if not 1 <= R <= 16:
-            raise ValueError(f"optimus_vae_next: decodes 1 to 16 latents per call, got {R}")
+            raise ValueError(f"optimus_vae_next: decodes 1 to 16 latents per call, got {R}" if not K else
+                             f"optimus_vae_next: beam search runs n * num_beams <= 16 rows per call, got {z.shape[0]} x {K}")
         ops = _ops()
         p = self.packed()
         st = self._state(R, z.device)
@@ -627,7 +678,8 @@ class optimus_vae_next(PackedModule):
         if nsteps > CACHE_SLOTS:
             raise ValueError(f"optimus_vae_next: at most {CACHE_SLOTS} steps")
         # per-call state: latent projections (the memory slices and the embedding offset), tokens, flags, seed
-        zs = (z.float() * float(pre_scale)).contiguous()
+        zs = z.float() * float(pre_scale)
+        zs = (zs.repeat_interleave(K, 0) if K else zs).contiguous()
         ops.textdec_gemv(zs, p["w_emb"], st.emb)
         ops.textdec_gemv(zs, p["w_lin"], st.mem)
         init = torch.full((R, CACHE_SLOTS + 1), eos, dtype=torch.int32)
@@ -643,10 +695,15 @@ class optimus_vae_next(PackedModule):
         elif mode == "uniforms":
             st.uniforms.zero_()
             st.uniforms[:, :uniforms.shape[1]].copy_(uniforms)
+        elif mode == "beam":
+            scores = torch.full((R,), -math.inf, dtype=torch.float64)
+            scores[::K] = 0.0                     # only beam 0 of each latent is live at step 0
+            st.scores.copy_(scores)
+            st.src.copy_(torch.arange(R, dtype=torch.int32)[:, None].expand(R, CACHE_SLOTS))
         else:
             st.forced.zero_()
             st.forced[:, :forced.shape[1]].copy_(forced)
-        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p)
+        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p, K)
         s = 0
         while s < nsteps:
             n = min(STEPS_PER_CHECK, nsteps - s)
@@ -655,7 +712,7 @@ class optimus_vae_next(PackedModule):
                 g.replay()
             else:
                 for _ in range(n):
-                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p)
+                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K)
                 if graph and n == STEPS_PER_CHECK and key not in st.graphs:
                     # the chunk just ran eagerly (kernels configured, caches warm); capture one for the later chunks
                     torch.cuda.current_stream().synchronize()
@@ -663,7 +720,7 @@ class optimus_vae_next(PackedModule):
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
                         for _ in range(n):
-                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p)
+                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K)
                     st.step.copy_(step_before)        # capture does not execute, but keep the counter exactly as the eager chunk left it
                     st.graphs[key] = g
             s += n
@@ -671,13 +728,54 @@ class optimus_vae_next(PackedModule):
                 break
         return st, s
 
+    def _beam_group(self, z, num_beams, temperature, pre_scale, eos, length_penalty, record=False, graph=True):
+        """Beam search of n latents with n * num_beams <= 16 -> (per latent, its num_beams (ids, score, normalized score) best
+        first; the state; the steps run)."""
+        st, ran = self._run(z, temperature, eos, pre_scale=pre_scale, mode="beam", record=record, graph=graph, num_beams=num_beams)
+        tokens, lengths, scores = st.tokens.cpu(), st.lengths.cpu().tolist(), st.scores.cpu().tolist()
+        out = []
+        for i in range(z.shape[0]):
+            beams = []
+            for j in range(num_beams):
+                r = i * num_beams + j
+                n = min(lengths[r] - 1, MAX_LENGTH - 2)   # scored tokens: a forced final <EOS> has none
+                beams.append((tokens[r, :lengths[r]].long(), scores[r], scores[r] / n ** length_penalty))
+            out.append([beams[j] for j in sorted(range(num_beams), key=lambda j: (-beams[j][2], j))])
+        return out, st, ran
+
+    @torch.no_grad()
+    def decode_beams(self, z, num_beams, temperature=1.0, pre_scale=1.0, length_penalty=1.0, eos_token=EOS_ID, graph=True):
+        """Beam search (see the module docstring): for each latent, its num_beams final hypotheses as (ids int64 CPU tensor from
+        <BOS> to <EOS>, score = summed fp64 log-probability, score / n ** length_penalty), best normalized score first.
+        num_beams latents' worth of rows run per token step, at most 16: more latents are decoded in groups of 16 // num_beams,
+        one after the other, each re-streaming the weights."""
+        num_beams, length_penalty = _check_beams(num_beams, length_penalty, 0, 0.0)
+        if num_beams < 1:
+            raise ValueError(f"optimus_vae_next.decode_beams: num_beams must be >= 1, got {num_beams}")
+        require_cuda(z, "optimus_vae_next.decode")
+        if z.dim() != 2 or z.shape[0] < 1:
+            raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
+        per = MAX_BEAMS // num_beams
+        out = []
+        for i0 in range(0, z.shape[0], per):
+            out += self._beam_group(z[i0:i0 + per], num_beams, temperature, pre_scale, int(eos_token), length_penalty,
+                                    graph=graph)[0]
+        return out
+
     @torch.no_grad()
     def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True,
-                   top_k=0, top_p=0.0):
+                   top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0):
         """Sampled token rows, each an int64 CPU tensor starting with <BOS> and (unless eos_token never occurs and is never forced)
         ending with eos_token, length <= 30.  uniforms (fp64 [n, >=28]) replaces the Philox draws; return_logits also returns the
         fp32 logits of every step that ran, [steps, n, 50260] on the device.  top_k > 0 keeps the top_k most likely tokens (ties
-        included), 0 < top_p < 1 the nucleus of mass top_p (optimus.py:690-719); the defaults sample the full softmax."""
+        included), 0 < top_p < 1 the nucleus of mass top_p (optimus.py:690-719); the defaults sample the full softmax.
+        num_beams >= 1: each latent's best beam-search hypothesis instead (decode_beams; no cuts, uniforms or logits)."""
+        num_beams, length_penalty = _check_beams(num_beams, length_penalty, top_k, top_p)
+        if num_beams:
+            if uniforms is not None or return_logits:
+                raise ValueError("optimus_vae_next: beam search takes no uniforms and returns no logits")
+            return [b[0][0] for b in self.decode_beams(z, num_beams, temperature=temperature, pre_scale=pre_scale,
+                                                       length_penalty=length_penalty, eos_token=eos_token, graph=graph)]
         st, ran = self._run(z, temperature, int(eos_token), pre_scale=pre_scale, mode="uniforms" if uniforms is not None else "seed",
                             uniforms=uniforms, record=return_logits, graph=graph, top_k=top_k, top_p=top_p)
         tokens, lengths = st.tokens.cpu(), st.lengths.cpu()
@@ -697,7 +795,9 @@ class optimus_vae_next(PackedModule):
         return st.record[:L].permute(1, 0, 2).contiguous()
 
     @torch.no_grad()
-    def decode(self, z, temperature=1.0, pre_scale=1.0, top_k=0, top_p=0.0):
-        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row; top_k / top_p as in decode_ids."""
-        rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale, top_k=top_k, top_p=top_p)
+    def decode(self, z, temperature=1.0, pre_scale=1.0, top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0):
+        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row; top_k / top_p / num_beams / length_penalty as
+        in decode_ids (num_beams >= 1: the best beam-search hypothesis)."""
+        rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale, top_k=top_k, top_p=top_p, num_beams=num_beams,
+                               length_penalty=length_penalty)
         return [self.tokenizer_decoder.sentence(r.tolist()) for r in rows]

@@ -738,6 +738,41 @@ def textdec_sample(logits, tokens, done, lengths, step, temperature=1.0, seed=No
                                               *args), "textdec_sample_filtered")
 
 
+def textdec_attention_indexed(qkv, mem, kcache, vcache, src, step, out, scale=0.125):
+    """textdec_attention with cache slot j of row r read from physical row src[r, j] (int32 [R, T]; see
+    vdb_textdec_attention_indexed)."""
+    for n, t in (("qkv", qkv), ("mem", mem), ("out", out)):
+        _need(t, torch.float32, n, rows_ok=True)
+    _need(kcache, torch.float32, "kcache"); _need(vcache, torch.float32, "vcache"); _need(step, torch.int32, "step")
+    _need(src, torch.int32, "src")
+    R, H, T, _ = kcache.shape
+    if tuple(src.shape) != (R, T):
+        raise ValueError(f"textdec_attention_indexed: src must be [{R}, {T}], got {list(src.shape)}")
+    check(lib.vdb_textdec_attention_indexed(_ptr(qkv), qkv.stride(0), _ptr(mem), mem.stride(0), _ptr(kcache), _ptr(vcache),
+                                            _ptr(src), R, H, T, _ptr(step), float(scale), _ptr(out), out.stride(0), _stream()),
+          "textdec_attention_indexed")
+    return out
+
+
+def textdec_beam_step(logits, num_beams, tokens, src, scores, done, lengths, step, cand_tok, cand_logp, temperature=1.0,
+                      eos=50259, max_len=30, record=None, trace=None):
+    """One beam-search step over rows r = latent * num_beams + beam (see vdb_textdec_beam_step): tokens int32 [R, L], src int32
+    [R, T], scores fp64 [R], done / lengths int32 [R]; cand_tok int32 / cand_logp fp64 with >= R * num_beams elements (scratch);
+    record fp32 [steps, R, V], trace fp64 [steps, R, 3] (parent beam, token or -1, score)."""
+    _need(logits, torch.float32, "logits", rows_ok=True)
+    for n, t in (("tokens", tokens), ("src", src), ("done", done), ("lengths", lengths), ("step", step), ("cand_tok", cand_tok)):
+        _need(t, torch.int32, n)
+    _need(scores, torch.float64, "scores"); _need(cand_logp, torch.float64, "cand_logp")
+    _need(record, torch.float32, "record"); _need(trace, torch.float64, "trace")
+    R, V = logits.shape
+    if cand_tok.numel() < R * num_beams or cand_logp.numel() < R * num_beams:
+        raise ValueError(f"textdec_beam_step: the candidate buffers need {R * num_beams} elements")
+    check(lib.vdb_textdec_beam_step(_ptr(logits), R, V, logits.stride(0), float(temperature), int(num_beams), _ptr(tokens),
+                                    tokens.stride(0), _ptr(src), src.stride(0), _ptr(scores), _ptr(done), _ptr(lengths), _ptr(step),
+                                    int(eos), int(max_len), _ptr(cand_tok), _ptr(cand_logp), _ptr(record), _ptr(trace), _stream()),
+          "textdec_beam_step")
+
+
 # ------------------------------------------------------------------------------------------------
 # Semantic/style disentanglement (app.py:48-127): the rank adjustment of the image context, one launch
 # ------------------------------------------------------------------------------------------------
