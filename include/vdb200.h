@@ -46,6 +46,19 @@ int vdb_num_sms(void);
 int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* noise,
                       const float* coef, const int* step_idx, float scale, float temperature, float* x_prev,
                       float* x_prev_dup, float* pred_x0, long long n, void* stream);
+/* ---- CFG mix + one multistep DPM-Solver++ update — DPMSolverSampler, lib/model_zoo/dpm_solver.py (an addition: the reference
+ * has no such sampler; the algorithm and the table are specified in that module's docstring) -------------------------------------
+ * coef: device fp32 rows of 8 {P, Q, A, B, C, D, 0, 0}; row *step_idx (device int, required) is used, so one captured CUDA graph
+ * serves every step, warm-up and lower-order final steps included.  hist: a ring of 3 x n fp32 (slot s at hist + s*n) holding
+ * the data predictions of the last steps.  In this op order, fp32 with explicit round-to-nearest (no FMA contraction):
+ *   e = e_u + scale*(e_c - e_u);  x0 = P*x + Q*e  (-> hist slot idx % 3, and pred_x0);
+ *   x_next = ((A*x + B*x0) + C*h1) + D*h2,  h1 = slot (idx+1) % 3, h2 = slot (idx+2) % 3.
+ * A C or D term whose coefficient is exactly 0 is skipped and its slot not read (the ring is uninitialised at the first steps).
+ * e_uncond may be NULL (scale==1 path: e = e_c); pred_x0 and x_next_dup may be NULL.  x_next may alias x; x_next_dup receives a
+ * second copy (the cond half of the next step's batch).  VDB_ERR_INVALID before any launch: a null e_cond / x / coef / step_idx /
+ * hist / x_next, n <= 0, a pointer not 16-byte aligned, or hist overlapping x, x_next, x_next_dup or pred_x0. */
+int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
+                       float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n, void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */

@@ -69,6 +69,84 @@ __global__ void ddim_cfg_step_kernel(const float* __restrict__ e_uncond, const f
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// CFG mix + one multistep DPM-Solver++ update (lib/model_zoo/dpm_solver.py), row *step_idx of the 8-float table
+// coef = {P, Q, A, B, C, D, 0, 0}, in this op order (explicit _rn: no FMA contraction, so an fp32 CPU restatement is bitwise):
+//   e   = e_u + s * (e_c - e_u)
+//   x0  = P*x + Q*e                                  -> hist slot idx % 3, pred_x0
+//   x'  = ((A*x + B*x0) [+ C*h1]) [+ D*h2]           h1 = hist slot (idx+1) % 3, h2 = slot (idx+2) % 3
+// A bracketed term is skipped (and its slot not read) when its coefficient is exactly 0: the ring holds no data yet at the
+// first steps.  The slot pointers are 16-byte aligned only when n % 4 == 0, so the ring is accessed by vectors only then.
+// ---------------------------------------------------------------------------------------------
+__global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const float* __restrict__ e_cond,
+                                      const float* x, const float* __restrict__ coef, const int* __restrict__ step_idx,
+                                      float scale, float* __restrict__ hist, float* x_next, float* __restrict__ x_next_dup,
+                                      float* __restrict__ pred_x0, long long n) {
+  const int idx = *step_idx;
+  const float* c = coef + 8 * idx;
+  const float P = c[0], Q = c[1], A = c[2], B = c[3], C = c[4], D = c[5];
+  float* h0 = hist + static_cast<long long>(idx % 3) * n;
+  const float* h1 = hist + static_cast<long long>((idx + 1) % 3) * n;
+  const float* h2 = hist + static_cast<long long>((idx + 2) % 3) * n;
+  const bool hvec = (n & 3) == 0;
+  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) * 4; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x * 4) {
+    const bool full = i + 3 < n;
+    float ec[4], eu[4], xv[4], a1[4] = {0.f, 0.f, 0.f, 0.f}, a2[4] = {0.f, 0.f, 0.f, 0.f}, xn[4], p0[4];
+    if (full) {
+      *reinterpret_cast<float4*>(ec) = __ldg(reinterpret_cast<const float4*>(e_cond + i));
+      if (e_uncond) *reinterpret_cast<float4*>(eu) = __ldg(reinterpret_cast<const float4*>(e_uncond + i));
+      *reinterpret_cast<float4*>(xv) = *reinterpret_cast<const float4*>(x + i);   // x may alias x_next: no __ldg
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          ec[q] = e_cond[i + q];
+          if (e_uncond) eu[q] = e_uncond[i + q];
+          xv[q] = x[i + q];
+        }
+    }
+    if (full && hvec) {
+      if (C != 0.f) *reinterpret_cast<float4*>(a1) = *reinterpret_cast<const float4*>(h1 + i);
+      if (D != 0.f) *reinterpret_cast<float4*>(a2) = *reinterpret_cast<const float4*>(h2 + i);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          if (C != 0.f) a1[q] = h1[i + q];
+          if (D != 0.f) a2[q] = h2[i + q];
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      float e = ec[q];
+      if (e_uncond) e = __fadd_rn(eu[q], __fmul_rn(scale, __fsub_rn(ec[q], eu[q])));
+      const float px0 = __fadd_rn(__fmul_rn(P, xv[q]), __fmul_rn(Q, e));
+      float v = __fadd_rn(__fmul_rn(A, xv[q]), __fmul_rn(B, px0));
+      if (C != 0.f) v = __fadd_rn(v, __fmul_rn(C, a1[q]));
+      if (D != 0.f) v = __fadd_rn(v, __fmul_rn(D, a2[q]));
+      xn[q] = v;
+      p0[q] = px0;
+    }
+    if (full) {
+      *reinterpret_cast<float4*>(x_next + i) = *reinterpret_cast<float4*>(xn);
+      if (x_next_dup) *reinterpret_cast<float4*>(x_next_dup + i) = *reinterpret_cast<float4*>(xn);
+      if (pred_x0) *reinterpret_cast<float4*>(pred_x0 + i) = *reinterpret_cast<float4*>(p0);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          x_next[i + q] = xn[q];
+          if (x_next_dup) x_next_dup[i + q] = xn[q];
+          if (pred_x0) pred_x0[i + q] = p0[q];
+        }
+    }
+    if (full && hvec) {
+      *reinterpret_cast<float4*>(h0 + i) = *reinterpret_cast<float4*>(p0);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) h0[i + q] = p0[q];
+    }
+  }
+}
+
 __global__ void add_int_kernel(int* p, int delta) { *p += delta; }
 
 // y = c0*x0 + c1*x1 + c2*x2 + c3*x3 (null pointers skipped) — the Adams-Bashforth eps combination of the PLMS
@@ -1552,6 +1630,30 @@ int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x
   VDB_PREFER_MAX_SMEM(ddim_cfg_step_kernel);
   ddim_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       e_uncond, e_cond, x, noise, coef, step_idx, scale, temperature, x_prev, x_prev_dup, pred_x0, n);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
+                       float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n, void* stream) {
+  if (!e_cond || !x || !coef || !step_idx || !hist || !x_next || n <= 0)
+    return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: null/empty argument");
+  if ((reinterpret_cast<uintptr_t>(e_cond) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_next) |
+       reinterpret_cast<uintptr_t>(e_uncond) | reinterpret_cast<uintptr_t>(hist) | reinterpret_cast<uintptr_t>(pred_x0) |
+       reinterpret_cast<uintptr_t>(x_next_dup)) & 15)
+    return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: pointers must be 16-byte aligned");
+  // the ring is written while x is read and x_next / x_next_dup / pred_x0 are written: it must not share a byte with them
+  const uintptr_t h_lo = reinterpret_cast<uintptr_t>(hist), h_hi = h_lo + 3 * static_cast<uintptr_t>(n) * sizeof(float);
+  for (const float* p : {x, static_cast<const float*>(x_next), static_cast<const float*>(x_next_dup),
+                         static_cast<const float*>(pred_x0)}) {
+    const uintptr_t lo = reinterpret_cast<uintptr_t>(p), hi = lo + static_cast<uintptr_t>(n) * sizeof(float);
+    if (p && lo < h_hi && h_lo < hi) return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: hist overlaps x, x_next, x_next_dup or pred_x0");
+  }
+  const int threads = 256;
+  VDB_PREFER_MAX_SMEM(dpmpp_cfg_step_kernel);
+  dpmpp_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;

@@ -150,11 +150,7 @@ class DDIMSampler(object):
             x = x.reshape(bs, shape[1], 1, 1)
 
         # device-side per-step tables, indexed by the DDIM index (total_steps-1 ... 0)
-        coef = torch.tensor(np.stack([np.asarray(self.ddim_alphas.cpu() if isinstance(self.ddim_alphas, torch.Tensor) else self.ddim_alphas, dtype=np.float32)[:total_steps],
-                                      np.asarray(self.ddim_alphas_prev, dtype=np.float32)[:total_steps],
-                                      sigmas.astype(np.float32)[:total_steps],
-                                      np.asarray(self.ddim_sqrt_one_minus_alphas.cpu() if isinstance(self.ddim_sqrt_one_minus_alphas, torch.Tensor) else self.ddim_sqrt_one_minus_alphas, dtype=np.float32)[:total_steps]], axis=1),
-                            dtype=torch.float32, device=device).contiguous()
+        coef = torch.tensor(self._coef_table(timesteps, sigmas), dtype=torch.float32, device=device).contiguous()
         ts_table = torch.tensor(np.asarray(timesteps, dtype=np.int64), device=device)
 
         st = self._state(bs, B, H, W, shape[1], device)
@@ -171,9 +167,7 @@ class DDIMSampler(object):
             if flat:
                 eps = eps.view(B, 1, 1, -1)
             e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
-            ops.ddim_cfg_step(e_u, e_c, st['x_in'][:bs], st['coef'], scale, x_prev=st['x_in'][:bs],
-                              x_prev_dup=st['x_in'][bs:] if cfg else None, pred_x0=st['pred_x0'], noise=noise,
-                              temperature=temperature, step_idx=st['idx'])
+            self._update(st, e_u, e_c, scale, bs, cfg, noise, temperature)
             ops.add_int(st['idx'], -1)
 
         intermediates = {'pred_xt': [], 'pred_x0': []}
@@ -196,7 +190,7 @@ class DDIMSampler(object):
         else:
             from .diffusion_utils import pack_epoch
             key = (pack_epoch(), bs, B, H, W, x_type, tuple(c_types), tuple(ratios), scale, float(temperature), time_from,
-                   tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs))
+                   tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs)) + self._graph_tag()
             ent = self._graphs.get(key)
             if ent is not None and ent[1] == model.context_kv_signature(c_types, ctxs):
                 # steady state: the context projections were just refreshed in place; every step is a graph replay
@@ -232,6 +226,27 @@ class DDIMSampler(object):
         x_info['x'] = pred_xt
         return pred_xt, intermediates
 
+    # ------------------------------------------------------------------ per-step update (overridden by DPMSolverSampler)
+    _coef_cols = 4      # width of a row of the device coefficient table
+
+    def _coef_table(self, timesteps, sigmas):
+        """fp32 [len(timesteps), 4] rows {a_t, a_prev, sigma_t, sqrt(1 - a_t)} of the walk, indexed by the DDIM index."""
+        total_steps = timesteps.shape[0]
+        return np.stack([np.asarray(self.ddim_alphas.cpu() if isinstance(self.ddim_alphas, torch.Tensor) else self.ddim_alphas, dtype=np.float32)[:total_steps],
+                         np.asarray(self.ddim_alphas_prev, dtype=np.float32)[:total_steps],
+                         sigmas.astype(np.float32)[:total_steps],
+                         np.asarray(self.ddim_sqrt_one_minus_alphas.cpu() if isinstance(self.ddim_sqrt_one_minus_alphas, torch.Tensor) else self.ddim_sqrt_one_minus_alphas, dtype=np.float32)[:total_steps]], axis=1)
+
+    def _update(self, st, e_u, e_c, scale, bs, cfg, noise, temperature):
+        """CFG mix + x_{t-1} from row st['idx'] of st['coef']: x_in[:bs] in place, its copy into x_in[bs:], pred_x0."""
+        _ops().ddim_cfg_step(e_u, e_c, st['x_in'][:bs], st['coef'], scale, x_prev=st['x_in'][:bs],
+                             x_prev_dup=st['x_in'][bs:] if cfg else None, pred_x0=st['pred_x0'], noise=noise,
+                             temperature=temperature, step_idx=st['idx'])
+
+    def _graph_tag(self):
+        """What else, besides the shapes and contexts, the captured step graph depends on."""
+        return ()
+
     def _ctx_buffer(self, i, c):
         """Persistent zero-padded bf16 copy of context i ([B, L, C] -> [B, ceil8(L), C]); refilled in place."""
         bufs = self.__dict__.setdefault('_ctx_bufs', {})
@@ -251,7 +266,7 @@ class DDIMSampler(object):
             st = {'key': key,
                   'x_in': torch.zeros(B, H, W, C, dtype=torch.float32, device=device),
                   'pred_x0': torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
-                  'coef': torch.zeros(1000, 4, dtype=torch.float32, device=device),
+                  'coef': torch.zeros(1000, self._coef_cols, dtype=torch.float32, device=device),
                   'ts': torch.zeros(1000, dtype=torch.int64, device=device),
                   'idx': torch.zeros(1, dtype=torch.int32, device=device)}
             self._st = st

@@ -26,6 +26,7 @@ SIGNATURES = {
     "vdb_reset_launch_count": (None, []),
     "vdb_num_sms": (i, []),
     "vdb_ddim_cfg_step": (i, [p, p, p, p, p, p, f, f, p, p, p, ll, p]),
+    "vdb_dpmpp_cfg_step": (i, [p, p, p, p, p, f, p, p, p, p, ll, p]),
     "vdb_axpby_f32": (i, [p, p, f, f, p, ll, p]),
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),

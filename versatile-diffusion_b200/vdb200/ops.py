@@ -182,6 +182,26 @@ def ddim_cfg_step(e_uncond, e_cond, x, coef, scale, x_prev=None, pred_x0=None, n
     return x_prev, pred_x0
 
 
+def dpmpp_cfg_step(e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next=None, x_next_dup=None, pred_x0=None):
+    """CFG mix + one multistep DPM-Solver++ update (lib/model_zoo/dpm_solver.py).  e_*/x fp32 of n elements; coef fp32 [., 8]
+    device table, row step_idx[0] (int32 device tensor); hist fp32 ring of 3 n elements."""
+    for name, t in (("e_uncond", e_uncond), ("e_cond", e_cond), ("x", x), ("coef", coef), ("hist", hist),
+                    ("x_next_dup", x_next_dup), ("pred_x0", pred_x0)):
+        _need(t, torch.float32, name)
+    _need(step_idx, torch.int32, "step_idx")
+    if coef.dim() != 2 or coef.shape[1] != 8:
+        raise ValueError(f"coef: expected [rows, 8], got {tuple(coef.shape)}")
+    n = x.numel()
+    if hist.numel() != 3 * n:
+        raise ValueError(f"hist: expected 3 x {n} elements, got {hist.numel()}")
+    if x_next is None:
+        x_next = torch.empty_like(x)
+    check(lib.vdb_dpmpp_cfg_step(_ptr(e_uncond), _ptr(e_cond), _ptr(x), _ptr(coef), _ptr(step_idx), float(scale), _ptr(hist),
+                                 _ptr(x_next), _ptr(x_next_dup), _ptr(pred_x0), n, _stream()),
+          "dpmpp_cfg_step")
+    return x_next, pred_x0
+
+
 def axpby(x, z, a, b, out=None):
     _need(x, torch.float32, "x"); _need(z, torch.float32, "z")
     if out is None:
