@@ -59,6 +59,27 @@ int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x
  * hist / x_next, n <= 0, a pointer not 16-byte aligned, or hist overlapping x, x_next, x_next_dup or pred_x0. */
 int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
                        float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n, void* stream);
+/* ---- inpainting: blended latent diffusion — lib/model_zoo/inpaint.py (an addition: the reference has no inpainting; the
+ * semantics are specified in that module's docstring) ------------------------------------------------------------------------------
+ * vdb_inpaint_blend_f32, after each sampler step: x, x0, noise fp32 NHWC [bs, hw, c]; mask fp32 [bs, hw] (mask_per_item != 0) or
+ * [1, hw] (broadcast over the batch), 1 = generate, 0 = keep, broadcast over c.  table: device fp32 rows {a, b}; row *step_idx
+ * (device int, required) is used.  z = noise when non-NULL, else four normals per element quad from Philox4x32-10 at counter
+ * (quad, *step_idx, 0x696e7074 "inpt", 0) under the 64-bit key *seed (two Box-Muller pairs, u = (b + 0.5) 2^-32).  Per element,
+ * fp32 with explicit round-to-nearest:  k = a*x0 + b*z;  x = m == 1 ? x : m == 0 ? k : m*x + (1 - m)*k;  x_dup (may be NULL)
+ * receives a copy.  VDB_ERR_INVALID before any launch: a null x / x0 / mask / table / step_idx, neither seed nor noise, a size
+ * <= 0, a pointer not 16-byte aligned, or x0, mask or noise overlapping x or x_dup. */
+int vdb_inpaint_blend_f32(float* x, float* x_dup, const float* x0, const float* mask, int mask_per_item, const float* table,
+                          const int* step_idx, const unsigned long long* seed, const float* noise, int bs, long long hw, int c,
+                          void* stream);
+/* the blend's Philox draws of step *step_idx for elements [0, n) of a latent, into out (fp32) */
+int vdb_inpaint_noise_f32(const unsigned long long* seed, const int* step_idx, long long n, float* out, void* stream);
+/* pixel mask fp32 [n, H8, W8] -> latent mask [n, H8/8, W8/8]: the max over each 8x8 cell (max_pool2d's rule: NaN propagates);
+ * H8 and W8 multiples of 8 */
+int vdb_mask_to_latent(const float* mask, int n, int H8, int W8, float* out, void* stream);
+/* post-decode paste-back, fp32 NCHW [n, c, hw]: out = m*decoded + (1 - m)*image per pixel (m == 1 and m == 0 select exactly),
+ * mask [n, hw] (mask_per_item != 0) or [1, hw]; out may alias decoded or image */
+int vdb_composite_f32(const float* decoded, const float* image, const float* mask, int mask_per_item, int n, int c, long long hw,
+                      float* out, void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */

@@ -2,6 +2,8 @@
 // and apply(+SiLU, +channel concat), LayerNorm, nearest 2x upsample, small-Cin im2col, skinny
 // (M <= 16) linears for the timestep-embedding MLP, sinusoidal timestep embedding, row softmax,
 // layout permutes. All vectorised to 16-byte accesses on NHWC / token-major bf16 tensors.
+#include <curand_philox4x32_x.h>
+
 #include "common.cuh"
 #include "host_util.h"
 
@@ -144,6 +146,127 @@ __global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const 
       for (int q = 0; q < 4; ++q)
         if (i + q < n) h0[i + q] = p0[q];
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Inpainting (lib/model_zoo/inpaint.py): blended latent diffusion.  After every sampler step the kept region (mask 0) is
+// overwritten with the original latent re-noised to the step's target point, row *step_idx of the table {a, b}:
+//   k  = a*x0 + b*z                       (explicit _rn: an fp32 CPU restatement is bitwise)
+//   x' = m == 1 ? x' : m == 0 ? k : m*x' + (1 - m)*k
+// z is the explicit noise when given, else the Philox4x32-10 stream below.  The exact selects at m = 0 and m = 1 make a hard
+// mask keep x0 bit for bit at the last row {1, 0} and leave the generated region bit for bit as the step wrote it.
+// ---------------------------------------------------------------------------------------------
+constexpr unsigned kInpaintTag = 0x696e7074u;   // "inpt": the text decoder's stream uses "text" (0x74657874)
+
+// Four standard normals of counter (quad, step, "inpt", 0) under a 64-bit key: two Box-Muller pairs, u = (b + 0.5) 2^-32 in
+// fp64 (never 0 or 1), (r cos 2 pi u', r sin 2 pi u') with r = sqrt(-2 ln u), rounded to fp32.
+__device__ __forceinline__ void inpaint_normals(unsigned long long key, unsigned quad, int step, float z[4]) {
+  const uint4 b = curand_Philox4x32_10(make_uint4(quad, static_cast<unsigned>(step), kInpaintTag, 0u),
+                                       make_uint2(static_cast<unsigned>(key), static_cast<unsigned>(key >> 32)));
+  const unsigned w[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int p = 0; p < 2; ++p) {
+    const double u0 = (static_cast<double>(w[2 * p]) + 0.5) * 0x1.0p-32;
+    const double u1 = (static_cast<double>(w[2 * p + 1]) + 0.5) * 0x1.0p-32;
+    const double r = sqrt(-2.0 * log(u0));
+    double s, c;
+    sincospi(2.0 * u1, &s, &c);
+    z[2 * p] = static_cast<float>(r * c);
+    z[2 * p + 1] = static_cast<float>(r * s);
+  }
+}
+
+// x, x0, noise: fp32 NHWC [bs, hw, c] flattened to n = bs*hw*c; mask [bs | 1, hw], broadcast over c.  Element quad i/4 draws
+// counter quad i/4.  The slots are 16-byte aligned only when n % 4 == 0, so vectors are used on full quads only.
+__global__ void inpaint_blend_kernel(float* x, float* __restrict__ x_dup, const float* __restrict__ x0,
+                                     const float* __restrict__ mask, int mask_per_item, const float* __restrict__ table,
+                                     const int* __restrict__ step_idx, const unsigned long long* __restrict__ seed,
+                                     const float* __restrict__ noise, long long n, long long hw, int c) {
+  const int idx = *step_idx;
+  const float a = table[2 * idx], b = table[2 * idx + 1];
+  const unsigned long long key = noise ? 0ull : *seed;
+  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) * 4; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x * 4) {
+    const bool full = i + 3 < n;
+    float xv[4], kv[4], zv[4];
+    if (full) {
+      *reinterpret_cast<float4*>(xv) = *reinterpret_cast<const float4*>(x + i);
+      *reinterpret_cast<float4*>(kv) = __ldg(reinterpret_cast<const float4*>(x0 + i));
+      if (noise) *reinterpret_cast<float4*>(zv) = __ldg(reinterpret_cast<const float4*>(noise + i));
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          xv[q] = x[i + q];
+          kv[q] = x0[i + q];
+          if (noise) zv[q] = noise[i + q];
+        }
+    }
+    if (!noise) inpaint_normals(key, static_cast<unsigned>(i >> 2), idx, zv);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (i + q >= n) break;
+      const long long pix = (i + q) / c;
+      const float m = mask[mask_per_item ? pix : pix % hw];
+      const float k = __fadd_rn(__fmul_rn(a, kv[q]), __fmul_rn(b, zv[q]));
+      xv[q] = m == 1.f ? xv[q] : m == 0.f ? k : __fadd_rn(__fmul_rn(m, xv[q]), __fmul_rn(__fsub_rn(1.f, m), k));
+    }
+    if (full) {
+      *reinterpret_cast<float4*>(x + i) = *reinterpret_cast<float4*>(xv);
+      if (x_dup) *reinterpret_cast<float4*>(x_dup + i) = *reinterpret_cast<float4*>(xv);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          x[i + q] = xv[q];
+          if (x_dup) x_dup[i + q] = xv[q];
+        }
+    }
+  }
+}
+
+// the blend kernel's draws of step *step_idx for elements [0, n)
+__global__ void inpaint_noise_kernel(const unsigned long long* __restrict__ seed, const int* __restrict__ step_idx, long long n,
+                                     float* __restrict__ out) {
+  const unsigned long long key = *seed;
+  const int idx = *step_idx;
+  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) * 4; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x * 4) {
+    float z[4];
+    inpaint_normals(key, static_cast<unsigned>(i >> 2), idx, z);
+    for (int q = 0; q < 4; ++q)
+      if (i + q < n) out[i + q] = z[q];
+  }
+}
+
+// pixel mask [n, H8, W8] -> latent mask [n, H8/8, W8/8]: max over each 8x8 cell, first maximum in row-major order, NaN wins
+// (max_pool2d's rule, so the result is bitwise torch's)
+__global__ void mask_to_latent_kernel(const float* __restrict__ mask, int n, int H8, int W8, float* __restrict__ out) {
+  const int H = H8 / 8, W = W8 / 8;
+  const long long total = static_cast<long long>(n) * H * W;
+  for (long long o = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; o < total;
+       o += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int xw = static_cast<int>(o % W), yh = static_cast<int>((o / W) % H);
+    const long long b = o / (static_cast<long long>(W) * H);
+    const float* p = mask + (b * H8 + 8LL * yh) * W8 + 8 * xw;
+    float best = p[0];
+    for (int r = 0; r < 8; ++r)
+      for (int s = 0; s < 8; ++s) {
+        const float v = p[static_cast<long long>(r) * W8 + s];
+        if (v > best || v != v) best = v;
+      }
+    out[o] = best;
+  }
+}
+
+// out = m*decoded + (1 - m)*image per pixel, NCHW [n, c, hw], mask [n | 1, hw]; exact selects at m = 0 and m = 1
+__global__ void composite_kernel(const float* decoded, const float* image, const float* __restrict__ mask, int mask_per_item,
+                                 int c, long long hw, long long total, float* out) {
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long p = e % hw;
+    const float m = mask[(mask_per_item ? e / (hw * c) * hw : 0) + p];
+    const float d = decoded[e], im = image[e];
+    out[e] = m == 1.f ? d : m == 0.f ? im : __fadd_rn(__fmul_rn(m, d), __fmul_rn(__fsub_rn(1.f, m), im));
   }
 }
 
@@ -1654,6 +1777,64 @@ int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* 
   VDB_PREFER_MAX_SMEM(dpmpp_cfg_step_kernel);
   dpmpp_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_inpaint_blend_f32(float* x, float* x_dup, const float* x0, const float* mask, int mask_per_item, const float* table,
+                          const int* step_idx, const unsigned long long* seed, const float* noise, int bs, long long hw, int c,
+                          void* stream) {
+  if (!x || !x0 || !mask || !table || !step_idx || (!seed && !noise) || bs <= 0 || hw <= 0 || c <= 0)
+    return set_error(VDB_ERR_INVALID, "inpaint_blend: null/empty argument");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_dup) | reinterpret_cast<uintptr_t>(x0) |
+       reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(noise)) & 15)
+    return set_error(VDB_ERR_INVALID, "inpaint_blend: pointers must be 16-byte aligned");
+  const long long n = static_cast<long long>(bs) * hw * c;
+  // x / x_dup are written while x0, the mask and the noise are read through the read-only path: no byte may be shared
+  const long long in_len[3] = {n, (mask_per_item ? bs : 1) * hw, n};
+  const float* ins[3] = {x0, mask, noise};
+  for (const float* o : {static_cast<const float*>(x), static_cast<const float*>(x_dup)}) {
+    const uintptr_t o_lo = reinterpret_cast<uintptr_t>(o), o_hi = o_lo + static_cast<uintptr_t>(n) * sizeof(float);
+    for (int k = 0; k < 3; ++k) {
+      const uintptr_t lo = reinterpret_cast<uintptr_t>(ins[k]), hi = lo + static_cast<uintptr_t>(in_len[k]) * sizeof(float);
+      if (o && ins[k] && lo < o_hi && o_lo < hi)
+        return set_error(VDB_ERR_INVALID, "inpaint_blend: x0, mask or noise overlaps x or x_dup");
+    }
+  }
+  const int threads = 256;
+  inpaint_blend_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, x_dup, x0, mask, mask_per_item, table, step_idx, seed, noise, n, hw, c);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_inpaint_noise_f32(const unsigned long long* seed, const int* step_idx, long long n, float* out, void* stream) {
+  if (!seed || !step_idx || !out || n <= 0) return set_error(VDB_ERR_INVALID, "inpaint_noise: null/empty argument");
+  inpaint_noise_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(seed, step_idx, n, out);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_mask_to_latent(const float* mask, int n, int H8, int W8, float* out, void* stream) {
+  if (!mask || !out || n <= 0 || H8 <= 0 || W8 <= 0) return set_error(VDB_ERR_INVALID, "mask_to_latent: null/empty argument");
+  if (H8 % 8 || W8 % 8) return set_error(VDB_ERR_INVALID, "mask_to_latent: H8 and W8 must be multiples of 8");
+  mask_to_latent_kernel<<<ew_blocks(static_cast<long long>(n) * (H8 / 8) * (W8 / 8), 256), 256, 0,
+                          reinterpret_cast<cudaStream_t>(stream)>>>(mask, n, H8, W8, out);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_composite_f32(const float* decoded, const float* image, const float* mask, int mask_per_item, int n, int c, long long hw,
+                      float* out, void* stream) {
+  if (!decoded || !image || !mask || !out || n <= 0 || c <= 0 || hw <= 0)
+    return set_error(VDB_ERR_INVALID, "composite: null/empty argument");
+  const long long total = static_cast<long long>(n) * c * hw;
+  composite_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(decoded, image, mask, mask_per_item,
+                                                                                               c, hw, total, out);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;

@@ -112,12 +112,25 @@ class DDIMSampler(object):
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         model = self.model
         device = torch.device(model.device)
+        # inpainting (lib/model_zoo/inpaint.py): refuse bad inputs before any device work; the Philox key comes from torch's CPU
+        # generator, drawn only when a mask is given
+        inpaint = x_info.get('inpaint_mask', None) is not None
+        if inpaint:
+            from .inpaint import check_inputs
+            x0_in, mask_in = check_inputs(x_info, shape)
+            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64)
         if device.type != 'cuda':
             raise RuntimeError("DDIMSampler: the H100 build has no CPU path (model.to('cuda') first)")
         ops = _ops()
         dtype = c_infos[0]['conditioning'].dtype
         bs = shape[0]
-        x, timesteps = self._initial_latent(shape, x_info, dtype, device)
+        full_walk = inpaint and x_info.get('x0_forward_timesteps', None) is None
+        start_info = x_info
+        if full_walk:       # a masked full walk starts from x_T as an unmasked one does, never from the img2img start
+            start_info = {k: v for k, v in x_info.items() if k != 'x0'}
+        elif inpaint:       # the img2img start noises x0 row by row: a batch-1 x0 is noised once per item
+            start_info = dict(x_info, x0=x0_in.expand(bs, *x0_in.shape[1:]))
+        x, timesteps = self._initial_latent(shape, start_info, dtype, device)
         x_info['x'] = x
         scale = float(c_infos[0]['unconditional_guidance_scale'])
         cfg = scale != 1.
@@ -155,6 +168,8 @@ class DDIMSampler(object):
 
         st = self._state(bs, B, H, W, shape[1], device)
         ops.nchw_to_nhwc(x.float().contiguous(), out=st['x_in'][:bs])
+        if inpaint:
+            mask_per_item = self._inpaint_state(st, x0_in, mask_in, seed, total_steps, x if full_walk else None, bs, device)
         if cfg:
             st['x_in'][bs:].copy_(st['x_in'][:bs])
         st['coef'][:total_steps].copy_(coef)
@@ -168,6 +183,9 @@ class DDIMSampler(object):
                 eps = eps.view(B, 1, 1, -1)
             e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
             self._update(st, e_u, e_c, scale, bs, cfg, noise, temperature)
+            if inpaint:
+                ops.inpaint_blend(st['x_in'][:bs], st['x0'], st['mask'] if mask_per_item else st['mask'][:1], st['blend'],
+                                  st['idx'], seed=st['seed'], x_dup=st['x_in'][bs:] if cfg else None)
             ops.add_int(st['idx'], -1)
 
         intermediates = {'pred_xt': [], 'pred_x0': []}
@@ -191,6 +209,8 @@ class DDIMSampler(object):
             from .diffusion_utils import pack_epoch
             key = (pack_epoch(), bs, B, H, W, x_type, tuple(c_types), tuple(ratios), scale, float(temperature), time_from,
                    tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs)) + self._graph_tag()
+            if inpaint:
+                key += (('inpaint', mask_per_item),)
             ent = self._graphs.get(key)
             if ent is not None and ent[1] == model.context_kv_signature(c_types, ctxs):
                 # steady state: the context projections were just refreshed in place; every step is a graph replay
@@ -272,6 +292,34 @@ class DDIMSampler(object):
             self._st = st
             self._graphs = {}
         return st
+
+    def _inpaint_state(self, st, x0, mask, seed, total_steps, x_T, bs, device):
+        """Refill the inpainting buffers of st in place, so a cached step graph replays on a new image, mask and seed ->
+        whether the mask is per item.  With x_T (the full walk) the kept region of x_in[:bs] becomes x0 noised to t_top with
+        x_T's own draw.  lib/model_zoo/inpaint.py specifies the semantics."""
+        from .inpaint import blend_table
+        ops = _ops()
+        _, H, W, C = st['x_in'].shape
+        if 'x0' not in st:
+            st.update(x0=torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
+                      mask=torch.zeros(bs, H * W, dtype=torch.float32, device=device),
+                      blend=torch.zeros(1000, 2, dtype=torch.float32, device=device),
+                      seed=torch.zeros(1, dtype=torch.int64, device=device))
+        st['x0'].copy_(ops.nchw_to_nhwc(x0.to(device=device, dtype=torch.float32).contiguous()))   # broadcasts a [1] batch
+        mask = mask.to(device=device, dtype=torch.float32).contiguous()
+        if mask.shape[-1] != W:
+            mask = ops.mask_to_latent(mask)
+        st['mask'][:mask.shape[0]].copy_(mask.view(mask.shape[0], H * W))
+        st['blend'][:total_steps].copy_(torch.from_numpy(blend_table(self.ddim_alphas_prev[:total_steps])))
+        st['seed'].copy_(seed)
+        mask_per_item = int(mask.shape[0] != 1)
+        if x_T is not None:
+            a_top = float(self.ddim_alphas[total_steps - 1])
+            row = torch.tensor([[np.sqrt(a_top), np.sqrt(1.0 - a_top)]], dtype=torch.float32, device=device)
+            ops.inpaint_blend(st['x_in'][:bs], st['x0'], st['mask'] if mask_per_item else st['mask'][:1], row,
+                              torch.zeros(1, dtype=torch.int32, device=device),
+                              noise=ops.nchw_to_nhwc(x_T.float().contiguous()))
+        return mask_per_item
 
     # ------------------------------------------------------------------ single-step API (reference parity)
     @torch.no_grad()

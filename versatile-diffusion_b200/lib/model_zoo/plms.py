@@ -34,6 +34,9 @@ class PLMSSampler(DDIMSampler):
         super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)
 
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
+        if x_info.get('inpaint_mask', None) is not None:
+            raise NotImplementedError("PLMSSampler has no inpainting: use DDIMSampler or DPMSolverSampler "
+                                      "(lib/model_zoo/inpaint.py)")
         ops = _ops()
         model = self.model
         device = torch.device(model.device)

@@ -202,6 +202,69 @@ def dpmpp_cfg_step(e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next=None
     return x_next, pred_x0
 
 
+def inpaint_blend(x, x0, mask, table, step_idx, seed=None, noise=None, x_dup=None):
+    """Inpainting blend after a sampler step (lib/model_zoo/inpaint.py), in place on x.  x / x0 / noise / x_dup fp32 NHWC
+    [bs, H, W, C]; mask fp32 of H*W (broadcast over the batch) or bs*H*W elements; table fp32 [., 2] device rows, row
+    step_idx[0] (int32 device tensor); seed int64 device word keying the Philox draws, unused when noise is given."""
+    for name, t in (("x", x), ("x0", x0), ("mask", mask), ("table", table), ("noise", noise), ("x_dup", x_dup)):
+        _need(t, torch.float32, name)
+    _need(step_idx, torch.int32, "step_idx")
+    _need(seed, torch.int64, "seed")
+    bs, C = x.shape[0], x.shape[-1]
+    hw = x.numel() // (bs * C)
+    for name, t in (("x0", x0), ("noise", noise), ("x_dup", x_dup)):
+        if t is not None and t.shape != x.shape:
+            raise ValueError(f"{name}: expected {tuple(x.shape)}, got {tuple(t.shape)}")
+    if mask.numel() not in (hw, bs * hw):
+        raise ValueError(f"mask: expected {hw} or {bs * hw} elements, got {mask.numel()}")
+    if table.dim() != 2 or table.shape[1] != 2:
+        raise ValueError(f"table: expected [rows, 2], got {tuple(table.shape)}")
+    check(lib.vdb_inpaint_blend_f32(_ptr(x), _ptr(x_dup), _ptr(x0), _ptr(mask), int(mask.numel() != hw), _ptr(table),
+                                    _ptr(step_idx), _ptr(seed), _ptr(noise), bs, hw, C, _stream()),
+          "inpaint_blend")
+    return x
+
+
+def inpaint_noise(seed, step_idx, n, out=None):
+    """The inpainting blend's Philox draws at step step_idx[0] for the first n elements of a latent -> fp32 [n]."""
+    _need(seed, torch.int64, "seed")
+    _need(step_idx, torch.int32, "step_idx")
+    if out is None:
+        out = torch.empty(n, dtype=torch.float32, device=seed.device)
+    _need(out, torch.float32, "out")
+    check(lib.vdb_inpaint_noise_f32(_ptr(seed), _ptr(step_idx), int(n), _ptr(out), _stream()), "inpaint_noise")
+    return out
+
+
+def mask_to_latent(mask, out=None):
+    """Pixel mask fp32 [n, 1, 8H, 8W] -> latent mask [n, 1, H, W], the max over each 8x8 cell."""
+    _need(mask, torch.float32, "mask")
+    if mask.dim() != 4 or mask.shape[1] != 1 or mask.shape[2] % 8 or mask.shape[3] % 8:
+        raise ValueError(f"mask: expected [n, 1, 8H, 8W], got {tuple(mask.shape)}")
+    n, _, H8, W8 = mask.shape
+    if out is None:
+        out = torch.empty((n, 1, H8 // 8, W8 // 8), dtype=torch.float32, device=mask.device)
+    check(lib.vdb_mask_to_latent(_ptr(mask), n, H8, W8, _ptr(out), _stream()), "mask_to_latent")
+    return out
+
+
+def composite(decoded, image, mask, out=None):
+    """out = m*decoded + (1 - m)*image per pixel: decoded / image fp32 NCHW [n, C, H, W], mask fp32 [n or 1, 1, H, W]."""
+    for name, t in (("decoded", decoded), ("image", image), ("mask", mask)):
+        _need(t, torch.float32, name)
+    if decoded.dim() != 4 or image.shape != decoded.shape:
+        raise ValueError(f"image: expected {tuple(decoded.shape)}, got {tuple(image.shape)}")
+    n, C, H, W = decoded.shape
+    if mask.dim() != 4 or mask.shape[0] not in (1, n) or tuple(mask.shape[1:]) != (1, H, W):
+        raise ValueError(f"mask: expected [{n} or 1, 1, {H}, {W}], got {tuple(mask.shape)}")
+    if out is None:
+        out = torch.empty_like(decoded)
+    check(lib.vdb_composite_f32(_ptr(decoded), _ptr(image), _ptr(mask), int(mask.shape[0] != 1), n, C, H * W, _ptr(out),
+                                _stream()),
+          "composite")
+    return out
+
+
 def axpby(x, z, a, b, out=None):
     _need(x, torch.float32, "x"); _need(z, torch.float32, "z")
     if out is None:
