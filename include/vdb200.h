@@ -103,8 +103,8 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
                   size_t ws_bytes, void* stream);
 
 /* The tiling the last vdb_gemm_bf16 / vdb_gemm_ln_bf16 / vdb_conv3x3_bf16 call on this thread launched (host-side record, no
- * device work): out[0..n) receives {BN, STAGES, epilogue MODE, ksplit, grid, M tiles, N tiles, nfast, chunked} (as many as n
- * allows).  Returns the number of fields (9).  For tests and tools that need to know which kernel instantiation ran. */
+ * device work): out[0..n) receives {BN, STAGES, epilogue MODE, ksplit, grid, M tiles, N tiles} (as many as n
+ * allows).  Returns the number of fields (7).  For tests and tools that need to know which kernel instantiation ran. */
 int vdb_igemm_last_plan(int* out, int n);
 
 /* ---- the same GEMM with a LayerNorm folded in — BasicTransformerBlock norm1/2/3, attention.py:206-208,214-218 -------------
@@ -120,22 +120,11 @@ int vdb_igemm_last_plan(int* out, int n);
  * PRODUCER (stats_out != NULL):  out = A W^T + bias + resid as vdb_gemm_bf16, and stats_out (room for [2 * ceil(N/64)][M][2] fp32)
  *   receives *stats_parts partial (sum, sum of squares) per output row (fp32 values before the bf16 rounding; one partial per N tile
  *   and epilogue warp, so *stats_parts = 2 * N tiles is known on the host when the call returns), N % 32 == 0.
- * Exactly one of ln_stats / stats_out; bf16 out, 16-byte aligned out / resid rows; needs the TMA-store epilogue (VDB_EPI_TMA != 0). */
+ * Exactly one of ln_stats / stats_out; bf16 out, 16-byte aligned out / resid rows. */
 int vdb_gemm_ln_bf16(const void* A, long long M, long long K, long long lda, const void* W, long long N, long long ldw,
                      const float* bias, const void* resid, long long ldr, void* out, long long ldo, int act,
                      const float* ln_stats, long long ln_rows, int ln_parts, int ln_dim, float ln_eps, const float* ln_colsum,
                      int ln_on_cols, const float* ln_rowbias, float* stats_out, int* stats_parts, int bn, void* stream);
-
-/* ---- skinny GEMM on the CUDA cores for a small operand of <= 64 rows — the 0-D diffuser's Linear_MultiDim / FCBlock_MultiDim GEMMs
- *      (openaimodel.py:2084-2141, 2275-2354; M = batch rows) and the 32-row projections of its context blocks --------------------
- * small = [S, K1 (+K2)] bf16 rows (two sources concatenated along K, small2 may be NULL), big = [R, K1+K2] bf16 rows, fp32 accumulate.
- * transpose_out 0:  out[s, r] = small[s] . big[r] + bias[s * bias_bstride + r] + resid[s, r]     (activations x weights^T)
- * transpose_out 1:  out[r, s] = small[s] . big[r]                                               (no bias / residual: V^T projection)
- * The small operand must fit shared memory: vdb_gemm_skinny_fits(S, K) != 0 (S padded to 8 / 16 / 32 / 64 rows x K x 2 B <= 200 KB). */
-int vdb_gemm_skinny_fits(int S, long long K);
-int vdb_gemm_skinny_bf16(const void* small1, int S, long long K1, long long lds1, const void* small2, long long K2, long long lds2,
-                         const void* big, long long R, long long ldb, const float* bias, long long bias_bstride,
-                         const void* resid, long long ldr, void* out, long long ldo, int transpose_out, void* stream);
 
 /* ---- wgmma implicit-GEMM 3x3 conv on NHWC — ResBlock convs openaimodel.py:203,229; Downsample
  *      :150-152; Upsample.conv :105; VAE autokl_modules.py:48-76,93-111 ---------------------------
@@ -143,10 +132,9 @@ int vdb_gemm_skinny_bf16(const void* small1, int S, long long K1, long long lds1
  * mode 3 + 2*py + px: parity (py,px) of "nearest 2x upsample then 3x3 conv" (Upsample.forward, openaimodel.py:107-117;
  *      autokl_modules.py:54-58) evaluated on the SOURCE image with the 9 taps folded into 2x2: X = source [B,H,W,C],
  *      out = [B,H,W,N] (that parity sub-lattice), Wt = [N, 4*C] (ty,tx,c) pre-summed on the host; no skip inputs.
- *      vdb_interleave2x2_nhwc assembles the four parities into [B,2H,2W,N].
  * mode 7 + 2*py + px: the same parity conv, but `out` is the full [B,2H,2W,N] tensor and the tile is stored straight into pixels
  *      (2y+py, 2x+px) through the output tensor map (no interleave pass, no parity temporaries); bf16 out, no residual / skips /
- *      split-K, N % 32 == 0 (needs the TMA-store epilogue).
+ *      split-K, N % 32 == 0.
  * Wt [N, 9*C + Cs1 + Cs2], K order (ky,kx,c) then the 1x1 skip_connection columns whose inputs
  * skip1/skip2 (raw NHWC at output resolution; the two halves of torch.cat([h, hs.pop()]),
  * vd.py:372) are accumulated into the same accumulator tile (ResBlock.skip_connection, openaimodel.py:240).
@@ -221,9 +209,6 @@ int vdb_resample_h_u8(const void* x /* u8 [n,H,Win,3] */, int n, int H, int Win,
 int vdb_resample_v_crop_norm(const void* x /* u8 [n,Hin,W,3] */, int n, int Hin, int W, const int* bounds, const int* kk,
                              int ksize /* 0: no vertical resize */, int top, int left, int S, const float* mean3,
                              const float* std3, float* y /* fp32 [n,3,S,S] */, void* stream);
-
-/* [4 parities (py,px)][B,H,W,C] bf16 -> [B,2H,2W,C]: out[b,2y+py,2x+px,:] = src[py*2+px][b,y,x,:] (see conv mode 3..6). */
-int vdb_interleave2x2_nhwc(const void* src, int B, int H, int W, int C, void* y, void* stream);
 
 /* ---- im2col for tiny-Cin 3x3 convs (latent 4ch / RGB 3ch inputs): fp32 NHWC -> bf16 [B*H*W, Kpad]
  *      (x*in_scale + in_shift applied first: AutoencoderKL.encode's x*2-1, autokl.py:34) ----------- */

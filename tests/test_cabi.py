@@ -73,10 +73,10 @@ def test_attention_dispatch_edges():
     assert lib.vdb_launch_count() == before
 
 
-def test_igemm_last_plan_reports_nine_fields():
+def test_igemm_last_plan_reports_seven_fields():
     from vdb200._lib import lib
-    buf = (ctypes.c_int * 9)()
-    assert lib.vdb_igemm_last_plan(buf, 9) == 9 and lib.vdb_igemm_last_plan(None, 0) == 9
+    buf = (ctypes.c_int * 7)()
+    assert lib.vdb_igemm_last_plan(buf, 7) == 7 and lib.vdb_igemm_last_plan(None, 0) == 7
 
 
 def test_norm_last_plan_reports_nine_fields_and_refused_calls_leave_it():

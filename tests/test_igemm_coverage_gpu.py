@@ -1,8 +1,8 @@
 """Every instantiation of the implicit-GEMM kernel (igemm.cu), and the state it carries from one tile to the next, against an
 fp64 reference.
 
-The launcher compiles 23 instantiations: BN in {64, 128, 160, 256} x epilogue modes {0, 1, 3, 5, 7}, plus BN 256 x the GEGLU
-modes {2, 4, 6}.  Each row of CASES names the (BN, MODE) it means to reach and the inputs that get there; the test asserts the
+The launcher compiles 18 instantiations: BN in {64, 128, 160, 256} x epilogue modes {0, 3, 5, 7}, plus BN 256 x the GEGLU
+modes {4, 6}.  Each row of CASES names the (BN, MODE) it means to reach and the inputs that get there; the test asserts the
 plan the launcher reports (ops.igemm_last_plan) and compares every output element with the fp64 result on the same
 bf16-rounded operands.  BN and ksplit are forced, so the plan does not depend on the SM count.
 
@@ -11,8 +11,6 @@ grid with test_tile_schedule.walk): that is when the bias / LayerNorm tables cac
 tile's row statistics are prefetched, the parked accumulator is reused and the TMA-store staging alternates.  They also have an
 M tail (M % 128 != 0), a K tail (K % 64 != 0) and, except for GEGLU (N % 256 == 0 by contract), a partial last N tile.
 test_tile_schedule checks on the CPU that every instantiation has such a row at 132 SMs.
-
-Modes 1 and 2 (the non-TMA epilogues) are only chosen with VDB_EPI_TMA=0; their rows run in a subprocess under that switch.
 
 Tolerance, per element (U = 2^-24, fp32 unit roundoff; K = reduction length):
     |out - ref| <= rtol * |ref| + atol
@@ -23,9 +21,6 @@ Tolerance, per element (U = 2^-24, fp32 unit roundoff; K = reduction length):
   top of that.  The cosine >= 0.999 check of test_kernels_gpu is kept as well.
 """
 import math
-import os
-import subprocess
-import sys
 from collections import defaultdict
 
 import pytest
@@ -36,8 +31,6 @@ from test_tile_schedule import walk
 
 DEV = "cuda"
 U = 2.0 ** -24
-SWITCHES = ("VDB_EPI_TMA", "VDB_IGEMM_SPEC", "VDB_NFAST", "VDB_CHUNKED", "VDB_BN_MODEL")
-NO_TMA = {"VDB_EPI_TMA": "0"}
 STAGES = {64: 8, 128: 6, 160: 5, 256: 4}
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_QGELU, ACT_GEGLU = 0, 1, 2, 3, 4
 
@@ -52,8 +45,8 @@ N_WALK_ODD = {64: 16 * 64 + 40, 128: 16 * 128 + 40, 160: 16 * 160 + 104, 256: 16
 N_GEGLU = 17 * 256
 
 
-def _case(cid, kind, bn, mode, walk=False, env=None, ksplit=1, **kw):
-    return dict(id=cid, kind=kind, bn=bn, mode=mode, walk=walk, env=env or {}, ksplit=ksplit, **kw)
+def _case(cid, kind, bn, mode, walk=False, ksplit=1, **kw):
+    return dict(id=cid, kind=kind, bn=bn, mode=mode, walk=walk, ksplit=ksplit, **kw)
 
 
 CASES = []
@@ -62,13 +55,11 @@ for _bn, _act, _alpha in ((64, ACT_SILU, 1.0), (128, ACT_GELU, 1.0), (160, ACT_Q
     CASES.append(_case(f"m0-bn{_bn}", "gemm", _bn, 0, walk=True, M=M_WALK, N=N_WALK_ODD[_bn], K=K_WALK, bias="vec", resid=True,
                        act=_act, alpha=_alpha))
 for _bn in (64, 128, 160, 256):
-    CASES.append(_case(f"m1-bn{_bn}", "gemm", _bn, 1, walk=True, env=NO_TMA, M=M_WALK, N=N_WALK[_bn], K=K_WALK, bias="vec", resid=True))
     CASES.append(_case(f"m3-bn{_bn}", "gemm", _bn, 3, walk=True, M=M_WALK, N=N_WALK[_bn], K=K_WALK, bias="vec", resid=True))
     CASES.append(_case(f"m5-bn{_bn}", "ln", _bn, 5, walk=True, M=M_WALK, N=N_WALK[_bn], K=K_WALK,
                        parts={64: 5, 128: 25, 160: 8, 256: 20}[_bn]))          # ln_parts <= 16: prefetched a tile ahead; > 16: not
     CASES.append(_case(f"m7-bn{_bn}", "stats", _bn, 7, walk=True, M=M_WALK, N=N_WALK[_bn], K=K_WALK, bias="vec", resid=_bn != 128))
 CASES += [
-    _case("m2-bn256", "gemm", 256, 2, walk=True, env=NO_TMA, M=M_WALK, N=N_GEGLU, K=K_WALK, bias="vec", act=ACT_GEGLU),
     _case("m4-bn256", "gemm", 256, 4, walk=True, M=M_WALK, N=N_GEGLU, K=K_WALK, bias="vec", act=ACT_GEGLU),
     _case("m6-bn256", "ln", 256, 6, walk=True, M=M_WALK, N=N_GEGLU, K=K_WALK, parts=5, geglu=True),
     _case("m6-bn256-parts20", "ln", 256, 6, walk=True, M=M_WALK, N=N_GEGLU, K=K_WALK, parts=20, geglu=True),
@@ -93,12 +84,19 @@ CASES += [
     # non-power-of-two grids: the (TW, TH, TB) box hangs past the image; those rows are masked on store
     _case("conv-24x40-silu", "conv", 64, 0, walk=True, B=3, H=24, W=40, C=64, N=320, cmode=0, bias="vec", resid=True, act=ACT_SILU),
     _case("conv-24x40-batchbias", "conv", 64, 3, walk=True, B=3, H=24, W=40, C=64, N=320, cmode=0, bias="batch", resid=True),
-    _case("conv-24x40-batchbias-notma", "conv", 64, 1, walk=True, env=NO_TMA, B=3, H=24, W=40, C=64, N=320, cmode=0, bias="batch",
-          resid=True),
     _case("conv-12x8", "conv", 128, 3, B=3, H=12, W=8, C=128, N=160, cmode=0, bias="batch", resid=True),
     _case("conv-s2-24x40", "conv", 64, 3, B=3, H=24, W=40, C=128, N=128, cmode=1, bias="vec"),
     _case("conv-s2vae-24x40-f32", "conv", 128, 0, B=1, H=24, W=40, C=64, N=96, cmode=2, bias="vec", f32=True),
     _case("conv-s2vae-12x8-b5", "conv", 64, 0, B=5, H=12, W=8, C=64, N=96, cmode=2, bias="batch"),
+    # folded nearest-2x upsample + 3x3 conv (2x2 taps on the source image, one launch per output parity): modes 7..10 store the
+    # parity straight into the interleaved [B, 2H, 2W, N] result through the output tensor map, modes 3..6 into a dense
+    # [B, H, W, N] tensor; both run the TMA-store epilogue (plan mode 3)
+    _case("conv-up-p0", "conv", 64, 3, B=3, H=12, W=20, C=64, N=96, cmode=7, bias="vec"),
+    _case("conv-up-p1", "conv", 128, 3, B=3, H=12, W=20, C=128, N=160, cmode=8, bias="vec"),
+    _case("conv-up-p2", "conv", 160, 3, B=2, H=16, W=16, C=64, N=320, cmode=9, bias="batch"),
+    _case("conv-up-p3", "conv", 256, 3, B=3, H=12, W=20, C=64, N=320, cmode=10, bias="vec"),
+    _case("conv-upc-p1", "conv", 64, 3, B=3, H=12, W=20, C=64, N=160, cmode=4, bias="batch", resid=True),
+    _case("conv-upc-p2", "conv", 160, 3, B=2, H=24, W=40, C=128, N=320, cmode=5, bias="vec", resid=True),
 ]
 
 
@@ -121,7 +119,7 @@ def tile_geometry(case):
         TH = min(_pow2_ceil(Ho), 128 // TW)
         TB = 128 // (TW * TH)
         tiles_m = -(-Wo // TW) * -(-Ho // TH) * -(-Bo // TB)
-        kb = 9 * case["C"] // 64
+        kb = (4 if case["cmode"] >= 3 else 9) * case["C"] // 64
     else:
         tiles_m = -(-case["M"] // 128)
         kb = -(-case["K"] // 64)
@@ -131,10 +129,10 @@ def tile_geometry(case):
     return tiles_m, tiles_n, -(-kb // per), kb
 
 
-def multi_tile_n_change(grid, tiles_m, tiles_n, ksplit, nfast=0, chunked=0):
+def multi_tile_n_change(grid, tiles_m, tiles_n, ksplit):
     """some CTA runs >= 2 tiles and not all of them on one N tile"""
     seq = defaultdict(list)
-    for cta, _m, n, _k in walk(grid, tiles_m, tiles_n, ksplit, bool(nfast), bool(chunked)):
+    for cta, _m, n, _k in walk(grid, tiles_m, tiles_n, ksplit):
         seq[cta].append(n)
     return any(len(s) >= 2 and len(set(s)) >= 2 for s in seq.values())
 
@@ -216,12 +214,8 @@ def check_plan(case, plan):
         tm, tn, _, _ = tile_geometry(case)
         assert (plan["tiles_m"], plan["tiles_n"]) == (tm, tn), (plan, tm, tn)
     if case["walk"]:
-        assert multi_tile_n_change(plan["grid"], plan["tiles_m"], plan["tiles_n"], plan["ksplit"], plan["nfast"], plan["chunked"]), \
+        assert multi_tile_n_change(plan["grid"], plan["tiles_m"], plan["tiles_n"], plan["ksplit"]), \
             f"{case['id']}: no CTA runs two tiles on different N tiles ({plan})"
-
-
-def _env_matches(case):
-    return all(os.environ.get(k) == case["env"].get(k) for k in SWITCHES)
 
 
 def _bias(case, rows, N, seed):
@@ -379,24 +373,44 @@ def _im2col64(x, cmode):
     return cols.view(B, C, 9, L).permute(0, 3, 2, 1).reshape(B * L, 9 * C)
 
 
+def _taps64(x, par):
+    """NHWC bf16 [B, H, W, C] -> fp64 [B * H * W, 4 C]: the 2x2 source taps of output parity par = 2 py + px of the folded
+    upsample conv, K ordered (ty, tx, c), source pixel (y + ty - 1 + py, x + tx - 1 + px), zero outside the image"""
+    B, H, W, C = x.shape
+    py, px = par >> 1, par & 1
+    xp = F.pad(x.double().permute(0, 3, 1, 2), (1, 1, 1, 1))
+    taps = [xp[:, :, py + ty:py + ty + H, px + tx:px + tx + W] for ty in (0, 1) for tx in (0, 1)]
+    return torch.cat(taps, 1).permute(0, 2, 3, 1).reshape(B * H * W, 4 * C)
+
+
 def run_conv(case):
-    """vdb_conv3x3_bf16 as the GEMM im2col(x) W^T (+ bias, act, residual), bounded as a plain GEMM with K = 9 C."""
+    """vdb_conv3x3_bf16 as the GEMM im2col(x) W^T (+ bias, act, residual), bounded as a plain GEMM with K = 9 C (4 C for the
+    folded upsample modes).  Modes 7..10 write one parity of a zero-filled [B, 2H, 2W, N] tensor: the other three parities
+    must stay zero."""
     ops = _ops()
     B, H, W, C, N, cmode, act = case["B"], case["H"], case["W"], case["C"], case["N"], case["cmode"], case.get("act", 0)
     Ho, Wo = (H // 2, W // 2) if cmode in (1, 2) else (H, W)
+    taps = 4 if cmode >= 3 else 9
     x = rnd(B, H, W, C, seed=1)
-    w = rnd(N, 9 * C, seed=2, scale=(9 * C) ** -0.5)
+    w = rnd(N, taps * C, seed=2, scale=(taps * C) ** -0.5)
     rows = B * Ho * Wo
     b, bstride, _ = _bias(dict(case, rpb=Ho * Wo), rows, N, 3)
     r = rnd(B, Ho, Wo, N, seed=4) if case.get("resid") else None
     f32 = case.get("f32", False)
+    full = torch.zeros(B, 2 * H, 2 * W, N, dtype=torch.bfloat16, device=DEV) if cmode >= 7 else None
     out = ops.conv3x3(x, w, bias=b, bias_bstride=bstride, resid=r, act=act, mode=cmode, bn=case["bn"], ksplit=case["ksplit"],
-                      out_dtype=torch.float32 if f32 else torch.bfloat16)
+                      out=full, out_dtype=torch.float32 if f32 else torch.bfloat16)
     plan = ops.igemm_last_plan()
-    xc = _im2col64(x, cmode)
+    if cmode >= 7:
+        py, px = (cmode - 7) >> 1, (cmode - 7) & 1
+        others = torch.ones(2 * H, 2 * W, dtype=torch.bool, device=DEV)
+        others[py::2, px::2] = False
+        assert torch.count_nonzero(full[:, others]) == 0, f"{case['id']}: a store left its parity"
+        out = full[:, py::2, px::2, :].contiguous()
+    xc = _taps64(x, (cmode - 3) % 4) if cmode >= 3 else _im2col64(x, cmode)
     pre = mm64(xc, w) + _bias_rows(b, bstride, Ho * Wo, rows)
     ref = act64(pre, act)
-    atol = 1.25 * (4 * 9 * C * U * rss64(xc, w) + 2 * U * pre.abs()) + 2.0 ** -20 * pre.abs()
+    atol = 1.25 * (4 * taps * C * U * rss64(xc, w) + 2 * U * pre.abs()) + 2.0 ** -20 * pre.abs()
     if r is not None:
         ref = ref + r.double().view(rows, N)
         atol = atol + 2.0 ** -20 * r.double().view(rows, N).abs()
@@ -408,23 +422,8 @@ RUN = {"gemm": run_gemm, "ln": run_ln, "stats": run_stats, "conv": run_conv}
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES, ids=[c["id"] for c in CASES])
-def test_case(case):
-    if not _env_matches(case):
-        pytest.skip(f"needs {case['env'] or 'the default kernel switches'} (run by test_non_tma_epilogues)")
+def test_instantiation(case):
     out, ref, atol, plan = RUN[case["kind"]](case)
     check_plan(case, plan)
     check(out, ref, atol, 2.0 ** -16 if case.get("f32") else 2.0 ** -8, case["id"])
 
-
-@pytest.mark.gpu
-@pytest.mark.skipif(any(os.environ.get(k) is not None for k in SWITCHES), reason="launched from the default configuration")
-def test_non_tma_epilogues():
-    """modes 1 and 2 (bf16 stores and residual loads as 16-byte vectors from the transposed tile) are chosen only with
-    VDB_EPI_TMA=0, read once per process: their rows run in a process of their own"""
-    env = dict(os.environ, **NO_TMA)
-    ids = [c["id"] for c in CASES if c["env"] == NO_TMA]
-    out = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.abspath(__file__),
-                          "-k", "test_case and (" + " or ".join(ids) + ")"],
-                         capture_output=True, text=True, env=env, timeout=600, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    assert out.returncode == 0, out.stdout[-4000:] + out.stderr[-1000:]
-    assert f"{len(ids)} passed" in out.stdout, out.stdout[-2000:]

@@ -122,9 +122,11 @@ def test_unet_forward_matches_oracle_fresh_inputs(mini):
     _cmp(out, ref, what="apply_model vs oracle (24x24, B=3, L=50)")
 
 
-def test_layernorm_fold_equals_the_layernorm_kernels(mini, monkeypatch):
-    """The three LayerNorms of every transformer block run inside the neighbouring GEMMs' epilogues by default (vdb_gemm_ln_bf16);
-    VDB_LN_FOLD=0 runs them as kernels.  Same eps prediction (both are checked against the reference golden), fewer launches."""
+def test_folded_layernorms_equal_the_layernorm_kernels(mini, monkeypatch):
+    """The three LayerNorms of every transformer block run inside the neighbouring GEMMs' epilogues wherever the token grid allows
+    it (vdb_gemm_ln_bf16); elsewhere they run as kernels, here forced on every block.  Same eps prediction (both are checked
+    against the reference golden), fewer launches."""
+    from lib.model_zoo import attention
     from vdb200 import ops
     net, sd, gi, gold = mini
     args = ({"type": "image", "x": gi["x"].to(DEV)}, gi["t"].to(DEV), {"type": "text", "c": gi["c_text"].to(DEV)})
@@ -133,7 +135,7 @@ def test_layernorm_fold_equals_the_layernorm_kernels(mini, monkeypatch):
         ops.reset_launch_count()
         out_fold = net.apply_model(*args)
         n_fold = ops.launch_count()
-        monkeypatch.setenv("VDB_LN_FOLD", "0")
+        monkeypatch.setattr(attention, "ln_fold_fits", lambda *shape: False)
         ops.reset_launch_count()
         out_ln = net.apply_model(*args)
         n_ln = ops.launch_count()
@@ -268,6 +270,24 @@ def test_vae_decode_encode_vs_reference_golden(mini):
     _cmp(img, gold["vae_decode"], what="vae_decode (clamped image)")
     _cmp(raw.permute(0, 3, 1, 2), gold["vae_decode_raw"], what="decoder output before clamp")
     _cmp(post.parameters, gold["vae_moments"], what="vae_encode moments")
+
+
+def test_folded_upsample_in_the_model_paths(mini, monkeypatch):
+    """With the fold threshold lowered to 0, every Upsample of the mini UNet and VAE runs as four parity convs on the source
+    image (ops.upsample2x never runs): the apply_model, VAE-decode and 5-step DDIM parity checks must hold on that path."""
+    from lib.model_zoo import diffusion_utils
+    from vdb200 import ops
+
+    def unfolded(*args, **kw):
+        raise AssertionError("an Upsample took the unfolded path")
+    monkeypatch.setattr(diffusion_utils, "UPSAMPLE_FOLD_MIN_PIXELS", 0)
+    monkeypatch.setattr(ops, "upsample2x", unfolded)
+    test_apply_model_text_vs_reference_golden(mini)
+    test_apply_model_image_ctx_vs_reference_golden(mini)
+    test_apply_model_multicontext_vs_reference_golden(mini)
+    test_vae_decode_encode_vs_reference_golden(mini)
+    for graph in (False, True):
+        test_ddim_5_steps_vs_reference_golden(mini, graph)
 
 
 def test_vae_encode_sample_matches_oracle(mini):

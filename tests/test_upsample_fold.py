@@ -1,6 +1,6 @@
-"""Folding "nearest-2x upsample + 3x3 conv" into four 2x2-tap convs on the source image (opt-in VDB_UPFOLD): the weight
-folding and the tap / parity conventions handed to the kernel (conv modes 3..6 of vdb_conv3x3_bf16, then
-vdb_interleave2x2_nhwc) are checked here on the CPU against torch's own upsample + conv2d (reference semantics:
+"""Folding "nearest-2x upsample + 3x3 conv" into four 2x2-tap convs on the source image: the weight folding and the tap /
+parity conventions handed to the kernel (conv modes 7..10 of vdb_conv3x3_bf16, each storing one parity of the interleaved
+result) are checked here on the CPU against torch's own upsample + conv2d (reference semantics:
 openaimodel.py:107-117, autokl_modules.py:54-58).  The emulation below consumes the folded weights exactly as the kernel
 does: K ordered (ty, tx, ci), source pixel (y + ty - 1 + py, x + tx - 1 + px), zero fill outside the image."""
 import pytest
@@ -9,7 +9,7 @@ import torch.nn.functional as F
 
 
 def emulate_kernel(x, wf, bias):
-    """x [B,C,H,W] fp32, wf [4, N, 4*C] (any float dtype) -> [B,N,2H,2W], mirroring modes 3..6 + interleave2x2."""
+    """x [B,C,H,W] fp32, wf [4, N, 4*C] (any float dtype) -> [B,N,2H,2W], mirroring modes 7..10."""
     B, C, H, W = x.shape
     N = wf.shape[1]
     xp = F.pad(x, (1, 1, 1, 1))                         # TMA zero-fills out-of-image source pixels
@@ -23,7 +23,7 @@ def emulate_kernel(x, wf, bias):
             src = xp[:, :, 1 + dh:1 + dh + H, 1 + dw:1 + dw + W]
             wt = wf[par].float()[:, t * C:(t + 1) * C]  # [N, C]
             acc += torch.einsum("bchw,nc->bnhw", src, wt)
-        out[:, :, py::2, px::2] = acc + bias[None, :, None, None]     # interleave2x2: out[b, 2y+py, 2x+px]
+        out[:, :, py::2, px::2] = acc + bias[None, :, None, None]     # out[b, 2y+py, 2x+px]
     return out
 
 
@@ -50,11 +50,9 @@ def test_folded_weights_reproduce_upsample_then_conv(B, C, N, H, W):
     assert (wf.float() - wf_exact).abs().max() <= 8e-3 * wf_exact.abs().max() + 1e-6
 
 
-def test_fold_switch(monkeypatch):
+def test_fold_rule():
+    """fold where the source grid fills the machine (>= 2048 pixels) and the output channels suit the interleaved TMA store"""
     from lib.model_zoo.diffusion_utils import upsample_fold_enabled
-    monkeypatch.setenv("VDB_UPFOLD", "0")
-    assert not upsample_fold_enabled(1 << 20)
-    monkeypatch.delenv("VDB_UPFOLD", raising=False)          # default since round 2: on for grids that fill the machine
-    assert upsample_fold_enabled(4096) and not upsample_fold_enabled(512)
-    monkeypatch.setenv("VDB_UPFOLD", "1")
-    assert upsample_fold_enabled(4096) and not upsample_fold_enabled(512)
+    assert upsample_fold_enabled(4096, 320) and upsample_fold_enabled(2048, 32)
+    assert not upsample_fold_enabled(512, 320) and not upsample_fold_enabled(2047, 320)
+    assert not upsample_fold_enabled(4096, 48) and not upsample_fold_enabled(1 << 20, 3)

@@ -293,9 +293,7 @@ static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t strea
   static bool configured = false;
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    if (TMA_WARP)
-      prefer_max_smem(kernel);
-    else   // the second CTA per SM is the point of this form: ask for the whole carveout, not the driver's pick
+    if (!TMA_WARP)   // the second CTA per SM is the point of this form: ask for the whole carveout, not the driver's pick
       VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }

@@ -1149,27 +1149,6 @@ __global__ void resample_v_crop_norm_kernel(const uint8_t* __restrict__ x, int n
   }
 }
 
-// [4 parities (py, px)][B, H, W, C] bf16 -> [B, 2H, 2W, C]: out[b, 2y+py, 2x+px, :] = src[py*2+px][b, y, x, :]
-// (assembles the four parity sub-lattices produced by the folded-upsample conv modes)
-__global__ void interleave2x2_kernel(const __nv_bfloat16* __restrict__ src, int B, int H, int W, int C,
-                                     __nv_bfloat16* __restrict__ y) {
-  const int V = C / 8;
-  const long long per = static_cast<long long>(B) * H * W * V;      // vectors per parity tensor
-  const long long total = 4 * per;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    // iterate in OUTPUT order so that the stores are fully coalesced
-    const int v = static_cast<int>(i % V);
-    long long p = i / V;
-    const int xo = static_cast<int>(p % (2 * W)); p /= 2 * W;
-    const int yo = static_cast<int>(p % (2 * H));
-    const long long b = p / (2 * H);
-    const int par = (yo & 1) * 2 + (xo & 1);
-    const long long sidx = par * per + ((b * H + (yo >> 1)) * W + (xo >> 1)) * V + v;
-    reinterpret_cast<uint4*>(y)[i] = __ldg(reinterpret_cast<const uint4*>(src) + sidx);
-  }
-}
-
 // nearest-neighbour 2x upsample of NHWC bf16           (openaimodel.py:114, autokl_modules.py:54)
 __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ x, int B, int H, int W, int C,
                                   __nv_bfloat16* __restrict__ y) {
@@ -1387,127 +1366,6 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const float* __restri
   }
 }
 
-// ---------------------------------------------------------------------------------------------
-// Skinny GEMM on the CUDA cores for a SMALL operand of <= 64 rows (the 0-D diffuser: M = 8 FCBlock / Linear_MultiDim GEMMs that
-// stream 3.4 GB of weights per evaluation, and the 32-row projections of its context blocks).  On the tensor-core kernel these
-// launches are a latency chain (tensor-map fetch -> TMA -> MMA -> epilogue, plus a split-K reduction launch): 6-10 us
-// for 3 MB of weights.  Here the small operand lives in shared memory (bf16, whole K), every warp streams RW rows of the BIG
-// operand with 16-byte loads (lanes split K) and keeps RW x S fp32 accumulators; one shuffle reduction per row group.
-//   small = [S, K1 (+K2)] bf16 rows (two sources concatenated along K), big = [R, K] bf16 rows
-//   transpose_out 0: out[s, r] = dot + bias[s * bias_bstride + r] + resid[s, r]   (small = activations, big = weights)
-//   transpose_out 1: out[r, s] = dot                                                (small = tokens, big = weights: V^T projection)
-// ---------------------------------------------------------------------------------------------
-template <int S, int RW>
-__global__ void __launch_bounds__(256) gemm_skinny_kernel(const __nv_bfloat16* __restrict__ sm1, int K1, long long lds1,
-                                                          const __nv_bfloat16* __restrict__ sm2, int K2, long long lds2, int Srows,
-                                                          const __nv_bfloat16* __restrict__ big, long long R, long long ldb,
-                                                          const float* __restrict__ bias, long long bias_bstride,
-                                                          const __nv_bfloat16* __restrict__ resid, long long ldr,
-                                                          __nv_bfloat16* __restrict__ out, long long ldo, int transpose_out) {
-  extern __shared__ __align__(16) uint8_t skinny_smem[];
-  const int K = K1 + K2;
-  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(skinny_smem);   // [S][K], rows >= Srows zero
-  {
-    // stage the small operand: 8 independent 16-byte loads in flight per thread (a one-load-per-iteration loop is a chain of L2
-    // round trips: 20 of them for 80 KB made this stage cost more than the whole GEMM, first GPU run of this kernel: 30 us per launch)
-    const int vec_per_row = K >> 3;
-    const int nvec = S * vec_per_row;
-    for (int i0 = threadIdx.x; i0 < nvec; i0 += blockDim.x * 8) {
-      uint4 v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int i = i0 + u * blockDim.x;
-        v[u] = make_uint4(0u, 0u, 0u, 0u);
-        if (i < nvec) {
-          const int srow = i / vec_per_row, kv = (i - srow * vec_per_row) << 3;
-          if (srow < Srows)
-            v[u] = (kv < K1) ? __ldg(reinterpret_cast<const uint4*>(sm1 + srow * lds1 + kv))
-                             : __ldg(reinterpret_cast<const uint4*>(sm2 + srow * lds2 + (kv - K1)));
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int i = i0 + u * blockDim.x;
-        if (i < nvec) {
-          const int srow = i / vec_per_row, kv = (i - srow * vec_per_row) << 3;
-          *reinterpret_cast<uint4*>(xs + static_cast<size_t>(srow) * K + kv) = v[u];
-        }
-      }
-    }
-  }
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nwarps = blockDim.x >> 5;
-  const uint32_t xs_s = smem_u32(xs);
-  for (long long r0 = (static_cast<long long>(blockIdx.x) * nwarps + warp) * RW; r0 < R;
-       r0 += static_cast<long long>(gridDim.x) * nwarps * RW) {
-    float acc[RW][S];
-#pragma unroll
-    for (int r = 0; r < RW; ++r)
-#pragma unroll
-      for (int q = 0; q < S; ++q) acc[r][q] = 0.f;
-    // the next k-vector of every row is requested before the current one is multiplied (two loads per row in flight: with
-    // 8-16 warps per SM a single one leaves the HBM pipe two thirds empty on the 50-150 MB weight streams)
-    uint4 nxt[RW];
-    auto fetch = [&](int k) {
-#pragma unroll
-      for (int r = 0; r < RW; ++r) {
-        nxt[r] = make_uint4(0u, 0u, 0u, 0u);
-        if (k < K && r0 + r < R) nxt[r] = __ldg(reinterpret_cast<const uint4*>(big + (r0 + r) * ldb + k));
-      }
-    };
-    fetch(lane * 8);
-    for (int k = lane * 8; k < K; k += 256) {
-      float w[RW][8];
-      uint4 cur[RW];
-#pragma unroll
-      for (int r = 0; r < RW; ++r) cur[r] = nxt[r];
-      fetch(k + 256);
-#pragma unroll
-      for (int r = 0; r < RW; ++r) {
-        const uint4 u = cur[r];
-        const uint32_t uu[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) { const float2 t = unpack_bf16x2(uu[q]); w[r][2 * q] = t.x; w[r][2 * q + 1] = t.y; }
-      }
-#pragma unroll
-      for (int q = 0; q < S; ++q) {
-        uint4 xv;
-        asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(xv.x), "=r"(xv.y), "=r"(xv.z), "=r"(xv.w)
-                     : "r"(xs_s + static_cast<uint32_t>((q * K + k) * 2)));
-        const uint32_t xu[4] = {xv.x, xv.y, xv.z, xv.w};
-        float xf[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { const float2 t = unpack_bf16x2(xu[i]); xf[2 * i] = t.x; xf[2 * i + 1] = t.y; }
-#pragma unroll
-        for (int r = 0; r < RW; ++r)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[r][q] = fmaf(w[r][i], xf[i], acc[r][q]);
-      }
-    }
-    // reduce over the 32 lanes; lane (r * S + q) % 32 keeps result (r, q)
-#pragma unroll
-    for (int r = 0; r < RW; ++r) {
-#pragma unroll
-      for (int q = 0; q < S; ++q) {
-        float v = acc[r][q];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == ((r * S + q) & 31) && q < Srows && r0 + r < R) {
-          const long long row = r0 + r;
-          if (transpose_out) {
-            out[row * ldo + q] = __float2bfloat16(v);
-          } else {
-            if (bias) v += __ldg(bias + q * bias_bstride + row);
-            if (resid) v += __bfloat162float(resid[q * ldr + row]);
-            out[q * ldo + row] = __float2bfloat16(v);
-          }
-        }
-      }
-    }
-  }
-}
-
 // row softmax over [rows, n] bf16 with scale, fp32 math, bf16 out (VAE AttnBlock, autokl_modules.py:186-188)
 __global__ void __launch_bounds__(256) softmax_rows_kernel(const __nv_bfloat16* __restrict__ x, long long rows,
                                                            int n, long long ld, float scale,
@@ -1715,30 +1573,6 @@ static int ew_blocks(long long work_items, int threads) {
 
 using namespace vdb;
 
-namespace vdb {
-template <int S, int RW>
-static int launch_gemm_skinny(const void* sm1, int K1, long long lds1, const void* sm2, int K2, long long lds2, int Srows,
-                              const void* big, long long R, long long ldb, const float* bias, long long bias_bstride,
-                              const void* resid, long long ldr, void* out, long long ldo, int transpose_out, cudaStream_t st) {
-  const size_t smem = static_cast<size_t>(S) * (K1 + K2) * 2;
-  static size_t configured = 0;
-  if (smem > configured) {
-    VDB_CUDA_CHECK(cudaFuncSetAttribute(gemm_skinny_kernel<S, RW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    configured = 200 * 1024;
-  }
-  const long long groups = (R + RW - 1) / RW;                       // one warp per group of RW rows
-  const int blocks = static_cast<int>(std::min<long long>((groups + 7) / 8, static_cast<long long>(num_sms()) * (smem > 100 * 1024 ? 1 : 2)));
-  gemm_skinny_kernel<S, RW><<<blocks, 256, smem, st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(sm1), K1, lds1, reinterpret_cast<const __nv_bfloat16*>(sm2), K2, lds2, Srows,
-      reinterpret_cast<const __nv_bfloat16*>(big), R, ldb, bias, bias_bstride, reinterpret_cast<const __nv_bfloat16*>(resid), ldr,
-      reinterpret_cast<__nv_bfloat16*>(out), ldo, transpose_out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
-}
-
-}  // namespace vdb
-
 extern "C" {
 
 int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* noise,
@@ -1750,7 +1584,6 @@ int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x
        reinterpret_cast<uintptr_t>(x_prev_dup)) & 15)
     return set_error(VDB_ERR_INVALID, "ddim_cfg_step: pointers must be 16-byte aligned");
   const int threads = 256;
-  VDB_PREFER_MAX_SMEM(ddim_cfg_step_kernel);
   ddim_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       e_uncond, e_cond, x, noise, coef, step_idx, scale, temperature, x_prev, x_prev_dup, pred_x0, n);
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -1774,7 +1607,6 @@ int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* 
     if (p && lo < h_hi && h_lo < hi) return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: hist overlaps x, x_next, x_next_dup or pred_x0");
   }
   const int threads = 256;
-  VDB_PREFER_MAX_SMEM(dpmpp_cfg_step_kernel);
   dpmpp_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n);
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -1859,7 +1691,6 @@ int vdb_lincomb4_f32(const float* x0, const float* x1, const float* x2, const fl
 
 int vdb_add_int(int* p, int delta, void* stream) {
   if (!p) return set_error(VDB_ERR_INVALID, "add_int: null");
-  VDB_PREFER_MAX_SMEM(add_int_kernel);
   add_int_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, delta);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
@@ -1902,9 +1733,8 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
     return set_error(VDB_ERR_UNSUPPORTED, "groupnorm: need 32 groups, C %% 32 == 0, C/8 <= 512 (C=%d)", C);
   if (!x2) C2 = 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // group-bundle kernel (default; VDB_GN_BUNDLE=0 turns it off): see gn_bundle_kernel
-  static const bool bundle_ok = [] { const char* ev = getenv("VDB_GN_BUNDLE"); return !(ev && ev[0] == '0'); }();
-  if (bundle_ok && groups == 32) {
+  // group-bundle kernel: see gn_bundle_kernel
+  if (groups == 32) {
     const int cpg = C / groups;
     int G = 1;
     while (G <= 4 && ((G * cpg) % 8)) G *= 2;
@@ -1931,9 +1761,7 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       // a 4096-pixel C = 320 layer is ONE wave of 128 CTAs (2-CTA clusters) — with 512-thread register-resident CTAs it needs
       // 8-CTA clusters = 512 CTAs = 1.7 waves of the 296 resident slots (18 us measured) — and the C = 960 / 1920 concat
       // layers that fit neither variant before no longer fall back to the pixel-range kernel
-      // (VDB_GN_BIG=0 turns this off)
-      static const bool big_ok = [] { const char* ev = getenv("VDB_GN_BIG"); return !(ev && ev[0] == '0'); }();
-      if (big_ok && static_cast<long long>(HW) * B >= 16384) {
+      if (static_cast<long long>(HW) * B >= 16384) {
         for (int S = 1; S <= 8; S *= 2) {
           if (static_cast<long long>(groups / G) * S * B > 4LL * num_sms()) break;   // (at most ~4 waves of one CTA per SM)
           if (nper_t(1024, S) <= 11) {
@@ -1959,21 +1787,18 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       if (n <= 12) return launch(gn_bundle_kernel<12, 512>, 12, 512, S);
     }
   }
-  static const bool fused_ok = [] { const char* ev = getenv("VDB_GN_FUSED"); return !(ev && ev[0] == '0'); }();
-  // register-resident variant for the small layers (VDB_GN_REG=0 turns it off)
-  static const bool reg_ok = [] { const char* ev = getenv("VDB_GN_REG"); return !(ev && ev[0] == '0'); }();
   // every CTA of the single-launch kernel must be resident: ask the runtime how many fit (registers / shared memory)
   static const int occ0 = [] { int n = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gn_fused_kernel<0>, kGnThreads, 0); return n; }();
   static const int occ4 = [] { int n = 0; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, gn_fused_kernel<4>, kGnThreads, 0); return n; }();
   const int max_resident = std::min(2, std::min(occ0, occ4)) * num_sms();   // (the scratch is sized for 2 CTAs / SM)
-  if (fused_ok && max_resident >= B && C <= 3072) {   // (shared-memory plan of the single-launch kernel)
+  if (max_resident >= B && C <= 3072) {   // (shared-memory plan of the single-launch kernel)
     const int max_ns = max_resident / B;
     const int lanes = kGnThreads / (C / 8);
     const int ns4 = (HW + 4 * lanes - 1) / (4 * lanes);   // splits needed for <= 4 pixels per thread
     const __nv_bfloat16* x1b = reinterpret_cast<const __nv_bfloat16*>(x1);
     const __nv_bfloat16* x2b = reinterpret_cast<const __nv_bfloat16*>(x2);
     __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(y);
-    if (reg_ok && ns4 <= max_ns) {
+    if (ns4 <= max_ns) {   // register-resident variant for the small layers
       const int ns = std::max(1, std::min(max_ns, std::max(ns4, (HW + 7) / 8)));
       set_norm_plan(2, 4, 0, 0, 0, ns, dim3(ns, B));
       VDB_CUDA_CHECK(launch_pdl(gn_fused_kernel<4>, dim3(ns, B), dim3(kGnThreads), 0, st, x1b, C1, x2b, C2, HW, groups, eps,
@@ -1988,8 +1813,6 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
     return VDB_OK;
   }
   const int nsplit = vdb_groupnorm_nsplit(B, HW);
-  VDB_PREFER_MAX_SMEM(gn_stats_kernel);
-  VDB_PREFER_MAX_SMEM(gn_apply_kernel);
   set_norm_plan(3, 0, 0, 0, 0, nsplit, dim3(nsplit, B));
   VDB_CUDA_CHECK(launch_pdl(gn_stats_kernel, dim3(nsplit, B), dim3(kGnThreads), 0, st,
                             reinterpret_cast<const __nv_bfloat16*>(x1), C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2,
@@ -2016,35 +1839,29 @@ int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, cons
   const int blocks = static_cast<int>(std::min<long long>((rows + 8 * R - 1) / (8 * R), num_sms() * 8LL));
   const __nv_bfloat16* xp = reinterpret_cast<const __nv_bfloat16*>(x);
   __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(y);
-  // row-group kernel (default; VDB_LN_RG=0 falls back to the warp-per-row kernels): C = 8 * VPL * LPR
-  static const bool ln_rg = [] { const char* ev = getenv("VDB_LN_RG"); return !(ev && ev[0] == '0'); }();
-  if (ln_rg) {
-    auto launch_rg = [&](auto kernel, int vpl, int rpw) -> int {
-      int occ = 0;
-      const size_t smem = 2 * static_cast<size_t>(C) * sizeof(float);
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1) occ = 1;
-      const long long steps = (rows + rpw - 1) / rpw;                         // warp steps
-      const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>((steps + 7) / 8, static_cast<long long>(occ) * num_sms())));
-      set_norm_plan(4, vpl, 32 / rpw, 0, 0, 0, dim3(grid));
-      VDB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(threads), smem, st, xp, rows, C, gamma, beta, eps, yp));
-      count_launch();
-      return VDB_OK;
-    };
-    switch (V) {
-      case 40: return launch_rg(layernorm_rg_kernel<5, 8>, 5, 4);      // C 320
-      case 80: return launch_rg(layernorm_rg_kernel<5, 16>, 5, 2);     // C 640
-      case 160: return launch_rg(layernorm_rg_kernel<5, 32>, 5, 1);    // C 1280
-      case 96: return launch_rg(layernorm_rg_kernel<3, 32>, 3, 1);     // C 768  (CLIP text)
-      case 128: return launch_rg(layernorm_rg_kernel<4, 32>, 4, 1);    // C 1024 (CLIP vision)
-      case 8: return launch_rg(layernorm_rg_kernel<1, 8>, 1, 4);       // C 64   (reduced-width test nets)
-      case 16: return launch_rg(layernorm_rg_kernel<2, 8>, 2, 4);      // C 128
-      case 32: return launch_rg(layernorm_rg_kernel<4, 8>, 4, 4);      // C 256
-      default: break;
-    }
+  // row-group kernel where C = 8 * VPL * LPR has an instantiation, else the warp-per-row kernels
+  auto launch_rg = [&](auto kernel, int vpl, int rpw) -> int {
+    int occ = 0;
+    const size_t smem = 2 * static_cast<size_t>(C) * sizeof(float);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) != cudaSuccess || occ < 1) occ = 1;
+    const long long steps = (rows + rpw - 1) / rpw;                         // warp steps
+    const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>((steps + 7) / 8, static_cast<long long>(occ) * num_sms())));
+    set_norm_plan(4, vpl, 32 / rpw, 0, 0, 0, dim3(grid));
+    VDB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(threads), smem, st, xp, rows, C, gamma, beta, eps, yp));
+    count_launch();
+    return VDB_OK;
+  };
+  switch (V) {
+    case 40: return launch_rg(layernorm_rg_kernel<5, 8>, 5, 4);      // C 320
+    case 80: return launch_rg(layernorm_rg_kernel<5, 16>, 5, 2);     // C 640
+    case 160: return launch_rg(layernorm_rg_kernel<5, 32>, 5, 1);    // C 1280
+    case 96: return launch_rg(layernorm_rg_kernel<3, 32>, 3, 1);     // C 768  (CLIP text)
+    case 128: return launch_rg(layernorm_rg_kernel<4, 32>, 4, 1);    // C 1024 (CLIP vision)
+    case 8: return launch_rg(layernorm_rg_kernel<1, 8>, 1, 4);       // C 64   (reduced-width test nets)
+    case 16: return launch_rg(layernorm_rg_kernel<2, 8>, 2, 4);      // C 128
+    case 32: return launch_rg(layernorm_rg_kernel<4, 8>, 4, 4);      // C 256
+    default: break;
   }
-  VDB_PREFER_MAX_SMEM((layernorm_kernel<2, 4>));
-  VDB_PREFER_MAX_SMEM((layernorm_kernel<5, 2>));
-  VDB_PREFER_MAX_SMEM((layernorm_kernel<8, 1>));
   set_norm_plan(5, V <= 64 ? 2 : (V <= 160 ? 5 : 8), R, 0, 0, 0, dim3(blocks));
   if (V <= 64)
     VDB_CUDA_CHECK(launch_pdl(layernorm_kernel<2, 4>, dim3(blocks), dim3(threads), 0, st, xp, rows, C, gamma, beta, eps, yp));
@@ -2098,7 +1915,6 @@ int vdb_pad_heads(const float* w, int H, int d, int dpad, int K, void* out, void
 int vdb_upsample2x_nhwc(const void* x, int B, int H, int W, int C, void* y, void* stream) {
   if (!x || !y || (C % 8)) return set_error(VDB_ERR_INVALID, "upsample2x: null argument or C %% 8 != 0");
   const long long total = static_cast<long long>(B) * 4 * H * W * (C / 8);
-  VDB_PREFER_MAX_SMEM(upsample2x_kernel);
   upsample2x_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const __nv_bfloat16*>(x), B, H, W, C, reinterpret_cast<__nv_bfloat16*>(y));
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -2139,21 +1955,10 @@ int vdb_resample_v_crop_norm(const void* x, int n, int Hin, int W, const int* bo
   return VDB_OK;
 }
 
-int vdb_interleave2x2_nhwc(const void* src, int B, int H, int W, int C, void* y, void* stream) {
-  if (!src || !y || B <= 0 || H <= 0 || W <= 0 || (C % 8)) return set_error(VDB_ERR_INVALID, "interleave2x2: null argument or C %% 8 != 0");
-  const long long total = static_cast<long long>(B) * 4 * H * W * (C / 8);
-  interleave2x2_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(src), B, H, W, C, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
-}
-
 int vdb_im2col3x3_small(const float* x, int B, int H, int W, int Cin, int Kpad, float in_scale, float in_shift,
                         void* y, void* stream) {
   if (!x || !y || 9 * Cin > Kpad || (Kpad % 8)) return set_error(VDB_ERR_INVALID, "im2col3x3_small: bad argument");
   const long long total = static_cast<long long>(B) * H * W * (Kpad / 8);
-  VDB_PREFER_MAX_SMEM(im2col3x3_small_kernel);
   im2col3x3_small_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, B, H, W, Cin, Kpad, in_scale, in_shift, reinterpret_cast<__nv_bfloat16*>(y));
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -2165,7 +1970,6 @@ int vdb_permute_f32(const float* x, int B, int C, long long HW, int to_nhwc, flo
                     float* y, void* stream) {
   if (!x || !y) return set_error(VDB_ERR_INVALID, "permute_f32: null argument");
   const long long total = static_cast<long long>(B) * C * HW;
-  VDB_PREFER_MAX_SMEM(permute_f32_kernel);
   permute_f32_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       x, B, C, static_cast<int>(HW), to_nhwc, mul, add, clamp01, y);
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -2214,7 +2018,6 @@ int vdb_cast_bf16_f32(const void* x, float* y, long long n, void* stream) {
 int vdb_timestep_embedding(const long long* ts, const int* step_idx, int B, int dim, float neg_log_period, float* out,
                            void* stream) {
   if (!ts || !out || B <= 0 || dim <= 1) return set_error(VDB_ERR_INVALID, "timestep_embedding: bad argument");
-  VDB_PREFER_MAX_SMEM(timestep_embedding_kernel);
   timestep_embedding_kernel<<<ew_blocks(static_cast<long long>(B) * (dim / 2), 128), 128, 0,
                               reinterpret_cast<cudaStream_t>(stream)>>>(ts, step_idx, B, dim, neg_log_period, out);
   VDB_CUDA_CHECK(cudaGetLastError());
@@ -2230,7 +2033,6 @@ int vdb_linear_small(const float* x, int M, int K, const void* Wt, int N, const 
   static bool configured = false;
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(linear_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    prefer_max_smem(linear_small_kernel);
     configured = true;
   }
   const int blocks = std::min((N + 31) / 32, num_sms() * 2);
@@ -2239,25 +2041,6 @@ int vdb_linear_small(const float* x, int M, int K, const void* Wt, int N, const 
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;
-}
-
-int vdb_gemm_skinny_fits(int S, long long K) { return S >= 1 && S <= 64 && K > 0 && (K % 8) == 0 && ((S <= 8 ? 8 : S <= 16 ? 16 : S <= 32 ? 32 : 64) * K * 2 <= 200 * 1024) ? 1 : 0; }
-
-int vdb_gemm_skinny_bf16(const void* small1, int S, long long K1, long long lds1, const void* small2, long long K2, long long lds2,
-                         const void* big, long long R, long long ldb, const float* bias, long long bias_bstride,
-                         const void* resid, long long ldr, void* out, long long ldo, int transpose_out, void* stream) {
-  if (!small1 || !big || !out || S <= 0 || R <= 0 || K1 <= 0) return set_error(VDB_ERR_INVALID, "gemm_skinny: null/empty argument");
-  const long long K = K1 + (small2 ? K2 : 0);
-  if ((K1 % 8) || (small2 && (K2 % 8)) || (lds1 % 8) || (small2 && (lds2 % 8)) || (ldb % 8))
-    return set_error(VDB_ERR_INVALID, "gemm_skinny: K and leading dimensions must be multiples of 8");
-  if (!vdb_gemm_skinny_fits(S, K)) return set_error(VDB_ERR_UNSUPPORTED, "gemm_skinny: %d rows x K %lld do not fit shared memory (use vdb_gemm_bf16)", S, K);
-  if (transpose_out && (bias || resid)) return set_error(VDB_ERR_UNSUPPORTED, "gemm_skinny: transposed output takes no bias / residual");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int k1 = static_cast<int>(K1), k2 = small2 ? static_cast<int>(K2) : 0;
-  if (S <= 8) return launch_gemm_skinny<8, 4>(small1, k1, lds1, small2, k2, lds2, S, big, R, ldb, bias, bias_bstride, resid, ldr, out, ldo, transpose_out, st);
-  if (S <= 16) return launch_gemm_skinny<16, 4>(small1, k1, lds1, small2, k2, lds2, S, big, R, ldb, bias, bias_bstride, resid, ldr, out, ldo, transpose_out, st);
-  if (S <= 32) return launch_gemm_skinny<32, 2>(small1, k1, lds1, small2, k2, lds2, S, big, R, ldb, bias, bias_bstride, resid, ldr, out, ldo, transpose_out, st);
-  return launch_gemm_skinny<64, 1>(small1, k1, lds1, small2, k2, lds2, S, big, R, ldb, bias, bias_bstride, resid, ldr, out, ldo, transpose_out, st);
 }
 
 int vdb_clip_text_embed(const long long* tokens, const float* tok_emb, const float* pos_emb, int B, int L, int Lp, int C,

@@ -34,21 +34,6 @@ int make_tmap_4d_sw64(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1,
                       uint64_t stride1, uint64_t stride2, uint64_t stride3, uint32_t box0, uint32_t box1,
                       uint32_t box2, uint32_t box3);   // SWIZZLE_64B (epilogue store tiles: 64-byte rows)
 
-// Ask for the maximum shared-memory carveout for a kernel (once).  The tensor-core kernels need up to 227 KB of shared memory;
-// if the small kernels between them ran with a different L1/shared split the SMs would have to be reconfigured (which
-// needs them idle) at every transition of the ~470-kernel step.  Measured: no effect on the step time, so this is
-// opt-in (VDB_CARVEOUT=1).
-template <typename K>
-inline void prefer_max_smem(K kernel) {
-  static const bool on = [] { const char* e = getenv("VDB_CARVEOUT"); return e && e[0] == '1'; }();   // measured neutral: opt-in
-  if (on) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-}
-#define VDB_PREFER_MAX_SMEM(kernel)              \
-  do {                                           \
-    static bool _done = false;                   \
-    if (!_done) { ::vdb::prefer_max_smem(kernel); _done = true; } \
-  } while (0)
-
 // Launch with the programmatic-stream-serialization attribute: the kernel's prologue may overlap the tail of
 // the previous kernel in the stream; every kernel launched this way calls pdl_wait() before reading its inputs.
 template <typename... KArgs, typename... Args>

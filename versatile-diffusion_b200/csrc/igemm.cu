@@ -71,11 +71,8 @@ struct alignas(64) IgemmParams {
   const float* ln_rowbias;    // on_cols 1: [M] beta-term of the output row (null = 0); on_cols 0 the beta term lives in `bias`
   float* stats_out;           // mode 7: [2 * tilesN][M][2] fp32: (sum, sum of squares) over the even (slot 2n) and the odd
                               // (slot 2n + 1) 32-column chunks of N tile n, for every OUTPUT row
-  int epi_alt;                // 1: the two warps of a 32-row quarter swap chunk parity every tile (odd chunk counts)
-  int nfast;                  // 1: N is the fast tile index (tile t -> n = t % tilesN, m = t / tilesN); needs ksplit == 1
   unsigned long long* timeline; // debug: per-tile role timestamps of CTA 0 (null = off)
   unsigned smem_bytes;        // dynamic shared memory of the launch (LN modes check their carve-up against it)
-  int chunked;                // 1: every CTA walks a contiguous range of tiles instead of a grid-strided one
 };
 
 enum { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU = 2, ACT_QGELU = 3, ACT_GEGLU = 4 };
@@ -98,10 +95,9 @@ VDB_DEVINL float apply_act(float v, int act) {
 }
 
 // MODE selects the epilogue that is compiled in: 0 = every path (split-K partials, GEGLU, fp32 / ragged / per-row-bias
-// tiles), 1 = only the bf16 fast path (act none, alpha 1, N % 32 == 0, one bias row per tile) with the residual of the
-// NEXT chunk prefetched, 2 = only GEGLU.  Keeping the rarely used paths out of the common instantiations keeps the
-// epilogue's instruction footprint small.
-// Modes 3 / 4 are modes 1 / 2 with the tile leaving through shared memory + TMA stores.  Modes 5 / 6 are modes 3 / 4 for a GEMM whose
+// tiles), 3 = only the bf16 fast path (act none, alpha 1, N % 32 == 0, one bias row per tile), 4 = only GEGLU, both with the
+// tile leaving through shared memory + TMA stores.  Keeping the rarely used paths out of the common instantiations keeps the
+// epilogue's instruction footprint small.  Modes 5 / 6 are modes 3 / 4 for a GEMM whose
 // input is a LayerNorm: the operand is the RAW activation x and the weights carry gamma (W' = W * gamma), so with the row's mean mu
 // and rstd r       LN(x) W^T + b  =  r * (x W'^T  -  mu * s) + c,     s[n] = sum_k W'[n,k],  c[n] = sum_k beta_k W[n,k] + b[n]
 // is a rank-1 correction in the epilogue (2 FMAs per element) — the normalised tensor is never written or read.  mu and r come
@@ -114,8 +110,8 @@ VDB_DEVINL float apply_act(float v, int act) {
 // 32-column chunks, staging each as a 16 x 32 bf16 box (stmatrix) for a TMA store.  The warpgroups do not wait for each other
 // after the mainloop, and the producer is gated by the empty barriers alone: it loads the next tile's first STAGES k-blocks while
 // the epilogue runs, so the next mainloop starts on a full ring.  tests/test_igemm_protocol_tma_epi.py models this protocol.
-// Modes 0-2 park the accumulator in shared memory (sacc, [128][BN + 4] fp32, aliasing the operand ring) after the mainloop and
-// run the epilogue on it: each warp reads 32-column chunks of one ROW per thread (acc_ld32), the layout those paths are written
+// Mode 0 parks the accumulator in shared memory (sacc, [128][BN + 4] fp32, aliasing the operand ring) after the mainloop and
+// runs the epilogue on it: each warp reads 32-column chunks of one ROW per thread (acc_ld32), the layout its paths are written
 // for.  The producer starts the next tile's loads once every consumer warp is done with sacc (acc_free;
 // tests/test_igemm_protocol.py).
 template <int BN, int STAGES, int EW, int MODE>
@@ -179,13 +175,8 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
   const int tilesM = p.tilesW * p.tilesH * p.tilesB;
   const int unitsM = tilesM;
   const int num_tiles = unitsM * p.tilesN * p.ksplit;
-  // Tile walk of this CTA (both roles use the same bounds): strided (tile c, c + grid, ...) or, p.chunked, a contiguous range.
-  // With M as the fast tile index a strided walk changes its N tile every unitsM / grid tiles and every change reloads the
-  // bias / LayerNorm tables behind two barriers; a contiguous range changes it once or twice per launch.
-  const int n_ctas = gridDim.x, cta_id = blockIdx.x;
-  const int per_cta = (num_tiles + n_ctas - 1) / n_ctas;
-  const int t_first = p.chunked ? cta_id * per_cta : cta_id, t_step = p.chunked ? 1 : n_ctas;
-  const int t_end = p.chunked ? min(num_tiles, t_first + per_cta) : num_tiles;
+  // Tile walk of this CTA (both roles use the same bounds): tiles c, c + grid, ..., with M as the fast tile index.
+  const int t_first = blockIdx.x, t_step = gridDim.x, t_end = num_tiles;
 
   if (warp == EW) {
     // ------------------------------ TMA producer ------------------------------
@@ -194,17 +185,11 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       const bool flat = (p.tilesH == 1) && (p.tilesB == 1);
       const int step_m = t_step % unitsM, step_r = t_step / unitsM;
       int unit_m = t_first % unitsM, rest = t_first / unitsM;
-      // N-fast order (opt-in): the N tiles of one M tile run on neighbouring CTAs at the same time, so an A operand larger
-      // than L2 is fetched from DRAM once instead of once per N tile
-      const int nf_step_n = p.nfast ? t_step % p.tilesN : 0, nf_step_m = p.nfast ? t_step / p.tilesN : 0;
-      int nf_n = p.nfast ? t_first % p.tilesN : 0, nf_m = p.nfast ? t_first / p.tilesN : 0;
       int it = 0;
       for (int t = t_first; t < t_end; t += t_step, ++it) {
-        const int m_idx = p.nfast ? nf_m : unit_m;
-        int n_idx = p.nfast ? nf_n : rest, ks = 0;
+        const int m_idx = unit_m;
+        int n_idx = rest, ks = 0;
         if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
-        nf_n += nf_step_n; nf_m += nf_step_m;
-        if (p.nfast && nf_n >= p.tilesN) { nf_n -= p.tilesN; ++nf_m; }
         int wt = m_idx, ht = 0, bt = 0;
         if (!flat) {
           wt = m_idx % p.tilesW;
@@ -219,7 +204,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         const int kb_begin = ks * p.kb_per_split;
         const int kb_end = min(p.kb_total, kb_begin + p.kb_per_split);
         int kb = 0;
-        // modes 0-2: the ring holds the previous tile's accumulator until its epilogue ends.  The TMA-store modes keep it in
+        // mode 0: the ring holds the previous tile's accumulator until its epilogue ends.  The TMA-store modes keep it in
         // registers, so only the empty barriers gate the ring and the next tile's first STAGES k-blocks load during the epilogue.
         if (!kTmaEpi && it > 0) mbar_wait(acc_free, (it - 1) & 1);
         VDB_TL(0, it);   // producer: starts issuing this tile
@@ -327,8 +312,6 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
     const bool flat = (p.tilesH == 1) && (p.tilesB == 1);   // GEMM view: M tiles along W only
     const int step_m = t_step % unitsM, step_r = t_step / unitsM;
     int unit_m = t_first % unitsM, rest = t_first / unitsM;
-    const int nf_step_n = p.nfast ? t_step % p.tilesN : 0, nf_step_m = p.nfast ? t_step / p.tilesN : 0;   // (see the producer)
-    int nf_n = p.nfast ? t_first % p.tilesN : 0, nf_m = p.nfast ? t_first / p.tilesN : 0;
     // TMA-store epilogues: the accumulator stays in the wgmma fragment layout, so warp w owns the 16 tile rows from e_row0 on
     // (warpgroup w / 4, quarter w % 4) and this thread rows e_row0 + lane / 4 and e_row0 + lane / 4 + 8, at columns
     // 8 j + 2 (lane % 4) + {0, 1}
@@ -358,11 +341,9 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t_first < t_end) ln_prefetch((t_first % unitsM) * kBlockM + e_row0 + (lane & 15));
     }
     for (int t = t_first; t < t_end; t += t_step, ++it) {
-      const int m_idx = p.nfast ? nf_m : unit_m;
-      int n_idx = p.nfast ? nf_n : rest, ks = 0;
+      const int m_idx = unit_m;
+      int n_idx = rest, ks = 0;
       if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
-      nf_n += nf_step_n; nf_m += nf_step_m;
-      if (p.nfast && nf_n >= p.tilesN) { nf_n -= p.tilesN; ++nf_m; }
       int wt = m_idx, ht = 0, bt = 0;
       if (!flat) {
         wt = m_idx % p.tilesW;
@@ -441,19 +422,8 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       const float* bias_g = (p.bias && !bias_uniform)
                                 ? p.bias + (p.bias_bstride ? static_cast<long long>(gp / p.rows_per_batch) * p.bias_bstride : 0) : nullptr;
 
-      // MODE 1: this warp's chunk range and the residual rows of its first chunk, requested BEFORE the accumulator wait
       const int f_nchunks = min(BN / 32, (p.N - n0) / 32);
       const bool has_resid = p.resid != nullptr;
-      const int f_first = (((BN / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half;
-      auto load_resid_fast = [&](int c, uint4 (&rr)[4]) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          if (ok_k[k]) rr[k] = __ldg(reinterpret_cast<const uint4*>(p.resid + static_cast<long long>(gp_k[k]) * p.ldr + n0 + c * 32 + tr_q * 8));
-      };
-      uint4 rr_first[4];
-      if constexpr (MODE == 1) {
-        if (has_resid && f_first < f_nchunks) load_resid_fast(f_first, rr_first);
-      }
 
       // TMA-store epilogues: output pixels (GEMM rows) of this thread's two accumulator rows
       int e_gp[2];
@@ -710,49 +680,6 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
                     make_float2(su, sq);
             }
         }
-      } else if constexpr (MODE == 1) {
-        // lean fast path: every chunk is a full 32-column bf16 chunk with one bias row; the residual rows of the
-        // next chunk are requested before this chunk is processed (their first use otherwise exposes ~1 us)
-        uint4 rr[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) rr[k] = rr_first[k];
-#pragma unroll 1
-        for (int c = f_first; c < f_nchunks; c += kWPQ) {
-          uint32_t v[32];
-          acc_ld32(c * 32, v);
-          uint4 rn[4];
-          if (has_resid && c + kWPQ < f_nchunks) load_resid_fast(c + kWPQ, rn);
-          stage_write(v);
-          __syncwarp();
-          float bb[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) bb[i] = p.bias ? sbias[c * 32 + tr_q * 8 + i] : 0.f;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float o[8];
-            stage_read(k, o);
-            if (ok_k[k]) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) o[i] += bb[i];
-              if (has_resid) {
-                const uint32_t w4[4] = {rr[k].x, rr[k].y, rr[k].z, rr[k].w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 x = unpack_bf16x2(w4[q]);
-                  o[2 * q] += x.x;
-                  o[2 * q + 1] += x.y;
-                }
-              }
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(gp_k[k]) * p.ldo + n0 + c * 32 + tr_q * 8) =
-                  make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-            }
-          }
-          __syncwarp();   // the staging tile is rewritten by this warp's next chunk
-#pragma unroll
-          for (int k = 0; k < 4; ++k) rr[k] = rn[k];
-        }
-      } else if constexpr (MODE == 2) {
-        geglu_tile();
       } else if (p.ksplit > 1) {
         // fp32 partials, reduced (+bias/act/residual) by splitk_reduce_kernel
         const long long Mtot = static_cast<long long>(p.Bo) * p.Ho * p.Wo;
@@ -860,7 +787,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         // this warp's chunks: half, half+2, ... (kept un-pipelined: double-buffering the 32-register accumulator chunk
         // pushed the kernel into spills and was measured slower)
         // chunk count not a multiple of the warps per quarter (BN = 160: five): rotate who takes the extra chunk
-        const int first = (p.epi_alt && ((BN / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half;
+        const int first = (((BN / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half;
 #pragma unroll 1
         for (int c = first; c < nchunks; c += kWPQ) {
           uint4 rr[4];
@@ -941,7 +868,6 @@ static int launch_igemm(const IgemmParams& p0, int num_units, cudaStream_t strea
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(igemm_kernel<BN, STAGES, EW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         static_cast<int>(smem)));
-    prefer_max_smem(igemm_kernel<BN, STAGES, EW, MODE>);
     configured = true;
   }
   const int grid = std::min(num_units, num_sms());
@@ -964,13 +890,13 @@ static int pick_bn(int N, int act, int forced) {
 
 static unsigned long long* g_timeline = nullptr;
 
-// The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN, nfast, chunked
-constexpr int kPlanFields = 9;
+// The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN
+constexpr int kPlanFields = 7;
 static thread_local int g_last_plan[kPlanFields] = {0};
 
-// The non-TMA epilogues store bf16 output rows and load residual rows as 16-byte vectors, and the split-K reduction stores fp32
-// rows as float4, so out / resid must be 16-byte aligned.  Checked before any tensor map is built: a misaligned `out` fails the
-// TMA-store map, and the launch would otherwise fall back to exactly those vector stores.
+// Mode 0 stores bf16 output rows and loads residual rows as 16-byte vectors, the split-K reduction stores fp32 rows as float4,
+// and the TMA-store epilogues need a 16-byte aligned output map, so out / resid must be 16-byte aligned.  Checked before any
+// tensor map is built, so that a bad pointer is reported as an argument error.
 static int check_epilogue_pointers(const void* out, long long ldo, int out_f32, const void* resid, long long ldr, const char* who) {
   if ((reinterpret_cast<uintptr_t>(out) & 15) || (resid && (reinterpret_cast<uintptr_t>(resid) & 15)))
     return set_error(VDB_ERR_INVALID, "%s: out and resid must be 16-byte aligned", who);
@@ -1013,12 +939,11 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   const bool ln_in = e.ln_stats != nullptr, st_out = e.stats_out != nullptr;
   if (ln_in || st_out) ksplit_forced = 1;               // the statistics ride on the single-pass TMA-store epilogues
   int BN = pick_bn(static_cast<int>(N), e.act, bn_forced);
-  // Tile-width model (round 2; VDB_BN_MODEL=0 restores the divisibility rule above): the persistent grid runs
+  // Tile-width model: the persistent grid runs
   // waves = ceil(tiles / #SMs) rounds of one tile per CTA, a tile costs kb * c(BN) cycles of mainloop (operand fill at ~90 B/clk
   // per SM or the MMA itself, whichever is longer) plus ~1500 cycles of pipeline fill / epilogue tail.  The divisibility rule sent
   // e.g. M 2048 x N 1280 x K 1280 (15 launches per step) to BN 256 = 80 tiles on 148 SMs; BN 160 gives 128 shorter tiles.
-  static const int bn_model = [] { const char* ev = getenv("VDB_BN_MODEL"); return (ev && ev[0] == '0') ? 0 : 1; }();
-  if (bn_model && !bn_forced && e.act != ACT_GEGLU && p.kb_total >= 8) {
+  if (!bn_forced && e.act != ACT_GEGLU && p.kb_total >= 8) {
     const long long tm = static_cast<long long>(p.tilesW) * p.tilesH * p.tilesB;
     const int cand[4] = {256, 160, 128, 64};
     double best = 1e30;
@@ -1035,13 +960,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
       const double cost = static_cast<double>(waves) * (kb_unit * per_kb + 1500.0) + (ks > 1 ? 12000.0 : 0.0);
       if (cost < best * 0.97) { best = cost; BN = c; }     // (prefer the wider tile unless the gain is clear)
     }
-  }
-  if (!bn_forced && !bn_model && e.act != ACT_GEGLU && p.kb_total < 32) {
-    // short K and a small MN grid (the 8x8 level): narrower tiles fill more SMs and need no split-K reduction pass
-    // (M 512, N 1280, K 1280: 10.7 us with BN 64 vs 18.1 us with BN 256 + split-K 2, tools/bn_sweep.py)
-    const int tm = p.tilesW * p.tilesH * p.tilesB;
-    auto tiles = [&](int bn) { return tm * static_cast<int>((N + bn - 1) / bn); };
-    while (BN > 64 && tiles(BN) * 2 <= num_sms()) BN = (BN == 256) ? 160 : (BN == 160 ? 128 : 64);
   }
   if (BN != 64 && BN != 128 && BN != 160 && BN != 256) return set_error(VDB_ERR_INVALID, "igemm: bad BN");
   if (e.act == ACT_GEGLU && (N % BN) != 0) return set_error(VDB_ERR_INVALID, "igemm: GEGLU needs N % 256 == 0");
@@ -1077,77 +995,53 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   p.ln_inv_dim = e.ln_dim > 0 ? 1.f / static_cast<float>(e.ln_dim) : 0.f; p.ln_eps = e.ln_eps;
   p.ln_colsum = e.ln_colsum; p.ln_rowbias = e.ln_rowbias; p.stats_out = e.stats_out;
   p.timeline = g_timeline;
-  static const int epi_alt = [] { const char* ev = getenv("VDB_EPI_ALT"); return (ev && ev[0] == '0') ? 0 : 1; }();
-  p.epi_alt = epi_alt;
-  // N-fast tile order (VDB_NFAST=1, opt-in until measured): only when every CTA keeps its N tile from one of its tiles to
-  // the next (grid % tilesN == 0: the bias tile cached in shared memory stays valid) and A is too big to survive in L2
-  // between two M sweeps (FF-out at the 64x64 level re-reads its 84 MB A operand)
-  static const int nfast_mode = [] { const char* ev = getenv("VDB_NFAST"); return ev ? atoi(ev) : 0; }();
-  {
-    const int grid = std::min(mn_tiles * p.ksplit, num_sms());
-    const double a_bytes = static_cast<double>(M) * static_cast<double>(Ktot) * 2.0;
-    p.nfast = (nfast_mode != 0 && p.ksplit == 1 && p.tilesN > 1 && (grid % p.tilesN) == 0 &&
-               (nfast_mode == 2 || a_bytes > 48e6) && !ln_in) ? 1 : 0;   // (the LN modes prefetch along the M-fast order)
-  }
-  // contiguous tile ranges (VDB_CHUNKED=1; default off) where the strided walk would change its N tile within a CTA's sequence
-  // more than a contiguous one does: several N tiles and a few tiles per CTA.  Measured neutral on every UNet shape: the table reloads it saves were not
-  // on the critical path.
-  {
-    static const int chunked_mode = [] { const char* ev = getenv("VDB_CHUNKED"); return ev ? atoi(ev) : 0; }();
-    const long long units = static_cast<long long>(tilesM) * p.tilesN * p.ksplit;
-    const int grid = static_cast<int>(std::min<long long>(units, num_sms()));
-    p.chunked = (chunked_mode != 0 && !p.nfast && p.ksplit == 1 && p.tilesN > 1 && units >= 3LL * grid) ? 1 : 0;
-  }
   int rc = make_tmap_2d(&p.tmB, Wt, static_cast<uint64_t>(Ktot), static_cast<uint64_t>(N),
                         static_cast<uint64_t>(ldw) * 2, kBlockK, BN);
   if (rc) return rc;
   const int num_tiles = mn_tiles * p.ksplit;
-  // epilogue specialisation (see igemm_kernel): 1 = plain bf16 fast path, 2 = GEGLU, 0 = everything else
-  static const int spec = [] { const char* ev = getenv("VDB_IGEMM_SPEC"); return (ev && ev[0] == '0') ? 0 : 1; }();
+  // epilogue specialisation (see igemm_kernel): 3 = plain bf16 fast path, 4 = GEGLU, 0 = everything else
   int mode = 0;
   // one bias row per tile: shared bias, or per-image rows with tiles that never straddle two images
   const bool one_bias_row = e.bias == nullptr || e.bias_bstride == 0 ||
                             (p.TB == 1 && (static_cast<long long>(p.Ho) * p.Wo == p.rows_per_batch ||
                                            (p.Ho == 1 && p.Bo == 1 && p.rows_per_batch % kBlockM == 0)));
-  if (spec && p.ksplit == 1 && !e.out_f32 && one_bias_row) {
-    if (e.act == ACT_GEGLU && BN == 256) mode = 2;
-    else if (e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0) mode = 1;
+  if (p.ksplit == 1 && !e.out_f32 && one_bias_row) {
+    if (e.act == ACT_GEGLU && BN == 256) mode = 4;
+    else if (e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0) mode = 3;
   }
-  // TMA-store epilogues (modes 3 / 4 = modes 1 / 2 with the output tile leaving through shared memory + cp.async.bulk.tensor;
-  // VDB_EPI_TMA=0 keeps the transposing epilogues): a warp's 16 rows x 32 columns must be one box of the output tensor map
-  static const int epi_tma = [] { const char* ev = getenv("VDB_EPI_TMA"); return (ev && ev[0] == '0') ? 0 : 1; }();
-  if (epi_tma && (mode == 1 || mode == 2) && (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 &&
-      (!e.resid || (reinterpret_cast<uintptr_t>(e.resid) & 15) == 0)) {
+  // modes 3 / 4 store the output tile through shared memory + cp.async.bulk.tensor: a warp's 16 rows x 32 columns are one box
+  // of the output tensor map (the M tile shapes hold at least 16 / (bw * bh) images; check_epilogue_pointers has checked the
+  // alignment of out / resid)
+  if (mode == 3 || mode == 4) {
     const int bw = std::min(p.TW, 16), bh = std::min(p.TH, 16 / bw), bb = 16 / (bw * bh);
-    const long long ncols = (mode == 2) ? N / 2 : N;
+    const long long ncols = (mode == 4) ? N / 2 : N;
     // out_parity >= 0: the same tile, written into every second pixel of every second row of the [B, 2Ho, 2Wo, N] tensor —
     // only the strides and the base of the output tensor map change, the kernel does not know
     const int py = e.out_parity >= 0 ? (e.out_parity >> 1) : 0, px = e.out_parity >= 0 ? (e.out_parity & 1) : 0;
     const uint64_t il = e.out_parity >= 0 ? 2 : 1;
     const void* obase = reinterpret_cast<const __nv_bfloat16*>(e.out) + (static_cast<long long>(py) * (il * p.Wo) + px) * e.ldo;
-    if (bb <= p.TB &&
-        make_tmap_4d_sw64(&p.tmO, obase, static_cast<uint64_t>(ncols), static_cast<uint64_t>(p.Wo), static_cast<uint64_t>(p.Ho),
-                          static_cast<uint64_t>(p.Bo), il * static_cast<uint64_t>(e.ldo) * 2,
-                          il * il * static_cast<uint64_t>(p.Wo) * e.ldo * 2,
-                          il * il * static_cast<uint64_t>(p.Ho) * p.Wo * e.ldo * 2, 32, bw, bh, bb) == 0)
-      mode += 2;
+    rc = make_tmap_4d_sw64(&p.tmO, obase, static_cast<uint64_t>(ncols), static_cast<uint64_t>(p.Wo), static_cast<uint64_t>(p.Ho),
+                           static_cast<uint64_t>(p.Bo), il * static_cast<uint64_t>(e.ldo) * 2,
+                           il * il * static_cast<uint64_t>(p.Wo) * e.ldo * 2,
+                           il * il * static_cast<uint64_t>(p.Ho) * p.Wo * e.ldo * 2, 32, bw, bh, bb);
+    if (rc) return rc;
   }
   if (e.out_parity >= 0 && mode != 3)
     return set_error(VDB_ERR_UNSUPPORTED, "igemm: the interleaved-output upsample modes need the TMA-store epilogue (bf16 out, no "
-                                          "activation, N %% 32 == 0, aligned out, VDB_EPI_TMA != 0)");
+                                          "activation, N %% 32 == 0)");
   if (ln_in || st_out) {
-    // folded LayerNorm: only on the TMA-store epilogues (bf16 out, act none / GEGLU, alpha 1, N % 32 == 0, aligned pointers)
+    // folded LayerNorm: only on the TMA-store epilogues (bf16 out, act none / GEGLU, alpha 1, N % 32 == 0)
     if (ln_in && st_out) return set_error(VDB_ERR_UNSUPPORTED, "igemm: a launch either consumes or produces LayerNorm statistics");
     if (mode != 3 && !(mode == 4 && ln_in))
       return set_error(VDB_ERR_UNSUPPORTED, "igemm: LayerNorm statistics need the TMA-store epilogue (bf16 out, no activation or "
-                                            "GEGLU, alpha 1, N %% 32 == 0, 16-byte aligned out / resid, VDB_EPI_TMA != 0)");
+                                            "GEGLU, alpha 1, N %% 32 == 0)");
     if (ln_in && e.resid) return set_error(VDB_ERR_UNSUPPORTED, "igemm: a folded-LayerNorm GEMM takes no residual");
     if (ln_in && mode == 4 && e.ln_on_cols) return set_error(VDB_ERR_UNSUPPORTED, "igemm: GEGLU with column statistics");
     mode = st_out ? 7 : mode + 2;
   }
   {
     const int stages = BN == 64 ? 8 : BN == 128 ? 6 : BN == 160 ? 5 : 4;   // (as instantiated below)
-    const int plan[kPlanFields] = {BN, stages, mode, p.ksplit, std::min(num_tiles, num_sms()), tilesM, p.tilesN, p.nfast, p.chunked};
+    const int plan[kPlanFields] = {BN, stages, mode, p.ksplit, std::min(num_tiles, num_sms()), tilesM, p.tilesN};
     for (int i = 0; i < kPlanFields; ++i) g_last_plan[i] = plan[i];
   }
   if (mode == 7) {
@@ -1175,15 +1069,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
       case 160: rc = launch_igemm<160, 5, 8, 3>(p, num_tiles, stream); break;
       default: rc = launch_igemm<256, 4, 8, 3>(p, num_tiles, stream); break;
     }
-  } else if (mode == 2) {
-    rc = launch_igemm<256, 4, 8, 2>(p, num_tiles, stream);
-  } else if (mode == 1) {
-    switch (BN) {
-      case 64: rc = launch_igemm<64, 8, 8, 1>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 6, 8, 1>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<160, 5, 8, 1>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<256, 4, 8, 1>(p, num_tiles, stream); break;
-    }
   } else {
     switch (BN) {
       case 64: rc = launch_igemm<64, 8, 8, 0>(p, num_tiles, stream); break;
@@ -1197,7 +1082,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     const long long total = M * (N / 4);
     const int threads = 256;
     const int blocks = static_cast<int>(std::min<long long>((total + threads - 1) / threads, num_sms() * 8LL));
-    VDB_PREFER_MAX_SMEM(splitk_reduce_kernel);
     VDB_CUDA_CHECK(launch_pdl(splitk_reduce_kernel, dim3(blocks), dim3(threads), 0, stream, (const float*)p.partial,
                               p.ksplit, M, static_cast<int>(N), p.bias, p.bias_bstride, p.rows_per_batch, p.resid,
                               p.ldr, p.out, p.ldo, p.out_f32, p.act, p.alpha));

@@ -6,12 +6,10 @@ Kernel schedule of one SpatialTransformer (x: [B,H,W,C] bf16):
   GN32(eps 1e-6) -> proj_in GEMM -> [LN -> fused q|k GEMM + V^T GEMM -> flash attention -> to_out GEMM(+resid)]
   -> [LN -> q GEMM (K, V^T of the context cached across DDIM steps) -> flash attention -> to_out GEMM(+resid)]
   -> LN -> GEGLU GEMM -> FF-out GEMM(+resid) -> proj_out GEMM (+ x_in, * mixing ratio)
-The three LayerNorms are not kernels (round 2, VDB_LN_FOLD=0 restores them): gamma is folded into the weights of the GEMMs that
+The three LayerNorms are not kernels where the token grid allows it (ln_fold_fits): gamma is folded into the weights of the GEMMs that
 consume the normalised tokens, mean / rstd arrive as per-32-channel partial sums written by the epilogue of the GEMM that PRODUCED
 the tokens (proj_in, the two to_out), and the consumer applies r * (x W'^T - mu * s) + c in its own epilogue (vdb_gemm_ln_bf16).
 """
-import os
-
 import torch
 from torch import nn
 
@@ -32,11 +30,10 @@ class PaddedContext(object):
         self.data, self.length = data, length
 
 
-def ln_fold_enabled():
-    """LayerNorm folded into the neighbouring GEMMs (default on; VDB_LN_FOLD=0: LayerNorm kernels).  Needs the TMA-store
-    epilogues (VDB_EPI_TMA != 0)."""
-    return os.environ.get("VDB_LN_FOLD", "1") != "0" and os.environ.get("VDB_EPI_TMA", "1") != "0" and \
-        os.environ.get("VDB_IGEMM_SPEC", "1") != "0"
+def ln_fold_fits(inner, B, H, W):
+    """LayerNorms folded into the neighbouring GEMMs need their TMA-store epilogues: inner % 32 == 0, and the B * H * W tokens
+    are the N of the V^T projection.  Other token grids run the LayerNorm kernels."""
+    return inner % 32 == 0 and (H * W) % 8 == 0 and (B * H * W) % 32 == 0
 
 
 def fold_layernorm(w, b, gamma, beta):
@@ -257,7 +254,7 @@ class BasicTransformerBlock(PackedModule):
     def _pack(self):
         out = {n: (f32(getattr(self, n).weight), f32(getattr(self, n).bias)) for n in ("norm1", "norm2", "norm3")} | \
             {"w2": bf16(self.ff.net[2].weight), "b2": f32(self.ff.net[2].bias)}
-        if ln_fold_enabled() and self.norm1.weight.shape[0] % 32 == 0:
+        if self.norm1.weight.shape[0] % 32 == 0:
             g = self.ff.net[0]
             idx = g.packed()["idx"]                          # GEGLU row order (value / gate halves per 256-column tile)
             wf, sf, cf = fold_layernorm(g.proj.weight, g.proj.bias, self.norm3.weight, self.norm3.bias)
@@ -312,7 +309,7 @@ class SpatialTransformer(PackedModule):
         B, H, W, C = x.shape
         xn = ops.groupnorm(x, p["g"], p["b"], self.norm.eps)
         inner = p["win"].shape[0]
-        if ln_fold_enabled() and inner % 32 == 0 and (H * W) % 8 == 0 and (B * H * W) % 32 == 0:   # (tokens are the N of V^T)
+        if ln_fold_fits(inner, B, H, W):
             # proj_in also writes the LayerNorm statistics of its output rows: norm1 of the first block runs inside attn1's GEMMs
             st = ops.ln_stats_buffer(B * H * W, inner, x.device)
             t, parts = ops.gemm_ln(xn.view(B * H * W, C), p["win"], bias=p["bin"], stats_out=st)

@@ -70,14 +70,14 @@ class Upsample(PackedModule):
         if not self.use_conv:
             return {}
         d = {"w": pack_conv3x3(self.conv.weight), "b": f32(self.conv.bias)}
-        if upsample_fold_enabled(1 << 30):           # (the folded copy is only built when the switch is on)
+        if upsample_fold_enabled(1 << 30, self.out_channels):   # (the folded copy is only built when some input can use it)
             d["wf"] = fold_upsample_conv3x3(self.conv.weight)
         return d
 
     def forward(self, x):
         ops = _ops()
         require_cuda(x, "Upsample")
-        if self.use_conv and upsample_fold_enabled(x.shape[0] * x.shape[1] * x.shape[2]):
+        if self.use_conv and upsample_fold_enabled(x.shape[0] * x.shape[1] * x.shape[2], self.out_channels):
             p = self.packed()
             return ops.upsample2x_conv3x3_folded(x, p["wf"], bias=p["b"])     # 2.25x fewer FLOPs, no upsampled temporary
         x = ops.upsample2x(x)

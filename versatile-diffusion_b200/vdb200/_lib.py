@@ -37,8 +37,6 @@ SIGNATURES = {
     "vdb_gemm_bf16": (i, [p, ll, ll, ll, p, ll, ll, p, ll, ll, p, ll, ll, p, ll, p, ll, i, i, f, i, i, p, sz, p]),
     "vdb_igemm_last_plan": (i, [C.POINTER(i), i]),
     "vdb_gemm_ln_bf16":(i, [p, ll, ll, ll, p, ll, ll, p, p, ll, p, ll, i, p, ll, i, i, f, p, i, p, p, p, i, p]),
-    "vdb_gemm_skinny_fits": (i, [i, ll]),
-    "vdb_gemm_skinny_bf16": (i, [p, i, ll, ll, p, ll, ll, p, ll, ll, p, ll, p, ll, p, ll, i, p]),
     "vdb_conv3x3_bf16": (i, [p, i, i, i, i, i, p, i, ll, p, i, p, i, p, ll, p, ll, p, ll, i, i, i, i, p, sz, p]),
     "vdb_attention_dk_pad": (i, [i]),
     "vdb_attention_dv_pad": (i, [i]),
@@ -50,7 +48,6 @@ SIGNATURES = {
     "vdb_layernorm": (i, [p, ll, i, p, p, f, p, p]),
     "vdb_norm_last_plan": (i, [C.POINTER(i), i]),
     "vdb_upsample2x_nhwc": (i, [p, i, i, i, i, p, p]),
-    "vdb_interleave2x2_nhwc": (i, [p, i, i, i, i, p, p]),
     "vdb_clip_to_u8_hwc": (i, [p, i, i, i, p, p]),
     "vdb_resample_h_u8": (i, [p, i, i, i, i, p, p, i, p, p]),
     "vdb_resample_v_crop_norm": (i, [p, i, i, i, p, p, i, i, i, i, C.POINTER(f), C.POINTER(f), p, p]),

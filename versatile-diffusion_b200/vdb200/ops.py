@@ -6,7 +6,6 @@ CUDA-graph capturable (no host syncs, scratch comes from the caller or torch's c
 """
 import ctypes
 import math
-import os
 
 import torch
 
@@ -292,13 +291,6 @@ def add_int(t, delta):
     check(lib.vdb_add_int(_ptr(t), int(delta), _stream()), "add_int")
 
 
-def _skinny_rows():
-    """largest small operand (rows) that ops.gemm sends to vdb_gemm_skinny_bf16 instead of the tensor-core kernel
-    (VDB_SKINNY=<rows>; default 0 = never: on the full-size 0-D diffuser the CUDA-core kernel was measured slower than the
-    split-K tensor-core tiles)"""
-    return int(os.environ.get("VDB_SKINNY", "0"))
-
-
 def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype=BF16, alpha=1.0,
          bias_bstride=0, rows_per_batch=1, bn=0, ksplit=0):
     """out[M,N'] = act(alpha*[a|a2] @ w^T + bias) + resid ; a [M,K] bf16, w [N,K(+K2)] bf16."""
@@ -312,19 +304,6 @@ def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype
     if out is None:
         out = torch.empty((M, n_out), dtype=out_dtype, device=a.device)
     _need(out, out_dtype, "out", True)
-    smax = _skinny_rows()
-    if act == ACT_NONE and alpha == 1.0 and out_dtype == BF16 and bn == 0 and ksplit == 0 and smax > 0:
-        # a small operand of <= 64 rows: weight-streaming CUDA-core kernel instead of the tensor-core latency chain
-        if M <= smax and (bias_bstride == 0 or rows_per_batch == 1) and lib.vdb_gemm_skinny_fits(M, K + K2):
-            check(lib.vdb_gemm_skinny_bf16(_ptr(a), M, K, a.stride(0), _ptr(a2), K2, a2.stride(0) if a2 is not None else 0,
-                                           _ptr(w), N, w.stride(0), _ptr(bias), int(bias_bstride), _ptr(resid),
-                                           resid.stride(0) if resid is not None else 0, _ptr(out), out.stride(0), 0, _stream()),
-                  "gemm_skinny_bf16")
-            return out
-        if N <= smax and M > N and a2 is None and bias is None and resid is None and lib.vdb_gemm_skinny_fits(N, K):
-            check(lib.vdb_gemm_skinny_bf16(_ptr(w), N, K, w.stride(0), None, 0, 0, _ptr(a), M, a.stride(0), None, 0, None, 0,
-                                           _ptr(out), out.stride(0), 1, _stream()), "gemm_skinny_bf16")
-            return out
     ws, ws_bytes = None, 0
     if ksplit != 1 and M <= 8192:   # split-K only ever triggers for small MN grids
         ws, ws_bytes = workspace(a.device), WORKSPACE_BYTES
@@ -340,12 +319,12 @@ def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype
     return out
 
 
-IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n", "nfast", "chunked")
+IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n")
 
 
 def igemm_last_plan():
     """The tiling of the last gemm / gemm_ln / conv3x3 launch on this thread (vdb_igemm_last_plan): which kernel instantiation
-    (BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile walk."""
+    (BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile counts."""
     buf = (ctypes.c_int * len(IGEMM_PLAN_FIELDS))()
     n = lib.vdb_igemm_last_plan(buf, len(buf))
     assert n == len(IGEMM_PLAN_FIELDS), n
@@ -550,34 +529,20 @@ def upsample2x(x, out=None):
     return out
 
 
-def interleave2x2(src, out=None):
-    """src bf16 [4, B, H, W, C] (parity py*2+px major) -> [B, 2H, 2W, C]."""
-    _need(src, BF16, "src")
-    _, B, H, W, C = src.shape
-    if out is None:
-        out = torch.empty((B, 2 * H, 2 * W, C), dtype=BF16, device=src.device)
-    check(lib.vdb_interleave2x2_nhwc(_ptr(src), B, H, W, C, _ptr(out), _stream()), "interleave2x2")
-    return out
-
-
 def upsample2x_conv3x3_folded(x, wf, bias=None):
     """nearest-2x upsample + 3x3 conv (pad 1) without materialising the upsampled image: four 2x2-tap convs on the source
-    (one per output parity, weights folded by diffusion_utils.fold_upsample_conv3x3) + one interleave pass.
-    x bf16 [B,H,W,C]; wf bf16 [4, N, 4*C]; -> [B,2H,2W,N]."""
+    (one per output parity, weights folded by diffusion_utils.fold_upsample_conv3x3).
+    x bf16 [B,H,W,C]; wf bf16 [4, N, 4*C] with N % 32 == 0; -> [B,2H,2W,N]."""
     B, H, W, _ = x.shape
     N = wf.shape[1]
-    if N % 32 == 0 and os.environ.get("VDB_UPFOLD_DIRECT", "1") != "0" and os.environ.get("VDB_EPI_TMA", "1") != "0" \
-            and os.environ.get("VDB_IGEMM_SPEC", "1") != "0":
-        # modes 7..10: every parity conv stores straight into its pixels of the [B,2H,2W,N] result (output tensor map with
-        # doubled strides): no interleave pass, no parity temporaries
-        out = torch.empty((B, 2 * H, 2 * W, N), dtype=BF16, device=x.device)
-        for par in range(4):
-            conv3x3(x, wf[par], bias=bias, out=out, mode=7 + par, ksplit=1)
-        return out
-    parts = torch.empty((4, B, H, W, N), dtype=BF16, device=x.device)
+    if N % 32:
+        raise ValueError(f"upsample2x_conv3x3_folded: N = {N} is not a multiple of 32 (use upsample2x + conv3x3)")
+    # modes 7..10: every parity conv stores straight into its pixels of the [B,2H,2W,N] result (output tensor map with
+    # doubled strides): no interleave pass, no parity temporaries
+    out = torch.empty((B, 2 * H, 2 * W, N), dtype=BF16, device=x.device)
     for par in range(4):
-        conv3x3(x, wf[par], bias=bias, out=parts[par], mode=3 + par, ksplit=1)
-    return interleave2x2(parts)
+        conv3x3(x, wf[par], bias=bias, out=out, mode=7 + par, ksplit=1)
+    return out
 
 
 def im2col3x3_small(x, kpad=64, in_scale=1.0, in_shift=0.0, out=None):
