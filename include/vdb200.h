@@ -362,6 +362,26 @@ int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* 
 int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, float temperature, int K, int* tokens, int ldt, int* src,
                           int lds, double* scores, int* done, int* lengths, const int* step, int eos, int max_len, int* cand_tok,
                           double* cand_logp, float* record, double* trace, void* stream);
+/* The repetition logits processors, in place on the fp32 logits [R, ldl] of one token step, before vdb_textdec_sample(_filtered)
+ * or vdb_textdec_beam_step reads them (so those see, and `record` holds, the edited logits).  Row r's history is
+ * h = tokens[r, 0 .. s], s = *step: <BOS>, then every token so far, including this step's input token.
+ *   Repetition penalty p (finite, > 0; 1 = off), as HF's RepetitionPenaltyLogitsProcessor: for each DISTINCT id v of h with
+ *     0 <= v < V, l[v] = l[v] < 0 ? l[v] * p : l[v] / p, IEEE round-to-nearest fp32 (a true division, no reciprocal).  An id is
+ *     penalised once however often it occurs; ids outside [0, V) are ignored.
+ *   No-repeat n-gram n (0 = off), as HF's NoRepeatNGramLogitsProcessor: for every 0 <= j <= s - n + 1 with
+ *     h[j .. j+n-2] == h[s-n+2 .. s] (the last n - 1 tokens), l[h[j+n-1]] = -inf (ids outside [0, V) ignored).  n = 1 bans every
+ *     token of h; nothing is banned while s + 1 < n.
+ * The penalty runs first; the two commute (the penalty maps -inf to -inf).  Both act on the raw logits, before the sampler's
+ * division by temperature and its top-k / nucleus cuts.  Rows with done[r] != 0 are left untouched, and a step with s < 0 or
+ * s + 1 >= ldt does nothing.  Beam search applies the edit to each beam's own row; the beam step's fp64 log-softmax then
+ * renormalises over the edited logits (HF edits log-probabilities and does not renormalise).
+ * Precondition for small vocabularies: a banned token is never drawn, and never extends a beam, only while a row keeps at least
+ * one finite logit (beam search: at least K finite logits per live beam).  V = 50260 with at most 32 history tokens always does.
+ * One launch, one CTA per row, reading only the row's history and at most 2 (s + 1) of its logits.  penalty == 1 and ngram == 0
+ * return 0 without a launch.  Returns VDB_ERR_INVALID before any launch unless 1 <= R <= 16, V >= 1, ldl >= V, ldt >= 1, penalty
+ * is finite and > 0, 0 <= ngram <= ldt, the pointers are non-null and 4-byte aligned. */
+int vdb_textdec_repetition(float* logits, int R, int V, long long ldl, const int* tokens, int ldt, const int* done, const int* step,
+                           float penalty, int ngram, void* stream);
 
 /* ---- semantic/style disentanglement of the image context — decompose / adjust_rank of the reference app.py:48-127 -----------
  * For each item b < n_items of x [n_items, m, n] (fp32, contiguous):  X = x - rowmean(x);  the randomized PCA of torch.pca_lowrank

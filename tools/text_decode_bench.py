@@ -6,7 +6,10 @@ With --top-k / --top-p: ms per token step at 4 and 16 rows with the sampler's cu
 alternately in one session, and the launches per step of each.
 With --num-beams K: 4 latents sampled (4 rows) against the same 4 latents under beam search (4 K rows, groups of 16 // K latents),
 the two step graphs replayed alternately: ms per token step, launches per step and the time of a whole decode call of each.
-    python tools/text_decode_bench.py [--no-i2t] [--top-k K] [--top-p P] [--num-beams K]"""
+With --repetition-penalty / --no-repeat-ngram: ms per token step and launches per step with the repetition processors off and
+on, the two graphs replayed alternately, best of 5, at 4 and 16 sampled rows and, with --num-beams K, at 16 // K latents x K beams.
+    python tools/text_decode_bench.py [--no-i2t] [--top-k K] [--top-p P] [--num-beams K] [--repetition-penalty P]
+                                      [--no-repeat-ngram N]"""
 import argparse
 import json
 import os
@@ -30,6 +33,8 @@ ap.add_argument("--no-i2t", action="store_true")
 ap.add_argument("--top-k", type=int, default=0)
 ap.add_argument("--top-p", type=float, default=0.0)
 ap.add_argument("--num-beams", type=int, default=0)
+ap.add_argument("--repetition-penalty", type=float, default=1.0)
+ap.add_argument("--no-repeat-ngram", type=int, default=0)
 args = ap.parse_args()
 HBM = 3.35e12
 dev = torch.device("cuda", 0)
@@ -62,7 +67,7 @@ with torch.no_grad():
         vae.decode_ids(z, eos_token=-1)                      # warm-up: packs weights, captures the step-chunk graph
     p = vae.packed()
     st = vae._state(R, dev)
-    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0, 0)]
+    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0, 0, 1.0, 0)]
     n0 = ops.launch_count()
     vae._step(st, p, 1.0, -1, 30, "seed", False)
     launches = ops.launch_count() - n0
@@ -113,7 +118,7 @@ def step_ms_off_and_on(R, top_k, top_p, rounds=5, reps=10):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
             for name, (k, p) in cuts.items():
-                g = st.graphs[(1.0, -1, 30, "seed", False, k, p, 0)]
+                g = st.graphs[(1.0, -1, 30, "seed", False, k, p, 0, 1.0, 0)]
                 e0.record()
                 for _ in range(reps):
                     st.step.zero_()
@@ -151,7 +156,7 @@ def sampling_and_beams(K, n=4, rounds=5, reps=10):
             st = vae._state(rows, dev)
             n0 = ops.launch_count()
             vae._step(st, vae.packed(), 1.0, -1, 30, mode, False, 0, 0.0, k)
-            out[name] = dict(rows=rows, graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, k)], st=st,
+            out[name] = dict(rows=rows, graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, k, 1.0, 0)], st=st,
                              launches_per_step=ops.launch_count() - n0, ms=[], ms_decode=[])
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
@@ -186,6 +191,55 @@ def sampling_and_beams(K, n=4, rounds=5, reps=10):
 
 if args.num_beams:
     print(json.dumps(sampling_and_beams(args.num_beams)))
+
+
+def repetition_off_and_on(n, K, penalty, ngram, rounds=5, reps=10):
+    """ms per token step of the captured chunk with the repetition processors off and on, the two graphs replayed alternately on
+    live rows (done = 0 and the step counter rewound before each timed chunk); launches per step of each.  K = 0 samples n rows,
+    K >= 1 runs beam search on n K rows."""
+    zr = torch.randn(n, 768, generator=torch.Generator().manual_seed(7)).to(dev) * 3.0
+    mode, R = ("beam", n * K) if K else ("seed", n)
+    knobs = {"off": (1.0, 0), "on": (float(penalty), int(ngram))}
+    out = {}
+    with torch.no_grad():
+        st = vae._state(R, dev)
+        for name, (rp, nr) in knobs.items():
+            for _ in range(2):
+                if K:
+                    vae.decode_beams(zr, K, eos_token=-1, repetition_penalty=rp, no_repeat_ngram_size=nr)
+                else:
+                    vae.decode_ids(zr, eos_token=-1, repetition_penalty=rp, no_repeat_ngram_size=nr)
+            st.step.zero_()
+            n0 = ops.launch_count()
+            vae._step(st, vae.packed(), 1.0, -1, 30, mode, False, 0, 0.0, K, rp, nr)
+            out[name] = dict(launches_per_step=ops.launch_count() - n0, ms=[],
+                             graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, K, rp, nr)])
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for _ in range(rounds):
+            for name in knobs:
+                torch.cuda.synchronize()
+                e0.record()
+                for _ in range(reps):
+                    st.step.zero_()
+                    st.done.zero_()
+                    out[name]["graph"].replay()
+                e1.record()
+                torch.cuda.synchronize()
+                out[name]["ms"].append(e0.elapsed_time(e1) / (reps * STEPS_PER_CHECK))
+    res = dict(card=card, rows=R, num_beams=K, repetition_penalty=penalty, no_repeat_ngram_size=ngram)
+    for name in knobs:
+        res[f"ms_per_step_{name}"] = round(min(out[name]["ms"]), 4)
+        res[f"ms_per_step_{name}_all"] = [round(v, 4) for v in out[name]["ms"]]
+        res[f"launches_per_step_{name}"] = out[name]["launches_per_step"]
+    res["processor_cost_ms_per_step"] = round(res["ms_per_step_on"] - res["ms_per_step_off"], 4)
+    return res
+
+
+if args.repetition_penalty != 1.0 or args.no_repeat_ngram:
+    for rows_ in (4, 16):
+        print(json.dumps(repetition_off_and_on(rows_, 0, args.repetition_penalty, args.no_repeat_ngram)))
+    if args.num_beams:
+        print(json.dumps(repetition_off_and_on(16 // args.num_beams, args.num_beams, args.repetition_penalty, args.no_repeat_ngram)))
 
 if not args.no_i2t:
     bs = 4

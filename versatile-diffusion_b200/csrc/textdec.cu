@@ -4,7 +4,7 @@
 // through ~247 MB of bf16 weights per token: every kernel here is bound by weight bandwidth or by launch latency, none is
 // tensor-core sized.  A token step is
 //   embed -> 12 x [ln_1+c_attn, attention over the KV cache, attn.c_proj(+resid), ln_2+c_fc+gelu, mlp.c_proj(+resid)]
-//         -> ln_f+lm_head -> sampler -> step += 1
+//         -> ln_f+lm_head [-> repetition penalty / n-gram bans] -> sampler -> step += 1
 // and reads the step index from a device counter, so one captured CUDA graph serves every step.
 #include <curand_philox4x32_x.h>
 
@@ -677,6 +677,47 @@ textdec_beam_select_kernel(int R, int K, const int* __restrict__ cand_tok, const
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Repetition penalty and no-repeat n-gram bans (vdb_textdec_repetition), one CTA per row, editing the row's logits in place
+// before the sampler or the beam step reads them.  h = tokens[r, 0 .. s], s = *step.  Thread j takes history position j:
+//   penalty pass: the first occurrence of each id in [0, V) scales its logit once (later occurrences of the id skip it);
+//   ban pass (after a barrier, so a ban lands on the penalised value): position j <= s - n + 1 whose n - 1 tokens equal the
+//   last n - 1 tokens of h sets logit h[j + n - 1] to -inf.  Two positions may ban one id: they write the same value.
+// Reads the s + 1 history tokens only and touches at most 2 (s + 1) logits of the row, never the whole vocabulary.
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int kRepThreads = 32;                   // one warp: the history of a decode is at most 32 tokens
+
+__global__ void __launch_bounds__(kRepThreads)
+textdec_repetition_kernel(float* __restrict__ logits, int V, long long ldl, const int* __restrict__ tokens, int ldt,
+                          const int* __restrict__ done, const int* __restrict__ step, float penalty, int ngram) {
+  const int r = blockIdx.x, s = *step;
+  if (s < 0 || s + 1 >= ldt || done[r]) return;
+  float* lr = logits + static_cast<size_t>(r) * ldl;
+  const int* h = tokens + static_cast<size_t>(r) * ldt;
+  if (penalty != 1.0f) {
+    for (int j = threadIdx.x; j <= s; j += blockDim.x) {
+      const int v = h[j];
+      if (v < 0 || v >= V) continue;
+      bool first = true;
+      for (int k = 0; k < j && first; ++k) first = h[k] != v;
+      if (first) {
+        const float l = lr[v];
+        lr[v] = l < 0.0f ? __fmul_rn(l, penalty) : __fdiv_rn(l, penalty);
+      }
+    }
+  }
+  __syncthreads();
+  if (ngram > 0) {
+    const int tail = s - ngram + 2;               // h[tail .. s]: the last n - 1 tokens
+    for (int j = threadIdx.x; j <= s - ngram + 1; j += blockDim.x) {
+      bool match = true;
+      for (int k = 0; k < ngram - 1 && match; ++k) match = h[j + k] == h[tail + k];
+      const int v = h[j + ngram - 1];
+      if (match && v >= 0 && v < V) lr[v] = -INFINITY;
+    }
+  }
+}
+
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
@@ -858,6 +899,25 @@ int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, floa
   count_launch();
   textdec_beam_select_kernel<<<R / K, kSelectThreads, 0, as_stream(stream)>>>(R, K, cand_tok, cand_logp, tokens, ldt, src, lds, scores,
                                                                               done, lengths, step, eos, max_len, trace);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_textdec_repetition(float* logits, int R, int V, long long ldl, const int* tokens, int ldt, const int* done, const int* step,
+                           float penalty, int ngram, void* stream) {
+  if (!logits || !tokens || !done || !step) return set_error(VDB_ERR_INVALID, "textdec_repetition: null pointer");
+  if (R < 1 || R > kGvMaxRows || V < 1 || ldl < V || ldt < 1)
+    return set_error(VDB_ERR_INVALID, "textdec_repetition: need 1 <= R <= 16, ldl >= V >= 1 and ldt >= 1, got R = %d, V = %d", R, V);
+  if (!(penalty > 0.0f) || !isfinite(penalty))
+    return set_error(VDB_ERR_INVALID, "textdec_repetition: penalty must be finite and > 0, got %g", static_cast<double>(penalty));
+  if (ngram < 0 || ngram > ldt)
+    return set_error(VDB_ERR_INVALID, "textdec_repetition: need 0 <= ngram <= ldt, got ngram = %d, ldt = %d", ngram, ldt);
+  if ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(tokens) | reinterpret_cast<uintptr_t>(done) |
+       reinterpret_cast<uintptr_t>(step)) & 3)
+    return set_error(VDB_ERR_INVALID, "textdec_repetition: buffers must be 4-byte aligned");
+  if (penalty == 1.0f && ngram == 0) return VDB_OK;
+  textdec_repetition_kernel<<<R, kRepThreads, 0, as_stream(stream)>>>(logits, V, ldl, tokens, ldt, done, step, penalty, ngram);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;

@@ -58,6 +58,22 @@ The KV cache is not moved when beams are reordered: each physical (row, slot) is
 slot j of beam r from row src[r, j], a table the beam step permutes with the token rows.  A step streams the weights once for all
 n * K rows (the GEMV is one 16-row tile), so n * K <= 16 rows run together; more latents are split into groups of 16 // K,
 decoded one after the other, each group re-streaming the weights.
+
+Repetition: decode / decode_ids / decode_beams(..., repetition_penalty=p, no_repeat_ngram_size=n) apply the two logits processors
+of Hugging Face generation (RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor) in one kernel inside the captured step
+graph (vdb_textdec_repetition), right after the LM head.  At step s the history of row r is h = tokens[r, 0 .. s] (<BOS>, every
+token so far, this step's input token included), and the row's fp32 logits are edited in place:
+  - penalty p (finite, > 0; 1.0 = off): for each distinct id v of h, l[v] = l[v] < 0 ? l[v] * p : l[v] / p in IEEE fp32, once
+    per id however often it occurs;
+  - n-gram n (0 = off, at most MAX_LENGTH): for every j <= s - n + 1 with h[j .. j+n-2] equal to the last n - 1 tokens of h,
+    l[h[j+n-1]] = -inf, so no n-gram occurs twice; n = 1 bans every token of h; nothing is banned while s + 1 < n.
+The penalty runs first (the two commute: the penalty keeps -inf).  Both act on the raw logits, before / temperature and before the
+top_k / top_p cuts, as HF runs processors before warpers; finished rows are not edited.  Every mode sees the edited logits and
+return_logits returns them.  Beam search edits each beam's own row and then takes its fp64 log-softmax of the edited logits, so a
+ban renormalises the beam's distribution; HF edits log-probabilities instead and does not renormalise.  The reference has no
+working beam path, so this definition stands.  A banned token is never drawn nor extends a beam while a row keeps a finite logit
+(K of them for beams), which a 50260-token vocabulary and at most 30 history tokens always leave.  teacher_forced_logits takes no
+processors.  With both off no launch is added and every output is bitwise what it is without the arguments.
 """
 import json
 import math
@@ -112,6 +128,17 @@ def _check_beams(num_beams, length_penalty, top_k, top_p):
     if num_beams and (top_k != 0 or top_p != 0.0):
         raise ValueError("optimus_vae_next: beam search (num_beams >= 1) takes no top_k / top_p cut")
     return int(num_beams), float(length_penalty)
+
+
+def _check_repetition(repetition_penalty, no_repeat_ngram_size):
+    """-> (float repetition_penalty, int no_repeat_ngram_size) of the repetition logits processors, or ValueError."""
+    p, n = repetition_penalty, no_repeat_ngram_size
+    if (isinstance(p, bool) or not isinstance(p, numbers.Real) or not math.isfinite(p) or not p > 0
+            or not 0.0 < float(torch.tensor(float(p), dtype=torch.float32)) < math.inf):     # the kernel takes it as fp32
+        raise ValueError(f"optimus_vae_next: repetition_penalty must be a finite float > 0 (1: off), got {p!r}")
+    if isinstance(n, bool) or not isinstance(n, numbers.Integral) or not 0 <= n <= MAX_LENGTH:
+        raise ValueError(f"optimus_vae_next: no_repeat_ngram_size must be an int in [0, {MAX_LENGTH}] (0: off), got {n!r}")
+    return float(p), int(n)
 
 
 class VocabularyMissingError(RuntimeError):
@@ -631,7 +658,8 @@ class optimus_vae_next(PackedModule):
         self.__dict__['_states'] = {}        # captured graphs hold the old weight addresses
 
     # ------------------------------------------------------------------ one token step (5 launches per layer + 4)
-    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0, num_beams=0):
+    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0, num_beams=0, repetition_penalty=1.0,
+              no_repeat_ngram_size=0):
         ops = _ops()
         dec = self.decoder
         D = dec.n_embd
@@ -647,6 +675,8 @@ class optimus_vae_next(PackedModule):
             ops.textdec_gemv(st.h, L["w_fc"], st.m, bias=L["b_fc"], ln=L["ln2"], act=ops.ACT_GELU_TANH)
             ops.textdec_gemv(st.m, L["w_mproj"], st.h, bias=L["b_mproj"], accumulate=True)
         ops.textdec_gemv(st.h, p["lm_head"], st.logits, ln=p["lnf"])
+        if mode != "forced" and (repetition_penalty != 1.0 or no_repeat_ngram_size):
+            ops.textdec_repetition(st.logits, st.tokens, st.done, st.step, repetition_penalty, no_repeat_ngram_size)
         if num_beams:
             ops.textdec_beam_step(st.logits, num_beams, st.tokens, st.src, st.scores, st.done, st.lengths, st.step, st.cand_tok,
                                   st.cand_logp, temperature=temperature, eos=eos, max_len=max_len,
@@ -660,9 +690,10 @@ class optimus_vae_next(PackedModule):
 
     @torch.no_grad()
     def _run(self, z, temperature, eos, pre_scale=1.0, max_len=MAX_LENGTH, nsteps=None, mode="seed", uniforms=None, forced=None,
-             record=False, graph=True, top_k=0, top_p=0.0, num_beams=0):
+             record=False, graph=True, top_k=0, top_p=0.0, num_beams=0, repetition_penalty=1.0, no_repeat_ngram_size=0):
         """mode "beam" (num_beams >= 1) decodes the n latents of z as rows latent * num_beams + beam, n * num_beams <= 16."""
         top_k, top_p = _check_cuts(top_k, top_p)
+        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
         require_cuda(z, "optimus_vae_next.decode")
         if z.dim() != 2 or z.shape[1] != self.nz:
             raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
@@ -703,7 +734,7 @@ class optimus_vae_next(PackedModule):
         else:
             st.forced.zero_()
             st.forced[:, :forced.shape[1]].copy_(forced)
-        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p, K)
+        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p, K, rp, nr)
         s = 0
         while s < nsteps:
             n = min(STEPS_PER_CHECK, nsteps - s)
@@ -712,7 +743,7 @@ class optimus_vae_next(PackedModule):
                 g.replay()
             else:
                 for _ in range(n):
-                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K)
+                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K, rp, nr)
                 if graph and n == STEPS_PER_CHECK and key not in st.graphs:
                     # the chunk just ran eagerly (kernels configured, caches warm); capture one for the later chunks
                     torch.cuda.current_stream().synchronize()
@@ -720,7 +751,7 @@ class optimus_vae_next(PackedModule):
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
                         for _ in range(n):
-                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K)
+                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K, rp, nr)
                     st.step.copy_(step_before)        # capture does not execute, but keep the counter exactly as the eager chunk left it
                     st.graphs[key] = g
             s += n
@@ -728,10 +759,12 @@ class optimus_vae_next(PackedModule):
                 break
         return st, s
 
-    def _beam_group(self, z, num_beams, temperature, pre_scale, eos, length_penalty, record=False, graph=True):
+    def _beam_group(self, z, num_beams, temperature, pre_scale, eos, length_penalty, record=False, graph=True,
+                    repetition_penalty=1.0, no_repeat_ngram_size=0):
         """Beam search of n latents with n * num_beams <= 16 -> (per latent, its num_beams (ids, score, normalized score) best
         first; the state; the steps run)."""
-        st, ran = self._run(z, temperature, eos, pre_scale=pre_scale, mode="beam", record=record, graph=graph, num_beams=num_beams)
+        st, ran = self._run(z, temperature, eos, pre_scale=pre_scale, mode="beam", record=record, graph=graph, num_beams=num_beams,
+                            repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
         tokens, lengths, scores = st.tokens.cpu(), st.lengths.cpu().tolist(), st.scores.cpu().tolist()
         out = []
         for i in range(z.shape[0]):
@@ -744,11 +777,14 @@ class optimus_vae_next(PackedModule):
         return out, st, ran
 
     @torch.no_grad()
-    def decode_beams(self, z, num_beams, temperature=1.0, pre_scale=1.0, length_penalty=1.0, eos_token=EOS_ID, graph=True):
+    def decode_beams(self, z, num_beams, temperature=1.0, pre_scale=1.0, length_penalty=1.0, eos_token=EOS_ID, graph=True,
+                     repetition_penalty=1.0, no_repeat_ngram_size=0):
         """Beam search (see the module docstring): for each latent, its num_beams final hypotheses as (ids int64 CPU tensor from
         <BOS> to <EOS>, score = summed fp64 log-probability, score / n ** length_penalty), best normalized score first.
         num_beams latents' worth of rows run per token step, at most 16: more latents are decoded in groups of 16 // num_beams,
-        one after the other, each re-streaming the weights."""
+        one after the other, each re-streaming the weights.  repetition_penalty / no_repeat_ngram_size edit each beam's logits
+        before its log-softmax (see the module docstring); the scores are then log-probabilities of the edited logits."""
+        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
         num_beams, length_penalty = _check_beams(num_beams, length_penalty, 0, 0.0)
         if num_beams < 1:
             raise ValueError(f"optimus_vae_next.decode_beams: num_beams must be >= 1, got {num_beams}")
@@ -759,25 +795,30 @@ class optimus_vae_next(PackedModule):
         out = []
         for i0 in range(0, z.shape[0], per):
             out += self._beam_group(z[i0:i0 + per], num_beams, temperature, pre_scale, int(eos_token), length_penalty,
-                                    graph=graph)[0]
+                                    graph=graph, repetition_penalty=rp, no_repeat_ngram_size=nr)[0]
         return out
 
     @torch.no_grad()
     def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True,
-                   top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0):
+                   top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0, repetition_penalty=1.0, no_repeat_ngram_size=0):
         """Sampled token rows, each an int64 CPU tensor starting with <BOS> and (unless eos_token never occurs and is never forced)
         ending with eos_token, length <= 30.  uniforms (fp64 [n, >=28]) replaces the Philox draws; return_logits also returns the
         fp32 logits of every step that ran, [steps, n, 50260] on the device.  top_k > 0 keeps the top_k most likely tokens (ties
         included), 0 < top_p < 1 the nucleus of mass top_p (optimus.py:690-719); the defaults sample the full softmax.
+        repetition_penalty != 1 / no_repeat_ngram_size > 0 edit the logits before the draw (see the module docstring); the
+        returned logits are the edited ones.
         num_beams >= 1: each latent's best beam-search hypothesis instead (decode_beams; no cuts, uniforms or logits)."""
+        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
         num_beams, length_penalty = _check_beams(num_beams, length_penalty, top_k, top_p)
         if num_beams:
             if uniforms is not None or return_logits:
                 raise ValueError("optimus_vae_next: beam search takes no uniforms and returns no logits")
             return [b[0][0] for b in self.decode_beams(z, num_beams, temperature=temperature, pre_scale=pre_scale,
-                                                       length_penalty=length_penalty, eos_token=eos_token, graph=graph)]
+                                                       length_penalty=length_penalty, eos_token=eos_token, graph=graph,
+                                                       repetition_penalty=rp, no_repeat_ngram_size=nr)]
         st, ran = self._run(z, temperature, int(eos_token), pre_scale=pre_scale, mode="uniforms" if uniforms is not None else "seed",
-                            uniforms=uniforms, record=return_logits, graph=graph, top_k=top_k, top_p=top_p)
+                            uniforms=uniforms, record=return_logits, graph=graph, top_k=top_k, top_p=top_p, repetition_penalty=rp,
+                            no_repeat_ngram_size=nr)
         tokens, lengths = st.tokens.cpu(), st.lengths.cpu()
         rows = [tokens[r, :int(lengths[r])].long() for r in range(st.R)]
         if return_logits:
@@ -795,9 +836,11 @@ class optimus_vae_next(PackedModule):
         return st.record[:L].permute(1, 0, 2).contiguous()
 
     @torch.no_grad()
-    def decode(self, z, temperature=1.0, pre_scale=1.0, top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0):
-        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row; top_k / top_p / num_beams / length_penalty as
-        in decode_ids (num_beams >= 1: the best beam-search hypothesis)."""
+    def decode(self, z, temperature=1.0, pre_scale=1.0, top_k=0, top_p=0.0, num_beams=0, length_penalty=1.0, repetition_penalty=1.0,
+               no_repeat_ngram_size=0):
+        """optimus_vae_next.decode (optimus.py:746-763): one string per latent row; top_k / top_p / num_beams / length_penalty /
+        repetition_penalty / no_repeat_ngram_size as in decode_ids (num_beams >= 1: the best beam-search hypothesis)."""
         rows = self.decode_ids(z, temperature=temperature, pre_scale=pre_scale, top_k=top_k, top_p=top_p, num_beams=num_beams,
-                               length_penalty=length_penalty)
+                               length_penalty=length_penalty, repetition_penalty=repetition_penalty,
+                               no_repeat_ngram_size=no_repeat_ngram_size)
         return [self.tokenizer_decoder.sentence(r.tolist()) for r in rows]

@@ -821,6 +821,18 @@ def textdec_beam_step(logits, num_beams, tokens, src, scores, done, lengths, ste
           "textdec_beam_step")
 
 
+def textdec_repetition(logits, tokens, done, step, penalty=1.0, ngram=0):
+    """The repetition penalty and no-repeat n-gram bans on logits fp32 [R, V] in place (see vdb_textdec_repetition): row r's
+    history is tokens[r, :*step + 1] (int32 [R, L]); rows with done[r] != 0 are left as they are.  penalty 1 and ngram 0
+    launch nothing."""
+    _need(logits, torch.float32, "logits", rows_ok=True)
+    _need(tokens, torch.int32, "tokens"); _need(done, torch.int32, "done"); _need(step, torch.int32, "step")
+    R, V = logits.shape
+    check(lib.vdb_textdec_repetition(_ptr(logits), R, V, logits.stride(0), _ptr(tokens), tokens.stride(0), _ptr(done), _ptr(step),
+                                     float(penalty), int(ngram), _stream()), "textdec_repetition")
+    return logits
+
+
 # ------------------------------------------------------------------------------------------------
 # Semantic/style disentanglement (app.py:48-127): the rank adjustment of the image context, one launch
 # ------------------------------------------------------------------------------------------------
