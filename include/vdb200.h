@@ -95,7 +95,9 @@ int vdb_lincomb4_f32(const float* x0, const float* x1, const float* x2, const fl
  * [.., N] selected by row / rows_per_batch.  act = VDB_ACT_*; VDB_ACT_GEGLU expects W/bias rows packed
  * per 256-column tile as 128 value rows then their 128 gate rows and writes N/2 columns
  * (GEGLU.forward, attention.py:42-44).  out bf16 (out_f32==0) or fp32.  bn: 0 = auto, else force
- * tile N in {64,128,160,256}.  ksplit: 0 = auto, 1 = off; split-K needs workspace >= ksplit*M*N*4 B. */
+ * tile N in {64,128,160,256} on a 128-row tile, or 160 | VDB_IGEMM_BM256 for the 256-row tile (bf16 out, act 0,
+ * alpha 1, N % 32 == 0, one bias row per 256 rows, no split-K; the same in the other igemm entry points).  ksplit: 0 = auto, 1 = off; split-K needs workspace >= ksplit*M*N*4 B. */
+#define VDB_IGEMM_BM256 0x1000
 int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const void* A2, long long K2,
                   long long lda2, const void* W, long long N, long long ldw, const float* bias,
                   long long bias_bstride, long long rows_per_batch, const void* resid, long long ldr, void* out,
@@ -106,6 +108,8 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
  * device work): out[0..n) receives {BN, STAGES, epilogue MODE, ksplit, grid, M tiles, N tiles} (as many as n
  * allows).  Returns the number of fields (7).  For tests and tools that need to know which kernel instantiation ran. */
 int vdb_igemm_last_plan(int* out, int n);
+/* The tile height BM (128 or 256 rows) of that same launch; 0 before the first one. */
+int vdb_igemm_last_bm(void);
 
 /* ---- the same GEMM with a LayerNorm folded in — BasicTransformerBlock norm1/2/3, attention.py:206-208,214-218 -------------
  * CONSUMER (ln_stats != NULL):  out = act( LN(x) W0^T + b0 )  computed from the RAW x without ever forming LN(x):

@@ -4,7 +4,7 @@ Records the GEMM / conv launches (igemm_kernel: every conv and linear layer of t
 config (ops.record_start / record_stop), groups them by shape and kernel plan, and replays each group alone inside a CUDA graph
 (--copies back-to-back copies per graph, so the graph launch is amortised), timed with CUDA events, best of --reps.  Prints per
 group: launches per step, us per step, TFLOP/s, share of the whole step (the CUDA-graph step of the sampler, timed the same way)
-and the plan (BN, STAGES, MODE, ksplit, grid), with the card's name and power limit.  A group replayed alone runs with a warmer
+and the plan (BM, BN, STAGES, MODE, ksplit, grid), with the card's name and power limit.  A group replayed alone runs with a warmer
 L2 than inside the step, so the per-group times are a lower bound on what the same launches cost there.
 
 VDB200_LIB=<other libvdb200.so> times another build of the kernels on the same shapes; --json writes the rows, and --baseline
@@ -134,13 +134,16 @@ def main():
         recs = ops.record_stop()
         torch.cuda.synchronize()
 
-        groups = OrderedDict()
+        groups, key_plans = OrderedDict(), {}
         for rec in recs:
             fn, cargs, _keep, flops = rec
             ops.check(fn(*cargs, ops._stream()), "igemm_step_shapes")
             plan = ops.igemm_last_plan()
-            key = "%s | BN %d ST %d MODE %d ks %d grid %d" % (describe(fn, cargs, flops), plan["bn"], plan["stages"], plan["mode"],
+            # (the key is the shape alone, so that --baseline lines a group up with a build that plans it differently)
+            key = describe(fn, cargs, flops)
+            tile = "BM %d BN %d ST %d MODE %d ks %d grid %d" % (plan["bm"], plan["bn"], plan["stages"], plan["mode"],
                                                                 plan["ksplit"], plan["grid"])
+            key_plans.setdefault(key, tile)
             grp = groups.setdefault(key, {"recs": [], "flops": 0.0})
             grp["recs"].append(rec)
             grp["flops"] += flops
@@ -152,7 +155,8 @@ def main():
                 for _ in range(args.copies):
                     ops.replay(grp["recs"])
             ms = time_graph(run, args.reps) / args.copies
-            rows.append({"key": key, "launches": len(grp["recs"]), "us": ms * 1e3, "tflops": grp["flops"] / ms / 1e9})
+            rows.append({"key": key, "plan": key_plans[key], "launches": len(grp["recs"]), "us": ms * 1e3,
+                         "tflops": grp["flops"] / ms / 1e9})
         all_ms = time_graph(lambda: ops.replay(recs), args.reps)
 
     base = {}
@@ -166,10 +170,13 @@ def main():
         hdr = "%9s %7s " % ("base us", "change") + hdr
     print(hdr)
     for r in sorted(rows, key=lambda r: -r["us"]):
-        line = "%9.1f %7.1f %5d %5.1f%%  %s" % (r["us"], r["tflops"], r["launches"], 100.0 * r["us"] / 1e3 / best_step, r["key"])
+        line = "%9.1f %7.1f %5d %5.1f%%  %s | %s" % (r["us"], r["tflops"], r["launches"], 100.0 * r["us"] / 1e3 / best_step, r["key"],
+                                                      r["plan"])
         if base:
             b = base.get(r["key"])
             line = ("%9.1f %+6.1f%% " % (b["us"], 100.0 * (r["us"] / b["us"] - 1)) if b else "%9s %7s " % ("-", "-")) + line
+            if b and b.get("plan") != r["plan"]:
+                line += "   (baseline: %s)" % b.get("plan")
         print(line)
     if base:
         bt = sum(b["us"] for b in base.values())

@@ -186,6 +186,13 @@ VDB_DEVINL void wgmma_fence_regs(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Register reallocation between warpgroups (every warp of the warpgroup executes it): a producer warpgroup gives registers
+// back, the consumer warpgroups take them.  R is a multiple of 8 in [24, 256].
+template <int R>
+VDB_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+VDB_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // nanosecond wall clock shared by all SMs (debug timelines, watchdogs)
 VDB_DEVINL unsigned long long gtime() {
   unsigned long long t;

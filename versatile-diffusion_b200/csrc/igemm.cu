@@ -9,24 +9,29 @@
 //     autokl_modules.py:42-141), with the 1x1 skip_connection of a channel-changing ResBlock folded
 //     in as extra K segments of the same accumulator.
 //
-// Structure: grid = #SMs (persistent, static round-robin over output tiles), 288 threads:
-//   warps 0-7: two consumer warpgroups (wgmma m64 x BN x 16 each, fp32 accumulators in registers), then the epilogue
+// Structure: grid = #SMs (persistent, static round-robin over output tiles), 288 threads (384 where the accumulator needs the
+// producer's registers, see igemm_realloc):
+//   warps 0-7: two consumer warpgroups (BM / 128 wgmma m64 x BN x 16 each per k16 step, fp32 accumulators in registers), then the epilogue
 //              (TMA-store modes: straight from the registers -> bias / LayerNorm / GEGLU / residual -> bf16 TMA stores;
 //              other modes: accumulator parked in shared memory -> bias/act/residual -> coalesced bf16 / fp32 stores)
 //   warp 8   : TMA producer  (cp.async.bulk.tensor 4D box loads of A, 2D box loads of W)
-// smem ring of STAGES x (A 128x64 bf16 | W BNx64 bf16), both 128B-swizzled K-major.
+// smem ring of STAGES x (A BMx64 bf16 | W BNx64 bf16), both 128B-swizzled K-major; the tile is BM = 128 or 256 rows high.
 #include "common.cuh"
 #include "host_util.h"
 
 namespace vdb {
 
-constexpr int kBlockM = 128;
+constexpr int kBlockM = 128;  // tile height of every launch the 256-row rule in choose_tile does not take
 constexpr int kBlockK = 64;  // bf16 elements = 128 B = one swizzle row
 constexpr int kMaxA = 6;     // A tensor maps per launch
 constexpr int kMaxSeg = 12;  // K segments per launch
-// threads = 64 + 32 * EW: warp 0 TMA, warp 1 MMA, EW epilogue warps (8, or 16 for the short-K GEMMs whose tiles
-// are bound by the epilogue's instruction latency rather than by the mainloop)
-constexpr uint32_t kABytes = kBlockM * kBlockK * 2;
+// A 256-row tile (160 accumulator registers per thread) or a 256-column one (128) does not fit the 168 registers that 288
+// threads leave each thread: those instantiations launch a whole producer warpgroup (384 threads, one warp of it works) that
+// hands its registers to the consumers (setmaxnreg: 128 x 40 + 256 x 232 = 64512 of the SM's 65536).
+__host__ __device__ constexpr bool igemm_realloc(int BM, int BN) { return BM == 256 || BN == 256; }
+__host__ __device__ constexpr int igemm_threads(int BM, int BN, int EW) { return 32 * EW + (igemm_realloc(BM, BN) ? 128 : 32); }
+// TMA-store staging boxes (1 KB) per epilogue warp: four, or two where four 52 KB stages leave no room for more
+__host__ __device__ constexpr int igemm_boxes(int BM) { return BM == 256 ? 2 : 4; }
 
 struct ASeg {
   int16_t tmap;  // which A tensor map
@@ -45,7 +50,7 @@ struct alignas(64) IgemmParams {
   int kb_total;      // total k-blocks over all segments
   int ksplit;        // split-K factor (>=1); >1 => fp32 partial output
   int kb_per_split;  // ceil(kb_total / ksplit)
-  int TW, TH, TB;    // M tile = TW*TH*TB = 128 output pixels
+  int TW, TH, TB;    // M tile = TW*TH*TB = BM output pixels
   int Wo, Ho, Bo;    // output pixel grid (GEMM view: Wo = M, Ho = Bo = 1)
   int tilesW, tilesH, tilesB, tilesN;
   int N;             // valid output columns (GEGLU: packed columns, output has N/2)
@@ -104,8 +109,8 @@ VDB_DEVINL float apply_act(float v, int act) {
 // from per-32-channel partial sums that the PRODUCER of x wrote from its own epilogue (mode 7 = mode 3 + those sums).  When x is
 // the B operand (the transposed V^T projection) the statistics belong to the output columns instead (ln_on_cols).
 //
-// Roles: warps 0-7 are two consumer warpgroups (warpgroup g computes output rows [64 g, 64 g + 64) of the tile with wgmma, fp32
-// accumulators in registers), warp 8 is the TMA producer.
+// Roles: warps 0-7 are two consumer warpgroups (warpgroup g computes output rows [BM / 2 * g, BM / 2 * (g + 1)) of the tile with
+// wgmma, as BM / 128 blocks of 64 rows that share the W descriptor, fp32 accumulators in registers), warp 8 is the TMA producer.
 // Modes 3-7 run the epilogue from the registers, in the wgmma fragment layout: warp w owns 16 rows of the tile and walks their
 // 32-column chunks, staging each as a 16 x 32 bf16 box (stmatrix) for a TMA store.  The warpgroups do not wait for each other
 // after the mainloop, and the producer is gated by the empty barriers alone: it loads the next tile's first STAGES k-blocks while
@@ -114,8 +119,8 @@ VDB_DEVINL float apply_act(float v, int act) {
 // runs the epilogue on it: each warp reads 32-column chunks of one ROW per thread (acc_ld32), the layout its paths are written
 // for.  The producer starts the next tile's loads once every consumer warp is done with sacc (acc_free;
 // tests/test_igemm_protocol.py).
-template <int BN, int STAGES, int EW, int MODE>
-__global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
+template <int BM, int BN, int STAGES, int EW, int MODE>
+__global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
   constexpr bool kTmaEpi = MODE >= 3;                 // TMA-store epilogues
   constexpr bool kGegluEpi = MODE == 4 || MODE == 6;
   constexpr bool kLnIn = MODE == 5 || MODE == 6;
@@ -123,12 +128,17 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
   constexpr int kNumEpiWarps = EW;
   constexpr int kNumEpiThreads = EW * 32;
   constexpr int kWPQ = EW / 4;           // epilogue warps per 32-row quarter of the tile
-  static_assert(EW == 8, "two consumer warpgroups of 64 rows each");
+  static_assert(EW == 8, "two consumer warpgroups");
+  static_assert(BM == 128 || (BM == 256 && (MODE == 3 || MODE == 7) && BN <= 160), "256-row tiles: modes 3 and 7, 160 accumulator registers");
+  constexpr int kMB = BM / 128;          // 64-row blocks per consumer warpgroup
+  constexpr int kBoxes = igemm_boxes(BM);
+  constexpr uint32_t kStgWarp = kBoxes * 1024;   // staging bytes per epilogue warp
+  constexpr uint32_t kABytes = BM * kBlockK * 2;
   constexpr uint32_t kBBytes = BN * kBlockK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
   constexpr int kAccStride = BN + 4;     // sacc row stride in floats (row-per-thread 16-byte reads are conflict-free)
   constexpr uint32_t kRingBytes = STAGES * kStageBytes;
-  constexpr uint32_t kAccBytes = kBlockM * kAccStride * 4;
+  constexpr uint32_t kAccBytes = MODE >= 3 ? 0 : BM * kAccStride * 4;
   constexpr uint32_t kRegion = kRingBytes > kAccBytes ? kRingBytes : kAccBytes;
   static_assert(kBBytes % 1024 == 0, "B stage must keep 1024B alignment");
   static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "invalid wgmma N");
@@ -139,8 +149,8 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
   uint8_t* smemB = smem + STAGES * kABytes;
   float* sacc = reinterpret_cast<float*>(smem);                            // [128][kAccStride] fp32 accumulator of the tile
   float* sstage = reinterpret_cast<float*>(smem + kRegion);                // kNumEpiWarps x 4 KB, 1024-byte aligned: [32][32] fp32
-                                                                           // transposition tiles, or 2 x 2 KB bf16 TMA-store tiles
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRegion + EW * 4096);
+                                                                           // transposition tiles, or kBoxes 1 KB bf16 TMA-store boxes
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRegion + EW * kStgWarp);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* acc_free = empty_bar + STAGES;    // [1]
   float* sbias = reinterpret_cast<float*>(acc_free + 2);      // [BN] bias of the current output tile
@@ -178,9 +188,10 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
   // Tile walk of this CTA (both roles use the same bounds): tiles c, c + grid, ..., with M as the fast tile index.
   const int t_first = blockIdx.x, t_step = gridDim.x, t_end = num_tiles;
 
-  if (warp == EW) {
+  if (warp >= EW) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    if constexpr (igemm_realloc(BM, BN)) setmaxnreg_dec<40>();     // the whole producer warpgroup; warp EW alone works
+    if (warp == EW && lane == 0) {
       uint32_t stage = 0, phase = 0;
       const bool flat = (p.tilesH == 1) && (p.tilesB == 1);
       const int step_m = t_step % unitsM, step_r = t_step / unitsM;
@@ -232,6 +243,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
     // XOR-swizzled 4 KB shared-memory tile and read it back transposed, so every global access is 8 rows x 64 contiguous
     // bytes per instruction (4 lanes per row), and bias / activation / residual / bf16 conversion run on 8 fixed columns
     // per lane (bias lives in registers).
+    if constexpr (igemm_realloc(BM, BN)) setmaxnreg_inc<232>();
     const int quarter = warp & 3;          // 32-row quarter of the tile
     const int half = warp >> 2;            // which of the kWPQ warps of the quarter
     const int r = quarter * 32 + lane;
@@ -246,22 +258,29 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         v[4 * i + 2] = __float_as_uint(x.z); v[4 * i + 3] = __float_as_uint(x.w);
       }
     };
-    // mainloop of one tile: warpgroup g multiplies its 64 rows of A by the BN x 64 B tile of every k-block, then (modes 0-2)
-    // both warpgroups park the accumulator in sacc
+    // mainloop of one tile: warpgroup g multiplies its kMB blocks of 64 rows of A by the BN x 64 B tile of every k-block (block
+    // hb sits 8 KB after block hb - 1 in the stage), then (mode 0) both warpgroups park the accumulator in sacc
     uint32_t ml_stage = 0, ml_phase = 0;
-    float acc[BN / 2];
+    float acc[kMB][BN / 2];
     auto mainloop = [&](int kb_begin, int kb_end) {
       const int g = warp >> 2;
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int hb = 0; hb < kMB; ++hb)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[hb][i] = 0.f;
       uint32_t prev = 0;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&full_bar[ml_stage], ml_phase);
         wgmma_fence();
-        const uint64_t adesc = make_desc_sw128(smem_u32(smemA + ml_stage * kABytes + g * (64 * 128)));
+        uint64_t adesc[kMB];
+#pragma unroll
+        for (int hb = 0; hb < kMB; ++hb)
+          adesc[hb] = make_desc_sw128(smem_u32(smemA + ml_stage * kABytes + (g * kMB + hb) * (64 * 128)));
         const uint64_t bdesc = make_desc_sw128(smem_u32(smemB + ml_stage * kBBytes));
 #pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) wgmma_ss<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb > kb_begin || k > 0) ? 1u : 0u);
+        for (int k = 0; k < kBlockK / 16; ++k)
+#pragma unroll
+          for (int hb = 0; hb < kMB; ++hb) wgmma_ss<BN>(acc[hb], adesc[hb] + 2 * k, bdesc + 2 * k, (kb > kb_begin || k > 0) ? 1u : 0u);
         wgmma_commit();
         if (kb > kb_begin) {            // the previous k-block's MMAs have read their stage: hand it back to the producer
           wgmma_wait<1>();
@@ -272,7 +291,8 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         if (++ml_stage == STAGES) { ml_stage = 0; ml_phase ^= 1; }
       }
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int hb = 0; hb < kMB; ++hb) wgmma_fence_regs(acc[hb]);
       __syncwarp();
       if (lane == 0 && kb_end > kb_begin) mbar_arrive(&empty_bar[prev]);
       if constexpr (!kTmaEpi) {
@@ -280,8 +300,8 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         float* srow = sacc + (g * 64 + (warp & 3) * 16 + (lane >> 2)) * kAccStride + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(srow + 8 * kAccStride + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[0][4 * j], acc[0][4 * j + 1]);
+          *reinterpret_cast<float2*>(srow + 8 * kAccStride + 8 * j) = make_float2(acc[0][4 * j + 2], acc[0][4 * j + 3]);
         }
         epi_bar_sync();
       }
@@ -300,7 +320,7 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       o[0] = x0.x; o[1] = x0.y; o[2] = x0.z; o[3] = x0.w; o[4] = x1.x; o[5] = x1.y; o[6] = x1.z; o[7] = x1.w;
     };
     int it = 0;
-    int st_buf = 0;                     // TMA-store epilogues: which of this warp's four staging boxes is written next
+    int st_buf = 0;                     // TMA-store epilogues: which of this warp's kBoxes staging boxes is written next
     (void)st_buf;
     const float* sbias_src = nullptr;   // which bias row/offset currently sits in sbias
     // The per-tile bookkeeping sits on the critical path of epilogue-bound GEMMs (it was ~0.75 us of every ~3.6 us
@@ -312,16 +332,18 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
     const bool flat = (p.tilesH == 1) && (p.tilesB == 1);   // GEMM view: M tiles along W only
     const int step_m = t_step % unitsM, step_r = t_step / unitsM;
     int unit_m = t_first % unitsM, rest = t_first / unitsM;
-    // TMA-store epilogues: the accumulator stays in the wgmma fragment layout, so warp w owns the 16 tile rows from e_row0 on
-    // (warpgroup w / 4, quarter w % 4) and this thread rows e_row0 + lane / 4 and e_row0 + lane / 4 + 8, at columns
-    // 8 j + 2 (lane % 4) + {0, 1}
-    const int e_row0 = (warp >> 2) * 64 + (warp & 3) * 16;
-    int e_tw[2], e_th[2], e_tb[2];
+    // TMA-store epilogues: the accumulator stays in the wgmma fragment layout, so in each 64-row block hb of its warpgroup warp w
+    // owns the 16 tile rows from e_row0 + 64 hb on (warpgroup w / 4, quarter w % 4) and this thread rows + lane / 4 and
+    // + lane / 4 + 8 of them, at columns 8 j + 2 (lane % 4) + {0, 1}
+    const int e_row0 = (warp >> 2) * (BM / 2) + (warp & 3) * 16;
+    int e_tw[kMB][2], e_th[kMB][2], e_tb[kMB][2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int er = e_row0 + (lane >> 2) + 8 * h;
-      e_tw[h] = er % p.TW; e_th[h] = (er / p.TW) % p.TH; e_tb[h] = er / (p.TW * p.TH);
-    }
+    for (int hb = 0; hb < kMB; ++hb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int er = e_row0 + 64 * hb + (lane >> 2) + 8 * h;
+        e_tw[hb][h] = er % p.TW; e_th[hb][h] = (er / p.TW) % p.TH; e_tb[hb][h] = er / (p.TW * p.TH);
+      }
     // folded LayerNorm, row statistics: partial sums of the warp's rows in the NEXT tile, requested a tile ahead.  Lane l serves
     // row e_row0 + l % 16: lanes 0-15 load partials 0-7, lanes 16-31 partials 8-15 of the same rows (kLnPre each)
     constexpr int kLnPre = 8;
@@ -426,23 +448,25 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
       const bool has_resid = p.resid != nullptr;
 
       // TMA-store epilogues: output pixels (GEMM rows) of this thread's two accumulator rows
-      int e_gp[2];
-      bool e_ok[2];
+      int e_gp[kMB][2];
+      bool e_ok[kMB][2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int ew = wt * p.TW + e_tw[h], eh = ht * p.TH + e_th[h], eb = bt * p.TB + e_tb[h];
-        e_ok[h] = (ew < p.Wo) && (eh < p.Ho) && (eb < p.Bo);
-        e_gp[h] = (eb * p.Ho + eh) * p.Wo + ew;
-      }
+      for (int hb = 0; hb < kMB; ++hb)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int ew = wt * p.TW + e_tw[hb][h], eh = ht * p.TH + e_th[hb][h], eb = bt * p.TB + e_tb[hb][h];
+          e_ok[hb][h] = (ew < p.Wo) && (eh < p.Ho) && (eb < p.Bo);
+          e_gp[hb][h] = (eb * p.Ho + eh) * p.Wo + ew;
+        }
       // folded LayerNorm: the scalars of this thread's two rows (requested before the accumulator wait)
       float ln_a0[2] = {0.f, 0.f}, ln_a1[2] = {1.f, 1.f};   // on_cols 0: (mean, rstd) of the row;  on_cols 1: (s[m], c[m]) of the output row
       if constexpr (kLnIn) {
         if (p.ln_on_cols) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (e_ok[h]) {
-              ln_a0[h] = __ldg(p.ln_colsum + e_gp[h]);
-              ln_a1[h] = p.ln_rowbias ? __ldg(p.ln_rowbias + e_gp[h]) : 0.f;
+            if (e_ok[0][h]) {
+              ln_a0[h] = __ldg(p.ln_colsum + e_gp[0][h]);
+              ln_a1[h] = p.ln_rowbias ? __ldg(p.ln_rowbias + e_gp[0][h]) : 0.f;
             }
           }
         } else {
@@ -528,10 +552,10 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         // walks the 32-column chunks of its 16 rows: per-element fp32 arithmetic on the thread's 2 rows x 8 columns of the chunk,
         // bf16 pack, two stmatrix into one 1 KB staging box of this warp (16 rows of 64 B, SWIZZLE_64B pattern), then lane 0
         // hands the box to the TMA unit (cp.async.bulk.tensor store; out-of-range rows / columns are clipped by the tensor
-        // map).  Four boxes per warp rotate: a box is rewritten once the store issued from it three chunks ago has read it.
-        // Bias / LayerNorm tables are read from shared memory as 8-byte broadcasts (columns 2 (lane % 4) + {0, 1}).
-        const uint32_t stg_s = smem_u32(sstage) + warp * 4096;
-        const int ow = wt * p.TW + (e_row0 % p.TW), oh = ht * p.TH + ((e_row0 / p.TW) % p.TH), ob = bt * p.TB + e_row0 / (p.TW * p.TH);
+        // map).  The kBoxes boxes of a warp rotate: a box is rewritten once the store issued from it kBoxes - 1 chunks ago has
+        // read it.  Bias / LayerNorm tables are read from shared memory as 8-byte broadcasts (columns 2 (lane % 4) + {0, 1}).
+        // A 256-row tile runs this once per 64-row block of the warpgroup.
+        const uint32_t stg_s = smem_u32(sstage) + warp * kStgWarp;
         constexpr int OUTC = kGegluEpi ? BN / 2 : BN;                    // output columns per tile
         const int ochunks = kGegluEpi ? OUTC / 32 : f_nchunks;
         const int ocol0 = n_idx * OUTC;
@@ -539,146 +563,151 @@ __global__ void __launch_bounds__(32 + 32 * EW, 1) igemm_kernel(const __grid_con
         // residual (modes 3 / 7): the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each,
         // requested a chunk ahead
         const bool do_resid = (MODE == 3 || MODE == 7) && has_resid;
-        const uint32_t* rrow[2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-          rrow[h] = (do_resid && e_ok[h]) ? reinterpret_cast<const uint32_t*>(p.resid + static_cast<long long>(e_gp[h]) * p.ldr + ocol0 + tq2)
-                                          : nullptr;
-        auto load_resid = [&](int c, uint32_t (&rr)[2][4]) {
+        for (int hb = 0; hb < kMB; ++hb) {
+          const int b_row0 = e_row0 + 64 * hb;
+          const int ow = wt * p.TW + (b_row0 % p.TW), oh = ht * p.TH + ((b_row0 / p.TW) % p.TH), ob = bt * p.TB + b_row0 / (p.TW * p.TH);
+          const uint32_t* rrow[2];
 #pragma unroll
           for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rrow[h] ? __ldg(rrow[h] + (c * 32 + 8 * jj) / 2) : 0u;
-        };
-        uint32_t rr[2][4];
-        if (do_resid) load_resid(0, rr);
-        float st_su[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // mode 7: [row][chunk parity]
-        (void)st_su; (void)st_sq;
-        float nrm[2];                                                    // LN rows: -rstd * mean of the row
-#pragma unroll
-        for (int h = 0; h < 2; ++h) nrm[h] = -ln_a1[h] * ln_a0[h];
-        (void)nrm;
-#pragma unroll
-        for (int c = 0; c < OUTC / 32; ++c) {
-          if (c >= ochunks) break;
-          float o[4][2][2];                                              // [8-column group][row][column]
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int n = c * 32 + 8 * jj + tq2;                         // tile column of o[jj][.][0]
-            const float* va = acc + 4 * (4 * c + jj);                    // {row 0: n, n + 1; row 8: n, n + 1}
-            if constexpr (kGegluEpi) {
-              const float* vg = acc + 4 * (BN / 16 + 4 * c + jj);        // gate columns OUTC + n
-              if constexpr (kLnIn) {   // GEGLU over a folded LayerNorm: r * (acc - mu * s) + c == fma(r, acc, fma(-r mu, s, c))
-                const float2 sa = lds_f2(slnx_s + 4 * n), ca = lds_f2(sbias_s + 4 * n);
-                const float2 sg = lds_f2(slnx_s + 4 * (OUTC + n)), cg = lds_f2(sbias_s + 4 * (OUTC + n));
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h], fmaf(nrm[h], sg.x, cg.x)));
-                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h + 1], fmaf(nrm[h], sg.y, cg.y)));
-                }
-              } else {
-                const float2 ba = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
-                const float2 bg = p.bias ? lds_f2(sbias_s + 4 * (OUTC + n)) : make_float2(0.f, 0.f);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  o[jj][h][0] = (va[2 * h] + ba.x) * gelu_fast_f(vg[2 * h] + bg.x);
-                  o[jj][h][1] = (va[2 * h + 1] + ba.y) * gelu_fast_f(vg[2 * h + 1] + bg.y);
-                }
-              }
-            } else if constexpr (kLnIn) {
-              if (p.ln_on_cols) {      // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
-                const float2 mu = lds_f2(slnx_s + 4 * n), rs = lds_f2(sbias_s + 4 * n);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  o[jj][h][0] = fmaf(rs.x, fmaf(mu.x, -ln_a0[h], va[2 * h]), ln_a1[h]);
-                  o[jj][h][1] = fmaf(rs.y, fmaf(mu.y, -ln_a0[h], va[2 * h + 1]), ln_a1[h]);
-                }
-              } else {                 // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
-                const float2 sx = lds_f2(slnx_s + 4 * n), cx = lds_f2(sbias_s + 4 * n);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sx.x, cx.x));
-                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sx.y, cx.y));
-                }
-              }
-            } else {                   // modes 3 / 7: acc + bias, then + residual
-              const float2 bb = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                o[jj][h][0] = va[2 * h] + bb.x;
-                o[jj][h][1] = va[2 * h + 1] + bb.y;
-              }
-            }
-          }
-          if (do_resid) {
-            uint32_t rn[2][4];
-            const bool more = c + 1 < ochunks;
-            if (more) load_resid(c + 1, rn);
+            rrow[h] = (do_resid && e_ok[hb][h]) ? reinterpret_cast<const uint32_t*>(p.resid + static_cast<long long>(e_gp[hb][h]) * p.ldr + ocol0 + tq2)
+                                                : nullptr;
+          auto load_resid = [&](int c, uint32_t (&rr)[2][4]) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const float2 x = unpack_bf16x2(rr[h][jj]);
-                o[jj][h][0] += x.x;
-                o[jj][h][1] += x.y;
+              for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rrow[h] ? __ldg(rrow[h] + (c * 32 + 8 * jj) / 2) : 0u;
+          };
+          uint32_t rr[2][4];
+          if (do_resid) load_resid(0, rr);
+          float st_su[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // mode 7: [row][chunk parity]
+          (void)st_su; (void)st_sq;
+          float nrm[2];                                                    // LN rows: -rstd * mean of the row
+#pragma unroll
+          for (int h = 0; h < 2; ++h) nrm[h] = -ln_a1[h] * ln_a0[h];
+          (void)nrm;
+#pragma unroll
+          for (int c = 0; c < OUTC / 32; ++c) {
+            if (c >= ochunks) break;
+            float o[4][2][2];                                              // [8-column group][row][column]
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int n = c * 32 + 8 * jj + tq2;                         // tile column of o[jj][.][0]
+              const float* va = acc[hb] + 4 * (4 * c + jj);                // {row 0: n, n + 1; row 8: n, n + 1}
+              if constexpr (kGegluEpi) {
+                const float* vg = acc[hb] + 4 * (BN / 16 + 4 * c + jj);    // gate columns OUTC + n
+                if constexpr (kLnIn) {   // GEGLU over a folded LayerNorm: r * (acc - mu * s) + c == fma(r, acc, fma(-r mu, s, c))
+                  const float2 sa = lds_f2(slnx_s + 4 * n), ca = lds_f2(sbias_s + 4 * n);
+                  const float2 sg = lds_f2(slnx_s + 4 * (OUTC + n)), cg = lds_f2(sbias_s + 4 * (OUTC + n));
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h], fmaf(nrm[h], sg.x, cg.x)));
+                    o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h + 1], fmaf(nrm[h], sg.y, cg.y)));
+                  }
+                } else {
+                  const float2 ba = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
+                  const float2 bg = p.bias ? lds_f2(sbias_s + 4 * (OUTC + n)) : make_float2(0.f, 0.f);
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    o[jj][h][0] = (va[2 * h] + ba.x) * gelu_fast_f(vg[2 * h] + bg.x);
+                    o[jj][h][1] = (va[2 * h + 1] + ba.y) * gelu_fast_f(vg[2 * h + 1] + bg.y);
+                  }
+                }
+              } else if constexpr (kLnIn) {
+                if (p.ln_on_cols) {      // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
+                  const float2 mu = lds_f2(slnx_s + 4 * n), rs = lds_f2(sbias_s + 4 * n);
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    o[jj][h][0] = fmaf(rs.x, fmaf(mu.x, -ln_a0[h], va[2 * h]), ln_a1[h]);
+                    o[jj][h][1] = fmaf(rs.y, fmaf(mu.y, -ln_a0[h], va[2 * h + 1]), ln_a1[h]);
+                  }
+                } else {                 // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
+                  const float2 sx = lds_f2(slnx_s + 4 * n), cx = lds_f2(sbias_s + 4 * n);
+#pragma unroll
+                  for (int h = 0; h < 2; ++h) {
+                    o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sx.x, cx.x));
+                    o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sx.y, cx.y));
+                  }
+                }
+              } else {                   // modes 3 / 7: acc + bias, then + residual
+                const float2 bb = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = va[2 * h] + bb.x;
+                  o[jj][h][1] = va[2 * h + 1] + bb.y;
+                }
               }
-            if (more) {
+            }
+            if (do_resid) {
+              uint32_t rn[2][4];
+              const bool more = c + 1 < ochunks;
+              if (more) load_resid(c + 1, rn);
 #pragma unroll
               for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rn[h][jj];
+                for (int jj = 0; jj < 4; ++jj) {
+                  const float2 x = unpack_bf16x2(rr[h][jj]);
+                  o[jj][h][0] += x.x;
+                  o[jj][h][1] += x.y;
+                }
+              if (more) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                  for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rn[h][jj];
+              }
             }
+            if constexpr (kStatsOut) {
+              // LayerNorm statistics of the rows this GEMM produces (fp32, before the rounding), split by chunk parity
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    st_su[h][c & 1] += o[jj][h][e];
+                    st_sq[h][c & 1] = fmaf(o[jj][h][e], o[jj][h][e], st_sq[h][c & 1]);
+                  }
+            }
+            // the box about to be rewritten was handed to the TMA unit kBoxes - 1 chunks ago: wait until it has been read
+            if (lane == 0) bulk_wait_read<kBoxes - 1>();
+            __syncwarp();
+            const uint32_t box = stg_s + st_buf * 1024;
+            {
+              // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
+              // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
+              const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                const int unit = 2 * u + (mi >> 1);
+                stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
+                            pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
+                            pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
+              }
+            }
+            fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
+            __syncwarp();
+            if (lane == 0) {
+              tma_store_4d(&p.tmO, reinterpret_cast<const uint8_t*>(sstage) + warp * kStgWarp + st_buf * 1024, ocol0 + c * 32, ow, oh, ob);
+              bulk_commit();
+            }
+            st_buf = (st_buf + 1) & (kBoxes - 1);
           }
           if constexpr (kStatsOut) {
-            // LayerNorm statistics of the rows this GEMM produces (fp32, before the rounding), split by chunk parity
+            // one (sum, sum of squares) per row, N tile and chunk parity: slot 2 n_idx + parity of [2 tilesN][M][2].  The four lanes
+            // of a row reduce over the quad; a parity without chunks writes zeros
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
-              for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  st_su[h][c & 1] += o[jj][h][e];
-                  st_sq[h][c & 1] = fmaf(o[jj][h][e], o[jj][h][e], st_sq[h][c & 1]);
-                }
+              for (int par = 0; par < 2; ++par) {
+                float su = st_su[h][par], sq = st_sq[h][par];
+                su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+                su += __shfl_xor_sync(0xffffffffu, su, 2); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+                if ((lane & 3) == 0 && e_ok[hb][h])
+                  reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * 2 + par) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + e_gp[hb][h]] =
+                      make_float2(su, sq);
+              }
           }
-          // the box about to be rewritten was handed to the TMA unit three chunks ago: wait until it has been read
-          if (lane == 0) bulk_wait_read<3>();
-          __syncwarp();
-          const uint32_t box = stg_s + st_buf * 1024;
-          {
-            // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
-            // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
-            const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int unit = 2 * u + (mi >> 1);
-              stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
-                          pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
-                          pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
-            }
-          }
-          fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_4d(&p.tmO, reinterpret_cast<const uint8_t*>(sstage) + warp * 4096 + st_buf * 1024, ocol0 + c * 32, ow, oh, ob);
-            bulk_commit();
-          }
-          st_buf = (st_buf + 1) & 3;
-        }
-        if constexpr (kStatsOut) {
-          // one (sum, sum of squares) per row, N tile and chunk parity: slot 2 n_idx + parity of [2 tilesN][M][2].  The four lanes
-          // of a row reduce over the quad; a parity without chunks writes zeros
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int par = 0; par < 2; ++par) {
-              float su = st_su[h][par], sq = st_sq[h][par];
-              su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
-              su += __shfl_xor_sync(0xffffffffu, su, 2); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-              if ((lane & 3) == 0 && e_ok[h])
-                reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * 2 + par) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + e_gp[h]] =
-                    make_float2(su, sq);
-            }
         }
       } else if (p.ksplit > 1) {
         // fp32 partials, reduced (+bias/act/residual) by splitk_reduce_kernel
@@ -852,26 +881,26 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int kspl
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
-template <int BN, int STAGES, int EW, int MODE>
+template <int BM, int BN, int STAGES, int EW, int MODE>
 static int launch_igemm(const IgemmParams& p0, int num_units, cudaStream_t stream) {
   constexpr bool kLn = MODE == 5 || MODE == 6;       // one more [BN] fp32 table (colsum / column mean)
-  constexpr size_t ring = STAGES * (kABytes + BN * kBlockK * 2), acc = kBlockM * (BN + 4) * 4;   // (see igemm_kernel)
-  constexpr size_t need = (ring > acc ? ring : acc) + (2 * STAGES + 2) * 8 + BN * 4 + (kLn ? BN * 4 : 0) + EW * 4096;
+  constexpr size_t ring = STAGES * (BM + BN) * kBlockK * 2, acc = MODE >= 3 ? 0 : BM * (BN + 4) * 4;   // (see igemm_kernel)
+  constexpr size_t need = (ring > acc ? ring : acc) + (2 * STAGES + 2) * 8 + BN * 4 + (kLn ? BN * 4 : 0) + EW * igemm_boxes(BM) * 1024;
   // + up to 1024 bytes of slack for the 1024-byte alignment of the operand ring (the LN modes at BN 256 may get less: the dynamic
   // window starts 1024-aligned in practice, and the kernel traps if its carve-up would not fit)
   constexpr size_t smem = (need + 1024 <= 227 * 1024) ? need + 1024 : 227 * 1024;
   static_assert(need + 896 <= 227 * 1024, "igemm shared-memory budget");
-  constexpr int threads = 32 + 32 * EW;
+  constexpr int threads = igemm_threads(BM, BN, EW);
   IgemmParams p = p0;
   p.smem_bytes = static_cast<unsigned>(smem);
   static bool configured = false;
   if (!configured) {
-    VDB_CUDA_CHECK(cudaFuncSetAttribute(igemm_kernel<BN, STAGES, EW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    VDB_CUDA_CHECK(cudaFuncSetAttribute(igemm_kernel<BM, BN, STAGES, EW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         static_cast<int>(smem)));
     configured = true;
   }
   const int grid = std::min(num_units, num_sms());
-  VDB_CUDA_CHECK(launch_pdl(igemm_kernel<BN, STAGES, EW, MODE>, dim3(grid), dim3(threads), smem, stream, p));
+  VDB_CUDA_CHECK(launch_pdl(igemm_kernel<BM, BN, STAGES, EW, MODE>, dim3(grid), dim3(threads), smem, stream, p));
   count_launch();
   return VDB_OK;
 }
@@ -890,9 +919,11 @@ static int pick_bn(int N, int act, int forced) {
 
 static unsigned long long* g_timeline = nullptr;
 
-// The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN
+// The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN; and its tile
+// height (vdb_igemm_last_bm)
 constexpr int kPlanFields = 7;
 static thread_local int g_last_plan[kPlanFields] = {0};
+static thread_local int g_last_bm = 0;
 
 // Mode 0 stores bf16 output rows and loads residual rows as 16-byte vectors, the split-K reduction stores fp32 rows as float4,
 // and the TMA-store epilogues need a 16-byte aligned output map, so out / resid must be 16-byte aligned.  Checked before any
@@ -932,36 +963,97 @@ struct IgemmEpilogue {
   int out_parity = -1;
 };
 
-// Finish IgemmParams (tiling, split-K, B map) and launch.
+static int pow2_ceil(int v) { int t = 1; while (t < v) t <<= 1; return t; }
+
+// M tile = BM output pixels as a (TW, TH, TB) box of the (W, H, B) pixel grid; box extents are
+// powers of two so that TW*TH*TB == BM (rows past the grid are zero-filled by TMA and masked on store).
+// GEMM view (one row of M "pixels"): the box is always BM rows.
+static void set_tile_shape(IgemmParams& p, int BM, int Wo, int Ho, int Bo, bool gemm_view) {
+  p.Wo = Wo; p.Ho = Ho; p.Bo = Bo;
+  const int TW = gemm_view ? BM : std::min(pow2_ceil(Wo), BM);
+  const int TH = std::min(pow2_ceil(Ho), BM / TW);
+  const int TB = BM / (TW * TH);
+  p.TW = TW; p.TH = TH; p.TB = TB;
+  p.tilesW = (Wo + TW - 1) / TW;
+  p.tilesH = (Ho + TH - 1) / TH;
+  p.tilesB = (Bo + TB - 1) / TB;
+}
+
+// one bias row per tile: shared bias, or per-image rows with tiles that never straddle two images
+static bool one_bias_row(const IgemmParams& p, int BM, const IgemmEpilogue& e) {
+  const int rpb = e.rows_per_batch > 0 ? e.rows_per_batch : 1;
+  return e.bias == nullptr || e.bias_bstride == 0 ||
+         (p.TB == 1 && (static_cast<long long>(p.Ho) * p.Wo == rpb || (p.Ho == 1 && p.Bo == 1 && rpb % BM == 0)));
+}
+
+// `bn` argument of the entry points: a forced tile width, optionally with this flag for the 256-row tile (VDB_IGEMM_BM256)
+constexpr int kForceBM256 = 0x1000;
+
+// The (BM, BN) tile of a launch, from the shape alone unless the caller forces it.
+//
+// Model: the persistent grid runs waves = ceil(tiles / #SMs) rounds of one tile per CTA.  A k-block of a BM x BN tile costs the
+// longer of its wgmma time, 4 BN clocks per 128 rows (4096 dense bf16 FLOP per clock per SM), and its operand fill, (BM + BN) x
+// 128 bytes from L2 at kFillBytesPerClk per SM; a tile adds kTileClocks per 128 rows of pipeline fill and epilogue tail, a
+// split-K launch kSplitKClocks for its reduction pass.
+// kFillBytesPerClk = 42 is fitted to the 3x3 conv B 8, 64x64, 320 -> 320 timed alone at BN 64 / 128 / 160
+// (tools/igemm_tile_sweep.py) on an H100 80GB HBM3 at 700 W, taking 1.83 GHz: 590, 888 and 809 clocks per k-block.  So every
+// 128-row tile is fill-bound, (16384 + 128 BN) / 42 clocks per k-block against 4 BN of wgmma, and the 256 x 160 tile is the
+// first that is not: 1280 clocks of wgmma over 1268 of fill, for twice the rows of a 128 x 160 k-block that takes 878.
+// kTileClocks and kSplitKClocks were tuned against a fill term of 90 B/clk (1500 and 12000 clocks) on the 16x16 and 8x8 levels,
+// which have not been re-measured: they keep that ratio to the fill term, so no 128-row choice moves.
+//
+// A 256-row tile needs the plain TMA-store epilogue or its statistics-writing variant (modes 3 / 7 of igemm_kernel) and is
+// taken only where its tiles make one wave that covers at least 7/8 of the SMs (the 32x32 level of the UNet at batch 8: 128
+// tiles).  Fewer tiles (the 16x16 and 8x8 levels) would leave SMs idle for the whole launch.  More than one wave (the 64x64
+// level: 256 tiles) doubles the rows of A the CTAs of a wave hold in L2 between them: measured on the same card, its 3x3
+// convs from 640 and 960 channels ran 12 % and 44 % slower on 256 rows and the level as a whole lost.
+struct Tile { int BM, BN; };
+constexpr double kFillBytesPerClk = 42.0, kTileClocks = 1500.0 * 90.0 / kFillBytesPerClk, kSplitKClocks = 12000.0 * 90.0 / kFillBytesPerClk;
+
+static Tile choose_tile(int Wo, int Ho, int Bo, bool gemm_view, long long N, int kb_total, const IgemmEpilogue& e, int bn_arg,
+                        int ksplit_forced, const void* workspace) {
+  const int bn_forced = bn_arg & ~kForceBM256;
+  if (bn_arg & kForceBM256) return Tile{256, bn_forced};
+  Tile best_tile{kBlockM, pick_bn(static_cast<int>(N), e.act, bn_forced)};
+  if (bn_forced || e.act == ACT_GEGLU || kb_total < 8) return best_tile;
+  const bool stats = e.ln_stats != nullptr || e.stats_out != nullptr;
+  if (stats) ksplit_forced = 1;                          // the statistics ride on the single-pass TMA-store epilogues
+  IgemmParams s128, s256;
+  set_tile_shape(s128, 128, Wo, Ho, Bo, gemm_view);
+  set_tile_shape(s256, 256, Wo, Ho, Bo, gemm_view);
+  const bool can256 = !e.ln_stats && !e.out_f32 && e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0 && ksplit_forced <= 1 &&
+                      one_bias_row(s256, 256, e);
+  const Tile cand[5] = {{256, 160}, {128, 256}, {128, 160}, {128, 128}, {128, 64}};
+  double best = 1e30;
+  for (const Tile& c : cand) {
+    const IgemmParams& sh = c.BM == 256 ? s256 : s128;
+    const long long tiles = static_cast<long long>(sh.tilesW) * sh.tilesH * sh.tilesB * ((N + c.BN - 1) / c.BN);   // (a partial
+                                                                                         // last N tile is computed in full)
+    if (c.BM == 256 && (!can256 || tiles * 8 < num_sms() * 7LL || tiles > num_sms())) continue;
+    // split-K exactly as run_igemm decides it: small MN grids with a deep K run kb / ks blocks per unit plus a reduction pass
+    long long ks = 1;
+    if (ksplit_forced > 0) ks = ksplit_forced;
+    else if (tiles * 2 <= num_sms() && kb_total >= 16 && (N % 4) == 0 && workspace)
+      ks = std::max<long long>(1, std::min<long long>(std::min<long long>(num_sms() / tiles, kb_total / 8), 16));
+    const long long waves = (tiles * ks + num_sms() - 1) / num_sms();
+    const double rows = c.BM / 128.0;
+    const double per_kb = std::max(4.0 * c.BN * rows, (c.BM + c.BN) * 128.0 / kFillBytesPerClk);
+    const double kb_unit = static_cast<double>((kb_total + ks - 1) / ks);
+    const double cost = static_cast<double>(waves) * (kb_unit * per_kb + kTileClocks * rows) + (ks > 1 ? kSplitKClocks : 0.0);
+    if (cost < best * 0.97) { best = cost; best_tile = c; }     // (prefer the larger tile unless the gain is clear)
+  }
+  return best_tile;
+}
+
+// Finish IgemmParams (split-K, B map, epilogue) and launch; p holds the M tiling of `tile` (set_tile_shape).
 static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot, long long ldw,
-                     const IgemmEpilogue& e, int bn_forced, int ksplit_forced, void* workspace,
+                     const IgemmEpilogue& e, Tile tile, int ksplit_forced, void* workspace,
                      size_t ws_bytes, cudaStream_t stream) {
   const bool ln_in = e.ln_stats != nullptr, st_out = e.stats_out != nullptr;
   if (ln_in || st_out) ksplit_forced = 1;               // the statistics ride on the single-pass TMA-store epilogues
-  int BN = pick_bn(static_cast<int>(N), e.act, bn_forced);
-  // Tile-width model: the persistent grid runs
-  // waves = ceil(tiles / #SMs) rounds of one tile per CTA, a tile costs kb * c(BN) cycles of mainloop (operand fill at ~90 B/clk
-  // per SM or the MMA itself, whichever is longer) plus ~1500 cycles of pipeline fill / epilogue tail.  The divisibility rule sent
-  // e.g. M 2048 x N 1280 x K 1280 (15 launches per step) to BN 256 = 80 tiles on 148 SMs; BN 160 gives 128 shorter tiles.
-  if (!bn_forced && e.act != ACT_GEGLU && p.kb_total >= 8) {
-    const long long tm = static_cast<long long>(p.tilesW) * p.tilesH * p.tilesB;
-    const int cand[4] = {256, 160, 128, 64};
-    double best = 1e30;
-    for (int c : cand) {
-      const long long tiles = tm * ((N + c - 1) / c);      // (a partial last N tile is computed in full)
-      // split-K exactly as decided below: small MN grids with a deep K run kb / ks blocks per unit plus a reduction pass
-      long long ks = 1;
-      if (ksplit_forced > 0) ks = ksplit_forced;
-      else if (tiles * 2 <= num_sms() && p.kb_total >= 16 && (N % 4) == 0 && workspace)
-        ks = std::max<long long>(1, std::min<long long>(std::min<long long>(num_sms() / tiles, p.kb_total / 8), 16));
-      const long long waves = (tiles * ks + num_sms() - 1) / num_sms();
-      const double per_kb = std::max(2.0 * c, (16384.0 + 128.0 * c) / 90.0);
-      const double kb_unit = static_cast<double>((p.kb_total + ks - 1) / ks);
-      const double cost = static_cast<double>(waves) * (kb_unit * per_kb + 1500.0) + (ks > 1 ? 12000.0 : 0.0);
-      if (cost < best * 0.97) { best = cost; BN = c; }     // (prefer the wider tile unless the gain is clear)
-    }
-  }
+  const int BM = tile.BM, BN = tile.BN;
   if (BN != 64 && BN != 128 && BN != 160 && BN != 256) return set_error(VDB_ERR_INVALID, "igemm: bad BN");
+  if (BM == 256 && BN != 160) return set_error(VDB_ERR_INVALID, "igemm: the 256-row tile is 160 columns wide");
   if (e.act == ACT_GEGLU && (N % BN) != 0) return set_error(VDB_ERR_INVALID, "igemm: GEGLU needs N % 256 == 0");
   p.N = static_cast<int>(N);
   p.tilesN = static_cast<int>((N + BN - 1) / BN);
@@ -1001,11 +1093,7 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   const int num_tiles = mn_tiles * p.ksplit;
   // epilogue specialisation (see igemm_kernel): 3 = plain bf16 fast path, 4 = GEGLU, 0 = everything else
   int mode = 0;
-  // one bias row per tile: shared bias, or per-image rows with tiles that never straddle two images
-  const bool one_bias_row = e.bias == nullptr || e.bias_bstride == 0 ||
-                            (p.TB == 1 && (static_cast<long long>(p.Ho) * p.Wo == p.rows_per_batch ||
-                                           (p.Ho == 1 && p.Bo == 1 && p.rows_per_batch % kBlockM == 0)));
-  if (p.ksplit == 1 && !e.out_f32 && one_bias_row) {
+  if (p.ksplit == 1 && !e.out_f32 && one_bias_row(p, BM, e)) {
     if (e.act == ACT_GEGLU && BN == 256) mode = 4;
     else if (e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0) mode = 3;
   }
@@ -1039,42 +1127,48 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     if (ln_in && mode == 4 && e.ln_on_cols) return set_error(VDB_ERR_UNSUPPORTED, "igemm: GEGLU with column statistics");
     mode = st_out ? 7 : mode + 2;
   }
+  if (BM == 256 && mode != 3 && mode != 7)
+    return set_error(VDB_ERR_UNSUPPORTED, "igemm: the 256-row tile needs the plain TMA-store epilogue (bf16 out, no activation, alpha 1, "
+                                          "N %% 32 == 0, one bias row per tile, no split-K, no LayerNorm input)");
   {
-    const int stages = BN == 64 ? 8 : BN == 128 ? 6 : BN == 160 ? 5 : 4;   // (as instantiated below)
+    const int stages = BN == 64 ? 8 : BN == 128 ? 6 : (BN == 160 && BM == 128) ? 5 : 4;   // (as instantiated below)
     const int plan[kPlanFields] = {BN, stages, mode, p.ksplit, std::min(num_tiles, num_sms()), tilesM, p.tilesN};
     for (int i = 0; i < kPlanFields; ++i) g_last_plan[i] = plan[i];
+    g_last_bm = BM;
   }
-  if (mode == 7) {
+  if (BM == 256) {
+    rc = mode == 7 ? launch_igemm<256, 160, 4, 8, 7>(p, num_tiles, stream) : launch_igemm<256, 160, 4, 8, 3>(p, num_tiles, stream);
+  } else if (mode == 7) {
     switch (BN) {
-      case 64: rc = launch_igemm<64, 8, 8, 7>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 6, 8, 7>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<160, 5, 8, 7>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<256, 4, 8, 7>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 8, 7>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 8, 7>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 8, 7>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 8, 7>(p, num_tiles, stream); break;
     }
   } else if (mode == 6) {
-    rc = launch_igemm<256, 4, 8, 6>(p, num_tiles, stream);
+    rc = launch_igemm<128, 256, 4, 8, 6>(p, num_tiles, stream);
   } else if (mode == 5) {
     switch (BN) {
-      case 64: rc = launch_igemm<64, 8, 8, 5>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 6, 8, 5>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<160, 5, 8, 5>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<256, 4, 8, 5>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 8, 5>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 8, 5>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 8, 5>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 8, 5>(p, num_tiles, stream); break;
     }
   } else if (mode == 4) {
-    rc = launch_igemm<256, 4, 8, 4>(p, num_tiles, stream);
+    rc = launch_igemm<128, 256, 4, 8, 4>(p, num_tiles, stream);
   } else if (mode == 3) {
     switch (BN) {
-      case 64: rc = launch_igemm<64, 8, 8, 3>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 6, 8, 3>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<160, 5, 8, 3>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<256, 4, 8, 3>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 8, 3>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 8, 3>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 8, 3>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 8, 3>(p, num_tiles, stream); break;
     }
   } else {
     switch (BN) {
-      case 64: rc = launch_igemm<64, 8, 8, 0>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 6, 8, 0>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<160, 5, 8, 0>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<256, 4, 8, 0>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 8, 0>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 8, 0>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 8, 0>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 8, 0>(p, num_tiles, stream); break;
     }
   }
   if (rc) return rc;
@@ -1088,21 +1182,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     count_launch();
   }
   return VDB_OK;
-}
-
-static int pow2_ceil(int v) { int t = 1; while (t < v) t <<= 1; return t; }
-
-// M tile = 128 output pixels as a (TW, TH, TB) box of the (W, H, B) pixel grid; box extents are
-// powers of two so that TW*TH*TB == 128 (rows past the grid are zero-filled by TMA and masked on store).
-static void set_tile_shape(IgemmParams& p, int Wo, int Ho, int Bo) {
-  p.Wo = Wo; p.Ho = Ho; p.Bo = Bo;
-  const int TW = std::min(pow2_ceil(Wo), 128);
-  const int TH = std::min(pow2_ceil(Ho), 128 / TW);
-  const int TB = 128 / (TW * TH);
-  p.TW = TW; p.TH = TH; p.TB = TB;
-  p.tilesW = (Wo + TW - 1) / TW;
-  p.tilesH = (Ho + TH - 1) / TH;
-  p.tilesB = (Bo + TB - 1) / TB;
 }
 
 }  // namespace vdb
@@ -1123,6 +1202,9 @@ int vdb_igemm_last_plan(int* out, int n) {
   return kPlanFields;
 }
 
+// see include/vdb200.h
+int vdb_igemm_last_bm(void) { return g_last_bm; }
+
 // out[M,N] = act(alpha * ([A | A2] @ W^T + bias)) + resid     (see include/vdb200.h)
 int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const void* A2, long long K2,
                   long long lda2, const void* W, long long N, long long ldw, const float* bias,
@@ -1136,29 +1218,27 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
   if (M > 0x7fffffffLL || N > 0x7fffffffLL) return set_error(VDB_ERR_INVALID, "gemm: dimension too large");
   int rc = check_epilogue_pointers(out, ldo, out_f32, resid, ldr, "gemm");
   if (rc) return rc;
+  IgemmEpilogue e;
+  e.bias = bias; e.bias_bstride = bias_bstride; e.rows_per_batch = static_cast<int>(rows_per_batch);
+  e.resid = resid; e.ldr = ldr; e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.act = act; e.alpha = alpha;
   IgemmParams p;
   memset(&p, 0, sizeof(p));
-  // GEMM view of the pixel grid: one row of M "pixels"; the box is always 128 rows (TMA zero-fills past M)
-  p.Wo = static_cast<int>(M); p.Ho = 1; p.Bo = 1;
-  p.TW = kBlockM; p.TH = 1; p.TB = 1;
-  p.tilesW = static_cast<int>((M + kBlockM - 1) / kBlockM); p.tilesH = 1; p.tilesB = 1;
-  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
-  if (rc) return rc;
   p.seg[0] = ASeg{0, 0, 0, static_cast<int16_t>((K + kBlockK - 1) / kBlockK), 0};
   p.nseg = 1;
-  p.kb_total = p.seg[0].nkb;
+  p.kb_total = p.seg[0].nkb + (A2 ? static_cast<int>((K2 + kBlockK - 1) / kBlockK) : 0);
+  // GEMM view of the pixel grid: one row of M "pixels"; the box is always BM rows (TMA zero-fills past M)
+  const Tile tile = choose_tile(static_cast<int>(M), 1, 1, true, N, p.kb_total, e, bn, ksplit, workspace);
+  set_tile_shape(p, tile.BM, static_cast<int>(M), 1, 1, true);
+  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
+  if (rc) return rc;
   if (A2) {
     rc = make_tmap_4d(&p.tmA[1], A2, K2, M, 1, 1, lda2 * 2, lda2 * 2 * M, lda2 * 2 * M, kBlockK, p.TW, 1, 1);
     if (rc) return rc;
     p.seg[1] = ASeg{1, 0, 0, static_cast<int16_t>((K2 + kBlockK - 1) / kBlockK), 0};
     p.nseg = 2;
-    p.kb_total += p.seg[1].nkb;
   }
   for (int i = p.nseg; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
-  IgemmEpilogue e;
-  e.bias = bias; e.bias_bstride = bias_bstride; e.rows_per_batch = static_cast<int>(rows_per_batch);
-  e.resid = resid; e.ldr = ldr; e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.act = act; e.alpha = alpha;
-  return run_igemm(p, W, N, K + (A2 ? K2 : 0), ldw, e, bn, ksplit, workspace, ws_bytes,
+  return run_igemm(p, W, N, K + (A2 ? K2 : 0), ldw, e, tile, ksplit, workspace, ws_bytes,
                    reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -1179,22 +1259,21 @@ int vdb_gemm_ln_bf16(const void* A, long long M, long long K, long long lda, con
   if (stats_out && ((N % 32) || !stats_parts)) return set_error(VDB_ERR_INVALID, "gemm_ln: stats_out needs N %% 32 == 0 and stats_parts");
   int rc = check_epilogue_pointers(out, ldo, 0, resid, ldr, "gemm_ln");
   if (rc) return rc;
-  IgemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.Wo = static_cast<int>(M); p.Ho = 1; p.Bo = 1;
-  p.TW = kBlockM; p.TH = 1; p.TB = 1;
-  p.tilesW = static_cast<int>((M + kBlockM - 1) / kBlockM); p.tilesH = 1; p.tilesB = 1;
-  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
-  if (rc) return rc;
-  p.seg[0] = ASeg{0, 0, 0, static_cast<int16_t>((K + kBlockK - 1) / kBlockK), 0};
-  p.nseg = 1;
-  p.kb_total = p.seg[0].nkb;
-  for (int i = p.nseg; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
   IgemmEpilogue e;
   e.bias = bias; e.resid = resid; e.ldr = ldr; e.out = out; e.ldo = ldo; e.act = act;
   e.ln_stats = ln_stats; e.ln_mstat = ln_rows; e.ln_parts = ln_parts; e.ln_dim = ln_dim; e.ln_eps = ln_eps; e.ln_colsum = ln_colsum;
   e.ln_on_cols = ln_on_cols; e.ln_rowbias = ln_rowbias; e.stats_out = stats_out; e.stats_parts = stats_parts;
-  return run_igemm(p, W, N, K, ldw, e, bn, 1, nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
+  IgemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.seg[0] = ASeg{0, 0, 0, static_cast<int16_t>((K + kBlockK - 1) / kBlockK), 0};
+  p.nseg = 1;
+  p.kb_total = p.seg[0].nkb;
+  const Tile tile = choose_tile(static_cast<int>(M), 1, 1, true, N, p.kb_total, e, bn, 1, nullptr);
+  set_tile_shape(p, tile.BM, static_cast<int>(M), 1, 1, true);
+  rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
+  if (rc) return rc;
+  for (int i = p.nseg; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
+  return run_igemm(p, W, N, K, ldw, e, tile, 1, nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
 // 3x3 convolution on NHWC bf16 as implicit GEMM.
@@ -1230,9 +1309,15 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int Wd, int C, int mode, const
   IgemmParams p;
   memset(&p, 0, sizeof(p));
   const int Ho = strided ? H / 2 : H, Wo = strided ? Wd / 2 : Wd;
-  set_tile_shape(p, Wo, Ho, B);
   const uint64_t eb = 2;
   const int nkb = C / kBlockK;
+  IgemmEpilogue e;
+  e.bias = bias; e.bias_bstride = bias_bstride; e.rows_per_batch = Ho * Wo;
+  e.resid = resid; e.ldr = ldr; e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.act = act; e.alpha = 1.f;
+  e.out_parity = out_parity;
+  const Tile tile = choose_tile(Wo, Ho, B, false, N, (folded ? 4 : 9) * nkb + (skip1 ? Cs1 / kBlockK : 0) + (skip2 ? Cs2 / kBlockK : 0),
+                                e, bn, ksplit, workspace);
+  set_tile_shape(p, tile.BM, Wo, Ho, B, false);
   int nmaps = 0;
   int ntaps = 9;
   if (mode == 0 || folded) {
@@ -1288,11 +1373,7 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int Wd, int C, int mode, const
     ++nmaps;
   }
   for (int i = nmaps; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
-  IgemmEpilogue e;
-  e.bias = bias; e.bias_bstride = bias_bstride; e.rows_per_batch = Ho * Wo;
-  e.resid = resid; e.ldr = ldr; e.out = out; e.ldo = ldo; e.out_f32 = out_f32; e.act = act; e.alpha = 1.f;
-  e.out_parity = out_parity;
-  return run_igemm(p, Wt, N, static_cast<long long>(p.kb_total) * kBlockK, ldw, e, bn, ksplit, workspace, ws_bytes,
+  return run_igemm(p, Wt, N, static_cast<long long>(p.kb_total) * kBlockK, ldw, e, tile, ksplit, workspace, ws_bytes,
                    reinterpret_cast<cudaStream_t>(stream));
 }
 

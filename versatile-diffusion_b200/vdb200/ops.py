@@ -319,16 +319,17 @@ def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype
     return out
 
 
-IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n")
+IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n", "bm")   # (bm: vdb_igemm_last_bm)
+BM256 = 0x1000      # VDB_IGEMM_BM256: bn=160 | BM256 forces the 256-row tile of gemm / gemm_ln / conv3x3
 
 
 def igemm_last_plan():
     """The tiling of the last gemm / gemm_ln / conv3x3 launch on this thread (vdb_igemm_last_plan): which kernel instantiation
-    (BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile counts."""
-    buf = (ctypes.c_int * len(IGEMM_PLAN_FIELDS))()
+    (BM, BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile counts."""
+    buf = (ctypes.c_int * (len(IGEMM_PLAN_FIELDS) - 1))()
     n = lib.vdb_igemm_last_plan(buf, len(buf))
-    assert n == len(IGEMM_PLAN_FIELDS), n
-    return dict(zip(IGEMM_PLAN_FIELDS, buf))
+    assert n == len(buf), n
+    return dict(zip(IGEMM_PLAN_FIELDS, list(buf) + [lib.vdb_igemm_last_bm()]))
 
 
 class LnFold(object):
