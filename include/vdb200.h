@@ -80,6 +80,28 @@ int vdb_mask_to_latent(const float* mask, int n, int H8, int W8, float* out, voi
  * mask [n, hw] (mask_per_item != 0) or [1, hw]; out may alias decoded or image */
 int vdb_composite_f32(const float* decoded, const float* image, const float* mask, int mask_per_item, int n, int c, long long hw,
                       float* out, void* stream);
+/* ---- editing: DDIM inversion and DiffEdit — lib/model_zoo/edit.py (an addition: the reference has no inversion and no
+ * editing; the semantics are specified in that module's docstring) ------------------------------------------------------------------
+ * vdb_latent_store_slot_f32: ring[s] = x with s = *step_idx + offset (device int, required), slot s at ring + s*n; x and the ring
+ * fp32 of n and slots*n elements.  A slot outside [0, slots) is not written.  VDB_ERR_INVALID before any launch: a null x / ring /
+ * step_idx, n <= 0 or slots <= 0, a pointer not 16-byte aligned, or x overlapping the ring. */
+int vdb_latent_store_slot_f32(const float* x, float* ring, int slots, const int* step_idx, int offset, long long n, void* stream);
+/* vdb_inversion_blend_f32, after each step of a walk from an inversion: x fp32 NHWC [bs, hw, c]; ring fp32 [slots, bs, hw, c], the
+ * inversion's trajectory; mask fp32 [bs, hw] (mask_per_item != 0) or [1, hw], 1 = generate, 0 = keep, broadcast over c.  Per element,
+ * with k = ring[*step_idx] (device int, required), fp32 with explicit round-to-nearest, the formula of vdb_inpaint_blend_f32:
+ * x = m == 1 ? x : m == 0 ? k : m*x + (1 - m)*k;  x_dup (may be NULL) receives a copy.  A *step_idx outside [0, slots) reads
+ * nothing and leaves x and x_dup as they are.  VDB_ERR_INVALID before any launch: a null
+ * x / ring / mask / step_idx, a size <= 0, a pointer not 16-byte aligned, or the ring or mask overlapping x or x_dup. */
+int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots, const float* mask, int mask_per_item,
+                            const int* step_idx, int bs, long long hw, int c, void* stream);
+/* vdb_diffedit_mask_f32: DiffEdit's mask of bs images from D noise draws.  e_* fp32 NHWC [D*bs, hw, c] (draw d of image b at row
+ * d*bs + b); e_src_u / e_tgt_u may be NULL (that side has no CFG: E = e_c), else E = e_u + s*(e_c - e_u).  out fp32 [bs, hw]:
+ * dist(p) = (sum over d, then c, of |E_tgt - E_src|) / (D c);  cap = ratio * mean_p dist;  out = cap > 0 && min(dist, cap)/cap >= 0.5
+ * ? 1 : 0.  One CTA per image, every sum in an order fixed by the shape, so the result is bit-reproducible.  VDB_ERR_INVALID before
+ * any launch: a null e_src_c / e_tgt_c / out, a size <= 0, ratio not finite and > 0, a pointer not 16-byte aligned, or out
+ * overlapping an input. */
+int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,
+                          float s_tgt, int D, int bs, long long hw, int c, float ratio, float* out, void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */

@@ -159,6 +159,11 @@ __global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const 
 // ---------------------------------------------------------------------------------------------
 constexpr unsigned kInpaintTag = 0x696e7074u;   // "inpt": the text decoder's stream uses "text" (0x74657874)
 
+// the per-element blend of the inpainting and the inversion blends: m x + (1 - m) k, selecting exactly at m = 1 and m = 0
+__device__ __forceinline__ float mask_blend(float m, float x, float k) {
+  return m == 1.f ? x : m == 0.f ? k : __fadd_rn(__fmul_rn(m, x), __fmul_rn(__fsub_rn(1.f, m), k));
+}
+
 // Four standard normals of counter (quad, step, "inpt", 0) under a 64-bit key: two Box-Muller pairs, u = (b + 0.5) 2^-32 in
 // fp64 (never 0 or 1), (r cos 2 pi u', r sin 2 pi u') with r = sqrt(-2 ln u), rounded to fp32.
 __device__ __forceinline__ void inpaint_normals(unsigned long long key, unsigned quad, int step, float z[4]) {
@@ -209,7 +214,7 @@ __global__ void inpaint_blend_kernel(float* x, float* __restrict__ x_dup, const 
       const long long pix = (i + q) / c;
       const float m = mask[mask_per_item ? pix : pix % hw];
       const float k = __fadd_rn(__fmul_rn(a, kv[q]), __fmul_rn(b, zv[q]));
-      xv[q] = m == 1.f ? xv[q] : m == 0.f ? k : __fadd_rn(__fmul_rn(m, xv[q]), __fmul_rn(__fsub_rn(1.f, m), k));
+      xv[q] = mask_blend(m, xv[q], k);
     }
     if (full) {
       *reinterpret_cast<float4*>(x + i) = *reinterpret_cast<float4*>(xv);
@@ -268,6 +273,114 @@ __global__ void composite_kernel(const float* decoded, const float* image, const
     const float d = decoded[e], im = image[e];
     out[e] = m == 1.f ? d : m == 0.f ? im : __fadd_rn(__fmul_rn(m, d), __fmul_rn(__fsub_rn(1.f, m), im));
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Editing (lib/model_zoo/edit.py): DDIM inversion and DiffEdit.
+// ring[*step_idx + offset] = x: the inversion walk records its trajectory from inside the captured step graph, where a memcpy
+// node's destination would be fixed at capture time.  A slot outside [0, slots) is not written.  n = elements per slot.
+// ---------------------------------------------------------------------------------------------
+__global__ void latent_store_slot_kernel(const float* __restrict__ x, float* __restrict__ ring, int slots,
+                                         const int* __restrict__ step_idx, int offset, long long n) {
+  const int s = *step_idx + offset;
+  if (s < 0 || s >= slots) return;
+  float* dst = ring + static_cast<long long>(s) * n;
+  const bool vec = (n & 3) == 0;
+  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) * 4; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x * 4) {
+    if (vec) {
+      *reinterpret_cast<float4*>(dst + i) = __ldg(reinterpret_cast<const float4*>(x + i));
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) dst[i + q] = x[i + q];
+    }
+  }
+}
+
+// After forward step *step_idx of a walk from an inversion: x = m x + (1 - m) slot, slot = ring + *step_idx * n, the
+// trajectory's latent at the step's target level.  mask [bs | 1, hw] broadcast over c; x_dup (may be NULL) receives a copy.
+// A slot outside [0, slots) is not read: x and x_dup are left as they are.
+__global__ void inversion_blend_kernel(float* x, float* __restrict__ x_dup, const float* __restrict__ ring, int slots,
+                                       const float* __restrict__ mask, int mask_per_item, const int* __restrict__ step_idx,
+                                       long long n, long long hw, int c) {
+  const int s = *step_idx;
+  if (s < 0 || s >= slots) return;
+  const float* slot = ring + static_cast<long long>(s) * n;
+  const bool vec = (n & 3) == 0;
+  for (long long i = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) * 4; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x * 4) {
+    const bool full = i + 3 < n;
+    float xv[4], kv[4];
+    if (full) {
+      *reinterpret_cast<float4*>(xv) = *reinterpret_cast<const float4*>(x + i);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) xv[q] = x[i + q];
+    }
+    if (full && vec) {
+      *reinterpret_cast<float4*>(kv) = __ldg(reinterpret_cast<const float4*>(slot + i));
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) kv[q] = slot[i + q];
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (i + q >= n) break;
+      const long long pix = (i + q) / c;
+      xv[q] = mask_blend(mask[mask_per_item ? pix : pix % hw], xv[q], kv[q]);
+    }
+    if (full) {
+      *reinterpret_cast<float4*>(x + i) = *reinterpret_cast<float4*>(xv);
+      if (x_dup) *reinterpret_cast<float4*>(x_dup + i) = *reinterpret_cast<float4*>(xv);
+    } else {
+      for (int q = 0; q < 4; ++q)
+        if (i + q < n) {
+          x[i + q] = xv[q];
+          if (x_dup) x_dup[i + q] = xv[q];
+        }
+    }
+  }
+}
+
+// DiffEdit's mask, one CTA per image b.  e_* fp32 NHWC [D*bs, hw, c], draw d of image b at row d*bs + b.  Per pixel p, in fp32:
+//   E = e_u + s (e_c - e_u)  (e_c when e_u is NULL),  acc = sum over d, then c, of |E_tgt - E_src|,  dist = acc / (D c)
+//   mu = (sum over p of dist) / hw  (per-thread sums in p order, then a fixed tree over the threads),  cap = ratio mu
+//   out = cap > 0 && min(dist, cap) / cap >= 0.5 ? 1 : 0
+// dist is parked in out between the two passes.  The order of every sum depends only on the shape: bit-reproducible.
+constexpr int kDiffEditThreads = 256;
+
+__global__ void __launch_bounds__(kDiffEditThreads) diffedit_mask_kernel(
+    const float* __restrict__ es_u, const float* __restrict__ es_c, float s_src, const float* __restrict__ et_u,
+    const float* __restrict__ et_c, float s_tgt, int D, int bs, long long hw, int c, float ratio, float* out) {
+  __shared__ float red[kDiffEditThreads];
+  const int b = blockIdx.x;
+  float* o = out + static_cast<long long>(b) * hw;
+  const float dc = static_cast<float>(static_cast<long long>(D) * c);
+  float part = 0.f;
+  for (long long p = threadIdx.x; p < hw; p += blockDim.x) {
+    float acc = 0.f;
+    for (int d = 0; d < D; ++d) {
+      const long long base = ((static_cast<long long>(d) * bs + b) * hw + p) * c;
+      for (int ch = 0; ch < c; ++ch) {
+        float es = es_c[base + ch], et = et_c[base + ch];
+        if (es_u) es = __fadd_rn(es_u[base + ch], __fmul_rn(s_src, __fsub_rn(es, es_u[base + ch])));
+        if (et_u) et = __fadd_rn(et_u[base + ch], __fmul_rn(s_tgt, __fsub_rn(et, et_u[base + ch])));
+        acc = __fadd_rn(acc, fabsf(__fsub_rn(et, es)));
+      }
+    }
+    const float dist = __fdiv_rn(acc, dc);
+    o[p] = dist;
+    part = __fadd_rn(part, dist);
+  }
+  red[threadIdx.x] = part;
+  __syncthreads();
+  for (int w = kDiffEditThreads / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] = __fadd_rn(red[threadIdx.x], red[threadIdx.x + w]);
+    __syncthreads();
+  }
+  const float cap = __fmul_rn(ratio, __fdiv_rn(red[0], static_cast<float>(hw)));
+  for (long long p = threadIdx.x; p < hw; p += blockDim.x)
+    o[p] = (cap > 0.f && __fdiv_rn(fminf(o[p], cap), cap) >= 0.5f) ? 1.f : 0.f;
 }
 
 __global__ void add_int_kernel(int* p, int delta) { *p += delta; }
@@ -1667,6 +1780,66 @@ int vdb_composite_f32(const float* decoded, const float* image, const float* mas
   const long long total = static_cast<long long>(n) * c * hw;
   composite_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(decoded, image, mask, mask_per_item,
                                                                                                c, hw, total, out);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+// whether a_floats floats from a and b_floats floats from b share a byte (a NULL pointer shares none)
+static bool overlaps(const void* a, long long a_floats, const void* b, long long b_floats) {
+  if (!a || !b) return false;
+  const uintptr_t a_lo = reinterpret_cast<uintptr_t>(a), a_hi = a_lo + static_cast<uintptr_t>(a_floats) * sizeof(float);
+  const uintptr_t b_lo = reinterpret_cast<uintptr_t>(b), b_hi = b_lo + static_cast<uintptr_t>(b_floats) * sizeof(float);
+  return a_lo < b_hi && b_lo < a_hi;
+}
+
+int vdb_latent_store_slot_f32(const float* x, float* ring, int slots, const int* step_idx, int offset, long long n,
+                              void* stream) {
+  if (!x || !ring || !step_idx || slots <= 0 || n <= 0) return set_error(VDB_ERR_INVALID, "latent_store_slot: null/empty argument");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(ring)) & 15)
+    return set_error(VDB_ERR_INVALID, "latent_store_slot: pointers must be 16-byte aligned");
+  if (overlaps(x, n, ring, static_cast<long long>(slots) * n))
+    return set_error(VDB_ERR_INVALID, "latent_store_slot: x overlaps the ring");
+  latent_store_slot_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, ring, slots,
+                                                                                                            step_idx, offset, n);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots, const float* mask, int mask_per_item,
+                            const int* step_idx, int bs, long long hw, int c, void* stream) {
+  if (!x || !ring || !mask || !step_idx || slots <= 0 || bs <= 0 || hw <= 0 || c <= 0)
+    return set_error(VDB_ERR_INVALID, "inversion_blend: null/empty argument");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_dup) | reinterpret_cast<uintptr_t>(ring) |
+       reinterpret_cast<uintptr_t>(mask)) & 15)
+    return set_error(VDB_ERR_INVALID, "inversion_blend: pointers must be 16-byte aligned");
+  const long long n = static_cast<long long>(bs) * hw * c;
+  // x / x_dup are written while the ring and the mask are read through the read-only path: no byte may be shared
+  for (const float* o : {static_cast<const float*>(x), static_cast<const float*>(x_dup)})
+    if (overlaps(o, n, ring, static_cast<long long>(slots) * n) || overlaps(o, n, mask, (mask_per_item ? bs : 1) * hw))
+      return set_error(VDB_ERR_INVALID, "inversion_blend: ring or mask overlaps x or x_dup");
+  inversion_blend_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      x, x_dup, ring, slots, mask, mask_per_item, step_idx, n, hw, c);
+  VDB_CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  return VDB_OK;
+}
+
+int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,
+                          float s_tgt, int D, int bs, long long hw, int c, float ratio, float* out, void* stream) {
+  if (!e_src_c || !e_tgt_c || !out || D <= 0 || bs <= 0 || hw <= 0 || c <= 0)
+    return set_error(VDB_ERR_INVALID, "diffedit_mask: null/empty argument");
+  if (!(ratio > 0.f) || !(ratio < INFINITY)) return set_error(VDB_ERR_INVALID, "diffedit_mask: ratio must be finite and > 0");
+  if ((reinterpret_cast<uintptr_t>(e_src_u) | reinterpret_cast<uintptr_t>(e_src_c) | reinterpret_cast<uintptr_t>(e_tgt_u) |
+       reinterpret_cast<uintptr_t>(e_tgt_c) | reinterpret_cast<uintptr_t>(out)) & 15)
+    return set_error(VDB_ERR_INVALID, "diffedit_mask: pointers must be 16-byte aligned");
+  const long long n = static_cast<long long>(D) * bs * hw * c;
+  for (const float* e : {e_src_u, e_src_c, e_tgt_u, e_tgt_c})
+    if (overlaps(out, static_cast<long long>(bs) * hw, e, n))
+      return set_error(VDB_ERR_INVALID, "diffedit_mask: out overlaps an eps input");
+  diffedit_mask_kernel<<<bs, kDiffEditThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, bs, hw, c, ratio, out);
   VDB_CUDA_CHECK(cudaGetLastError());
   count_launch();
   return VDB_OK;

@@ -27,6 +27,7 @@ class DDIMSampler(object):
         self.schedule = schedule
         self.use_cuda_graph = kwargs.get("use_cuda_graph", True)
         self._graphs = {}
+        self._inv_graphs = {}
 
     def register_buffer(self, name, attr):
         # the reference forces .to('cuda') here (ddim.py:17-21); follow the model's device instead
@@ -95,9 +96,13 @@ class DDIMSampler(object):
 
     # ------------------------------------------------------------------ the loop
     def _initial_latent(self, shape, x_info, dtype, device):
-        """ddim.py:94-105: injected x_T ('xt'), img2img start (x0 + q_sample) or fresh noise."""
+        """ddim.py:94-105: injected x_T ('xt'), img2img start (x0 + q_sample) or fresh noise; or slot k of an inversion and the
+        first k grid points (lib/model_zoo/edit.py)."""
         timesteps = self.ddim_timesteps
-        if x_info.get('xt', None) is not None:
+        if x_info.get('inversion', None) is not None:
+            inv = x_info['inversion']
+            x, timesteps = inv.xt.to(dtype).to(device), timesteps[:inv.k]
+        elif x_info.get('xt', None) is not None:
             x = x_info['xt'].to(dtype).to(device)       # (the reference's `.astype` here is a bug, ddim.py:95)
         elif x_info.get('x0', None) is not None:
             x0 = x_info['x0'].type(dtype).to(device)
@@ -112,9 +117,15 @@ class DDIMSampler(object):
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         model = self.model
         device = torch.device(model.device)
+        # a walk from an inversion (lib/model_zoo/edit.py): its mask blends against the trajectory, with no draws
+        from_inv = x_info.get('inversion', None) is not None
+        if from_inv:
+            from .edit import check_sample_inputs
+            inv, inv_mask = check_sample_inputs(x_info, shape, self.ddim_timesteps)
+        inv_blend = from_inv and inv_mask is not None
         # inpainting (lib/model_zoo/inpaint.py): refuse bad inputs before any device work; the Philox key comes from torch's CPU
         # generator, drawn only when a mask is given
-        inpaint = x_info.get('inpaint_mask', None) is not None
+        inpaint = x_info.get('inpaint_mask', None) is not None and not from_inv
         if inpaint:
             from .inpaint import check_inputs
             x0_in, mask_in = check_inputs(x_info, shape)
@@ -142,18 +153,8 @@ class DDIMSampler(object):
         sigmas = np.asarray(self.ddim_sigmas.cpu() if isinstance(self.ddim_sigmas, torch.Tensor) else self.ddim_sigmas)
         fast = self.use_cuda_graph and noise_dropout == 0. and not np.any(sigmas[:total_steps] != 0)
 
-        # contexts: [uncond ; cond] built once (the reference re-concatenates every step, ddim.py:146)
-        from .attention import PaddedContext
-        ctxs = []
-        for i, ci in enumerate(c_infos):
-            c = torch.cat([ci['unconditional_conditioning'], ci['conditioning']]) if cfg else ci['conditioning']
-            ci['c'] = c
-            ctxs.append(PaddedContext(self._ctx_buffer(i, c), c.shape[1]))
-        c_types = [ci['type'] for ci in c_infos]
-        ratios = [float(ci.get('ratio', 1.0)) for ci in c_infos]
         x_type = x_info['type']
-        time_from = model.time_source(x_type, multi)
-        mch = model.diffuser[time_from].model_channels
+        ctxs, c_types, ratios, time_from, mch = self._contexts(c_infos, cfg, x_type, multi)
         B = 2 * bs if cfg else bs
         # text latents ([n, 768], the i2t / t2t flows: app.py:384-434) walk the same loop as a 1x1 "image" of 768 channels: the
         # NCHW <-> NHWC conversions are identities and the 0-D diffuser takes the flat view
@@ -170,6 +171,8 @@ class DDIMSampler(object):
         ops.nchw_to_nhwc(x.float().contiguous(), out=st['x_in'][:bs])
         if inpaint:
             mask_per_item = self._inpaint_state(st, x0_in, mask_in, seed, total_steps, x if full_walk else None, bs, device)
+        if inv_blend:
+            mask_per_item = self._inversion_blend_state(st, inv, inv_mask, device)
         if cfg:
             st['x_in'][bs:].copy_(st['x_in'][:bs])
         st['coef'][:total_steps].copy_(coef)
@@ -186,6 +189,9 @@ class DDIMSampler(object):
             if inpaint:
                 ops.inpaint_blend(st['x_in'][:bs], st['x0'], st['mask'] if mask_per_item else st['mask'][:1], st['blend'],
                                   st['idx'], seed=st['seed'], x_dup=st['x_in'][bs:] if cfg else None)
+            if inv_blend:
+                ops.inversion_blend(st['x_in'][:bs], st['traj'], st['mask'] if mask_per_item else st['mask'][:1], st['idx'],
+                                    x_dup=st['x_in'][bs:] if cfg else None)
             ops.add_int(st['idx'], -1)
 
         intermediates = {'pred_xt': [], 'pred_x0': []}
@@ -211,33 +217,11 @@ class DDIMSampler(object):
                    tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs)) + self._graph_tag()
             if inpaint:
                 key += (('inpaint', mask_per_item),)
-            ent = self._graphs.get(key)
-            if ent is not None and ent[1] == model.context_kv_signature(c_types, ctxs):
-                # steady state: the context projections were just refreshed in place; every step is a graph replay
-                for i in range(total_steps):
-                    ent[0].replay()
-                    log(total_steps - i - 1)
-            else:
-                n0 = ops.launch_count()
-                step()                      # first step eager: packs weights, sizes workspaces, warms caches
-                self.last_step_launches = ops.launch_count() - n0
-                log(total_steps - 1)
-                g = None
-                if total_steps > 1:
-                    torch.cuda.synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    idx_before = st['idx'].clone()
-                    x_before = st['x_in'].clone()
-                    with torch.cuda.graph(g):
-                        step()
-                    # capture does not execute; make sure state is exactly what the eager step left
-                    st['idx'].copy_(idx_before)
-                    st['x_in'].copy_(x_before)
-                    # keep one live graph (its private pool holds the activations) + the K / V^T buffers it reads
-                    self._graphs = {key: (g, model.context_kv_signature(c_types, ctxs))}
-                for i in range(1, total_steps):
-                    g.replay()
-                    log(total_steps - i - 1)
+            if inv_blend:
+                key += (('inversion', mask_per_item),)
+            n = self._walk(key, '_graphs', step, total_steps, st, c_types, ctxs, lambda i: log(total_steps - i - 1))
+            if n is not None:
+                self.last_step_launches = n
 
         pred_xt = ops.nhwc_to_nchw(st['x_in'][:bs].contiguous()).to(dtype)
         if flat:
@@ -245,6 +229,113 @@ class DDIMSampler(object):
             intermediates = {k: [v.reshape(bs, -1) for v in vs] for k, vs in intermediates.items()}
         x_info['x'] = pred_xt
         return pred_xt, intermediates
+
+    def _contexts(self, c_infos, cfg, x_type, multi, buffer_tag=None):
+        """[uncond ; cond] of every context, built once (the reference re-concatenates every step, ddim.py:146), in persistent
+        padded buffers (per buffer_tag, so the inversion keeps its own) -> (contexts, c_types, ratios, time_from, model_channels)"""
+        from .attention import PaddedContext
+        ctxs = []
+        for i, ci in enumerate(c_infos):
+            c = torch.cat([ci['unconditional_conditioning'], ci['conditioning']]) if cfg else ci['conditioning']
+            ci['c'] = c
+            ctxs.append(PaddedContext(self._ctx_buffer(i if buffer_tag is None else (buffer_tag, i), c), c.shape[1]))
+        c_types = [ci['type'] for ci in c_infos]
+        ratios = [float(ci.get('ratio', 1.0)) for ci in c_infos]
+        time_from = self.model.time_source(x_type, multi)
+        return ctxs, c_types, ratios, time_from, self.model.diffuser[time_from].model_channels
+
+    def _walk(self, key, graphs_attr, step, total_steps, st, c_types, ctxs, log):
+        """Run total_steps steps of `step` on a captured step graph kept in self.<graphs_attr>; log(i) after walk position i.
+        -> the launches of one step, or None when a cached graph replayed every step."""
+        model, ops = self.model, _ops()
+        ent = getattr(self, graphs_attr).get(key)
+        if ent is not None and ent[1] == model.context_kv_signature(c_types, ctxs):
+            # steady state: the context projections were just refreshed in place; every step is a graph replay
+            for i in range(total_steps):
+                ent[0].replay()
+                log(i)
+            return None
+        n0 = ops.launch_count()
+        step()                      # first step eager: packs weights, sizes workspaces, warms caches
+        launches = ops.launch_count() - n0
+        log(0)
+        g = None
+        if total_steps > 1:
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            idx_before = st['idx'].clone()
+            x_before = st['x_in'].clone()
+            with torch.cuda.graph(g):
+                step()
+            # capture does not execute; make sure state is exactly what the eager step left
+            st['idx'].copy_(idx_before)
+            st['x_in'].copy_(x_before)
+            # keep one live graph (its private pool holds the activations) + the K / V^T buffers it reads
+            setattr(self, graphs_attr, {key: (g, model.context_kv_signature(c_types, ctxs))})
+        for i in range(1, total_steps):
+            g.replay()
+            log(i)
+        return launches
+
+    # ------------------------------------------------------------------ DDIM inversion (lib/model_zoo/edit.py)
+    @torch.no_grad()
+    def invert(self, steps, x0, c_info, k=None, verbose=False):
+        """Run the DDIM ODE backwards from the image latent x0 over the first k grid points (all by default) -> Inversion."""
+        return self._invert(steps, x0, [c_info], False, k, verbose)
+
+    @torch.no_grad()
+    def invert_multicontext(self, steps, x0, c_info_list, k=None, verbose=False):
+        scale = c_info_list[0]['unconditional_guidance_scale']
+        for ci in c_info_list:
+            assert scale == ci['unconditional_guidance_scale'], \
+                "A different unconditional guidance scale between different context is not allowed!"
+        return self._invert(steps, x0, c_info_list, True, k, verbose)
+
+    def _invert(self, steps, x0, c_infos, multi, k, verbose):
+        from .edit import Inversion, check_invert_inputs, context_batch, inversion_rows
+        model = self.model
+        device = torch.device(model.device)
+        self.make_schedule(ddim_num_steps=steps, ddim_eta=0., verbose=verbose)
+        timesteps = self.ddim_timesteps
+        bs = context_batch(c_infos, float(c_infos[0]['unconditional_guidance_scale']))
+        k = check_invert_inputs(x0, bs, k, len(timesteps))
+        if device.type != 'cuda':
+            raise RuntimeError("DDIMSampler: the H100 build has no CPU path (model.to('cuda') first)")
+        ops = _ops()
+        _, C, H, W = x0.shape
+        scale = float(c_infos[0]['unconditional_guidance_scale'])
+        cfg = scale != 1.
+        B = 2 * bs if cfg else bs
+        ctxs, c_types, ratios, time_from, mch = self._contexts(c_infos, cfg, 'image', multi, buffer_tag='invert')
+        st = self._inv_state(bs, B, H, W, C, len(timesteps) + 1, device)
+        ring = st['ring']
+        ring[0].copy_(ops.nchw_to_nhwc(x0.to(device=device, dtype=torch.float32).expand(bs, C, H, W).contiguous()))
+        st['x_in'][:bs].copy_(ring[0])
+        if cfg:
+            st['x_in'][bs:].copy_(ring[0])
+        st['coef'][:k].copy_(torch.from_numpy(inversion_rows(self.ddim_alphas, self.ddim_alphas_prev, k)))
+        st['ts'][:len(timesteps)].copy_(torch.tensor(np.asarray(timesteps, dtype=np.int64)))
+        st['idx'].fill_(0)
+
+        def step():
+            t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=B)
+            eps = model.eps_nhwc(st['x_in'], 'image', t_emb, c_types, ctxs, ratios, time_from)
+            e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
+            DDIMSampler._update(self, st, e_u, e_c, scale, bs, cfg, None, 1.0)
+            ops.latent_store_slot(st['x_in'][:bs], ring, st['idx'], 1)
+            ops.add_int(st['idx'], 1)
+
+        if not self.use_cuda_graph:
+            for _ in range(k):
+                step()
+        else:
+            from .diffusion_utils import pack_epoch
+            key = (pack_epoch(), bs, B, H, W, tuple(c_types), tuple(ratios), scale, time_from,
+                   tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs), 'invert')
+            n = self._walk(key, '_inv_graphs', step, k, st, c_types, ctxs, lambda i: None)
+            if n is not None:
+                self.last_invert_step_launches = n
+        return Inversion(ring[:k + 1].clone(), steps, k, timesteps, (bs, C, H, W))
 
     # ------------------------------------------------------------------ per-step update (overridden by DPMSolverSampler)
     _coef_cols = 4      # width of a row of the device coefficient table
@@ -292,6 +383,41 @@ class DDIMSampler(object):
             self._st = st
             self._graphs = {}
         return st
+
+    def _inv_state(self, bs, B, H, W, C, slots, device):
+        """The inversion walk's own persistent buffers (so it never evicts the sampling graph) and its trajectory ring."""
+        key = (bs, B, H, W, C, slots, str(device))
+        st = getattr(self, '_inv_st', None)
+        if st is None or st['key'] != key:
+            st = {'key': key,
+                  'x_in': torch.zeros(B, H, W, C, dtype=torch.float32, device=device),
+                  'pred_x0': torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
+                  'coef': torch.zeros(1000, 4, dtype=torch.float32, device=device),
+                  'ts': torch.zeros(1000, dtype=torch.int64, device=device),
+                  'idx': torch.zeros(1, dtype=torch.int32, device=device),
+                  'ring': torch.zeros(slots, bs, H, W, C, dtype=torch.float32, device=device)}
+            self._inv_st = st
+            self._inv_graphs = {}
+        return st
+
+    def _inversion_blend_state(self, st, inv, mask, device):
+        """Refill the trajectory and mask buffers of st in place, so a cached step graph replays on a new inversion and mask ->
+        whether the mask is per item.  lib/model_zoo/edit.py specifies the semantics."""
+        ops = _ops()
+        bs, H, W = inv.bs, inv.shape[2], inv.shape[3]
+        traj = st.get('traj')
+        if traj is None or traj.shape[0] < inv.k or tuple(traj.shape[1:]) != tuple(inv.trajectory.shape[1:]):
+            st['traj'] = torch.zeros((max(inv.k, len(self.ddim_timesteps)),) + tuple(inv.trajectory.shape[1:]),
+                                     dtype=torch.float32, device=device)
+            self._graphs = {}           # a cached graph reads the old buffer
+        st['traj'][:inv.k].copy_(inv.trajectory[:inv.k])
+        if 'mask' not in st:
+            st['mask'] = torch.zeros(bs, H * W, dtype=torch.float32, device=device)
+        mask = mask.to(device=device, dtype=torch.float32).contiguous()
+        if mask.shape[-1] != W:
+            mask = ops.mask_to_latent(mask)
+        st['mask'][:mask.shape[0]].copy_(mask.view(mask.shape[0], H * W))
+        return int(mask.shape[0] != 1)
 
     def _inpaint_state(self, st, x0, mask, seed, total_steps, x_T, bs, device):
         """Refill the inpainting buffers of st in place, so a cached step graph replays on a new image, mask and seed ->

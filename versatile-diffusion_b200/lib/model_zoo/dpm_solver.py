@@ -121,6 +121,13 @@ class DPMSolverSampler(DDIMSampler):
     def _graph_tag(self):
         return ('dpmpp', self.order)
 
+    def invert(self, *args, **kwargs):
+        raise NotImplementedError("DPMSolverSampler has no inversion: inverting the multistep solver is a different algorithm "
+                                  "(invert with DDIMSampler, then sample here from its Inversion; lib/model_zoo/edit.py)")
+
+    def invert_multicontext(self, *args, **kwargs):
+        self.invert()
+
     def p_sample_ddim(self, *args, **kwargs):
         raise NotImplementedError("DPMSolverSampler is a multistep solver: it has no single-step form (use sample)")
 

@@ -33,10 +33,19 @@ class PLMSSampler(DDIMSampler):
             raise ValueError('ddim_eta must be 0 for PLMS')
         super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)
 
+    def invert(self, *args, **kwargs):
+        raise NotImplementedError("PLMSSampler has no inversion: invert with DDIMSampler (lib/model_zoo/edit.py)")
+
+    def invert_multicontext(self, *args, **kwargs):
+        self.invert()
+
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         if x_info.get('inpaint_mask', None) is not None:
             raise NotImplementedError("PLMSSampler has no inpainting: use DDIMSampler or DPMSolverSampler "
                                       "(lib/model_zoo/inpaint.py)")
+        if x_info.get('inversion', None) is not None:
+            raise NotImplementedError("PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
+                                      "(lib/model_zoo/edit.py)")
         ops = _ops()
         model = self.model
         device = torch.device(model.device)

@@ -31,6 +31,9 @@ SIGNATURES = {
     "vdb_inpaint_noise_f32": (i, [p, p, ll, p, p]),
     "vdb_mask_to_latent": (i, [p, i, i, i, p, p]),
     "vdb_composite_f32": (i, [p, p, p, i, i, i, ll, p, p]),
+    "vdb_latent_store_slot_f32": (i, [p, p, i, p, i, ll, p]),
+    "vdb_inversion_blend_f32": (i, [p, p, p, i, p, i, p, i, ll, i, p]),
+    "vdb_diffedit_mask_f32": (i, [p, p, f, p, p, f, i, i, ll, i, f, p, p]),
     "vdb_axpby_f32": (i, [p, p, f, f, p, ll, p]),
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),

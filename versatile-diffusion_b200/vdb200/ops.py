@@ -264,6 +264,64 @@ def composite(decoded, image, mask, out=None):
     return out
 
 
+def latent_store_slot(x, ring, step_idx, offset):
+    """ring[step_idx[0] + offset] = x (lib/model_zoo/edit.py): x fp32 of n elements, ring fp32 [slots, ...] of slots * n."""
+    _need(x, torch.float32, "x")
+    _need(ring, torch.float32, "ring")
+    _need(step_idx, torch.int32, "step_idx")
+    n = x.numel()
+    if ring.dim() < 1 or ring.numel() != ring.shape[0] * n:
+        raise ValueError(f"ring: expected [slots, {tuple(x.shape)}], got {tuple(ring.shape)}")
+    check(lib.vdb_latent_store_slot_f32(_ptr(x), _ptr(ring), ring.shape[0], _ptr(step_idx), int(offset), n, _stream()),
+          "latent_store_slot")
+    return ring
+
+
+def inversion_blend(x, ring, mask, step_idx, x_dup=None):
+    """x = m x + (1 - m) ring[step_idx[0]] after a step of a walk from an inversion (lib/model_zoo/edit.py), in place on x.  x /
+    x_dup fp32 NHWC [bs, H, W, C]; ring fp32 [slots, bs, H, W, C]; mask fp32 of H*W (broadcast over the batch) or bs*H*W."""
+    for name, t in (("x", x), ("ring", ring), ("mask", mask), ("x_dup", x_dup)):
+        _need(t, torch.float32, name)
+    _need(step_idx, torch.int32, "step_idx")
+    bs, C = x.shape[0], x.shape[-1]
+    hw = x.numel() // (bs * C)
+    if x_dup is not None and x_dup.shape != x.shape:
+        raise ValueError(f"x_dup: expected {tuple(x.shape)}, got {tuple(x_dup.shape)}")
+    if ring.dim() != x.dim() + 1 or tuple(ring.shape[1:]) != tuple(x.shape):
+        raise ValueError(f"ring: expected [slots, {', '.join(map(str, x.shape))}], got {tuple(ring.shape)}")
+    if mask.numel() not in (hw, bs * hw):
+        raise ValueError(f"mask: expected {hw} or {bs * hw} elements, got {mask.numel()}")
+    check(lib.vdb_inversion_blend_f32(_ptr(x), _ptr(x_dup), _ptr(ring), ring.shape[0], _ptr(mask), int(mask.numel() != hw),
+                                      _ptr(step_idx), bs, hw, C, _stream()),
+          "inversion_blend")
+    return x
+
+
+def diffedit_mask(e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, ratio, out=None):
+    """DiffEdit's {0, 1} mask (lib/model_zoo/edit.py) -> fp32 [bs, H, W].  e_* fp32 NHWC [D*bs, H, W, C], draw d of image b at row
+    d*bs + b; an e_*_u is None when that side has no CFG."""
+    for name, t in (("e_src_u", e_src_u), ("e_src_c", e_src_c), ("e_tgt_u", e_tgt_u), ("e_tgt_c", e_tgt_c)):
+        _need(t, torch.float32, name)
+        if t is not None and t.shape != e_src_c.shape:
+            raise ValueError(f"{name}: expected {tuple(e_src_c.shape)}, got {tuple(t.shape)}")
+    D = int(D)
+    if D < 1:
+        raise ValueError(f"D must be >= 1, got {D}")
+    if e_src_c.dim() != 4 or e_src_c.shape[0] % D:
+        raise ValueError(f"eps: expected [D*bs, H, W, C] with D = {D}, got {tuple(e_src_c.shape)}")
+    R, H, W, C = e_src_c.shape
+    bs = R // D
+    if out is None:
+        out = torch.empty(bs, H, W, dtype=torch.float32, device=e_src_c.device)
+    _need(out, torch.float32, "out")
+    if out.numel() != bs * H * W:
+        raise ValueError(f"out: expected {bs * H * W} elements ([{bs}, {H}, {W}]), got {tuple(out.shape)}")
+    check(lib.vdb_diffedit_mask_f32(_ptr(e_src_u), _ptr(e_src_c), float(s_src), _ptr(e_tgt_u), _ptr(e_tgt_c), float(s_tgt), int(D),
+                                    bs, H * W, C, float(ratio), _ptr(out), _stream()),
+          "diffedit_mask")
+    return out
+
+
 def axpby(x, z, a, b, out=None):
     _need(x, torch.float32, "x"); _need(z, torch.float32, "z")
     if out is None:
