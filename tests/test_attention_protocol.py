@@ -13,7 +13,8 @@ latencies and checks, at every access, that:
   * P_j is not written while PV_{j-1} may still read the P registers;
   * nobody passes an mbarrier wait early through parity aliasing; the run terminates (no deadlock).
 
-It knows nothing about arithmetic — only about who may touch what, when.  tests/test_igemm_protocol.py reuses the simulator.
+It knows nothing about arithmetic — only about who may touch what, when.  tests/test_igemm_protocol_tma_epi.py reuses the
+simulator.
 """
 import random
 

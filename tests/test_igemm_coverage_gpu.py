@@ -8,7 +8,7 @@ bf16-rounded operands.  BN and ksplit are forced, so the plan does not depend on
 
 Rows marked walk=True must make some CTA run two or more tiles and change its N tile in between (checked on the reported
 grid with test_tile_schedule.walk): that is when the bias / LayerNorm tables cached in shared memory are reloaded, the next
-tile's row statistics are prefetched, the parked accumulator is reused and the TMA-store staging alternates.  They also have an
+tile's row statistics are prefetched and the TMA-store staging alternates.  They also have an
 M tail (M % 128 != 0), a K tail (K % 64 != 0) and, except for GEGLU (N % 256 == 0 by contract), a partial last N tile.
 test_tile_schedule checks on the CPU that every instantiation has such a row at 132 SMs.
 
@@ -65,11 +65,14 @@ CASES += [
     _case("m6-bn256-parts20", "ln", 256, 6, walk=True, M=M_WALK, N=N_GEGLU, K=K_WALK, parts=20, geglu=True),
     # mode 0 paths the rows above do not take
     _case("m0-f32-ntail", "gemm", 128, 0, M=1000, N=200, K=328, bias="vec", f32=True),
+    _case("m0-bf16-n24", "gemm", 64, 0, M=300, N=24, K=72, bias="vec", resid=True, act=ACT_SILU),   # one chunk narrower than a box
     _case("m0-f32-silu-alpha", "gemm", 64, 0, walk=True, M=M_WALK, N=N_WALK_ODD[64], K=K_WALK, bias="vec", act=ACT_SILU, alpha=1.5, f32=True),
-    # per-row bias whose 128-row tiles straddle two (or, at 77 rows, three) batch items: the bias_g path; at 257 rows some
+    # per-row bias whose 128-row tiles straddle two (or, at 77 rows, three) batch items: each row reads its own bias row; at 257 rows some
     # tiles lie inside one item and take the shared-memory bias row, reloaded per item
     _case("m0-rowbias77", "gemm", 64, 0, walk=True, M=77 * 13, N=N_WALK[64], K=K_WALK, bias="batch", rpb=77, resid=True),
     _case("m0-rowbias257", "gemm", 160, 0, walk=True, M=257 * 5, N=N_WALK[160], K=K_WALK, bias="batch", rpb=257, resid=True),
+    # GEGLU with a per-row bias: tiles that straddle two of the 200-row items keep GEGLU on the generic epilogue
+    _case("m0-geglu-rowbias200", "gemm", 256, 0, walk=True, M=200 * 6, N=N_GEGLU, K=K_WALK, bias="batch", rpb=200, act=ACT_GEGLU),
     # split-K: fp32 partials, then splitk_reduce_kernel adds the per-batch bias, activation and residual
     _case("m0-splitk-rowbias", "gemm", 128, 0, ksplit=4, M=320, N=640, K=1288, bias="batch", rpb=80, resid=True, act=ACT_SILU),
     _case("m0-splitk-f32", "gemm", 64, 0, ksplit=3, M=300, N=200, K=520, bias="vec", f32=True, act=ACT_GELU),
@@ -77,7 +80,7 @@ CASES += [
     _case("m5-cols-bn128", "ln", 128, 5, walk=True, M=M_WALK, N=N_WALK[128], K=K_WALK, parts=5, on_cols=True),
     _case("m5-cols-bn64-parts20", "ln", 64, 5, walk=True, M=M_WALK, N=N_WALK[64], K=K_WALK, parts=20, on_cols=True),
     # 3x3 convs.  The 8x8 UNet level's ResBlock conv1 (B 8, 1280 -> 1280, the time embedding as a per-batch bias): the tile box
-    # is 8 x 8 x 2 images, so every tile straddles two bias rows (mode 0, bias_g); with split-K the reduction adds that bias
+    # is 8 x 8 x 2 images, so every tile straddles two bias rows (mode 0, per-row bias); with split-K the reduction adds that bias
     _case("conv-8x8-rb-ks1", "conv", 64, 0, ksplit=1, B=8, H=8, W=8, C=1280, N=1280, cmode=0, bias="batch"),
     _case("conv-8x8-rb-ks4", "conv", 160, 0, ksplit=4, B=8, H=8, W=8, C=1280, N=1280, cmode=0, bias="batch"),
     _case("conv-8x8-rb-auto", "conv", 0, 0, ksplit=0, B=8, H=8, W=8, C=1280, N=1280, cmode=0, bias="batch"),

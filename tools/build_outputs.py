@@ -7,7 +7,9 @@ parity tests (synthetic seeded weights):
   * an inpainting DDIM walk (soft latent mask, Philox noise keyed by torch.manual_seed),
   * the text-latent diffuser (4-step DDIM on a [2, 768] latent, image context),
   * a VAE decode whose Upsamples all take the folded path (64x64 latent) and one whose Upsamples all take the unfolded path
-    (8x8 latent).
+    (8x8 latent),
+  * a CLIP text encode and a CLIP image encode (quick_gelu MLPs) and a 2-layer Optimus BERT encode (GELU feed-forward), on
+    synthetic seeded weights as in the CLIP and text-encoder tests.
 
 Each build runs with its own tree's Python and library; then the dumps are compared with torch.equal:
 
@@ -54,6 +56,49 @@ def cinfo(c, u, typ="text"):
     return {"type": typ, "conditioning": c.to(DEV), "unconditional_conditioning": u.to(DEV), "unconditional_guidance_scale": 7.5}
 
 
+def synth_encoder(cfg_name, seed=3):
+    """a CLIP context encoder of the config bank with seeded synthetic weights"""
+    from lib.cfg_helper import model_cfg_bank
+    from lib.model_zoo import get_model
+    from oracle import weights
+    enc = get_model()(model_cfg_bank()(cfg_name), verbose=False)
+    shapes = {k: tuple(v.shape) for k, v in enc.model.named_parameters()}
+    enc.model.load_state_dict(weights.synth_state_dict(shapes, seed=seed), strict=False)
+    return enc.to(DEV)
+
+
+def synth_bert(n_layer=2, seed=7):
+    """the Optimus BERT encoder with seeded synthetic weights"""
+    from lib.model_zoo.optimus import optimus_vae_next
+    from oracle import weights
+    m = optimus_vae_next(decoder=dict(config=dict(n_layer=1)), encoder=dict(config=dict(num_hidden_layers=n_layer)))
+    shapes = {k: tuple(v.shape) for k, v in m.state_dict().items() if k.startswith("encoder.")}
+    m.load_state_dict({k: weights.tensor_for(k, s, seed) for k, s in shapes.items()}, strict=False)
+    return m.to(DEV)
+
+
+def run_encoders(g):
+    out = {}
+    with torch.no_grad():
+        tok = torch.full((3, 77), 49407, dtype=torch.long)
+        tok[:, 0] = 49406
+        for i in range(3):
+            tok[i, 1:6 + 7 * i] = torch.randint(1000, 40000, (5 + 7 * i,), generator=g)
+        enc = synth_encoder("clip_text_context_encoder")
+        out["clip_text_encode"] = enc.encode_tokens(tok)
+        del enc
+        enc = synth_encoder("clip_image_context_encoder")
+        out["clip_image_encode"] = enc.encode(torch.rand(2, 3, 300, 360, generator=g).to(DEV))
+        del enc
+        lengths = [9, 70, 33, 79]
+        ids = torch.zeros(len(lengths), max(lengths), dtype=torch.long)
+        for r, n in enumerate(lengths):
+            ids[r, 0], ids[r, n - 1] = 101, 102
+            ids[r, 1:n - 1] = torch.randint(999, 28996, (n - 2,), generator=g)
+        out["bert_encode"] = synth_bert().encode_ids(ids, lengths)
+    return out
+
+
 def run_cases():
     from lib.model_zoo.ddim import DDIMSampler
     from lib.model_zoo.dpm_solver import DPMSolverSampler
@@ -87,6 +132,8 @@ def run_cases():
         out["text_latent_ddim_4"] = DDIMSampler(net).sample(
             steps=4, shape=[2, 768], x_info={"type": "text", "xt": xt.to(DEV)}, c_info=cinfo(ci, ui, "image"),
             verbose=False, eta=0.)[0]
+    del net
+    out.update(run_encoders(g))
     return {k: v.detach().cpu() for k, v in out.items()}
 
 

@@ -11,9 +11,9 @@
 //
 // Structure: grid = #SMs (persistent, static round-robin over output tiles), 288 threads (384 where the accumulator needs the
 // producer's registers, see igemm_realloc):
-//   warps 0-7: two consumer warpgroups (BM / 128 wgmma m64 x BN x 16 each per k16 step, fp32 accumulators in registers), then the epilogue
-//              (TMA-store modes: straight from the registers -> bias / LayerNorm / GEGLU / residual -> bf16 TMA stores;
-//              other modes: accumulator parked in shared memory -> bias/act/residual -> coalesced bf16 / fp32 stores)
+//   warps 0-7: two consumer warpgroups (BM / 128 wgmma m64 x BN x 16 each per k16 step, fp32 accumulators in registers), then the
+//              epilogue straight from the registers: bias / LayerNorm / activation / GEGLU / residual -> bf16 TMA stores, or fp32
+//              stores (fp32 output, split-K partials)
 //   warp 8   : TMA producer  (cp.async.bulk.tensor 4D box loads of A, 2D box loads of W)
 // smem ring of STAGES x (A BMx64 bf16 | W BNx64 bf16), both 128B-swizzled K-major; the tile is BM = 128 or 256 rows high.
 #include "common.cuh"
@@ -76,19 +76,10 @@ struct alignas(64) IgemmParams {
   const float* ln_rowbias;    // on_cols 1: [M] beta-term of the output row (null = 0); on_cols 0 the beta term lives in `bias`
   float* stats_out;           // mode 7: [2 * tilesN][M][2] fp32: (sum, sum of squares) over the even (slot 2n) and the odd
                               // (slot 2n + 1) 32-column chunks of N tile n, for every OUTPUT row
-  unsigned long long* timeline; // debug: per-tile role timestamps of CTA 0 (null = off)
   unsigned smem_bytes;        // dynamic shared memory of the launch (LN modes check their carve-up against it)
 };
 
 enum { ACT_NONE = 0, ACT_SILU = 1, ACT_GELU = 2, ACT_QGELU = 3, ACT_GEGLU = 4 };
-
-#ifdef VDB_TIMELINE   // debug build only (tools/gemm_timeline.py): per-tile role timestamps of CTA 0
-#define VDB_TL(slot, it) do { if (p.timeline && blockIdx.x == 0 && (it) < 8) p.timeline[(it) * 16 + (slot)] = gtime(); } while (0)
-#define VDB_TLE(slot, it) do { if (warp == 0 && lane == 0) VDB_TL(slot, it); } while (0)
-#else
-#define VDB_TL(slot, it) do { } while (0)
-#define VDB_TLE(slot, it) do { } while (0)
-#endif
 
 VDB_DEVINL float apply_act(float v, int act) {
   switch (act) {
@@ -99,10 +90,33 @@ VDB_DEVINL float apply_act(float v, int act) {
   }
 }
 
-// MODE selects the epilogue that is compiled in: 0 = every path (split-K partials, GEGLU, fp32 / ragged / per-row-bias
-// tiles), 3 = only the bf16 fast path (act none, alpha 1, N % 32 == 0, one bias row per tile), 4 = only GEGLU, both with the
-// tile leaving through shared memory + TMA stores.  Keeping the rarely used paths out of the common instantiations keeps the
-// epilogue's instruction footprint small.  Modes 5 / 6 are modes 3 / 4 for a GEMM whose
+// v = act(alpha * v) over 8 of the values of a thread's epilogue chunk: one branch on the activation per 8 values, so the code a
+// chunk executes stays contiguous (a switch per element spreads it over every activation's code); 8 at a time, not 16, keeps the
+// interleaved activations inside the registers the accumulator leaves
+VDB_DEVINL void alpha_act8(float* v, float alpha, int act) {
+  switch (act) {
+    case ACT_SILU:
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = silu_f(__fmul_rn(v[i], alpha));
+      break;
+    case ACT_GELU:
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = gelu_erf_f(__fmul_rn(v[i], alpha));
+      break;
+    case ACT_QGELU:
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = quick_gelu_f(__fmul_rn(v[i], alpha));
+      break;
+    default:
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = __fmul_rn(v[i], alpha);
+  }
+}
+
+// MODE selects the epilogue that is compiled in: 0 = every path (split-K partials, GEGLU, activation / alpha, fp32 output,
+// ragged N, per-row bias), 3 = only plain bf16 (act none, alpha 1, N % 32 == 0, one bias row per tile), 4 = only GEGLU.  Keeping
+// the rarely used paths out of the common instantiations keeps the epilogue's instruction footprint small.  Modes 5 / 6 are
+// modes 3 / 4 for a GEMM whose
 // input is a LayerNorm: the operand is the RAW activation x and the weights carry gamma (W' = W * gamma), so with the row's mean mu
 // and rstd r       LN(x) W^T + b  =  r * (x W'^T  -  mu * s) + c,     s[n] = sum_k W'[n,k],  c[n] = sum_k beta_k W[n,k] + b[n]
 // is a rank-1 correction in the epilogue (2 FMAs per element) — the normalised tensor is never written or read.  mu and r come
@@ -111,23 +125,18 @@ VDB_DEVINL float apply_act(float v, int act) {
 //
 // Roles: warps 0-7 are two consumer warpgroups (warpgroup g computes output rows [BM / 2 * g, BM / 2 * (g + 1)) of the tile with
 // wgmma, as BM / 128 blocks of 64 rows that share the W descriptor, fp32 accumulators in registers), warp 8 is the TMA producer.
-// Modes 3-7 run the epilogue from the registers, in the wgmma fragment layout: warp w owns 16 rows of the tile and walks their
-// 32-column chunks, staging each as a 16 x 32 bf16 box (stmatrix) for a TMA store.  The warpgroups do not wait for each other
-// after the mainloop, and the producer is gated by the empty barriers alone: it loads the next tile's first STAGES k-blocks while
-// the epilogue runs, so the next mainloop starts on a full ring.  tests/test_igemm_protocol_tma_epi.py models this protocol.
-// Mode 0 parks the accumulator in shared memory (sacc, [128][BN + 4] fp32, aliasing the operand ring) after the mainloop and
-// runs the epilogue on it: each warp reads 32-column chunks of one ROW per thread (acc_ld32), the layout its paths are written
-// for.  The producer starts the next tile's loads once every consumer warp is done with sacc (acc_free;
-// tests/test_igemm_protocol.py).
+// Every mode runs the epilogue from the registers, in the wgmma fragment layout: warp w owns 16 rows of the tile and walks their
+// 32-column chunks, staging each as a 16 x 32 bf16 box (stmatrix) for a TMA store, or storing it to global memory directly when
+// the output is fp32.  The warpgroups do not wait for each other after the mainloop, and the producer is gated by the empty
+// barriers alone: it loads the next tile's first STAGES k-blocks while the epilogue runs, so the next mainloop starts on a full
+// ring.  tests/test_igemm_protocol_tma_epi.py models this protocol.
 template <int BM, int BN, int STAGES, int EW, int MODE>
 __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
-  constexpr bool kTmaEpi = MODE >= 3;                 // TMA-store epilogues
   constexpr bool kGegluEpi = MODE == 4 || MODE == 6;
   constexpr bool kLnIn = MODE == 5 || MODE == 6;
   constexpr bool kStatsOut = MODE == 7;
   constexpr int kNumEpiWarps = EW;
   constexpr int kNumEpiThreads = EW * 32;
-  constexpr int kWPQ = EW / 4;           // epilogue warps per 32-row quarter of the tile
   static_assert(EW == 8, "two consumer warpgroups");
   static_assert(BM == 128 || (BM == 256 && (MODE == 3 || MODE == 7) && BN <= 160), "256-row tiles: modes 3 and 7, 160 accumulator registers");
   constexpr int kMB = BM / 128;          // 64-row blocks per consumer warpgroup
@@ -136,10 +145,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   constexpr uint32_t kABytes = BM * kBlockK * 2;
   constexpr uint32_t kBBytes = BN * kBlockK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr int kAccStride = BN + 4;     // sacc row stride in floats (row-per-thread 16-byte reads are conflict-free)
   constexpr uint32_t kRingBytes = STAGES * kStageBytes;
-  constexpr uint32_t kAccBytes = MODE >= 3 ? 0 : BM * kAccStride * 4;
-  constexpr uint32_t kRegion = kRingBytes > kAccBytes ? kRingBytes : kAccBytes;
   static_assert(kBBytes % 1024 == 0, "B stage must keep 1024B alignment");
   static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "invalid wgmma N");
 
@@ -147,13 +153,10 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + STAGES * kABytes;
-  float* sacc = reinterpret_cast<float*>(smem);                            // [128][kAccStride] fp32 accumulator of the tile
-  float* sstage = reinterpret_cast<float*>(smem + kRegion);                // kNumEpiWarps x 4 KB, 1024-byte aligned: [32][32] fp32
-                                                                           // transposition tiles, or kBoxes 1 KB bf16 TMA-store boxes
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRegion + EW * kStgWarp);
+  uint8_t* sstage = smem + kRingBytes;                        // kNumEpiWarps x kBoxes 1 KB bf16 TMA-store boxes, 1024-byte aligned
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sstage + EW * kStgWarp);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_free = empty_bar + STAGES;    // [1]
-  float* sbias = reinterpret_cast<float*>(acc_free + 2);      // [BN] bias of the current output tile
+  float* sbias = reinterpret_cast<float*>(empty_bar + STAGES);  // [BN] bias of the current output tile
   float* slnx = sbias + BN;                                   // [BN] LN modes: colsum s (on_cols 0) / column mean (on_cols 1)
   const uint32_t sbias_s = smem_u32(sbias), slnx_s = smem_u32(slnx);   // (shared-space addresses: LDS, not generic LD)
   (void)slnx_s;
@@ -168,14 +171,13 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   if (warp == EW && lane == 0) {
     for (int i = 0; i < kMaxA; ++i) tma_prefetch_desc(&p.tmA[i]);
     tma_prefetch_desc(&p.tmB);
-    if constexpr (MODE >= 3) tma_prefetch_desc(&p.tmO);
+    if (MODE != 0 || (!p.out_f32 && p.ksplit == 1)) tma_prefetch_desc(&p.tmO);   // (mode 0 builds it for bf16 output only)
   }
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kNumEpiWarps);
     }
-    mbar_init(acc_free, kNumEpiWarps);
     fence_barrier_init();
   }
   __syncthreads();
@@ -196,8 +198,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
       const bool flat = (p.tilesH == 1) && (p.tilesB == 1);
       const int step_m = t_step % unitsM, step_r = t_step / unitsM;
       int unit_m = t_first % unitsM, rest = t_first / unitsM;
-      int it = 0;
-      for (int t = t_first; t < t_end; t += t_step, ++it) {
+      for (int t = t_first; t < t_end; t += t_step) {
         const int m_idx = unit_m;
         int n_idx = rest, ks = 0;
         if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
@@ -215,10 +216,6 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
         const int kb_begin = ks * p.kb_per_split;
         const int kb_end = min(p.kb_total, kb_begin + p.kb_per_split);
         int kb = 0;
-        // mode 0: the ring holds the previous tile's accumulator until its epilogue ends.  The TMA-store modes keep it in
-        // registers, so only the empty barriers gate the ring and the next tile's first STAGES k-blocks load during the epilogue.
-        if (!kTmaEpi && it > 0) mbar_wait(acc_free, (it - 1) & 1);
-        VDB_TL(0, it);   // producer: starts issuing this tile
         for (int s = 0; s < p.nseg; ++s) {
           const ASeg sg = p.seg[s];
           if (kb + sg.nkb <= kb_begin) { kb += sg.nkb; continue; }
@@ -238,28 +235,9 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
     }
   } else {
     // ------------------------------ consumers: wgmma mainloop, then the epilogue ------------------------------
-    // Epilogue: warps w and w+4 own the same 32-row quarter of the tile (w & 3) and alternate 32-column chunks.
-    // acc_ld32 hands each thread one ROW of 32 columns; the transposing paths write the raw fp32 block to a private
-    // XOR-swizzled 4 KB shared-memory tile and read it back transposed, so every global access is 8 rows x 64 contiguous
-    // bytes per instruction (4 lanes per row), and bias / activation / residual / bf16 conversion run on 8 fixed columns
-    // per lane (bias lives in registers).
     if constexpr (igemm_realloc(BM, BN)) setmaxnreg_inc<232>();
-    const int quarter = warp & 3;          // 32-row quarter of the tile
-    const int half = warp >> 2;            // which of the kWPQ warps of the quarter
-    const int r = quarter * 32 + lane;
-    const int tr_row = lane >> 2, tr_q = lane & 3;   // transposed role: rows tr_row + 8k, columns tr_q*8 .. +7
-    float* stage = sstage + warp * 1024;             // [32 rows][32 fp32], 16-byte chunk j of row i at (j ^ (i & 7))
-    const uint32_t sacc_row = smem_u32(sacc) + static_cast<uint32_t>(r * kAccStride * 4);
-    auto acc_ld32 = [&](int col, uint32_t (&v)[32]) {   // row r, columns [col, col + 32) of the parked accumulator
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 x = lds_f4(sacc_row + (col + 4 * i) * 4);
-        v[4 * i] = __float_as_uint(x.x); v[4 * i + 1] = __float_as_uint(x.y);
-        v[4 * i + 2] = __float_as_uint(x.z); v[4 * i + 3] = __float_as_uint(x.w);
-      }
-    };
     // mainloop of one tile: warpgroup g multiplies its kMB blocks of 64 rows of A by the BN x 64 B tile of every k-block (block
-    // hb sits 8 KB after block hb - 1 in the stage), then (mode 0) both warpgroups park the accumulator in sacc
+    // hb sits 8 KB after block hb - 1 in the stage)
     uint32_t ml_stage = 0, ml_phase = 0;
     float acc[kMB][BN / 2];
     auto mainloop = [&](int kb_begin, int kb_end) {
@@ -295,44 +273,15 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
       for (int hb = 0; hb < kMB; ++hb) wgmma_fence_regs(acc[hb]);
       __syncwarp();
       if (lane == 0 && kb_end > kb_begin) mbar_arrive(&empty_bar[prev]);
-      if constexpr (!kTmaEpi) {
-        epi_bar_sync();                 // sacc aliases the ring: both warpgroups' MMAs have finished reading it
-        float* srow = sacc + (g * 64 + (warp & 3) * 16 + (lane >> 2)) * kAccStride + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[0][4 * j], acc[0][4 * j + 1]);
-          *reinterpret_cast<float2*>(srow + 8 * kAccStride + 8 * j) = make_float2(acc[0][4 * j + 2], acc[0][4 * j + 3]);
-        }
-        epi_bar_sync();
-      }
     };
-    auto stage_write = [&](const uint32_t (&v)[32]) {
-      float* srow = stage + lane * 32;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint4*>(srow + ((j ^ (lane & 7)) << 2)) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-    };
-    auto stage_read = [&](int k, float (&o)[8]) {   // row tr_row + 8k, columns tr_q*8 .. +7
-      const int row = k * 8 + tr_row;
-      const float* srow = stage + row * 32;
-      const float4 x0 = *reinterpret_cast<const float4*>(srow + (((2 * tr_q) ^ (row & 7)) << 2));
-      const float4 x1 = *reinterpret_cast<const float4*>(srow + (((2 * tr_q + 1) ^ (row & 7)) << 2));
-      o[0] = x0.x; o[1] = x0.y; o[2] = x0.z; o[3] = x0.w; o[4] = x1.x; o[5] = x1.y; o[6] = x1.z; o[7] = x1.w;
-    };
-    int it = 0;
-    int st_buf = 0;                     // TMA-store epilogues: which of this warp's kBoxes staging boxes is written next
-    (void)st_buf;
+    int st_buf = 0;                     // which of this warp's kBoxes staging boxes is written next
     const float* sbias_src = nullptr;   // which bias row/offset currently sits in sbias
-    // The per-tile bookkeeping sits on the critical path of epilogue-bound GEMMs (it was ~0.75 us of every ~3.6 us
-    // tile): the tile index advances incrementally (no divisions in the GEMM view), row indices are 32-bit, and
-    // everything that depends only on the thread is hoisted.
-    const int tw = r % p.TW;
-    const int th = (r / p.TW) % p.TH;
-    const int tb = r / (p.TW * p.TH);
+    // The per-tile bookkeeping sits on the critical path of epilogue-bound GEMMs: the tile index advances incrementally (no
+    // divisions in the GEMM view), row indices are 32-bit, and everything that depends only on the thread is hoisted.
     const bool flat = (p.tilesH == 1) && (p.tilesB == 1);   // GEMM view: M tiles along W only
     const int step_m = t_step % unitsM, step_r = t_step / unitsM;
     int unit_m = t_first % unitsM, rest = t_first / unitsM;
-    // TMA-store epilogues: the accumulator stays in the wgmma fragment layout, so in each 64-row block hb of its warpgroup warp w
+    // the accumulator stays in the wgmma fragment layout, so in each 64-row block hb of its warpgroup warp w
     // owns the 16 tile rows from e_row0 + 64 hb on (warpgroup w / 4, quarter w % 4) and this thread rows + lane / 4 and
     // + lane / 4 + 8 of them, at columns 8 j + 2 (lane % 4) + {0, 1}
     const int e_row0 = (warp >> 2) * (BM / 2) + (warp & 3) * 16;
@@ -362,7 +311,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
     if constexpr (kLnIn) {
       if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t_first < t_end) ln_prefetch((t_first % unitsM) * kBlockM + e_row0 + (lane & 15));
     }
-    for (int t = t_first; t < t_end; t += t_step, ++it) {
+    for (int t = t_first; t < t_end; t += t_step) {
       const int m_idx = unit_m;
       int n_idx = rest, ks = 0;
       if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
@@ -375,24 +324,9 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
       }
       unit_m += step_m; rest += step_r;
       if (unit_m >= unitsM) { unit_m -= unitsM; ++rest; }
-      const int w = wt * p.TW + tw, h = ht * p.TH + th, b = bt * p.TB + tb;
-      const bool row_ok = (w < p.Wo) && (h < p.Ho) && (b < p.Bo);
-      const int gp = (b * p.Ho + h) * p.Wo + w;     // output pixel (row of the GEMM); host guarantees M < 2^31
       const int gp_first = ((bt * p.TB) * p.Ho + ht * p.TH) * p.Wo + wt * p.TW;
       const int n0 = n_idx * BN;
 
-      // per-tile row bookkeeping for the transposed role (independent of the accumulator: done before the wait)
-      int gp_k[4];
-      bool ok_k[4];
-      if constexpr (!kTmaEpi) {
-        const unsigned okmask = __ballot_sync(0xffffffffu, row_ok);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int src = k * 8 + tr_row;
-          gp_k[k] = __shfl_sync(0xffffffffu, gp, src);
-          ok_k[k] = (okmask >> src) & 1u;
-        }
-      }
       // bias tile -> shared memory (one global read per tile); one row serves the tile unless the bias is per-batch
       // and the tile's first / last rows belong to different batch items
       const int gp_last = ((bt * p.TB + p.TB - 1) * p.Ho + ht * p.TH + p.TH - 1) * p.Wo + wt * p.TW + p.TW - 1;
@@ -441,13 +375,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
           sbias_src = brow;
         }
       }
-      const float* bias_g = (p.bias && !bias_uniform)
-                                ? p.bias + (p.bias_bstride ? static_cast<long long>(gp / p.rows_per_batch) * p.bias_bstride : 0) : nullptr;
-
-      const int f_nchunks = min(BN / 32, (p.N - n0) / 32);
-      const bool has_resid = p.resid != nullptr;
-
-      // TMA-store epilogues: output pixels (GEMM rows) of this thread's two accumulator rows
+      // output pixels (GEMM rows) of this thread's two accumulator rows
       int e_gp[kMB][2];
       bool e_ok[kMB][2];
 #pragma unroll
@@ -504,339 +432,242 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
         // request the next tile's row partials (GEMM view, M-fast order: unit_m already points at the next tile)
         if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t + t_step < t_end) ln_prefetch(unit_m * kBlockM + e_row0 + (lane & 15));
       }
-      VDB_TLE(4, it);   // consumers: mainloop starts
       mainloop(ks * p.kb_per_split, min(p.kb_total, ks * p.kb_per_split + p.kb_per_split));
-      VDB_TLE(5, it);   // consumers: accumulator parked
 
-      auto geglu_tile = [&] {
-        // packed tile: columns [0,BN/2) = value rows, [BN/2,BN) = gate rows of the same outputs
-        constexpr int HALF = BN / 2;
-        const int nout0 = n_idx * HALF;
-        const int Nout = p.N / 2;
-#pragma unroll 1
-        for (int c = (((HALF / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half; c < HALF / 32; c += kWPQ) {
-          uint32_t v[32];
-          float a[4][8];
-          acc_ld32(c * 32, v);
-          stage_write(v);
-          __syncwarp();
+      // ---- the epilogue, straight from the wgmma registers (no barrier between the warpgroups).  Each warp walks the 32-column
+      // chunks of its 16 rows: per-element fp32 arithmetic on the thread's 2 rows x 8 columns of the chunk, bf16 pack, two
+      // stmatrix into one 1 KB staging box of this warp (16 rows of 64 B, SWIZZLE_64B pattern), then lane 0 hands the box to the
+      // TMA unit (cp.async.bulk.tensor store; out-of-range rows / columns are clipped by the tensor map).  The kBoxes boxes of a
+      // warp rotate: a box is rewritten once the store issued from it kBoxes - 1 chunks ago has read it.  fp32 output and split-K
+      // partials (mode 0) skip the boxes: each thread stores its column pairs to global memory.  Bias / LayerNorm tables are read
+      // from shared memory as 8-byte broadcasts (columns 2 (lane % 4) + {0, 1}).  A 256-row tile runs this once per 64-row block
+      // of the warpgroup.
+      const uint32_t stg_s = smem_u32(sstage) + warp * kStgWarp;
+      // what modes 3-7 fix at compile time, mode 0 reads from the launch
+      const bool split = MODE == 0 && p.ksplit > 1;                      // raw fp32 partials, reduced by splitk_reduce_kernel
+      const bool f32_out = MODE == 0 && (split || p.out_f32);
+      const bool geglu = kGegluEpi || (MODE == 0 && p.act == ACT_GEGLU);
+      constexpr int kChunks = kGegluEpi ? BN / 64 : BN / 32;            // 32-column output chunks per tile
+      const int outc = geglu ? BN / 2 : BN;                             // output columns per tile
+      const int ocol0 = n_idx * outc;
+      const int nvalid = (geglu ? p.N / 2 : p.N) - ocol0;               // output columns of this tile inside the output
+      const int ochunks = geglu ? BN / 64 : min(BN / 32, (nvalid + 31) / 32);
+      const int tq2 = 2 * (lane & 3);                                    // this thread's first column of every 8-column group
+      // residual (modes 0 / 3 / 7): the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each (mode 0:
+      // one 2-byte load for a pair that ends at N, none past it), requested a chunk ahead
+      const bool do_resid = (MODE == 3 || MODE == 7 || (MODE == 0 && !split && !geglu)) && p.resid != nullptr;
+      const bool row_bias = MODE == 0 && p.bias && !bias_uniform && !split;   // a tile that one bias row does not cover
 #pragma unroll
-          for (int k = 0; k < 4; ++k) stage_read(k, a[k]);
-          __syncwarp();
-          acc_ld32(HALF + c * 32, v);
-          stage_write(v);
-          __syncwarp();
-          float bv[8], bg[8];
+      for (int hb = 0; hb < kMB; ++hb) {
+        const int b_row0 = e_row0 + 64 * hb;
+        const int ow = wt * p.TW + (b_row0 % p.TW), oh = ht * p.TH + ((b_row0 / p.TW) % p.TH), ob = bt * p.TB + b_row0 / (p.TW * p.TH);
+        const uint32_t* rrow[2];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            bv[i] = p.bias ? sbias[c * 32 + tr_q * 8 + i] : 0.f;
-            bg[i] = p.bias ? sbias[HALF + c * 32 + tr_q * 8 + i] : 0.f;
-          }
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float g[8];
-            stage_read(k, g);
-            if (ok_k[k] && nout0 + c * 32 + tr_q * 8 + 7 < Nout) {
-              float o[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) o[i] = (a[k][i] + bv[i]) * gelu_fast_f(g[i] + bg[i]);
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(gp_k[k]) * p.ldo + nout0 + c * 32 + tr_q * 8) =
-                  make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
-            }
-          }
-          __syncwarp();
-        }
-      };
-      if constexpr (kTmaEpi) {
-        // ---- TMA-store epilogues, straight from the wgmma registers (no park, no barrier between the warpgroups).  Each warp
-        // walks the 32-column chunks of its 16 rows: per-element fp32 arithmetic on the thread's 2 rows x 8 columns of the chunk,
-        // bf16 pack, two stmatrix into one 1 KB staging box of this warp (16 rows of 64 B, SWIZZLE_64B pattern), then lane 0
-        // hands the box to the TMA unit (cp.async.bulk.tensor store; out-of-range rows / columns are clipped by the tensor
-        // map).  The kBoxes boxes of a warp rotate: a box is rewritten once the store issued from it kBoxes - 1 chunks ago has
-        // read it.  Bias / LayerNorm tables are read from shared memory as 8-byte broadcasts (columns 2 (lane % 4) + {0, 1}).
-        // A 256-row tile runs this once per 64-row block of the warpgroup.
-        const uint32_t stg_s = smem_u32(sstage) + warp * kStgWarp;
-        constexpr int OUTC = kGegluEpi ? BN / 2 : BN;                    // output columns per tile
-        const int ochunks = kGegluEpi ? OUTC / 32 : f_nchunks;
-        const int ocol0 = n_idx * OUTC;
-        const int tq2 = 2 * (lane & 3);                                  // this thread's first column of every 8-column group
-        // residual (modes 3 / 7): the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each,
-        // requested a chunk ahead
-        const bool do_resid = (MODE == 3 || MODE == 7) && has_resid;
-#pragma unroll
-        for (int hb = 0; hb < kMB; ++hb) {
-          const int b_row0 = e_row0 + 64 * hb;
-          const int ow = wt * p.TW + (b_row0 % p.TW), oh = ht * p.TH + ((b_row0 / p.TW) % p.TH), ob = bt * p.TB + b_row0 / (p.TW * p.TH);
-          const uint32_t* rrow[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            rrow[h] = (do_resid && e_ok[hb][h]) ? reinterpret_cast<const uint32_t*>(p.resid + static_cast<long long>(e_gp[hb][h]) * p.ldr + ocol0 + tq2)
-                                                : nullptr;
-          auto load_resid = [&](int c, uint32_t (&rr)[2][4]) {
+        for (int h = 0; h < 2; ++h)
+          rrow[h] = (do_resid && e_ok[hb][h]) ? reinterpret_cast<const uint32_t*>(p.resid + static_cast<long long>(e_gp[hb][h]) * p.ldr + ocol0 + tq2)
+                                              : nullptr;
+        // row_bias: the bias row of the thread's row h (computed where it is used: kept live, it costs registers the whole epilogue)
+        auto rbias = [&](int h) { return p.bias + static_cast<long long>(e_gp[hb][h] / p.rows_per_batch) * p.bias_bstride + n0; };
+        auto load_resid = [&](int c, uint32_t (&rr)[2][4]) {
+          if (MODE != 0 || c * 32 + 32 <= nvalid) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
               for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rrow[h] ? __ldg(rrow[h] + (c * 32 + 8 * jj) / 2) : 0u;
-          };
-          uint32_t rr[2][4];
-          if (do_resid) load_resid(0, rr);
-          float st_su[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // mode 7: [row][chunk parity]
-          (void)st_su; (void)st_sq;
-          float nrm[2];                                                    // LN rows: -rstd * mean of the row
-#pragma unroll
-          for (int h = 0; h < 2; ++h) nrm[h] = -ln_a1[h] * ln_a0[h];
-          (void)nrm;
-#pragma unroll
-          for (int c = 0; c < OUTC / 32; ++c) {
-            if (c >= ochunks) break;
-            float o[4][2][2];                                              // [8-column group][row][column]
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int n = c * 32 + 8 * jj + tq2;                         // tile column of o[jj][.][0]
-              const float* va = acc[hb] + 4 * (4 * c + jj);                // {row 0: n, n + 1; row 8: n, n + 1}
-              if constexpr (kGegluEpi) {
-                const float* vg = acc[hb] + 4 * (BN / 16 + 4 * c + jj);    // gate columns OUTC + n
-                if constexpr (kLnIn) {   // GEGLU over a folded LayerNorm: r * (acc - mu * s) + c == fma(r, acc, fma(-r mu, s, c))
-                  const float2 sa = lds_f2(slnx_s + 4 * n), ca = lds_f2(sbias_s + 4 * n);
-                  const float2 sg = lds_f2(slnx_s + 4 * (OUTC + n)), cg = lds_f2(sbias_s + 4 * (OUTC + n));
-#pragma unroll
-                  for (int h = 0; h < 2; ++h) {
-                    o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h], fmaf(nrm[h], sg.x, cg.x)));
-                    o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h + 1], fmaf(nrm[h], sg.y, cg.y)));
-                  }
-                } else {
-                  const float2 ba = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
-                  const float2 bg = p.bias ? lds_f2(sbias_s + 4 * (OUTC + n)) : make_float2(0.f, 0.f);
-#pragma unroll
-                  for (int h = 0; h < 2; ++h) {
-                    o[jj][h][0] = (va[2 * h] + ba.x) * gelu_fast_f(vg[2 * h] + bg.x);
-                    o[jj][h][1] = (va[2 * h + 1] + ba.y) * gelu_fast_f(vg[2 * h + 1] + bg.y);
-                  }
-                }
-              } else if constexpr (kLnIn) {
-                if (p.ln_on_cols) {      // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
-                  const float2 mu = lds_f2(slnx_s + 4 * n), rs = lds_f2(sbias_s + 4 * n);
-#pragma unroll
-                  for (int h = 0; h < 2; ++h) {
-                    o[jj][h][0] = fmaf(rs.x, fmaf(mu.x, -ln_a0[h], va[2 * h]), ln_a1[h]);
-                    o[jj][h][1] = fmaf(rs.y, fmaf(mu.y, -ln_a0[h], va[2 * h + 1]), ln_a1[h]);
-                  }
-                } else {                 // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
-                  const float2 sx = lds_f2(slnx_s + 4 * n), cx = lds_f2(sbias_s + 4 * n);
-#pragma unroll
-                  for (int h = 0; h < 2; ++h) {
-                    o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sx.x, cx.x));
-                    o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sx.y, cx.y));
-                  }
-                }
-              } else {                   // modes 3 / 7: acc + bias, then + residual
-                const float2 bb = p.bias ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  o[jj][h][0] = va[2 * h] + bb.x;
-                  o[jj][h][1] = va[2 * h + 1] + bb.y;
-                }
-              }
-            }
-            if (do_resid) {
-              uint32_t rn[2][4];
-              const bool more = c + 1 < ochunks;
-              if (more) load_resid(c + 1, rn);
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) {
-                  const float2 x = unpack_bf16x2(rr[h][jj]);
-                  o[jj][h][0] += x.x;
-                  o[jj][h][1] += x.y;
-                }
-              if (more) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                  for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rn[h][jj];
-              }
-            }
-            if constexpr (kStatsOut) {
-              // LayerNorm statistics of the rows this GEMM produces (fp32, before the rounding), split by chunk parity
-#pragma unroll
-              for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                  for (int e = 0; e < 2; ++e) {
-                    st_su[h][c & 1] += o[jj][h][e];
-                    st_sq[h][c & 1] = fmaf(o[jj][h][e], o[jj][h][e], st_sq[h][c & 1]);
-                  }
-            }
-            // the box about to be rewritten was handed to the TMA unit kBoxes - 1 chunks ago: wait until it has been read
-            if (lane == 0) bulk_wait_read<kBoxes - 1>();
-            __syncwarp();
-            const uint32_t box = stg_s + st_buf * 1024;
-            {
-              // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
-              // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
-              const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-                const int unit = 2 * u + (mi >> 1);
-                stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
-                            pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
-                            pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
-              }
-            }
-            fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
-            __syncwarp();
-            if (lane == 0) {
-              tma_store_4d(&p.tmO, reinterpret_cast<const uint8_t*>(sstage) + warp * kStgWarp + st_buf * 1024, ocol0 + c * 32, ow, oh, ob);
-              bulk_commit();
-            }
-            st_buf = (st_buf + 1) & (kBoxes - 1);
-          }
-          if constexpr (kStatsOut) {
-            // one (sum, sum of squares) per row, N tile and chunk parity: slot 2 n_idx + parity of [2 tilesN][M][2].  The four lanes
-            // of a row reduce over the quad; a parity without chunks writes zeros
+          } else {                       // the last chunk of a ragged N
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
-              for (int par = 0; par < 2; ++par) {
-                float su = st_su[h][par], sq = st_sq[h][par];
-                su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
-                su += __shfl_xor_sync(0xffffffffu, su, 2); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
-                if ((lane & 3) == 0 && e_ok[hb][h])
-                  reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * 2 + par) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + e_gp[hb][h]] =
-                      make_float2(su, sq);
+              for (int jj = 0; jj < 4; ++jj) {
+                const uint32_t* q = rrow[h] + (c * 32 + 8 * jj) / 2;
+                const int left = nvalid - (c * 32 + 8 * jj + tq2);     // columns of the pair inside the output
+                rr[h][jj] = !rrow[h] || left <= 0 ? 0u : left >= 2 ? __ldg(q) : __ldg(reinterpret_cast<const unsigned short*>(q));
               }
           }
-        }
-      } else if (p.ksplit > 1) {
-        // fp32 partials, reduced (+bias/act/residual) by splitk_reduce_kernel
-        const long long Mtot = static_cast<long long>(p.Bo) * p.Ho * p.Wo;
-        float* dst = p.partial + (static_cast<long long>(ks) * Mtot + gp) * p.N + n0;
-#pragma unroll 1
-        for (int c = half; c < BN / 32; c += kWPQ) {
-          if (n0 + c * 32 >= p.N) break;
-          uint32_t v[32];
-          acc_ld32(c * 32, v);
-          if (row_ok) {
+        };
+        uint32_t rr[2][4];
+        if (do_resid) load_resid(0, rr);
+        float st_su[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, st_sq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // mode 7: [row][chunk parity]
+        (void)st_su; (void)st_sq;
+        float nrm[2];                                                    // LN rows: -rstd * mean of the row
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const int n = n0 + c * 32 + j;
-              if (n + 3 < p.N) {
-                *reinterpret_cast<float4*>(dst + c * 32 + j) =
-                    make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+        for (int h = 0; h < 2; ++h) nrm[h] = -ln_a1[h] * ln_a0[h];
+        (void)nrm;
+#pragma unroll
+        for (int c = 0; c < kChunks; ++c) {
+          if (c >= ochunks) break;
+          float o[4][2][2];                                              // [8-column group][row][column]
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int n = c * 32 + 8 * jj + tq2;                         // tile column of o[jj][.][0]
+            const float* va = acc[hb] + 4 * (4 * c + jj);                // {row 0: n, n + 1; row 8: n, n + 1}
+            if (split) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) { o[jj][h][0] = va[2 * h]; o[jj][h][1] = va[2 * h + 1]; }
+            } else if (geglu && c < BN / 64) {   // (c: mode 0 unrolls BN / 32 chunks, GEGLU has BN / 64)
+              const float* vg = acc[hb] + 4 * (BN / 16 + 4 * c + jj);    // gate columns outc + n
+              if constexpr (kLnIn) {   // GEGLU over a folded LayerNorm: r * (acc - mu * s) + c == fma(r, acc, fma(-r mu, s, c))
+                const float2 sa = lds_f2(slnx_s + 4 * n), ca = lds_f2(sbias_s + 4 * n);
+                const float2 sg = lds_f2(slnx_s + 4 * (outc + n)), cg = lds_f2(sbias_s + 4 * (outc + n));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sa.x, ca.x)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h], fmaf(nrm[h], sg.x, cg.x)));
+                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sa.y, ca.y)) * gelu_fast_f(fmaf(ln_a1[h], vg[2 * h + 1], fmaf(nrm[h], sg.y, cg.y)));
+                }
               } else {
-                for (int q = 0; q < 4; ++q)
-                  if (n + q < p.N) dst[c * 32 + j + q] = __uint_as_float(v[j + q]);
-              }
-            }
-          }
-        }
-      } else if (p.act == ACT_GEGLU) {
-        geglu_tile();
-      } else {
-        const int nchunks = min(BN / 32, (p.N - n0 + 31) / 32);
-        auto chunk = [&](int c, const uint32_t (&v)[32], const uint4 (&rr)[4], bool fast) {
-          const int nb = n0 + c * 32;
-          if (fast) {
-            stage_write(v);
-            __syncwarp();
-            if (c == half) VDB_TLE(8, it);
-            float bb[8];
+                const float2 bas = bias_uniform ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
+                const float2 bgs = bias_uniform ? lds_f2(sbias_s + 4 * (outc + n)) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) bb[i] = p.bias ? sbias[c * 32 + tr_q * 8 + i] : 0.f;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              float o[8];
-              stage_read(k, o);
-              if (ok_k[k]) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) o[i] += bb[i];
-                if (p.alpha != 1.f) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) o[i] *= p.alpha;
-                }
-                if (p.act != ACT_NONE) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) o[i] = apply_act(o[i], p.act);
-                }
-                if (p.resid) {
-                  const uint32_t w4[4] = {rr[k].x, rr[k].y, rr[k].z, rr[k].w};
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) {
-                    const float2 x = unpack_bf16x2(w4[q]);
-                    o[2 * q] += x.x;
-                    o[2 * q + 1] += x.y;
+                for (int h = 0; h < 2; ++h) {
+                  float2 ba = bas, bg = bgs;
+                  if (MODE == 0 && row_bias && e_ok[hb][h]) {
+                    const float* b = rbias(h);
+                    ba = make_float2(__ldg(b + n), __ldg(b + n + 1));
+                    bg = make_float2(__ldg(b + outc + n), __ldg(b + outc + n + 1));
                   }
+                  o[jj][h][0] = (va[2 * h] + ba.x) * gelu_fast_f(vg[2 * h] + bg.x);
+                  o[jj][h][1] = (va[2 * h + 1] + ba.y) * gelu_fast_f(vg[2 * h + 1] + bg.y);
                 }
-                *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(gp_k[k]) * p.ldo + nb + tr_q * 8) =
-                    make_uint4(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], o[3]), pack_bf16x2(o[4], o[5]), pack_bf16x2(o[6], o[7]));
               }
-              if (c == half && k == 0) VDB_TLE(9, it);
-            }
-            __syncwarp();   // the tile is rewritten by this warp's next chunk
-            if (c == half) VDB_TLE(10, it);
-          } else if (row_ok) {
-            // slow path (fp32 output, partial last chunk, per-row bias): one row per thread
-            float f[32];
+            } else if constexpr (kLnIn) {
+              if (p.ln_on_cols) {      // out = rstd[n] * (acc - mean[n] * s[m]) + c[m]
+                const float2 mu = lds_f2(slnx_s + 4 * n), rs = lds_f2(sbias_s + 4 * n);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-            if (p.bias) {
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(rs.x, fmaf(mu.x, -ln_a0[h], va[2 * h]), ln_a1[h]);
+                  o[jj][h][1] = fmaf(rs.y, fmaf(mu.y, -ln_a0[h], va[2 * h + 1]), ln_a1[h]);
+                }
+              } else {                 // out = rstd[m] * (acc - mean[m] * s[n]) + c[n] == fma(r, acc, fma(-r mu, s, c))
+                const float2 sx = lds_f2(slnx_s + 4 * n), cx = lds_f2(sbias_s + 4 * n);
 #pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (nb + j < p.N) f[j] += bias_uniform ? sbias[c * 32 + j] : __ldg(bias_g + nb + j);
-            }
+                for (int h = 0; h < 2; ++h) {
+                  o[jj][h][0] = fmaf(ln_a1[h], va[2 * h], fmaf(nrm[h], sx.x, cx.x));
+                  o[jj][h][1] = fmaf(ln_a1[h], va[2 * h + 1], fmaf(nrm[h], sx.y, cx.y));
+                }
+              }
+            } else {                   // modes 0 / 3 / 7: acc + bias, then (mode 0) * alpha and the activation, then + residual
+              // (_rn: every step rounds on its own, as the kernel always has; no FMA contraction across them)
+              const float2 bb = bias_uniform ? lds_f2(sbias_s + 4 * n) : make_float2(0.f, 0.f);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j] * p.alpha, p.act);
-            if (p.resid) {
-              const __nv_bfloat16* rs = p.resid + static_cast<long long>(gp) * p.ldr + nb;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) if (nb + j < p.N) f[j] += __bfloat162float(rs[j]);
-            }
-            if (p.out_f32) {
-              float* dst = reinterpret_cast<float*>(p.out) + static_cast<long long>(gp) * p.ldo + nb;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) if (nb + j < p.N) dst[j] = f[j];
-            } else {
-              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(gp) * p.ldo + nb;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) if (nb + j < p.N) dst[j] = __float2bfloat16(f[j]);
+              for (int h = 0; h < 2; ++h) {
+                o[jj][h][0] = __fadd_rn(va[2 * h], bb.x);
+                o[jj][h][1] = __fadd_rn(va[2 * h + 1], bb.y);
+              }
             }
           }
-        };
-        auto is_fast = [&](int c) { return (n0 + c * 32 + 32 <= p.N) && !p.out_f32 && (bias_uniform || !p.bias); };
-        auto load_resid = [&](int c, uint4 (&rr)[4]) {
-          if (p.resid && is_fast(c)) {
+          if (MODE == 0 && !split && !geglu) {
+            if (row_bias) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              if (ok_k[k]) rr[k] = __ldg(reinterpret_cast<const uint4*>(p.resid + static_cast<long long>(gp_k[k]) * p.ldr + n0 + c * 32 + tr_q * 8));
+              for (int h = 0; h < 2; ++h) {
+                if (!e_ok[hb][h]) continue;
+                const float* b = rbias(h);
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                  const int n = c * 32 + 8 * jj + tq2;
+                  const float* va = acc[hb] + 4 * (4 * c + jj) + 2 * h;
+                  o[jj][h][0] = __fadd_rn(va[0], n < nvalid ? __ldg(b + n) : 0.f);
+                  o[jj][h][1] = __fadd_rn(va[1], n + 1 < nvalid ? __ldg(b + n + 1) : 0.f);
+                }
+              }
+            }
+            alpha_act8(&o[0][0][0], p.alpha, p.act);
+            alpha_act8(&o[2][0][0], p.alpha, p.act);
           }
-        };
-        // this warp's chunks: half, half+2, ... (kept un-pipelined: double-buffering the 32-register accumulator chunk
-        // pushed the kernel into spills and was measured slower)
-        // chunk count not a multiple of the warps per quarter (BN = 160: five): rotate who takes the extra chunk
-        const int first = (((BN / 32) % kWPQ) != 0) ? ((half + it) % kWPQ) : half;
-#pragma unroll 1
-        for (int c = first; c < nchunks; c += kWPQ) {
-          uint4 rr[4];
-          load_resid(c, rr);          // residual loads are in flight while the accumulator chunk is fetched
-          uint32_t v[32];
-          acc_ld32(c * 32, v);
-          if (c == first) VDB_TLE(7, it);
-          chunk(c, v, rr, is_fast(c));
+          if (do_resid) {
+            uint32_t rn[2][4];
+            const bool more = c + 1 < ochunks;
+            if (more) load_resid(c + 1, rn);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const float2 x = unpack_bf16x2(rr[h][jj]);
+                o[jj][h][0] = __fadd_rn(o[jj][h][0], x.x);
+                o[jj][h][1] = __fadd_rn(o[jj][h][1], x.y);
+              }
+            if (more) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) rr[h][jj] = rn[h][jj];
+            }
+          }
+          if constexpr (kStatsOut) {
+            // LayerNorm statistics of the rows this GEMM produces (fp32, before the rounding), split by chunk parity
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  st_su[h][c & 1] += o[jj][h][e];
+                  st_sq[h][c & 1] = fmaf(o[jj][h][e], o[jj][h][e], st_sq[h][c & 1]);
+                }
+          }
+          if (f32_out) {
+            // fp32 columns pairs straight to global memory: float2 where the row stride keeps the pair 8-byte aligned (out is
+            // 16-byte aligned, the partials' row stride N is a multiple of 4), single floats otherwise and at the end of a row
+            float* const base = split ? p.partial + static_cast<long long>(ks) * p.Bo * p.Ho * p.Wo * p.N : reinterpret_cast<float*>(p.out);
+            const long long ld = split ? p.N : p.ldo;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (!e_ok[hb][h]) continue;
+              float* const row = base + static_cast<long long>(e_gp[hb][h]) * ld + ocol0 + c * 32 + tq2;
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const int left = nvalid - (c * 32 + 8 * jj + tq2);
+                if (left >= 2 && !(ld & 1)) {
+                  *reinterpret_cast<float2*>(row + 8 * jj) = make_float2(o[jj][h][0], o[jj][h][1]);
+                } else {
+                  if (left >= 1) row[8 * jj] = o[jj][h][0];
+                  if (left >= 2) row[8 * jj + 1] = o[jj][h][1];
+                }
+              }
+            }
+            continue;
+          }
+          // the box about to be rewritten was handed to the TMA unit kBoxes - 1 chunks ago: wait until it has been read
+          if (lane == 0) bulk_wait_read<kBoxes - 1>();
+          __syncwarp();
+          const uint32_t box = stg_s + st_buf * 1024;
+          {
+            // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
+            // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
+            const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int unit = 2 * u + (mi >> 1);
+              stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
+                          pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
+                          pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
+            }
+          }
+          fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
+          __syncwarp();
+          if (lane == 0) {
+            tma_store_4d(&p.tmO, sstage + warp * kStgWarp + st_buf * 1024, ocol0 + c * 32, ow, oh, ob);
+            bulk_commit();
+          }
+          st_buf = (st_buf + 1) & (kBoxes - 1);
+        }
+        if constexpr (kStatsOut) {
+          // one (sum, sum of squares) per row, N tile and chunk parity: slot 2 n_idx + parity of [2 tilesN][M][2].  The four lanes
+          // of a row reduce over the quad; a parity without chunks writes zeros
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int par = 0; par < 2; ++par) {
+              float su = st_su[h][par], sq = st_sq[h][par];
+              su += __shfl_xor_sync(0xffffffffu, su, 1); sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+              su += __shfl_xor_sync(0xffffffffu, su, 2); sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+              if ((lane & 3) == 0 && e_ok[hb][h])
+                reinterpret_cast<float2*>(p.stats_out)[static_cast<long long>(n_idx * 2 + par) * (static_cast<long long>(p.Bo) * p.Ho * p.Wo) + e_gp[hb][h]] =
+                    make_float2(su, sq);
+            }
         }
       }
-      if constexpr (!kTmaEpi) {
-        fence_proxy_async_smem();      // this warp's sacc reads are ordered before the producer's next TMA writes
-        __syncwarp();
-        VDB_TLE(6, it);   // epilogue: tile stored (this warp)
-        if (lane == 0) mbar_arrive(acc_free);
-      }
     }
-    if constexpr (MODE >= 3) {
-      if (lane == 0) bulk_wait<0>();     // every TMA store of this thread has completed before the CTA may exit
-    }
+    if (lane == 0) bulk_wait<0>();     // every TMA store of this thread has completed before the CTA may exit
   }
 }
 
@@ -884,8 +715,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int kspl
 template <int BM, int BN, int STAGES, int EW, int MODE>
 static int launch_igemm(const IgemmParams& p0, int num_units, cudaStream_t stream) {
   constexpr bool kLn = MODE == 5 || MODE == 6;       // one more [BN] fp32 table (colsum / column mean)
-  constexpr size_t ring = STAGES * (BM + BN) * kBlockK * 2, acc = MODE >= 3 ? 0 : BM * (BN + 4) * 4;   // (see igemm_kernel)
-  constexpr size_t need = (ring > acc ? ring : acc) + (2 * STAGES + 2) * 8 + BN * 4 + (kLn ? BN * 4 : 0) + EW * igemm_boxes(BM) * 1024;
+  constexpr size_t need = STAGES * (BM + BN) * kBlockK * 2 + 2 * STAGES * 8 + BN * 4 + (kLn ? BN * 4 : 0) + EW * igemm_boxes(BM) * 1024;   // (see igemm_kernel)
   // + up to 1024 bytes of slack for the 1024-byte alignment of the operand ring (the LN modes at BN 256 may get less: the dynamic
   // window starts 1024-aligned in practice, and the kernel traps if its carve-up would not fit)
   constexpr size_t smem = (need + 1024 <= 227 * 1024) ? need + 1024 : 227 * 1024;
@@ -917,17 +747,15 @@ static int pick_bn(int N, int act, int forced) {
   return 256;
 }
 
-static unsigned long long* g_timeline = nullptr;
-
 // The last run_igemm decision on this thread (vdb_igemm_last_plan): BN, STAGES, MODE, ksplit, grid, tilesM, tilesN; and its tile
 // height (vdb_igemm_last_bm)
 constexpr int kPlanFields = 7;
 static thread_local int g_last_plan[kPlanFields] = {0};
 static thread_local int g_last_bm = 0;
 
-// Mode 0 stores bf16 output rows and loads residual rows as 16-byte vectors, the split-K reduction stores fp32 rows as float4,
-// and the TMA-store epilogues need a 16-byte aligned output map, so out / resid must be 16-byte aligned.  Checked before any
-// tensor map is built, so that a bad pointer is reported as an argument error.
+// bf16 output leaves through a TMA output map (16-byte aligned base and row stride), the split-K reduction stores fp32 rows as
+// float4 and the fp32 epilogue column pairs as float2, so out / resid must be 16-byte aligned.  Checked before any tensor map is
+// built, so that a bad pointer is reported as an argument error.
 static int check_epilogue_pointers(const void* out, long long ldo, int out_f32, const void* resid, long long ldr, const char* who) {
   if ((reinterpret_cast<uintptr_t>(out) & 15) || (resid && (reinterpret_cast<uintptr_t>(resid) & 15)))
     return set_error(VDB_ERR_INVALID, "%s: out and resid must be 16-byte aligned", who);
@@ -1086,7 +914,6 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
   if (e.stats_parts) *e.stats_parts = 2 * p.tilesN;
   p.ln_inv_dim = e.ln_dim > 0 ? 1.f / static_cast<float>(e.ln_dim) : 0.f; p.ln_eps = e.ln_eps;
   p.ln_colsum = e.ln_colsum; p.ln_rowbias = e.ln_rowbias; p.stats_out = e.stats_out;
-  p.timeline = g_timeline;
   int rc = make_tmap_2d(&p.tmB, Wt, static_cast<uint64_t>(Ktot), static_cast<uint64_t>(N),
                         static_cast<uint64_t>(ldw) * 2, kBlockK, BN);
   if (rc) return rc;
@@ -1097,12 +924,12 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     if (e.act == ACT_GEGLU && BN == 256) mode = 4;
     else if (e.act == ACT_NONE && e.alpha == 1.f && (N % 32) == 0) mode = 3;
   }
-  // modes 3 / 4 store the output tile through shared memory + cp.async.bulk.tensor: a warp's 16 rows x 32 columns are one box
-  // of the output tensor map (the M tile shapes hold at least 16 / (bw * bh) images; check_epilogue_pointers has checked the
-  // alignment of out / resid)
-  if (mode == 3 || mode == 4) {
+  // bf16 output leaves through shared memory + cp.async.bulk.tensor: a warp's 16 rows x 32 columns are one box of the output
+  // tensor map, which clips the rows and columns past the output (the M tile shapes hold at least 16 / (bw * bh) images;
+  // check_epilogue_pointers has checked the alignment of out / resid).  fp32 output and split-K partials are stored directly.
+  if (!e.out_f32 && p.ksplit == 1) {
     const int bw = std::min(p.TW, 16), bh = std::min(p.TH, 16 / bw), bb = 16 / (bw * bh);
-    const long long ncols = (mode == 4) ? N / 2 : N;
+    const long long ncols = (e.act == ACT_GEGLU) ? N / 2 : N;
     // out_parity >= 0: the same tile, written into every second pixel of every second row of the [B, 2Ho, 2Wo, N] tensor —
     // only the strides and the base of the output tensor map change, the kernel does not know
     const int py = e.out_parity >= 0 ? (e.out_parity >> 1) : 0, px = e.out_parity >= 0 ? (e.out_parity & 1) : 0;
@@ -1192,9 +1019,6 @@ using namespace vdb;
 // C ABI
 // ---------------------------------------------------------------------------------------------
 extern "C" {
-
-// debug aid (not part of the product ABI): device buffer of 16*8 u64 receiving CTA 0's per-tile role timestamps
-void vdb_debug_igemm_timeline(void* buf) { g_timeline = reinterpret_cast<unsigned long long*>(buf); }
 
 // see include/vdb200.h
 int vdb_igemm_last_plan(int* out, int n) {
