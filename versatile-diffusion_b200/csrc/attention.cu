@@ -106,9 +106,7 @@ __global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();
-  if constexpr (VARLEN) {   // kv_len may be written by the kernel this launch overlaps: read it only after pdl_wait
+  if constexpr (VARLEN) {
     nk = max(0, min(p.kv_len[b], p.Nk));
     ntiles = (nk + BKV - 1) / BKV;
   }
@@ -285,7 +283,7 @@ struct AttnArgs {   // what the C ABI received; the tensor maps depend on the ke
 };
 
 template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false>
-static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t stream) {
+static int launch_attention(AttnParams& p, const AttnArgs& a, void* stream) {
   constexpr size_t smem = attention_smem_bytes<DK, DVP, BKV, KV_STAGES>();
   // two CTAs per SM need twice the dynamic window plus 1 KB each reserved by the system, within 228 KB
   static_assert(smem <= (TMA_WARP ? 227 * 1024 : 113 * 1024), "attention smem budget");
@@ -304,9 +302,7 @@ static int launch_attention(AttnParams& p, const AttnArgs& a, cudaStream_t strea
   rc = make_tmap_2d(&p.tmV, a.Vt, static_cast<uint64_t>(a.B) * a.kv_bstride, static_cast<uint64_t>(a.H) * DVP, a.ldv * 2, 64, DVP);
   if (rc) return rc;
   dim3 grid((p.Nq + kBQ - 1) / kBQ, a.H, a.B);
-  VDB_CUDA_CHECK(launch_pdl(kernel, grid, dim3(attention_threads(TMA_WARP)), smem, stream, p));
-  count_launch();
-  return VDB_OK;
+  return launch(kernel, grid, dim3(attention_threads(TMA_WARP)), smem, stream, p);
 }
 
 }  // namespace vdb
@@ -359,14 +355,13 @@ int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, 
                                    scale, causal, p, a);
   if (rc) return rc;
   const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // d_head <= 80: two CTAs per SM, each within 128 registers and half the shared memory (d_head <= 64: 128-key tiles,
   // 3 / 2 stages; d_head 80: 64-key tiles, 3 stages).  d_head 160 keeps the TMA warp and one CTA per SM: two CTAs' Q and
   // K / V^T stages do not fit; 64-key tiles keep its S + O + P within the register budget.
-  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false>(p, a, st);
-  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false>(p, a, st);
-  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false>(p, a, st);
-  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true>(p, a, st);
+  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false>(p, a, stream);
+  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false>(p, a, stream);
+  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false>(p, a, stream);
+  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true>(p, a, stream);
   return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel for d_head %d", d_head);
 }
 
@@ -385,7 +380,7 @@ int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const vo
                                    scale, causal, p, a);
   if (rc) return rc;
   p.kv_len = kv_len;
-  return launch_attention<64, 64, 128, 2, false, true>(p, a, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attention<64, 64, 128, 2, false, true>(p, a, stream);
 }
 
 }  // extern "C"

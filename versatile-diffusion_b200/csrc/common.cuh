@@ -193,20 +193,6 @@ VDB_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32
 template <int R>
 VDB_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// nanosecond wall clock shared by all SMs (debug timelines, watchdogs)
-VDB_DEVINL unsigned long long gtime() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
-// ----------------------------------------------------------------------------
-// programmatic dependent launch: a kernel launched with the PDL attribute may start while its predecessor
-// drains; it must not touch dependent global memory before pdl_wait(). No-ops for ordinary launches.
-// ----------------------------------------------------------------------------
-VDB_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-VDB_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // ----------------------------------------------------------------------------
 // small math / packing helpers
 // ----------------------------------------------------------------------------

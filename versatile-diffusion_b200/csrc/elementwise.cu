@@ -423,8 +423,6 @@ constexpr int kGnMaxBatch = 1024;
 __global__ void __launch_bounds__(kGnThreads) gn_stats_kernel(const __nv_bfloat16* __restrict__ x1, int C1,
                                                               const __nv_bfloat16* __restrict__ x2, int C2,
                                                               int HW, int groups, float eps, float* __restrict__ scratch) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int C = C1 + C2;
   const int V = C / 8;
   const int cpg = C / groups;
@@ -530,8 +528,6 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __nv_bfloat16* __re
                                                        const float* __restrict__ beta, int act,
                                                        __nv_bfloat16* __restrict__ y) {
   extern __shared__ float sm[];
-  pdl_launch_dependents();
-  pdl_wait();
   const int C = C1 + C2;
   const int cpg = C / groups;
   float* scale = sm;
@@ -587,16 +583,6 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __nv_bfloat16* __re
 }
 
 // ---------------------------------------------------------------------------------------------
-// Debug build only (-DVDB_TIMELINE, tools/gn_timeline.py): globaltimer stamps of thread 0 of CTA (0,0) of the single-launch
-// GroupNorm: 0 start, 1 statistics loads + accumulation done, 2 partial published, 3 every CTA of the image arrived,
-// 4 statistics folded, 5 scale / shift table ready, 6 normalised + stored.
-__device__ unsigned long long* g_gn_timeline_dev = nullptr;
-#ifdef VDB_TIMELINE
-#define VDB_GTL(slot) do { if (g_gn_timeline_dev && threadIdx.x == 0 && blockIdx.x == 0 && blockIdx.y == 0) g_gn_timeline_dev[slot] = gtime(); } while (0)
-#else
-#define VDB_GTL(slot) do { } while (0)
-#endif
-
 // Single-launch GroupNorm: statistics + apply in ONE kernel.  grid (nsplit, B) with nsplit*B <= the number of CTAs that
 // are resident at once (occupancy query on the host), so that every CTA of the grid is resident; each CTA reduces its
 // pixel range (deterministic, as gn_stats_kernel), publishes its partial, waits on a per-image arrival counter for
@@ -624,9 +610,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
   const int V = C / 8;
   const int cpg = C / groups;
   const int b = blockIdx.y, split = blockIdx.x, nsplit = gridDim.x, B = gridDim.y;
-  pdl_launch_dependents();
-  pdl_wait();
-  VDB_GTL(0);
   int* arrive = reinterpret_cast<int*>(scratch);
   int* depart = arrive + kGnMaxBatch;
   float* partial = scratch + 2 * kGnMaxBatch + static_cast<size_t>(B) * 2 * groups;
@@ -681,7 +664,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
     for (int i = 0; i < 8; ++i) { dst[i] = s[i]; dst[8 + i] = q[i]; }
   }
   __syncthreads();
-  VDB_GTL(1);
   for (int c = threadIdx.x; c < C; c += kGnThreads) {
     float s = 0.f, q = 0.f;
     for (int l = 0; l < lanes; ++l) {
@@ -712,7 +694,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
   // ---- publish, then wait for the other CTAs of this image (all CTAs of the grid are resident by construction) ----
   __threadfence();
   __syncthreads();
-  VDB_GTL(2);
   if (threadIdx.x == 0) {
     atomicAdd(&arrive[b], 1);
     int seen;
@@ -723,7 +704,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
     __threadfence();
   }
   __syncthreads();
-  VDB_GTL(3);
   // fold the image's nsplit partial rows (64 floats each: sum | sumsq per group) with the whole CTA: 8 row-lanes x 64
   // columns of coalesced L2 loads, then a fixed-order sum over the lanes -- every CTA of the image computes
   // bit-identical statistics.  (One thread per group walking all rows was ~4 us of serialised L2 latency.)
@@ -748,7 +728,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
     grstd[threadIdx.x] = rsqrtf(var + eps);
   }
   __syncthreads();
-  VDB_GTL(4);
   if (threadIdx.x == 0) {   // last CTA of the image to have read the partials re-arms both counters for the next launch
     if (atomicAdd(&depart[b], 1) == nsplit - 1) { arrive[b] = 0; depart[b] = 0; }
   }
@@ -765,7 +744,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
     }
   }
   __syncthreads();
-  VDB_GTL(5);
   // ---- phase 2: normalise this CTA's pixels ----
   if (active) {
     __nv_bfloat16* dstb = y + static_cast<long long>(b) * HW * C + v * 8;
@@ -801,7 +779,6 @@ __global__ void __launch_bounds__(kGnThreads, 2) gn_fused_kernel(const __nv_bflo
       }
     }
   }
-  VDB_GTL(6);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -844,8 +821,6 @@ __global__ void __launch_bounds__(THREADS, (THREADS == 512 && NVMAX <= 6) ? 2 : 
   const int lanes = THREADS / VPB;
   const int S = gridDim.y;
   const int b = blockIdx.z, bundle = blockIdx.x, part = blockIdx.y;
-  pdl_launch_dependents();
-  pdl_wait();
   __shared__ float wpart[THREADS / 32][8];          // per-warp partials: sum | sumsq of up to 4 groups
   __shared__ float xpart[8];              // this CTA's partials
   __shared__ float xall[8][8];            // S > 1: every rank's partials, WRITTEN BY THE PEERS (st.shared::cluster)
@@ -1029,8 +1004,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __nv_bfloat16* __r
                                                         const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, float eps,
                                                         __nv_bfloat16* __restrict__ y) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -1107,8 +1080,6 @@ __global__ void __launch_bounds__(256, 2) layernorm_rg_kernel(const __nv_bfloat1
                                                            float eps, __nv_bfloat16* __restrict__ y) {
   constexpr int RPW = 32 / LPR;           // rows per warp and step
   extern __shared__ float ln_gb[];        // gamma[C] | beta[C]
-  pdl_launch_dependents();
-  pdl_wait();
   for (int i = threadIdx.x; i < C; i += blockDim.x) { ln_gb[i] = __ldg(gamma + i); ln_gb[C + i] = __ldg(beta + i); }
   __syncthreads();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -1682,6 +1653,14 @@ static int ew_blocks(long long work_items, int threads) {
   return static_cast<int>(b);
 }
 
+// whether a_floats floats from a and b_floats floats from b share a byte (a NULL pointer shares none)
+static bool overlaps(const void* a, long long a_floats, const void* b, long long b_floats) {
+  if (!a || !b) return false;
+  const uintptr_t a_lo = reinterpret_cast<uintptr_t>(a), a_hi = a_lo + static_cast<uintptr_t>(a_floats) * sizeof(float);
+  const uintptr_t b_lo = reinterpret_cast<uintptr_t>(b), b_hi = b_lo + static_cast<uintptr_t>(b_floats) * sizeof(float);
+  return a_lo < b_hi && b_lo < a_hi;
+}
+
 }  // namespace vdb
 
 using namespace vdb;
@@ -1697,11 +1676,8 @@ int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x
        reinterpret_cast<uintptr_t>(x_prev_dup)) & 15)
     return set_error(VDB_ERR_INVALID, "ddim_cfg_step: pointers must be 16-byte aligned");
   const int threads = 256;
-  ddim_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      e_uncond, e_cond, x, noise, coef, step_idx, scale, temperature, x_prev, x_prev_dup, pred_x0, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(ddim_cfg_step_kernel, ew_blocks((n + 3) / 4, threads), threads, 0, stream, e_uncond, e_cond, x, noise, coef,
+                step_idx, scale, temperature, x_prev, x_prev_dup, pred_x0, n);
 }
 
 int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
@@ -1713,18 +1689,12 @@ int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* 
        reinterpret_cast<uintptr_t>(x_next_dup)) & 15)
     return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: pointers must be 16-byte aligned");
   // the ring is written while x is read and x_next / x_next_dup / pred_x0 are written: it must not share a byte with them
-  const uintptr_t h_lo = reinterpret_cast<uintptr_t>(hist), h_hi = h_lo + 3 * static_cast<uintptr_t>(n) * sizeof(float);
   for (const float* p : {x, static_cast<const float*>(x_next), static_cast<const float*>(x_next_dup),
-                         static_cast<const float*>(pred_x0)}) {
-    const uintptr_t lo = reinterpret_cast<uintptr_t>(p), hi = lo + static_cast<uintptr_t>(n) * sizeof(float);
-    if (p && lo < h_hi && h_lo < hi) return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: hist overlaps x, x_next, x_next_dup or pred_x0");
-  }
+                         static_cast<const float*>(pred_x0)})
+    if (overlaps(hist, 3 * n, p, n)) return set_error(VDB_ERR_INVALID, "dpmpp_cfg_step: hist overlaps x, x_next, x_next_dup or pred_x0");
   const int threads = 256;
-  dpmpp_cfg_step_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(dpmpp_cfg_step_kernel, ew_blocks((n + 3) / 4, threads), threads, 0, stream, e_uncond, e_cond, x, coef, step_idx,
+                scale, hist, x_next, x_next_dup, pred_x0, n);
 }
 
 int vdb_inpaint_blend_f32(float* x, float* x_dup, const float* x0, const float* mask, int mask_per_item, const float* table,
@@ -1737,40 +1707,24 @@ int vdb_inpaint_blend_f32(float* x, float* x_dup, const float* x0, const float* 
     return set_error(VDB_ERR_INVALID, "inpaint_blend: pointers must be 16-byte aligned");
   const long long n = static_cast<long long>(bs) * hw * c;
   // x / x_dup are written while x0, the mask and the noise are read through the read-only path: no byte may be shared
-  const long long in_len[3] = {n, (mask_per_item ? bs : 1) * hw, n};
-  const float* ins[3] = {x0, mask, noise};
-  for (const float* o : {static_cast<const float*>(x), static_cast<const float*>(x_dup)}) {
-    const uintptr_t o_lo = reinterpret_cast<uintptr_t>(o), o_hi = o_lo + static_cast<uintptr_t>(n) * sizeof(float);
-    for (int k = 0; k < 3; ++k) {
-      const uintptr_t lo = reinterpret_cast<uintptr_t>(ins[k]), hi = lo + static_cast<uintptr_t>(in_len[k]) * sizeof(float);
-      if (o && ins[k] && lo < o_hi && o_lo < hi)
-        return set_error(VDB_ERR_INVALID, "inpaint_blend: x0, mask or noise overlaps x or x_dup");
-    }
-  }
+  for (const float* o : {static_cast<const float*>(x), static_cast<const float*>(x_dup)})
+    if (overlaps(o, n, x0, n) || overlaps(o, n, mask, (mask_per_item ? bs : 1) * hw) || overlaps(o, n, noise, n))
+      return set_error(VDB_ERR_INVALID, "inpaint_blend: x0, mask or noise overlaps x or x_dup");
   const int threads = 256;
-  inpaint_blend_kernel<<<ew_blocks((n + 3) / 4, threads), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, x_dup, x0, mask, mask_per_item, table, step_idx, seed, noise, n, hw, c);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(inpaint_blend_kernel, ew_blocks((n + 3) / 4, threads), threads, 0, stream, x, x_dup, x0, mask, mask_per_item,
+                table, step_idx, seed, noise, n, hw, c);
 }
 
 int vdb_inpaint_noise_f32(const unsigned long long* seed, const int* step_idx, long long n, float* out, void* stream) {
   if (!seed || !step_idx || !out || n <= 0) return set_error(VDB_ERR_INVALID, "inpaint_noise: null/empty argument");
-  inpaint_noise_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(seed, step_idx, n, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(inpaint_noise_kernel, ew_blocks((n + 3) / 4, 256), 256, 0, stream, seed, step_idx, n, out);
 }
 
 int vdb_mask_to_latent(const float* mask, int n, int H8, int W8, float* out, void* stream) {
   if (!mask || !out || n <= 0 || H8 <= 0 || W8 <= 0) return set_error(VDB_ERR_INVALID, "mask_to_latent: null/empty argument");
   if (H8 % 8 || W8 % 8) return set_error(VDB_ERR_INVALID, "mask_to_latent: H8 and W8 must be multiples of 8");
-  mask_to_latent_kernel<<<ew_blocks(static_cast<long long>(n) * (H8 / 8) * (W8 / 8), 256), 256, 0,
-                          reinterpret_cast<cudaStream_t>(stream)>>>(mask, n, H8, W8, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(mask_to_latent_kernel, ew_blocks(static_cast<long long>(n) * (H8 / 8) * (W8 / 8), 256), 256, 0, stream, mask, n,
+                H8, W8, out);
 }
 
 int vdb_composite_f32(const float* decoded, const float* image, const float* mask, int mask_per_item, int n, int c, long long hw,
@@ -1778,19 +1732,7 @@ int vdb_composite_f32(const float* decoded, const float* image, const float* mas
   if (!decoded || !image || !mask || !out || n <= 0 || c <= 0 || hw <= 0)
     return set_error(VDB_ERR_INVALID, "composite: null/empty argument");
   const long long total = static_cast<long long>(n) * c * hw;
-  composite_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(decoded, image, mask, mask_per_item,
-                                                                                               c, hw, total, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
-}
-
-// whether a_floats floats from a and b_floats floats from b share a byte (a NULL pointer shares none)
-static bool overlaps(const void* a, long long a_floats, const void* b, long long b_floats) {
-  if (!a || !b) return false;
-  const uintptr_t a_lo = reinterpret_cast<uintptr_t>(a), a_hi = a_lo + static_cast<uintptr_t>(a_floats) * sizeof(float);
-  const uintptr_t b_lo = reinterpret_cast<uintptr_t>(b), b_hi = b_lo + static_cast<uintptr_t>(b_floats) * sizeof(float);
-  return a_lo < b_hi && b_lo < a_hi;
+  return launch(composite_kernel, ew_blocks(total, 256), 256, 0, stream, decoded, image, mask, mask_per_item, c, hw, total, out);
 }
 
 int vdb_latent_store_slot_f32(const float* x, float* ring, int slots, const int* step_idx, int offset, long long n,
@@ -1800,11 +1742,7 @@ int vdb_latent_store_slot_f32(const float* x, float* ring, int slots, const int*
     return set_error(VDB_ERR_INVALID, "latent_store_slot: pointers must be 16-byte aligned");
   if (overlaps(x, n, ring, static_cast<long long>(slots) * n))
     return set_error(VDB_ERR_INVALID, "latent_store_slot: x overlaps the ring");
-  latent_store_slot_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, ring, slots,
-                                                                                                            step_idx, offset, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(latent_store_slot_kernel, ew_blocks((n + 3) / 4, 256), 256, 0, stream, x, ring, slots, step_idx, offset, n);
 }
 
 int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots, const float* mask, int mask_per_item,
@@ -1819,11 +1757,8 @@ int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots
   for (const float* o : {static_cast<const float*>(x), static_cast<const float*>(x_dup)})
     if (overlaps(o, n, ring, static_cast<long long>(slots) * n) || overlaps(o, n, mask, (mask_per_item ? bs : 1) * hw))
       return set_error(VDB_ERR_INVALID, "inversion_blend: ring or mask overlaps x or x_dup");
-  inversion_blend_kernel<<<ew_blocks((n + 3) / 4, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, x_dup, ring, slots, mask, mask_per_item, step_idx, n, hw, c);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(inversion_blend_kernel, ew_blocks((n + 3) / 4, 256), 256, 0, stream, x, x_dup, ring, slots, mask, mask_per_item,
+                step_idx, n, hw, c);
 }
 
 int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,
@@ -1838,42 +1773,24 @@ int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_sr
   for (const float* e : {e_src_u, e_src_c, e_tgt_u, e_tgt_c})
     if (overlaps(out, static_cast<long long>(bs) * hw, e, n))
       return set_error(VDB_ERR_INVALID, "diffedit_mask: out overlaps an eps input");
-  diffedit_mask_kernel<<<bs, kDiffEditThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, bs, hw, c, ratio, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(diffedit_mask_kernel, bs, kDiffEditThreads, 0, stream, e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, bs,
+                hw, c, ratio, out);
 }
 
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream) {
   if (!x || !z || !y || n <= 0) return set_error(VDB_ERR_INVALID, "axpby: null/empty argument");
-  axpby_kernel<<<ew_blocks(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, z, a, b, y, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(axpby_kernel, ew_blocks(n, 256), 256, 0, stream, x, z, a, b, y, n);
 }
 
 int vdb_lincomb4_f32(const float* x0, const float* x1, const float* x2, const float* x3, float c0, float c1, float c2,
                      float c3, float* y, long long n, void* stream) {
   if (!x0 || !y || n <= 0) return set_error(VDB_ERR_INVALID, "lincomb4: null/empty argument");
-  lincomb4_kernel<<<ew_blocks(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x0, x1, x2, x3, c0, c1, c2, c3, y, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(lincomb4_kernel, ew_blocks(n, 256), 256, 0, stream, x0, x1, x2, x3, c0, c1, c2, c3, y, n);
 }
 
 int vdb_add_int(int* p, int delta, void* stream) {
   if (!p) return set_error(VDB_ERR_INVALID, "add_int: null");
-  add_int_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, delta);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
-}
-
-// debug aid (stamps exist only in a -DVDB_TIMELINE build): 8 x u64 device buffer receiving the single-launch GroupNorm's phases
-void vdb_debug_gn_timeline(void* buf) {
-  unsigned long long* p = reinterpret_cast<unsigned long long*>(buf);
-  cudaMemcpyToSymbol(vdb::g_gn_timeline_dev, &p, sizeof(p));
+  return launch(add_int_kernel, 1, 1, 0, stream, p, delta);
 }
 
 // see include/vdb200.h
@@ -1905,7 +1822,6 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
   if (groups != 32 || (C % groups) || (C1 % 8) || (x2 && (C2 % 8)) || C / 8 > kGnThreads)
     return set_error(VDB_ERR_UNSUPPORTED, "groupnorm: need 32 groups, C %% 32 == 0, C/8 <= 512 (C=%d)", C);
   if (!x2) C2 = 0;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // group-bundle kernel: see gn_bundle_kernel
   if (groups == 32) {
     const int cpg = C / groups;
@@ -1916,18 +1832,11 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       const __nv_bfloat16* x1b = reinterpret_cast<const __nv_bfloat16*>(x1);
       const __nv_bfloat16* x2b = reinterpret_cast<const __nv_bfloat16*>(x2);
       __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(y);
-      auto launch = [&](auto kernel, int nvmax, int threads, int S, size_t smem = 0) -> int {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(groups / G, S, B); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-        set_norm_plan(1, nvmax, threads, G, S, 0, cfg.gridDim);
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = S; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        VDB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, x1b, C1, x2b, C2, HW, groups, G, eps, act, gamma, beta, yb));
-        count_launch();
-        return VDB_OK;
+      auto launch_bundle = [&](auto kernel, int nvmax, int threads, int S, size_t smem = 0) -> int {
+        const dim3 grid(groups / G, S, B);
+        set_norm_plan(1, nvmax, threads, G, S, 0, grid);
+        return launch(dim3(1, S, 1), kernel, grid, dim3(threads), smem, stream, x1b, C1, x2b, C2, HW, groups, G, eps, act, gamma,
+                      beta, yb);
       };
       auto nper_t = [&](int threads, int S) { const int ln = threads / VPB; return (((HW + S - 1) / S) + ln - 1) / ln; };
       // big layers (the 64x64 level at B = 8): 1024-thread CTAs, one per SM, the pixels staged in up to 176 KB of shared memory:
@@ -1944,7 +1853,7 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
               VDB_CUDA_CHECK(cudaFuncSetAttribute(gn_bundle_kernel<11, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
               configured = true;
             }
-            return launch(gn_bundle_kernel<11, 1024>, 11, 1024, S, smem);
+            return launch_bundle(gn_bundle_kernel<11, 1024>, 11, 1024, S, smem);
           }
         }
       }
@@ -1955,9 +1864,9 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
       // small grids: more CTAs per image while every thread still keeps >= 2 pixels
       while (S < 8 && static_cast<long long>(groups / G) * S * B < num_sms() && nper(S * 2) >= 2) S *= 2;
       const int n = nper(S);
-      if (n <= 2) return launch(gn_bundle_kernel<2, 512>, 2, 512, S);
-      if (n <= 6) return launch(gn_bundle_kernel<6, 512>, 6, 512, S);
-      if (n <= 12) return launch(gn_bundle_kernel<12, 512>, 12, 512, S);
+      if (n <= 2) return launch_bundle(gn_bundle_kernel<2, 512>, 2, 512, S);
+      if (n <= 6) return launch_bundle(gn_bundle_kernel<6, 512>, 6, 512, S);
+      if (n <= 12) return launch_bundle(gn_bundle_kernel<12, 512>, 12, 512, S);
     }
   }
   // every CTA of the single-launch kernel must be resident: ask the runtime how many fit (registers / shared memory)
@@ -1974,38 +1883,32 @@ int vdb_groupnorm_nhwc(const void* x1, int C1, const void* x2, int C2, int B, in
     if (ns4 <= max_ns) {   // register-resident variant for the small layers
       const int ns = std::max(1, std::min(max_ns, std::max(ns4, (HW + 7) / 8)));
       set_norm_plan(2, 4, 0, 0, 0, ns, dim3(ns, B));
-      VDB_CUDA_CHECK(launch_pdl(gn_fused_kernel<4>, dim3(ns, B), dim3(kGnThreads), 0, st, x1b, C1, x2b, C2, HW, groups, eps,
-                                act, gamma, beta, scratch, yb));
-    } else {
-      const int ns = std::max(1, std::min(max_ns, (HW + 31) / 32));
-      set_norm_plan(2, 0, 0, 0, 0, ns, dim3(ns, B));
-      VDB_CUDA_CHECK(launch_pdl(gn_fused_kernel<0>, dim3(ns, B), dim3(kGnThreads), 0, st, x1b, C1, x2b, C2, HW, groups, eps,
-                                act, gamma, beta, scratch, yb));
+      return launch(gn_fused_kernel<4>, dim3(ns, B), dim3(kGnThreads), 0, stream, x1b, C1, x2b, C2, HW, groups, eps, act, gamma,
+                    beta, scratch, yb);
     }
-    count_launch(1);
-    return VDB_OK;
+    const int ns = std::max(1, std::min(max_ns, (HW + 31) / 32));
+    set_norm_plan(2, 0, 0, 0, 0, ns, dim3(ns, B));
+    return launch(gn_fused_kernel<0>, dim3(ns, B), dim3(kGnThreads), 0, stream, x1b, C1, x2b, C2, HW, groups, eps, act, gamma, beta,
+                  scratch, yb);
   }
   const int nsplit = vdb_groupnorm_nsplit(B, HW);
   set_norm_plan(3, 0, 0, 0, 0, nsplit, dim3(nsplit, B));
-  VDB_CUDA_CHECK(launch_pdl(gn_stats_kernel, dim3(nsplit, B), dim3(kGnThreads), 0, st,
-                            reinterpret_cast<const __nv_bfloat16*>(x1), C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2,
-                            HW, groups, eps, scratch));
+  const int rc = launch(gn_stats_kernel, dim3(nsplit, B), dim3(kGnThreads), 0, stream, reinterpret_cast<const __nv_bfloat16*>(x1),
+                        C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2, HW, groups, eps, scratch);
+  if (rc) return rc;
   const float* stats = scratch + 2 * kGnMaxBatch;
   const long long work = static_cast<long long>(HW) * (C / 8);
   // ~8 vectors per thread: amortises the per-CTA scale/shift prologue
   int nblk = static_cast<int>(std::min<long long>((work + 2047) / 2048, std::max(1, (num_sms() * 8) / std::max(B, 1))));
-  VDB_CUDA_CHECK(launch_pdl(gn_apply_kernel, dim3(nblk, B), dim3(256), 2 * C * sizeof(float), st,
-                            reinterpret_cast<const __nv_bfloat16*>(x1), C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2,
-                            HW, groups, stats, gamma, beta, act, reinterpret_cast<__nv_bfloat16*>(y)));
-  count_launch(2);
-  return VDB_OK;
+  return launch(gn_apply_kernel, dim3(nblk, B), dim3(256), 2 * C * sizeof(float), stream, reinterpret_cast<const __nv_bfloat16*>(x1),
+                C1, reinterpret_cast<const __nv_bfloat16*>(x2), C2, HW, groups, stats, gamma, beta, act,
+                reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, const float* beta, float eps, void* y,
                   void* stream) {
   if (!x || !gamma || !beta || !y || rows <= 0) return set_error(VDB_ERR_INVALID, "layernorm: null/empty argument");
   if ((C % 8) || C > 8 * 32 * 8) return set_error(VDB_ERR_UNSUPPORTED, "layernorm: C must be a multiple of 8, <= 2048");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int threads = 256;
   const int V = C / 8;
   const int R = V <= 64 ? 4 : (V <= 160 ? 2 : 1);
@@ -2020,9 +1923,7 @@ int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, cons
     const long long steps = (rows + rpw - 1) / rpw;                         // warp steps
     const int grid = static_cast<int>(std::max<long long>(1, std::min<long long>((steps + 7) / 8, static_cast<long long>(occ) * num_sms())));
     set_norm_plan(4, vpl, 32 / rpw, 0, 0, 0, dim3(grid));
-    VDB_CUDA_CHECK(launch_pdl(kernel, dim3(grid), dim3(threads), smem, st, xp, rows, C, gamma, beta, eps, yp));
-    count_launch();
-    return VDB_OK;
+    return launch(kernel, dim3(grid), dim3(threads), smem, stream, xp, rows, C, gamma, beta, eps, yp);
   };
   switch (V) {
     case 40: return launch_rg(layernorm_rg_kernel<5, 8>, 5, 4);      // C 320
@@ -2036,83 +1937,57 @@ int vdb_layernorm(const void* x, long long rows, int C, const float* gamma, cons
     default: break;
   }
   set_norm_plan(5, V <= 64 ? 2 : (V <= 160 ? 5 : 8), R, 0, 0, 0, dim3(blocks));
-  if (V <= 64)
-    VDB_CUDA_CHECK(launch_pdl(layernorm_kernel<2, 4>, dim3(blocks), dim3(threads), 0, st, xp, rows, C, gamma, beta, eps, yp));
-  else if (V <= 160)
-    VDB_CUDA_CHECK(launch_pdl(layernorm_kernel<5, 2>, dim3(blocks), dim3(threads), 0, st, xp, rows, C, gamma, beta, eps, yp));
-  else
-    VDB_CUDA_CHECK(launch_pdl(layernorm_kernel<8, 1>, dim3(blocks), dim3(threads), 0, st, xp, rows, C, gamma, beta, eps, yp));
-  count_launch();
-  return VDB_OK;
+  if (V <= 64) return launch(layernorm_kernel<2, 4>, dim3(blocks), dim3(threads), 0, stream, xp, rows, C, gamma, beta, eps, yp);
+  if (V <= 160) return launch(layernorm_kernel<5, 2>, dim3(blocks), dim3(threads), 0, stream, xp, rows, C, gamma, beta, eps, yp);
+  return launch(layernorm_kernel<8, 1>, dim3(blocks), dim3(threads), 0, stream, xp, rows, C, gamma, beta, eps, yp);
 }
 
 int vdb_affine_act_rows(const void* x, long long rows, int n, const float* gamma, const float* beta, int act, void* y, void* stream) {
   if (!x || !gamma || !beta || !y || rows <= 0 || n <= 0 || (n % 8)) return set_error(VDB_ERR_INVALID, "affine_act_rows: bad argument (n %% 8 == 0)");
-  affine_act_rows_kernel<<<ew_blocks(rows * (n / 8), 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), rows, n, gamma, beta, act, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(affine_act_rows_kernel, ew_blocks(rows * (n / 8), 256), 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x),
+                rows, n, gamma, beta, act, reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 int vdb_pack_conv_weight(const float* w, int Cout, int Cin, int kh, int kw, void* out, long long ldo, long long col0, void* stream) {
   if (!w || !out || Cout <= 0 || Cin <= 0 || kh <= 0 || kw <= 0) return set_error(VDB_ERR_INVALID, "pack_conv_weight: null/empty argument");
   if (ldo < col0 + static_cast<long long>(kh) * kw * Cin) return set_error(VDB_ERR_INVALID, "pack_conv_weight: ldo too small");
   const long long total = static_cast<long long>(Cout) * kh * kw * Cin;
-  pack_conv_weight_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      w, Cout, Cin, kh, kw, reinterpret_cast<__nv_bfloat16*>(out), ldo, col0);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(pack_conv_weight_kernel, ew_blocks(total, 256), 256, 0, stream, w, Cout, Cin, kh, kw,
+                reinterpret_cast<__nv_bfloat16*>(out), ldo, col0);
 }
 
 int vdb_pack_geglu(const float* w, const float* b, int n2, int K, void* w_out, float* b_out, void* stream) {
   if (!w || !w_out || n2 <= 0 || K <= 0 || (b && !b_out)) return set_error(VDB_ERR_INVALID, "pack_geglu: null/empty argument");
   if (n2 % 128) return set_error(VDB_ERR_INVALID, "pack_geglu: the GEGLU width must be a multiple of 128");
-  pack_geglu_kernel<<<ew_blocks(2LL * n2 * K, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      w, b, n2, K, reinterpret_cast<__nv_bfloat16*>(w_out), b_out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(pack_geglu_kernel, ew_blocks(2LL * n2 * K, 256), 256, 0, stream, w, b, n2, K,
+                reinterpret_cast<__nv_bfloat16*>(w_out), b_out);
 }
 
 int vdb_pad_heads(const float* w, int H, int d, int dpad, int K, void* out, void* stream) {
   if (!w || !out || H <= 0 || d <= 0 || dpad < d || K <= 0) return set_error(VDB_ERR_INVALID, "pad_heads: bad argument");
-  pad_heads_kernel<<<ew_blocks(static_cast<long long>(H) * dpad * K, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      w, H, d, dpad, K, reinterpret_cast<__nv_bfloat16*>(out));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(pad_heads_kernel, ew_blocks(static_cast<long long>(H) * dpad * K, 256), 256, 0, stream, w, H, d, dpad, K,
+                reinterpret_cast<__nv_bfloat16*>(out));
 }
 
 int vdb_upsample2x_nhwc(const void* x, int B, int H, int W, int C, void* y, void* stream) {
   if (!x || !y || (C % 8)) return set_error(VDB_ERR_INVALID, "upsample2x: null argument or C %% 8 != 0");
   const long long total = static_cast<long long>(B) * 4 * H * W * (C / 8);
-  upsample2x_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), B, H, W, C, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(upsample2x_kernel, ew_blocks(total, 256), 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x), B, H, W, C,
+                reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 int vdb_clip_to_u8_hwc(const float* x, int n, int H, int W, void* y, void* stream) {
   if (!x || !y || n <= 0 || H <= 0 || W <= 0) return set_error(VDB_ERR_INVALID, "clip_to_u8_hwc: bad argument");
-  clip_to_u8_hwc_kernel<<<ew_blocks(static_cast<long long>(n) * H * W * 3, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, n, H, W, reinterpret_cast<uint8_t*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(clip_to_u8_hwc_kernel, ew_blocks(static_cast<long long>(n) * H * W * 3, 256), 256, 0, stream, x, n, H, W,
+                reinterpret_cast<uint8_t*>(y));
 }
 
 int vdb_resample_h_u8(const void* x, int n, int H, int Win, int Wout, const int* bounds, const int* kk, int ksize, void* y,
                       void* stream) {
   if (!x || !y || !bounds || !kk || n <= 0 || H <= 0 || Win <= 0 || Wout <= 0 || ksize <= 0)
     return set_error(VDB_ERR_INVALID, "resample_h_u8: bad argument");
-  resample_h_u8_kernel<<<ew_blocks(static_cast<long long>(n) * H * Wout * 3, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const uint8_t*>(x), n, H, Win, Wout, bounds, kk, ksize, reinterpret_cast<uint8_t*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(resample_h_u8_kernel, ew_blocks(static_cast<long long>(n) * H * Wout * 3, 256), 256, 0, stream,
+                reinterpret_cast<const uint8_t*>(x), n, H, Win, Wout, bounds, kk, ksize, reinterpret_cast<uint8_t*>(y));
 }
 
 int vdb_resample_v_crop_norm(const void* x, int n, int Hin, int W, const int* bounds, const int* kk, int ksize, int top,
@@ -2120,82 +1995,54 @@ int vdb_resample_v_crop_norm(const void* x, int n, int Hin, int W, const int* bo
   if (!x || !y || !mean3 || !std3 || n <= 0 || Hin <= 0 || W <= 0 || S <= 0 || top < 0 || left < 0 || left + S > W ||
       (ksize > 0 && (!bounds || !kk)) || (ksize == 0 && top + S > Hin))
     return set_error(VDB_ERR_INVALID, "resample_v_crop_norm: bad argument");
-  resample_v_crop_norm_kernel<<<ew_blocks(static_cast<long long>(n) * 3 * S * S, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const uint8_t*>(x), n, Hin, W, bounds, kk, ksize, top, left, S, mean3[0], mean3[1], mean3[2], std3[0],
-      std3[1], std3[2], y);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(resample_v_crop_norm_kernel, ew_blocks(static_cast<long long>(n) * 3 * S * S, 256), 256, 0, stream,
+                reinterpret_cast<const uint8_t*>(x), n, Hin, W, bounds, kk, ksize, top, left, S, mean3[0], mean3[1], mean3[2],
+                std3[0], std3[1], std3[2], y);
 }
 
 int vdb_im2col3x3_small(const float* x, int B, int H, int W, int Cin, int Kpad, float in_scale, float in_shift,
                         void* y, void* stream) {
   if (!x || !y || 9 * Cin > Kpad || (Kpad % 8)) return set_error(VDB_ERR_INVALID, "im2col3x3_small: bad argument");
   const long long total = static_cast<long long>(B) * H * W * (Kpad / 8);
-  im2col3x3_small_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, B, H, W, Cin, Kpad, in_scale, in_shift, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(im2col3x3_small_kernel, ew_blocks(total, 256), 256, 0, stream, x, B, H, W, Cin, Kpad, in_scale, in_shift,
+                reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 int vdb_permute_f32(const float* x, int B, int C, long long HW, int to_nhwc, float mul, float add, int clamp01,
                     float* y, void* stream) {
   if (!x || !y) return set_error(VDB_ERR_INVALID, "permute_f32: null argument");
   const long long total = static_cast<long long>(B) * C * HW;
-  permute_f32_kernel<<<ew_blocks(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, B, C, static_cast<int>(HW), to_nhwc, mul, add, clamp01, y);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(permute_f32_kernel, ew_blocks(total, 256), 256, 0, stream, x, B, C, static_cast<int>(HW), to_nhwc, mul, add,
+                clamp01, y);
 }
 
 int vdb_pointwise_small(const float* x, long long npix, int Cin, int Cout, const float* Wm, const float* bias,
                         float pre_mul, float* y, void* stream) {
   if (!x || !Wm || !y || Cin <= 0 || Cin > 8 || Cout <= 0 || Cout > 8)
     return set_error(VDB_ERR_INVALID, "pointwise_small: need 1 <= Cin, Cout <= 8");
-  pointwise_small_kernel<<<ew_blocks(npix, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, npix, Cin, Cout, Wm,
-                                                                                                  bias, pre_mul, y);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(pointwise_small_kernel, ew_blocks(npix, 256), 256, 0, stream, x, npix, Cin, Cout, Wm, bias, pre_mul, y);
 }
 
 int vdb_gaussian_sample(const float* moments, const float* noise, int C, long long npix, float post_mul, float* z,
                         void* stream) {
   if (!moments || !z || C <= 0 || npix <= 0) return set_error(VDB_ERR_INVALID, "gaussian_sample: bad argument");
-  gaussian_sample_kernel<<<ew_blocks(npix * C, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      moments, noise, C, npix, post_mul, z);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(gaussian_sample_kernel, ew_blocks(npix * C, 256), 256, 0, stream, moments, noise, C, npix, post_mul, z);
 }
 
 int vdb_cast_f32_bf16(const float* x, void* y, long long n, void* stream) {
   if (!x || !y) return set_error(VDB_ERR_INVALID, "cast: null argument");
-  cast_f32_bf16_kernel<<<ew_blocks(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, reinterpret_cast<__nv_bfloat16*>(y), n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(cast_f32_bf16_kernel, ew_blocks(n, 256), 256, 0, stream, x, reinterpret_cast<__nv_bfloat16*>(y), n);
 }
 int vdb_cast_bf16_f32(const void* x, float* y, long long n, void* stream) {
   if (!x || !y) return set_error(VDB_ERR_INVALID, "cast: null argument");
-  cast_bf16_f32_kernel<<<ew_blocks(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), y, n);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(cast_bf16_f32_kernel, ew_blocks(n, 256), 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x), y, n);
 }
 
 int vdb_timestep_embedding(const long long* ts, const int* step_idx, int B, int dim, float neg_log_period, float* out,
                            void* stream) {
   if (!ts || !out || B <= 0 || dim <= 1) return set_error(VDB_ERR_INVALID, "timestep_embedding: bad argument");
-  timestep_embedding_kernel<<<ew_blocks(static_cast<long long>(B) * (dim / 2), 128), 128, 0,
-                              reinterpret_cast<cudaStream_t>(stream)>>>(ts, step_idx, B, dim, neg_log_period, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(timestep_embedding_kernel, ew_blocks(static_cast<long long>(B) * (dim / 2), 128), 128, 0, stream, ts, step_idx, B,
+                dim, neg_log_period, out);
 }
 
 int vdb_linear_small(const float* x, int M, int K, const void* Wt, int N, const float* bias, int act_in, int act_out,
@@ -2209,61 +2056,44 @@ int vdb_linear_small(const float* x, int M, int K, const void* Wt, int N, const 
     configured = true;
   }
   const int blocks = std::min((N + 31) / 32, num_sms() * 2);
-  linear_small_kernel<<<blocks, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
-      x, M, K, reinterpret_cast<const __nv_bfloat16*>(Wt), N, bias, act_in, act_out, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(linear_small_kernel, blocks, 256, smem, stream, x, M, K, reinterpret_cast<const __nv_bfloat16*>(Wt), N, bias,
+                act_in, act_out, out);
 }
 
 int vdb_clip_text_embed(const long long* tokens, const float* tok_emb, const float* pos_emb, int B, int L, int Lp, int C,
                         void* x, void* stream) {
   if (!tokens || !tok_emb || !pos_emb || !x || Lp < L) return set_error(VDB_ERR_INVALID, "clip_text_embed: bad argument");
-  clip_text_embed_kernel<<<ew_blocks(static_cast<long long>(B) * Lp * C, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      tokens, tok_emb, pos_emb, B, L, Lp, C, reinterpret_cast<__nv_bfloat16*>(x));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(clip_text_embed_kernel, ew_blocks(static_cast<long long>(B) * Lp * C, 256), 256, 0, stream, tokens, tok_emb,
+                pos_emb, B, L, Lp, C, reinterpret_cast<__nv_bfloat16*>(x));
 }
 
 int vdb_patchify(const float* pixels, int B, int Cin, int HW, int P, int Kpad, void* y, void* stream) {
   if (!pixels || !y || HW % P || Cin * P * P > Kpad || (Kpad % 8)) return set_error(VDB_ERR_INVALID, "patchify: bad argument");
   const int G = HW / P;
-  patchify_kernel<<<ew_blocks(static_cast<long long>(B) * G * G * Kpad, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      pixels, B, Cin, HW, P, Kpad, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(patchify_kernel, ew_blocks(static_cast<long long>(B) * G * G * Kpad, 256), 256, 0, stream, pixels, B, Cin, HW, P,
+                Kpad, reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 int vdb_vit_assemble(const void* patches, const float* cls, const float* pos, const float* tok_scale, int B, int L, int Lp,
                      int C, void* x, void* stream) {
   if (!patches || !cls || !pos || !x || Lp < L) return set_error(VDB_ERR_INVALID, "vit_assemble: bad argument");
-  vit_assemble_kernel<<<ew_blocks(static_cast<long long>(B) * Lp * C, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(patches), cls, pos, tok_scale, B, L, Lp, C, reinterpret_cast<__nv_bfloat16*>(x));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(vit_assemble_kernel, ew_blocks(static_cast<long long>(B) * Lp * C, 256), 256, 0, stream,
+                reinterpret_cast<const __nv_bfloat16*>(patches), cls, pos, tok_scale, B, L, Lp, C,
+                reinterpret_cast<__nv_bfloat16*>(x));
 }
 
 int vdb_scale_by_row_norm(const void* z, const int* idx, const float* row_scale, int B, int L, int Lp, int C, float* out,
                           void* stream) {
   if (!z || !out || B <= 0 || Lp < L) return set_error(VDB_ERR_INVALID, "scale_by_row_norm: bad argument");
-  scale_by_row_norm_kernel<<<B, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(z), idx, row_scale, L, Lp, C, out);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(scale_by_row_norm_kernel, B, 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(z), idx, row_scale, L, Lp, C,
+                out);
 }
 
 int vdb_softmax_rows(const void* x, long long rows, int n, long long ld, float scale, void* y, void* stream) {
   if (!x || !y || rows <= 0 || n <= 0) return set_error(VDB_ERR_INVALID, "softmax_rows: bad argument");
   const int blocks = static_cast<int>(std::min<long long>(rows, num_sms() * 8LL));
-  softmax_rows_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), rows, n, ld, scale, reinterpret_cast<__nv_bfloat16*>(y));
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(softmax_rows_kernel, blocks, 256, 0, stream, reinterpret_cast<const __nv_bfloat16*>(x), rows, n, ld, scale,
+                reinterpret_cast<__nv_bfloat16*>(y));
 }
 
 }  // extern "C"

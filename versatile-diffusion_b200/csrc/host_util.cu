@@ -1,6 +1,5 @@
 #include "host_util.h"
 #include <cstdarg>
-#include <cstdlib>
 #include <atomic>
 #include <mutex>
 
@@ -16,12 +15,7 @@ int set_error(int code, const char* fmt, ...) {
   va_end(ap);
   return code;
 }
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VDB_PDL"); v = (e && e[0] == '1') ? 1 : 0; }   // measured neutral inside the step graph: opt-in
-  return v != 0;
-}
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 int num_sms() {
   static int sms = 0;

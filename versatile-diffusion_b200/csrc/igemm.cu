@@ -25,11 +25,12 @@ constexpr int kBlockM = 128;  // tile height of every launch the 256-row rule in
 constexpr int kBlockK = 64;  // bf16 elements = 128 B = one swizzle row
 constexpr int kMaxA = 6;     // A tensor maps per launch
 constexpr int kMaxSeg = 12;  // K segments per launch
+constexpr int kNumEpiWarps = 8;  // the two consumer warpgroups, which run the epilogue too; the producer warp follows them
 // A 256-row tile (160 accumulator registers per thread) or a 256-column one (128) does not fit the 168 registers that 288
 // threads leave each thread: those instantiations launch a whole producer warpgroup (384 threads, one warp of it works) that
 // hands its registers to the consumers (setmaxnreg: 128 x 40 + 256 x 232 = 64512 of the SM's 65536).
 __host__ __device__ constexpr bool igemm_realloc(int BM, int BN) { return BM == 256 || BN == 256; }
-__host__ __device__ constexpr int igemm_threads(int BM, int BN, int EW) { return 32 * EW + (igemm_realloc(BM, BN) ? 128 : 32); }
+__host__ __device__ constexpr int igemm_threads(int BM, int BN) { return 32 * kNumEpiWarps + (igemm_realloc(BM, BN) ? 128 : 32); }
 // TMA-store staging boxes (1 KB) per epilogue warp: four, or two where four 52 KB stages leave no room for more
 __host__ __device__ constexpr int igemm_boxes(int BM) { return BM == 256 ? 2 : 4; }
 
@@ -130,14 +131,12 @@ VDB_DEVINL void alpha_act8(float* v, float alpha, int act) {
 // the output is fp32.  The warpgroups do not wait for each other after the mainloop, and the producer is gated by the empty
 // barriers alone: it loads the next tile's first STAGES k-blocks while the epilogue runs, so the next mainloop starts on a full
 // ring.  tests/test_igemm_protocol_tma_epi.py models this protocol.
-template <int BM, int BN, int STAGES, int EW, int MODE>
-__global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
+template <int BM, int BN, int STAGES, int MODE>
+__global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
   constexpr bool kGegluEpi = MODE == 4 || MODE == 6;
   constexpr bool kLnIn = MODE == 5 || MODE == 6;
   constexpr bool kStatsOut = MODE == 7;
-  constexpr int kNumEpiWarps = EW;
-  constexpr int kNumEpiThreads = EW * 32;
-  static_assert(EW == 8, "two consumer warpgroups");
+  constexpr int kNumEpiThreads = kNumEpiWarps * 32;
   static_assert(BM == 128 || (BM == 256 && (MODE == 3 || MODE == 7) && BN <= 160), "256-row tiles: modes 3 and 7, 160 accumulator registers");
   constexpr int kMB = BM / 128;          // 64-row blocks per consumer warpgroup
   constexpr int kBoxes = igemm_boxes(BM);
@@ -154,7 +153,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + STAGES * kABytes;
   uint8_t* sstage = smem + kRingBytes;                        // kNumEpiWarps x kBoxes 1 KB bf16 TMA-store boxes, 1024-byte aligned
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sstage + EW * kStgWarp);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sstage + kNumEpiWarps * kStgWarp);
   uint64_t* empty_bar = full_bar + STAGES;
   float* sbias = reinterpret_cast<float*>(empty_bar + STAGES);  // [BN] bias of the current output tile
   float* slnx = sbias + BN;                                   // [BN] LN modes: colsum s (on_cols 0) / column mean (on_cols 1)
@@ -163,12 +162,12 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   if constexpr (kLnIn) {
     if (reinterpret_cast<uint8_t*>(slnx + BN) > smem_raw + p.smem_bytes) __trap();
   }
-  auto epi_bar_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(EW * 32) : "memory"); };   // the consumer warps only
+  auto epi_bar_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNumEpiThreads) : "memory"); };   // the consumer warps only
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == EW && lane == 0) {
+  if (warp == kNumEpiWarps && lane == 0) {
     for (int i = 0; i < kMaxA; ++i) tma_prefetch_desc(&p.tmA[i]);
     tma_prefetch_desc(&p.tmB);
     if (MODE != 0 || (!p.out_f32 && p.ksplit == 1)) tma_prefetch_desc(&p.tmO);   // (mode 0 builds it for bf16 output only)
@@ -181,8 +180,6 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();
-  pdl_wait();   // everything above overlapped the previous kernel's tail; global inputs are valid from here
 
   const int tilesM = p.tilesW * p.tilesH * p.tilesB;
   const int unitsM = tilesM;
@@ -190,10 +187,10 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN, EW), 1) igemm_kernel(con
   // Tile walk of this CTA (both roles use the same bounds): tiles c, c + grid, ..., with M as the fast tile index.
   const int t_first = blockIdx.x, t_step = gridDim.x, t_end = num_tiles;
 
-  if (warp >= EW) {
+  if (warp >= kNumEpiWarps) {
     // ------------------------------ TMA producer ------------------------------
-    if constexpr (igemm_realloc(BM, BN)) setmaxnreg_dec<40>();     // the whole producer warpgroup; warp EW alone works
-    if (warp == EW && lane == 0) {
+    if constexpr (igemm_realloc(BM, BN)) setmaxnreg_dec<40>();     // the whole producer warpgroup; its first warp alone works
+    if (warp == kNumEpiWarps && lane == 0) {
       uint32_t stage = 0, phase = 0;
       const bool flat = (p.tilesH == 1) && (p.tilesB == 1);
       const int step_m = t_step % unitsM, step_r = t_step / unitsM;
@@ -676,8 +673,6 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int kspl
                                      const float* __restrict__ bias, long long bias_bstride, int rows_per_batch,
                                      const __nv_bfloat16* __restrict__ resid, long long ldr, void* out,
                                      long long ldo, int out_f32, int act, float alpha) {
-  pdl_launch_dependents();
-  pdl_wait();
   const long long total = M * (N / 4);
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -712,27 +707,25 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int kspl
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
-template <int BM, int BN, int STAGES, int EW, int MODE>
-static int launch_igemm(const IgemmParams& p0, int num_units, cudaStream_t stream) {
+template <int BM, int BN, int STAGES, int MODE>
+static int launch_igemm(const IgemmParams& p0, int num_units, void* stream) {
   constexpr bool kLn = MODE == 5 || MODE == 6;       // one more [BN] fp32 table (colsum / column mean)
-  constexpr size_t need = STAGES * (BM + BN) * kBlockK * 2 + 2 * STAGES * 8 + BN * 4 + (kLn ? BN * 4 : 0) + EW * igemm_boxes(BM) * 1024;   // (see igemm_kernel)
+  constexpr size_t need = STAGES * (BM + BN) * kBlockK * 2 + 2 * STAGES * 8 + BN * 4 + (kLn ? BN * 4 : 0) + kNumEpiWarps * igemm_boxes(BM) * 1024;   // (see igemm_kernel)
   // + up to 1024 bytes of slack for the 1024-byte alignment of the operand ring (the LN modes at BN 256 may get less: the dynamic
   // window starts 1024-aligned in practice, and the kernel traps if its carve-up would not fit)
   constexpr size_t smem = (need + 1024 <= 227 * 1024) ? need + 1024 : 227 * 1024;
   static_assert(need + 896 <= 227 * 1024, "igemm shared-memory budget");
-  constexpr int threads = igemm_threads(BM, BN, EW);
+  constexpr int threads = igemm_threads(BM, BN);
   IgemmParams p = p0;
   p.smem_bytes = static_cast<unsigned>(smem);
   static bool configured = false;
   if (!configured) {
-    VDB_CUDA_CHECK(cudaFuncSetAttribute(igemm_kernel<BM, BN, STAGES, EW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    VDB_CUDA_CHECK(cudaFuncSetAttribute(igemm_kernel<BM, BN, STAGES, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         static_cast<int>(smem)));
     configured = true;
   }
   const int grid = std::min(num_units, num_sms());
-  VDB_CUDA_CHECK(launch_pdl(igemm_kernel<BM, BN, STAGES, EW, MODE>, dim3(grid), dim3(threads), smem, stream, p));
-  count_launch();
-  return VDB_OK;
+  return launch(igemm_kernel<BM, BN, STAGES, MODE>, dim3(grid), dim3(threads), smem, stream, p);
 }
 
 static int pick_bn(int N, int act, int forced) {
@@ -876,7 +869,7 @@ static Tile choose_tile(int Wo, int Ho, int Bo, bool gemm_view, long long N, int
 // Finish IgemmParams (split-K, B map, epilogue) and launch; p holds the M tiling of `tile` (set_tile_shape).
 static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot, long long ldw,
                      const IgemmEpilogue& e, Tile tile, int ksplit_forced, void* workspace,
-                     size_t ws_bytes, cudaStream_t stream) {
+                     size_t ws_bytes, void* stream) {
   const bool ln_in = e.ln_stats != nullptr, st_out = e.stats_out != nullptr;
   if (ln_in || st_out) ksplit_forced = 1;               // the statistics ride on the single-pass TMA-store epilogues
   const int BM = tile.BM, BN = tile.BN;
@@ -964,51 +957,46 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     g_last_bm = BM;
   }
   if (BM == 256) {
-    rc = mode == 7 ? launch_igemm<256, 160, 4, 8, 7>(p, num_tiles, stream) : launch_igemm<256, 160, 4, 8, 3>(p, num_tiles, stream);
+    rc = mode == 7 ? launch_igemm<256, 160, 4, 7>(p, num_tiles, stream) : launch_igemm<256, 160, 4, 3>(p, num_tiles, stream);
   } else if (mode == 7) {
     switch (BN) {
-      case 64: rc = launch_igemm<128, 64, 8, 8, 7>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 128, 6, 8, 7>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<128, 160, 5, 8, 7>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<128, 256, 4, 8, 7>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 7>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 7>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 7>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 7>(p, num_tiles, stream); break;
     }
   } else if (mode == 6) {
-    rc = launch_igemm<128, 256, 4, 8, 6>(p, num_tiles, stream);
+    rc = launch_igemm<128, 256, 4, 6>(p, num_tiles, stream);
   } else if (mode == 5) {
     switch (BN) {
-      case 64: rc = launch_igemm<128, 64, 8, 8, 5>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 128, 6, 8, 5>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<128, 160, 5, 8, 5>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<128, 256, 4, 8, 5>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 5>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 5>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 5>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 5>(p, num_tiles, stream); break;
     }
   } else if (mode == 4) {
-    rc = launch_igemm<128, 256, 4, 8, 4>(p, num_tiles, stream);
+    rc = launch_igemm<128, 256, 4, 4>(p, num_tiles, stream);
   } else if (mode == 3) {
     switch (BN) {
-      case 64: rc = launch_igemm<128, 64, 8, 8, 3>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 128, 6, 8, 3>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<128, 160, 5, 8, 3>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<128, 256, 4, 8, 3>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 3>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 3>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 3>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 3>(p, num_tiles, stream); break;
     }
   } else {
     switch (BN) {
-      case 64: rc = launch_igemm<128, 64, 8, 8, 0>(p, num_tiles, stream); break;
-      case 128: rc = launch_igemm<128, 128, 6, 8, 0>(p, num_tiles, stream); break;
-      case 160: rc = launch_igemm<128, 160, 5, 8, 0>(p, num_tiles, stream); break;
-      default: rc = launch_igemm<128, 256, 4, 8, 0>(p, num_tiles, stream); break;
+      case 64: rc = launch_igemm<128, 64, 8, 0>(p, num_tiles, stream); break;
+      case 128: rc = launch_igemm<128, 128, 6, 0>(p, num_tiles, stream); break;
+      case 160: rc = launch_igemm<128, 160, 5, 0>(p, num_tiles, stream); break;
+      default: rc = launch_igemm<128, 256, 4, 0>(p, num_tiles, stream); break;
     }
   }
-  if (rc) return rc;
-  if (p.ksplit > 1) {
-    const long long total = M * (N / 4);
-    const int threads = 256;
-    const int blocks = static_cast<int>(std::min<long long>((total + threads - 1) / threads, num_sms() * 8LL));
-    VDB_CUDA_CHECK(launch_pdl(splitk_reduce_kernel, dim3(blocks), dim3(threads), 0, stream, (const float*)p.partial,
-                              p.ksplit, M, static_cast<int>(N), p.bias, p.bias_bstride, p.rows_per_batch, p.resid,
-                              p.ldr, p.out, p.ldo, p.out_f32, p.act, p.alpha));
-    count_launch();
-  }
-  return VDB_OK;
+  if (rc || p.ksplit == 1) return rc;
+  const long long total = M * (N / 4);
+  const int threads = 256;
+  const int blocks = static_cast<int>(std::min<long long>((total + threads - 1) / threads, num_sms() * 8LL));
+  return launch(splitk_reduce_kernel, dim3(blocks), dim3(threads), 0, stream, p.partial, p.ksplit, M, static_cast<int>(N), p.bias,
+                p.bias_bstride, p.rows_per_batch, p.resid, p.ldr, p.out, p.ldo, p.out_f32, p.act, p.alpha);
 }
 
 }  // namespace vdb
@@ -1062,8 +1050,7 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
     p.nseg = 2;
   }
   for (int i = p.nseg; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
-  return run_igemm(p, W, N, K + (A2 ? K2 : 0), ldw, e, tile, ksplit, workspace, ws_bytes,
-                   reinterpret_cast<cudaStream_t>(stream));
+  return run_igemm(p, W, N, K + (A2 ? K2 : 0), ldw, e, tile, ksplit, workspace, ws_bytes, stream);
 }
 
 // GEMM with a LayerNorm folded in (consumer) or LayerNorm statistics written out (producer); see include/vdb200.h
@@ -1097,7 +1084,7 @@ int vdb_gemm_ln_bf16(const void* A, long long M, long long K, long long lda, con
   rc = make_tmap_4d(&p.tmA[0], A, K, M, 1, 1, lda * 2, lda * 2 * M, lda * 2 * M, kBlockK, p.TW, 1, 1);
   if (rc) return rc;
   for (int i = p.nseg; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
-  return run_igemm(p, W, N, K, ldw, e, tile, 1, nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
+  return run_igemm(p, W, N, K, ldw, e, tile, 1, nullptr, 0, stream);
 }
 
 // 3x3 convolution on NHWC bf16 as implicit GEMM.
@@ -1197,8 +1184,7 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int Wd, int C, int mode, const
     ++nmaps;
   }
   for (int i = nmaps; i < kMaxA; ++i) p.tmA[i] = p.tmA[0];
-  return run_igemm(p, Wt, N, static_cast<long long>(p.kb_total) * kBlockK, ldw, e, tile, ksplit, workspace, ws_bytes,
-                   reinterpret_cast<cudaStream_t>(stream));
+  return run_igemm(p, Wt, N, static_cast<long long>(p.kb_total) * kBlockK, ldw, e, tile, ksplit, workspace, ws_bytes, stream);
 }
 
 }  // extern "C"

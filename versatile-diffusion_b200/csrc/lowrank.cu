@@ -333,7 +333,6 @@ rank_adjust_kernel(const float* __restrict__ xg, int m, const float* __restrict_
     s.mean = reinterpret_cast<float*>(p); p += ((rows_cap + 3) / 4) * 16;
     s.x = reinterpret_cast<float*>(p);
   }
-  pdl_wait();
 
   // ---- load this CTA's rows, centre them, and the statistics of x ----
   const float* xi = xg + (static_cast<long long>(item) * m + row0) * kN;
@@ -504,7 +503,6 @@ extern "C" int vdb_rank_adjust_f32(const float* x, int n_items, int m, int n, co
   const int rows_cap = (m + kCluster - 1) / kCluster;
   const int rw = (rows_cap + kWarps - 1) / kWarps;
   const size_t smem = rank_adjust_smem(m);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static bool configured = false;
   if (!configured) {
     for (auto kernel : {rank_adjust_kernel<4>, rank_adjust_kernel<5>})
@@ -512,17 +510,6 @@ extern "C" int vdb_rank_adjust_f32(const float* x, int n_items, int m, int n, co
                                           static_cast<int>(rank_adjust_smem(kMaxRows))));
     configured = true;
   }
-  auto launch = [&](auto kernel) -> int {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(kCluster, n_items); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = kCluster; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    VDB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, x, m, R, niter, factors, keep_remainder, out, s_out, u_out, v_out));
-    count_launch();
-    return VDB_OK;
-  };
-  return rw <= 4 ? launch(rank_adjust_kernel<4>) : launch(rank_adjust_kernel<5>);
+  return launch(dim3(kCluster), rw <= 4 ? rank_adjust_kernel<4> : rank_adjust_kernel<5>, dim3(kCluster, n_items), dim3(kThreads), smem,
+                stream, x, m, R, niter, factors, keep_remainder, out, s_out, u_out, v_out);
 }

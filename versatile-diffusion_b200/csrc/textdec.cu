@@ -718,7 +718,6 @@ textdec_repetition_kernel(float* __restrict__ logits, int V, long long ldl, cons
   }
 }
 
-inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 }  // namespace
@@ -753,12 +752,8 @@ int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const fl
   while (ks < kGvWarps && static_cast<long long>(tiles) * ks < want && chunks % (ks * 2) == 0) ks *= 2;
   const int slots = kGvWarps / ks;
   const int blocks = std::min((tiles + slots - 1) / slots, num_sms() * 2);
-  textdec_gemv_kernel<<<blocks, kGvWarps * 32, smem, as_stream(stream)>>>(
-      x, R, k, ldx, ln_gamma, ln_beta, ln_eps, reinterpret_cast<const __nv_bfloat16*>(W), n, ldw, bias, act, accumulate, out, ldo,
-      ks, ldxs);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_gemv_kernel, blocks, kGvWarps * 32, smem, stream, x, R, k, ldx, ln_gamma, ln_beta, ln_eps,
+                reinterpret_cast<const __nv_bfloat16*>(W), n, ldw, bias, act, accumulate, out, ldo, ks, ldxs);
 }
 
 int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache, int R,
@@ -772,11 +767,8 @@ int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, lon
        reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache)) & 3)
     return set_error(VDB_ERR_INVALID, "textdec_attention: fp32 buffers must be 4-byte aligned");
   const int warps = R * H;
-  textdec_attention_kernel<false><<<(warps + 3) / 4, 128, 0, as_stream(stream)>>>(qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step,
-                                                                                scale, out, ldo, nullptr);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_attention_kernel<false>, (warps + 3) / 4, 128, 0, stream, qkv, ldq, mem, ldm, kcache, vcache, R, H, T,
+                step, scale, out, ldo, nullptr);
 }
 
 int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
@@ -793,11 +785,8 @@ int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* 
        reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache) | reinterpret_cast<uintptr_t>(src)) & 3)
     return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: buffers must be 4-byte aligned");
   const int warps = R * H;
-  textdec_attention_kernel<true><<<(warps + 3) / 4, 128, 0, as_stream(stream)>>>(qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step,
-                                                                               scale, out, ldo, src);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_attention_kernel<true>, (warps + 3) / 4, 128, 0, stream, qkv, ldq, mem, ldm, kcache, vcache, R, H, T,
+                step, scale, out, ldo, src);
 }
 
 int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* wte, int V, const float* wpe, int P, int pos_offset,
@@ -805,10 +794,7 @@ int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* 
   if (!tokens || !step || !wte || !wpe || !emb || !h) return set_error(VDB_ERR_INVALID, "textdec_embed: null pointer");
   if (R < 1 || R > kGvMaxRows || D < 1 || V < 1 || P < 1 || ldt < 1 || pos_offset < 0)
     return set_error(VDB_ERR_INVALID, "textdec_embed: need 1 <= R <= 16 and positive sizes");
-  textdec_embed_kernel<<<R, 256, 0, as_stream(stream)>>>(tokens, ldt, step, wte, V, wpe, P, pos_offset, emb, D, h);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_embed_kernel, R, 256, 0, stream, tokens, ldt, step, wte, V, wpe, P, pos_offset, emb, D, h);
 }
 
 static int textdec_sample_launch(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
@@ -825,28 +811,21 @@ static int textdec_sample_launch(const float* logits, int R, int V, long long ld
     return set_error(VDB_ERR_INVALID, "textdec_sample: seed / uniforms must be 8-byte aligned");
   // forced tokens replace the draw, so the cuts have nothing to act on
   const bool filter = !forced && ((top_k > 0 && top_k < V) || (top_p > 0.0f && top_p < 1.0f));
-  if (!filter) {
-    textdec_sample_kernel<false><<<R, kSampleThreads, 0, as_stream(stream)>>>(
-        logits, R, V, ldl, temperature, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record,
-        0, 0.0f);
-  } else {
-    if (V > kFilterMaxV)
-      return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top-k / top-p stage at most %d logits per row, got V = %d",
-                       kFilterMaxV, V);
-    const size_t smem = kFilterHistBytes + static_cast<size_t>(V) * sizeof(uint32_t);
-    static bool configured = false;
-    if (!configured) {
-      VDB_CUDA_CHECK(cudaFuncSetAttribute(textdec_sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          static_cast<int>(kFilterHistBytes + kFilterMaxV * sizeof(uint32_t))));
-      configured = true;
-    }
-    textdec_sample_kernel<true><<<R, kSampleThreads, smem, as_stream(stream)>>>(
-        logits, R, V, ldl, temperature, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record,
-        top_k, top_p);
+  if (!filter)
+    return launch(textdec_sample_kernel<false>, R, kSampleThreads, 0, stream, logits, R, V, ldl, temperature, seed, uniforms, ldu,
+                  forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record, 0, 0.0f);
+  if (V > kFilterMaxV)
+    return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top-k / top-p stage at most %d logits per row, got V = %d",
+                     kFilterMaxV, V);
+  const size_t smem = kFilterHistBytes + static_cast<size_t>(V) * sizeof(uint32_t);
+  static bool configured = false;
+  if (!configured) {
+    VDB_CUDA_CHECK(cudaFuncSetAttribute(textdec_sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        static_cast<int>(kFilterHistBytes + kFilterMaxV * sizeof(uint32_t))));
+    configured = true;
   }
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_sample_kernel<true>, R, kSampleThreads, smem, stream, logits, R, V, ldl, temperature, seed, uniforms, ldu,
+                forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record, top_k, top_p);
 }
 
 int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
@@ -893,15 +872,11 @@ int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, floa
                                         static_cast<int>(kFilterHistBytes + kFilterMaxV * sizeof(uint32_t))));
     configured = true;
   }
-  textdec_beam_topk_kernel<<<R, kSampleThreads, smem, as_stream(stream)>>>(logits, R, V, ldl, temperature, K, done, step, cand_tok,
-                                                                           cand_logp, record);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  textdec_beam_select_kernel<<<R / K, kSelectThreads, 0, as_stream(stream)>>>(R, K, cand_tok, cand_logp, tokens, ldt, src, lds, scores,
-                                                                              done, lengths, step, eos, max_len, trace);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  const int rc = launch(textdec_beam_topk_kernel, R, kSampleThreads, smem, stream, logits, R, V, ldl, temperature, K, done, step,
+                       cand_tok, cand_logp, record);
+  if (rc) return rc;
+  return launch(textdec_beam_select_kernel, R / K, kSelectThreads, 0, stream, R, K, cand_tok, cand_logp, tokens, ldt, src, lds,
+                scores, done, lengths, step, eos, max_len, trace);
 }
 
 int vdb_textdec_repetition(float* logits, int R, int V, long long ldl, const int* tokens, int ldt, const int* done, const int* step,
@@ -917,10 +892,7 @@ int vdb_textdec_repetition(float* logits, int R, int V, long long ldl, const int
        reinterpret_cast<uintptr_t>(step)) & 3)
     return set_error(VDB_ERR_INVALID, "textdec_repetition: buffers must be 4-byte aligned");
   if (penalty == 1.0f && ngram == 0) return VDB_OK;
-  textdec_repetition_kernel<<<R, kRepThreads, 0, as_stream(stream)>>>(logits, V, ldl, tokens, ldt, done, step, penalty, ngram);
-  VDB_CUDA_CHECK(cudaGetLastError());
-  count_launch();
-  return VDB_OK;
+  return launch(textdec_repetition_kernel, R, kRepThreads, 0, stream, logits, V, ldl, tokens, ldt, done, step, penalty, ngram);
 }
 
 }  // extern "C"

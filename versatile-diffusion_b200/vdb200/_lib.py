@@ -2,7 +2,8 @@
 import ctypes as C
 import os
 
-# VDB200_LIB: load another build of the same library (debug builds with -DVDB_TIMELINE); default = the in-tree product build
+# VDB200_LIB: load another build of the same library (a debug build, or another revision to compare against); default = the
+# in-tree product build
 LIB_PATH = os.environ.get("VDB200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libvdb200.so")
 
 
