@@ -102,6 +102,17 @@ int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots
  * overlapping an input. */
 int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,
                           float s_tgt, int D, int bs, long long hw, int c, float ratio, float* out, void* stream);
+/* ---- Prompt-to-Prompt editing — lib/model_zoo/prompt_edit.py (an addition: the reference has no prompt editing; the semantics are
+ * specified in that module's docstring) ------------------------------------------------------------------------------------------
+ * vdb_local_blend_f32, after each step: x fp32 NHWC [n, H, W, C], row 0 the source image; map fp32 [n, h, w], the word maps; flags
+ * device int32 per step, read at *step_idx (device int, required): 0 leaves x untouched.  For each target b = 1 .. n-1 (one CTA each):
+ * pooled_s = 3x3 max-pool (stride 1, pad 1) of map[s], mask_s(y, x) = max(pooled_s) > 0 && pooled_s[floor(y h / H), floor(x w / W)] /
+ * max(pooled_s) > threshold (the division rounded to nearest), and x_b = (mask_b || mask_0) ? x_b : x_0 (a selection: the per-element
+ * blend of vdb_inpaint_blend_f32 at m in {0, 1}).  x_dup (may be NULL) receives the rows written.  VDB_ERR_INVALID before any launch:
+ * a null x / map / flags / step_idx, n < 2, a size <= 0, h * w > 4096, a threshold not finite, a pointer not 4-byte aligned, or x,
+ * x_dup and map overlapping. */
+int vdb_local_blend_f32(float* x, float* x_dup, const float* map, const int* flags, const int* step_idx, int n, int H, int W, int C,
+                        int h, int w, float threshold, void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */
@@ -199,6 +210,26 @@ int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const vo
                               const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
                               int q_bstride, int kv_bstride, int d_head, float scale, int causal, const int* kv_len,
                               void* stream);
+/* The same attention with the operands of each output item chosen by a device table — Prompt-to-Prompt's attention injection,
+ * lib/model_zoo/prompt_edit.py.  items: device int32 [rows][3][B]; output item b reads Q from item bq = items[r][0][b], K from item
+ * bk = items[r][1][b] and V^T from item bv = items[r][2][b] of row r = *step_idx (device int), and writes item b of out.  Entries must
+ * lie in [0, Bq) (bq) and [0, Bkv) (bk, bv), where Q holds Bq items and K / V^T hold Bkv items (the tensor maps are sized by them);
+ * bv < 0 skips item b: nothing is read or written for it.  accumulate != 0: out = bf16(float(out) + O).  With items[r][.][b] = b and
+ * accumulate 0 the output equals vdb_attention_bf16's bitwise.  A null or misaligned items / step_idx, or Bq / Bkv <= 0, return
+ * VDB_ERR_INVALID.  The other arguments are those of vdb_attention_bf16. */
+int vdb_attention_indexed_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                               const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                               int q_bstride, int kv_bstride, int d_head, float scale, int causal, int Bq, int Bkv,
+                               const int* items, const int* step_idx, int accumulate, void* stream);
+/* Prompt-to-Prompt's word maps from the operands of a cross-attention call, fp32 math: for r in [0, n) and query p in [0, N),
+ *   map[r, p] += sum over heads h of sum over keys j < L of w[r, j] * softmax_j(scale * q . k)
+ * with q = Q row (row0 + r) * N + p, k = K row (row0 + r) * kv_bstride + j, both at columns h*DK .. h*DK + d_head (DK =
+ * vdb_attention_dk_pad(d_head)), bf16.  w, map fp32 [n, L], [n, N].  One CTA per (16 queries, r), sums in an order fixed by the
+ * shape, one writer per entry: bit-reproducible.  L <= 80 (a text context) and d_head <= 160 a multiple of 8, else
+ * VDB_ERR_UNSUPPORTED.  VDB_ERR_INVALID before any launch: a null Q / K / w / map, a size <= 0, row0 < 0, kv_bstride < L (0 = L),
+ * odd or short ldq / ldk, a pointer not 4-byte aligned, or map overlapping w. */
+int vdb_xattn_word_map_f32(const void* Q, long long ldq, const void* K, long long ldk, const float* w, float* map, int n, int row0,
+                           int H, int N, int L, int kv_bstride, int d_head, float scale, void* stream);
 
 /* ---- GroupNorm(32) [+SiLU] [+channel concat] on NHWC — normalization()/Normalize():
  *      diffusion_utils.py:168-191 (eps 1e-5), attention.py:76-77 & autokl_modules.py:38-39 (1e-6) ----

@@ -44,6 +44,9 @@ struct alignas(64) AttnParams {
   __nv_bfloat16* out;
   long long ldo;
   const int* kv_len; // [B] valid keys per batch item (VARLEN instantiations only; key j of item b is visible iff j < kv_len[b])
+  const int* items;  // INDEXED: [rows][3][B] int32 source items {bq, bk, bv} of output item b, row *step_idx
+  const int* step_idx;
+  int accumulate;    // INDEXED: out = bf16(float(out) + O)
 };
 
 template <int DK, int DVP, int BKV, int KV_STAGES>
@@ -54,7 +57,9 @@ constexpr size_t attention_smem_bytes() {
 // DK = padded q/k head width (64-channel swizzle atoms), DVP = padded v head width (the N of the PV product),
 // BKV = keys per tile (the N of the QK^T product), TMA_WARP = a ninth warp issues the loads (see the top of the file).
 // VARLEN: batch item b sees only its first min(kv_len[b], Nk) keys (BERT's padding mask); an item with no key writes zero rows.
-template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false>
+// INDEXED: output item b takes its Q, K and V from items {bq, bk, bv} of row *step_idx of the table (Prompt-to-Prompt's attention
+// injection, lib/model_zoo/prompt_edit.py); bv < 0 skips the item.
+template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false, bool INDEXED = false>
 __global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
     attention_kernel(const __grid_constant__ AttnParams p) {
   constexpr int KA = DK / 64;                      // 64-wide K atoms of the QK^T reduction
@@ -87,6 +92,14 @@ __global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
   const int q0 = blockIdx.x * kBQ;
   const int head = blockIdx.y;
   const int b = blockIdx.z;
+  int bq = b, bk = b, bv = b;
+  if constexpr (INDEXED) {
+    const int* row = p.items + static_cast<long long>(*p.step_idx) * 3 * gridDim.z;
+    bq = row[b];
+    bk = row[gridDim.z + b];
+    bv = row[2 * gridDim.z + b];
+    if (bv < 0) return;                            // the whole CTA, before any barrier, load or write
+  }
 
   int nk = 0;                                      // VARLEN: this item's key count
   int ntiles = (p.Nk + BKV - 1) / BKV;
@@ -116,21 +129,21 @@ __global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
   auto load_q = [&] {
     mbar_arrive_expect_tx(q_full, kQBytes);
     for (int a = 0; a < KA; ++a)
-      tma_load_2d(sQ + a * kBQ * 128, &p.tmQ, q_full, p.q_col0 + head * DK + a * 64, b * p.q_bs + q0);
+      tma_load_2d(sQ + a * kBQ * 128, &p.tmQ, q_full, p.q_col0 + head * DK + a * 64, bq * p.q_bs + q0);
   };
   auto load_k = [&](int t) {
     const int st = t % KV_STAGES;
     mbar_wait(&k_empty[st], ((t / KV_STAGES) & 1) ^ 1);
     mbar_arrive_expect_tx(&k_full[st], kKBytes);
     for (int a = 0; a < KA; ++a)
-      tma_load_2d(sK + st * kKBytes + a * BKV * 128, &p.tmK, &k_full[st], p.k_col0 + head * DK + a * 64, b * p.kv_bs + t * BKV);
+      tma_load_2d(sK + st * kKBytes + a * BKV * 128, &p.tmK, &k_full[st], p.k_col0 + head * DK + a * 64, bk * p.kv_bs + t * BKV);
   };
   auto load_v = [&](int t) {
     const int st = t % KV_STAGES;
     mbar_wait(&v_empty[st], ((t / KV_STAGES) & 1) ^ 1);
     mbar_arrive_expect_tx(&v_full[st], kVBytes);
     for (int a = 0; a < KVA; ++a)
-      tma_load_2d(sV + st * kVBytes + a * kVAtom, &p.tmV, &v_full[st], b * p.kv_bs + t * BKV + a * 64, head * DVP);
+      tma_load_2d(sV + st * kVBytes + a * kVAtom, &p.tmV, &v_full[st], bv * p.kv_bs + t * BKV + a * 64, head * DVP);
   };
 
   if constexpr (TMA_WARP) {
@@ -270,8 +283,15 @@ __global__ void __launch_bounds__(attention_threads(TMA_WARP), TMA_WARP ? 1 : 2)
 #pragma unroll
     for (int jj = 0; jj < DVP / 8; ++jj) {
       const int col = 8 * jj + c2;
-      if (col < p.dv)   // (dv % 8 == 0: the pair never straddles the end)
-        *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(o[4 * jj + 2 * i] * inv_l, o[4 * jj + 2 * i + 1] * inv_l);
+      if (col < p.dv) {   // (dv % 8 == 0: the pair never straddles the end)
+        float v0 = o[4 * jj + 2 * i] * inv_l, v1 = o[4 * jj + 2 * i + 1] * inv_l;
+        if (INDEXED && p.accumulate) {
+          const __nv_bfloat162 prev = *reinterpret_cast<const __nv_bfloat162*>(orow + col);
+          v0 += __bfloat162float(prev.x);
+          v1 += __bfloat162float(prev.y);
+        }
+        *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(v0, v1);
+      }
     }
   }
 }
@@ -280,14 +300,15 @@ struct AttnArgs {   // what the C ABI received; the tensor maps depend on the ke
   const void *Q, *K, *Vt;
   long long ldq, ldk, ldv;
   int B, H, q_bstride, kv_bstride;
+  int Bq, Bkv;       // items in Q and in K / V^T (B unless indexed)
 };
 
-template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false>
+template <int DK, int DVP, int BKV, int KV_STAGES, bool TMA_WARP, bool VARLEN = false, bool INDEXED = false>
 static int launch_attention(AttnParams& p, const AttnArgs& a, void* stream) {
   constexpr size_t smem = attention_smem_bytes<DK, DVP, BKV, KV_STAGES>();
   // two CTAs per SM need twice the dynamic window plus 1 KB each reserved by the system, within 228 KB
   static_assert(smem <= (TMA_WARP ? 227 * 1024 : 113 * 1024), "attention smem budget");
-  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES, TMA_WARP, VARLEN>;
+  auto kernel = attention_kernel<DK, DVP, BKV, KV_STAGES, TMA_WARP, VARLEN, INDEXED>;
   static bool configured = false;
   if (!configured) {
     VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -295,14 +316,96 @@ static int launch_attention(AttnParams& p, const AttnArgs& a, void* stream) {
       VDB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  int rc = make_tmap_2d(&p.tmQ, a.Q, static_cast<uint64_t>(a.ldq), static_cast<uint64_t>(a.B) * a.q_bstride, a.ldq * 2, 64, kBQ);
+  int rc = make_tmap_2d(&p.tmQ, a.Q, static_cast<uint64_t>(a.ldq), static_cast<uint64_t>(a.Bq) * a.q_bstride, a.ldq * 2, 64, kBQ);
   if (rc) return rc;
-  rc = make_tmap_2d(&p.tmK, a.K, static_cast<uint64_t>(a.ldk), static_cast<uint64_t>(a.B) * a.kv_bstride, a.ldk * 2, 64, BKV);
+  rc = make_tmap_2d(&p.tmK, a.K, static_cast<uint64_t>(a.ldk), static_cast<uint64_t>(a.Bkv) * a.kv_bstride, a.ldk * 2, 64, BKV);
   if (rc) return rc;
-  rc = make_tmap_2d(&p.tmV, a.Vt, static_cast<uint64_t>(a.B) * a.kv_bstride, static_cast<uint64_t>(a.H) * DVP, a.ldv * 2, 64, DVP);
+  rc = make_tmap_2d(&p.tmV, a.Vt, static_cast<uint64_t>(a.Bkv) * a.kv_bstride, static_cast<uint64_t>(a.H) * DVP, a.ldv * 2, 64, DVP);
   if (rc) return rc;
   dim3 grid((p.Nq + kBQ - 1) / kBQ, a.H, a.B);
   return launch(kernel, grid, dim3(attention_threads(TMA_WARP)), smem, stream, p);
+}
+
+// Prompt-to-Prompt's word maps (lib/model_zoo/prompt_edit.py) from the bf16 operands of a cross-attention call, fp32 math:
+//   map[r, p] += sum over h of sum over j < L of w[r, j] softmax_j(scale q[(row0 + r) N + p, head h] . k[(row0 + r) kv_bs + j, head h])
+// One CTA per (block of kWmapQ queries, r).  K of one head at a time sits in shared memory; warp g owns queries
+// g*kWmapQ/8 .. of the block, lane l keys l, l + 32, l + 64.  The heads are summed in order, the keys by partial sums per lane
+// and a fixed xor tree, and every map entry has one writer: the result is bit-reproducible.
+constexpr int kWmapThreads = 256, kWmapQ = 16, kWmapMaxL = 80, kWmapMaxD = 160;
+
+__global__ void __launch_bounds__(kWmapThreads) xattn_word_map_kernel(
+    const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloat16* __restrict__ K, long long ldk,
+    const float* __restrict__ w, float* __restrict__ map, int row0, int H, int N, int L, int kv_bs, int d, int DK,
+    float scale_log2) {
+  constexpr int kPerWarp = kWmapQ / (kWmapThreads / 32);
+  constexpr int kRowWords = kWmapMaxD / 2 + 1;     // odd row stride in 4-byte words: lanes reading 32 rows hit 32 banks
+  __shared__ __nv_bfloat162 sK[kWmapMaxL * kRowWords];
+  __shared__ float sq[kWmapThreads / 32][kWmapMaxD];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.y, item = row0 + r;
+  const int rw = d / 2 + 1;
+  float wj[3];
+#pragma unroll
+  for (int t = 0; t < 3; ++t) wj[t] = lane + 32 * t < L ? w[static_cast<long long>(r) * L + lane + 32 * t] : 0.f;
+  float acc[kPerWarp];
+#pragma unroll
+  for (int qq = 0; qq < kPerWarp; ++qq) acc[qq] = 0.f;
+  for (int h = 0; h < H; ++h) {
+    __syncthreads();
+    for (int e = threadIdx.x; e < L * (d / 2); e += kWmapThreads) {
+      const int j = e / (d / 2), c2 = e % (d / 2);
+      sK[j * rw + c2] = *reinterpret_cast<const __nv_bfloat162*>(K + (static_cast<long long>(item) * kv_bs + j) * ldk + h * DK + 2 * c2);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int qq = 0; qq < kPerWarp; ++qq) {
+      const int p = blockIdx.x * kWmapQ + warp * kPerWarp + qq;
+      if (p >= N) break;
+      const __nv_bfloat16* qrow = Q + (static_cast<long long>(item) * N + p) * ldq + h * DK;
+      for (int c = lane; c < d; c += 32) sq[warp][c] = __bfloat162float(qrow[c]);
+      __syncwarp();
+      float sc[3];
+      float mx = -INFINITY;
+#pragma unroll
+      for (int t = 0; t < 3; ++t) {
+        const int j = lane + 32 * t;
+        sc[t] = -INFINITY;
+        if (j < L) {
+          float dot = 0.f;
+          for (int c2 = 0; c2 < d / 2; ++c2) {
+            const float2 kv = __bfloat1622float2(sK[j * rw + c2]);
+            dot = fmaf(sq[warp][2 * c2], kv.x, dot);
+            dot = fmaf(sq[warp][2 * c2 + 1], kv.y, dot);
+          }
+          sc[t] = dot;
+          mx = fmaxf(mx, dot);
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float den = 0.f, num = 0.f;
+#pragma unroll
+      for (int t = 0; t < 3; ++t) {
+        const float e = lane + 32 * t < L ? exp2f((sc[t] - mx) * scale_log2) : 0.f;
+        den += e;
+        num = fmaf(wj[t], e, num);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        den += __shfl_xor_sync(0xffffffffu, den, o);
+        num += __shfl_xor_sync(0xffffffffu, num, o);
+      }
+      acc[qq] += num / den;
+      __syncwarp();
+    }
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int qq = 0; qq < kPerWarp; ++qq) {
+      const int p = blockIdx.x * kWmapQ + warp * kPerWarp + qq;
+      if (p < N) map[static_cast<long long>(r) * N + p] += acc[qq];
+    }
+  }
 }
 
 }  // namespace vdb
@@ -338,7 +441,7 @@ static int attention_prepare(const void* Q, long long ldq, int q_col0, const voi
     return set_error(VDB_ERR_INVALID, "attention: need q_bstride >= Nq, kv_bstride >= Nk and kv_bstride %% 8 == 0 (got %d, %d)",
                      q_bstride, kv_bstride);
   memset(&p, 0, sizeof(p));
-  a = AttnArgs{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride};
+  a = AttnArgs{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride, B, B};
   p.Nq = Nq; p.Nk = Nk; p.q_bs = q_bstride; p.kv_bs = kv_bstride; p.q_col0 = q_col0; p.k_col0 = k_col0; p.dv = d_head; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
@@ -381,6 +484,54 @@ int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const vo
   if (rc) return rc;
   p.kv_len = kv_len;
   return launch_attention<64, 64, 128, 2, false, true>(p, a, stream);
+}
+
+int vdb_attention_indexed_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                               const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                               int q_bstride, int kv_bstride, int d_head, float scale, int causal, int Bq, int Bkv,
+                               const int* items, const int* step_idx, int accumulate, void* stream) {
+  if (!items || !step_idx || (reinterpret_cast<uintptr_t>(items) & 3) || (reinterpret_cast<uintptr_t>(step_idx) & 3))
+    return set_error(VDB_ERR_INVALID, "attention_indexed: items and step_idx must be non-null, 4-byte aligned device int32");
+  if (Bq <= 0 || Bkv <= 0) return set_error(VDB_ERR_INVALID, "attention_indexed: Bq and Bkv must be > 0 (got %d, %d)", Bq, Bkv);
+  AttnParams p;
+  AttnArgs a{};
+  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
+                                   scale, causal, p, a);
+  if (rc) return rc;
+  a.Bq = Bq;
+  a.Bkv = Bkv;
+  p.items = items;
+  p.step_idx = step_idx;
+  p.accumulate = accumulate ? 1 : 0;
+  const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
+  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false, false, true>(p, a, stream);
+  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false, false, true>(p, a, stream);
+  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false, false, true>(p, a, stream);
+  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true, false, true>(p, a, stream);
+  return set_error(VDB_ERR_UNSUPPORTED, "attention_indexed: no kernel for d_head %d", d_head);
+}
+
+int vdb_xattn_word_map_f32(const void* Q, long long ldq, const void* K, long long ldk, const float* w, float* map, int n, int row0,
+                           int H, int N, int L, int kv_bstride, int d_head, float scale, void* stream) {
+  if (!Q || !K || !w || !map || n <= 0 || row0 < 0 || H <= 0 || N <= 0 || L <= 0)
+    return set_error(VDB_ERR_INVALID, "xattn_word_map: null/empty argument");
+  if (L > kWmapMaxL) return set_error(VDB_ERR_UNSUPPORTED, "xattn_word_map: at most %d keys (a text context), got %d", kWmapMaxL, L);
+  const int DK = vdb_attention_dk_pad(d_head);
+  if (DK < 0 || d_head > kWmapMaxD || d_head % 8)
+    return set_error(VDB_ERR_UNSUPPORTED, "xattn_word_map: d_head %d not supported (a multiple of 8, <= %d)", d_head, kWmapMaxD);
+  if (kv_bstride <= 0) kv_bstride = L;
+  if (kv_bstride < L || ldq < static_cast<long long>(H) * DK || ldk < static_cast<long long>(H) * DK || (ldq & 1) || (ldk & 1))
+    return set_error(VDB_ERR_INVALID, "xattn_word_map: need kv_bstride >= L and even ldq, ldk >= H * %d", DK);
+  if ((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(K) | reinterpret_cast<uintptr_t>(w) |
+       reinterpret_cast<uintptr_t>(map)) & 3)
+    return set_error(VDB_ERR_INVALID, "xattn_word_map: pointers must be 4-byte aligned");
+  const char *m0 = reinterpret_cast<const char*>(map), *m1 = m0 + static_cast<long long>(n) * N * 4;
+  const char *w0 = reinterpret_cast<const char*>(w), *w1 = w0 + static_cast<long long>(n) * L * 4;
+  if (m0 < w1 && w0 < m1) return set_error(VDB_ERR_INVALID, "xattn_word_map: map overlaps w");
+  dim3 grid((N + kWmapQ - 1) / kWmapQ, n);
+  return launch(xattn_word_map_kernel, grid, dim3(kWmapThreads), 0, stream, reinterpret_cast<const __nv_bfloat16*>(Q), ldq,
+                reinterpret_cast<const __nv_bfloat16*>(K), ldk, w, map, row0, H, N, L, kv_bstride, d_head, DK,
+                scale * 1.4426950408889634f);
 }
 
 }  // extern "C"

@@ -383,6 +383,63 @@ __global__ void __launch_bounds__(kDiffEditThreads) diffedit_mask_kernel(
     o[p] = (cap > 0.f && __fdiv_rn(fminf(o[p], cap), cap) >= 0.5f) ? 1.f : 0.f;
 }
 
+// Prompt-to-Prompt's local blend (lib/model_zoo/prompt_edit.py) after a step, when flags[*step_idx] != 0.  One CTA per target image
+// b = 1 .. n-1 of x fp32 NHWC [n, H, W, C]; map fp32 [n, h, w], the word maps of the conditional rows.  For s in {0, b}:
+//   pooled_s = 3x3 max-pool (stride 1, pad 1) of map[s];  mx_s = max of pooled_s
+//   mask_s(y, x) = mx_s > 0 && pooled_s[floor(y h / H), floor(x w / W)] / mx_s > threshold   (division rounded to nearest)
+// then x_b = mask_blend(m, x_b, x_0) with m = mask_b || mask_0 in {0, 1}: a selection, so outside the mask x_b takes x_0's bits.
+// x_dup (may be NULL) receives the rows written.  Max is order-independent, so the result is bit-reproducible.
+constexpr int kBlendThreads = 256, kBlendMaxMap = 4096;
+
+__global__ void __launch_bounds__(kBlendThreads) local_blend_kernel(float* x, float* x_dup, const float* __restrict__ map,
+                                                                    const int* __restrict__ flags, const int* __restrict__ step_idx,
+                                                                    int H, int W, int C, int h, int w, float threshold) {
+  __shared__ float pooled[2][kBlendMaxMap];
+  __shared__ float red[2][kBlendThreads];
+  if (!flags[*step_idx]) return;
+  const int b = blockIdx.x + 1;
+  const int hw = h * w;
+  float part[2] = {-INFINITY, -INFINITY};
+  for (int i = threadIdx.x; i < hw; i += kBlendThreads) {
+    const int y = i / w, xx = i % w;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const float* m = map + static_cast<long long>(s ? b : 0) * hw;
+      float v = -INFINITY;
+      for (int dy = -1; dy <= 1; ++dy)
+        for (int dx = -1; dx <= 1; ++dx) {
+          const int yy = y + dy, xw = xx + dx;
+          if (yy >= 0 && yy < h && xw >= 0 && xw < w) v = fmaxf(v, m[yy * w + xw]);
+        }
+      pooled[s][i] = v;
+      part[s] = fmaxf(part[s], v);
+    }
+  }
+  red[0][threadIdx.x] = part[0];
+  red[1][threadIdx.x] = part[1];
+  __syncthreads();
+  for (int k = kBlendThreads / 2; k > 0; k >>= 1) {
+    if (threadIdx.x < k)
+      for (int s = 0; s < 2; ++s) red[s][threadIdx.x] = fmaxf(red[s][threadIdx.x], red[s][threadIdx.x + k]);
+    __syncthreads();
+  }
+  const float mx0 = red[0][0], mxb = red[1][0];
+  const long long hwc = static_cast<long long>(H) * W * C;
+  const float* x0 = x;
+  float* xb = x + b * hwc;
+  float* db = x_dup ? x_dup + b * hwc : nullptr;
+  for (long long e = threadIdx.x; e < hwc; e += kBlendThreads) {
+    const long long pix = e / C;
+    const int y = static_cast<int>(pix / W), xx = static_cast<int>(pix % W);
+    const int cell = static_cast<int>(static_cast<long long>(y) * h / H) * w + static_cast<int>(static_cast<long long>(xx) * w / W);
+    const bool m0 = mx0 > 0.f && __fdiv_rn(pooled[0][cell], mx0) > threshold;
+    const bool mb = mxb > 0.f && __fdiv_rn(pooled[1][cell], mxb) > threshold;
+    const float v = mask_blend(m0 || mb ? 1.f : 0.f, xb[e], x0[e]);
+    xb[e] = v;
+    if (db) db[e] = v;
+  }
+}
+
 __global__ void add_int_kernel(int* p, int delta) { *p += delta; }
 
 // y = c0*x0 + c1*x1 + c2*x2 + c3*x3 (null pointers skipped) — the Adams-Bashforth eps combination of the PLMS
@@ -1759,6 +1816,24 @@ int vdb_inversion_blend_f32(float* x, float* x_dup, const float* ring, int slots
       return set_error(VDB_ERR_INVALID, "inversion_blend: ring or mask overlaps x or x_dup");
   return launch(inversion_blend_kernel, ew_blocks((n + 3) / 4, 256), 256, 0, stream, x, x_dup, ring, slots, mask, mask_per_item,
                 step_idx, n, hw, c);
+}
+
+int vdb_local_blend_f32(float* x, float* x_dup, const float* map, const int* flags, const int* step_idx, int n, int H, int W, int C,
+                        int h, int w, float threshold, void* stream) {
+  if (!x || !map || !flags || !step_idx || n < 2 || H <= 0 || W <= 0 || C <= 0 || h <= 0 || w <= 0)
+    return set_error(VDB_ERR_INVALID, "local_blend: null/empty argument (n >= 2: a source and a target)");
+  if (static_cast<long long>(h) * w > kBlendMaxMap)
+    return set_error(VDB_ERR_INVALID, "local_blend: word maps of at most %d cells, got %d x %d", kBlendMaxMap, h, w);
+  if (!(threshold == threshold) || threshold == INFINITY || threshold == -INFINITY)
+    return set_error(VDB_ERR_INVALID, "local_blend: threshold must be finite");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_dup) | reinterpret_cast<uintptr_t>(map) |
+       reinterpret_cast<uintptr_t>(flags) | reinterpret_cast<uintptr_t>(step_idx)) & 3)
+    return set_error(VDB_ERR_INVALID, "local_blend: pointers must be 4-byte aligned");
+  const long long nx = static_cast<long long>(n) * H * W * C;
+  if (overlaps(x, nx, map, static_cast<long long>(n) * h * w) || (x_dup && (overlaps(x_dup, nx, map, static_cast<long long>(n) * h * w) ||
+                                                                         overlaps(x_dup, nx, x, nx))))
+    return set_error(VDB_ERR_INVALID, "local_blend: x, x_dup and map must not overlap");
+  return launch(local_blend_kernel, n - 1, kBlendThreads, 0, stream, x, x_dup, map, flags, step_idx, H, W, C, h, w, threshold);
 }
 
 int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,

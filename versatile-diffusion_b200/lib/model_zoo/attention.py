@@ -24,10 +24,11 @@ def _ops():
 class PaddedContext(object):
     """A context batch already in kernel layout: bf16 [B, Lp, C] with Lp = L rounded up to 8 and zero pad rows.
     DDIMSampler keeps one per context in a persistent buffer so the captured CUDA graph (and the cached K / V^T
-    of every cross-attention layer) stay valid when a new prompt is copied in."""
+    of every cross-attention layer) stay valid when a new prompt is copied in.  edit: the prompt_edit.EditState of a
+    Prompt-to-Prompt walk on this context (its rows past the batch's are the edited contexts), else None."""
 
-    def __init__(self, data, length):
-        self.data, self.length = data, length
+    def __init__(self, data, length, edit=None):
+        self.data, self.length, self.edit = data, length, edit
 
 
 def ln_fold_fits(inner, B, H, W):
@@ -187,8 +188,26 @@ class CrossAttention(PackedModule):
         self._kv_put((key, val, context))
         return val
 
-    def forward(self, x, context=None, resid=None, B=1):
-        """x: [B*N, C] bf16 (already layer-normed); returns to_out(attn) + resid as [B*N, C] bf16."""
+    def _attend(self, q, k, vt, o, B, N, Nk, edit, cross, q_col0=0, k_col0=0, kv_bstride=0):
+        """The layer's flash attention.  Under a prompt edit (lib/model_zoo/prompt_edit.py) the indexed form with the edit's
+        table for this layer, the refinement's accumulating second term, and the word maps at the 1/4-side cross layers."""
+        ops = _ops()
+        H, d = self.heads, self.dim_head
+        items = None if edit is None else edit.items(cross, N)
+        kw = dict(scale=self.scale, q_col0=q_col0, k_col0=k_col0, kv_bstride=kv_bstride)
+        if items is None:
+            ops.attention(q, k, vt, o, B, H, N, Nk, d, **kw)
+            return
+        Bkv = edit.ctx_batch if cross else B
+        ops.attention_indexed(q, k, vt, o, B, H, N, Nk, d, B, Bkv, items, edit.idx, **kw)
+        if cross and edit.cross2 is not None:
+            ops.attention_indexed(q, k, vt, o, B, H, N, Nk, d, B, Bkv, edit.cross2, edit.idx, accumulate=True, **kw)
+        if cross and edit.maps_at(N):
+            ops.xattn_word_map(q, k, edit.w, edit.map, edit.c0, H, N, Nk, d, kv_bstride=kv_bstride, scale=self.scale)
+
+    def forward(self, x, context=None, resid=None, B=1, edit=None):
+        """x: [B*N, C] bf16 (already layer-normed); returns to_out(attn) + resid as [B*N, C] bf16.  edit: the prompt edit of a
+        self-attention layer (a cross-attention layer reads it from its context)."""
         ops = _ops()
         p = self.packed()
         H, d, dk = self.heads, self.dim_head, p["dk"]
@@ -197,7 +216,7 @@ class CrossAttention(PackedModule):
         if context is None and N % 8 == 0:
             qk = ops.gemm(x, p["wqk"])                    # [B*N, 2*H*dk]: q | k
             vt = ops.gemm(p["wv"], x)                     # [H*dvp, B*N]
-            ops.attention(qk, qk, vt, o, B, H, N, N, d, scale=self.scale, q_col0=0, k_col0=H * dk)
+            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk)
         elif context is None:
             # ragged token count (latent sides not a multiple of 8 at this level): keys/values from a copy of
             # the tokens padded to a multiple of 8 per batch item (TMA alignment of the V^T columns)
@@ -208,14 +227,14 @@ class CrossAttention(PackedModule):
             q = ops.gemm(x, p["wq"])
             k = ops.gemm(xp, p["wk"])
             vt = ops.gemm(p["wv"], xp)
-            ops.attention(q, k, vt, o, B, H, N, N, d, scale=self.scale, kv_bstride=Np)
+            self._attend(q, k, vt, o, B, N, N, edit, False, kv_bstride=Np)
         else:
             q = ops.gemm(x, p["wq"])
             k, vt, L, Lp = self.context_kv(context)
-            ops.attention(q, k, vt, o, B, H, N, L, d, scale=self.scale, kv_bstride=Lp)
+            self._attend(q, k, vt, o, B, N, L, getattr(context, "edit", None), True, kv_bstride=Lp)
         return ops.gemm(o, p["wo"], bias=p["bo"], resid=resid)
 
-    def forward_folded(self, x, ln, fp, context=None, resid=None, B=1, stats_out=None):
+    def forward_folded(self, x, ln, fp, context=None, resid=None, B=1, stats_out=None, edit=None):
         """x: [B*N, C] bf16 RAW tokens, ln: ops.LnFold with their LayerNorm statistics, fp: pack_folded(); to_out writes the
         statistics of ITS output rows into stats_out (the next LayerNorm's input).  Self-attention needs N % 8 == 0."""
         ops = _ops()
@@ -226,11 +245,11 @@ class CrossAttention(PackedModule):
         if context is None:
             qk = ops.gemm_ln(x, fp["wqk"], bias=fp["cqk"], ln=ln, colsum=fp["sqk"])                       # [B*N, 2*H*dk]: q | k
             vt = ops.gemm_ln(fp["wv"], x, ln=ln, colsum=fp["sv"], on_cols=True, rowbias=fp["cv"])       # [H*dvp, B*N]
-            ops.attention(qk, qk, vt, o, B, H, N, N, d, scale=self.scale, q_col0=0, k_col0=H * dk)
+            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk)
         else:
             q = ops.gemm_ln(x, fp["wq"], bias=fp["cq"], ln=ln, colsum=fp["sq"])
             k, vt, L, Lp = self.context_kv(context)
-            ops.attention(q, k, vt, o, B, H, N, L, d, scale=self.scale, kv_bstride=Lp)
+            self._attend(q, k, vt, o, B, N, L, getattr(context, "edit", None), True, kv_bstride=Lp)
         if stats_out is None:
             return ops.gemm(o, p["wo"], bias=p["bo"], resid=resid)
         return ops.gemm_ln(o, p["wo"], bias=p["bo"], resid=resid, stats_out=stats_out)      # -> (tokens, partials per row)
@@ -269,15 +288,17 @@ class BasicTransformerBlock(PackedModule):
         ops = _ops()
         p = self.packed()
         C = x.shape[1]
+        edit = getattr(context, "edit", None)      # a prompt edit on this context also edits the block's self-attention
         if stats is not None and "fold" in p and (x.shape[0] // B) % 8 == 0 and x.shape[0] % 32 == 0:
             f = p["fold"]
             st1, parts1 = stats
             st2, st3 = ops.ln_stats_buffer(x.shape[0], C, x.device), ops.ln_stats_buffer(x.shape[0], C, x.device)
-            x, parts2 = self.attn1.forward_folded(x, ops.LnFold(st1, parts1, C, self.norm1.eps), f["a1"], None, resid=x, B=B, stats_out=st2)
+            x, parts2 = self.attn1.forward_folded(x, ops.LnFold(st1, parts1, C, self.norm1.eps), f["a1"], None, resid=x, B=B, stats_out=st2,
+                                                 edit=edit)
             x, parts3 = self.attn2.forward_folded(x, ops.LnFold(st2, parts2, C, self.norm2.eps), f["a2"], context, resid=x, B=B, stats_out=st3)
             h = ops.gemm_ln(x, f["ffw"], bias=f["ffc"], act=ops.ACT_GEGLU, ln=ops.LnFold(st3, parts3, C, self.norm3.eps), colsum=f["ffs"])
             return ops.gemm(h, p["w2"], bias=p["b2"], resid=x)
-        x = self.attn1(ops.layernorm(x, *p["norm1"], eps=self.norm1.eps), None, resid=x, B=B)
+        x = self.attn1(ops.layernorm(x, *p["norm1"], eps=self.norm1.eps), None, resid=x, B=B, edit=edit)
         x = self.attn2(ops.layernorm(x, *p["norm2"], eps=self.norm2.eps), context, resid=x, B=B)
         h = self.ff.net[0](ops.layernorm(x, *p["norm3"], eps=self.norm3.eps))
         return ops.gemm(h, p["w2"], bias=p["b2"], resid=x)

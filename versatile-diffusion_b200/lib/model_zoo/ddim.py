@@ -117,6 +117,11 @@ class DDIMSampler(object):
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         model = self.model
         device = torch.device(model.device)
+        # Prompt-to-Prompt (lib/model_zoo/prompt_edit.py): refuse unsupported inputs before any device work
+        pe_ctx = pe = None
+        if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
+            from .prompt_edit import check_sample_inputs
+            pe_ctx, pe = check_sample_inputs(x_info, shape, c_infos)
         # a walk from an inversion (lib/model_zoo/edit.py): its mask blends against the trajectory, with no draws
         from_inv = x_info.get('inversion', None) is not None
         if from_inv:
@@ -141,6 +146,11 @@ class DDIMSampler(object):
             start_info = {k: v for k, v in x_info.items() if k != 'x0'}
         elif inpaint:       # the img2img start noises x0 row by row: a batch-1 x0 is noised once per item
             start_info = dict(x_info, x0=x0_in.expand(bs, *x0_in.shape[1:]))
+        elif pe is not None:    # every prompt starts from the same noise: one draw, or the given x_T, expanded to the n rows
+            xt = x_info.get('xt', None)
+            if xt is None:
+                xt = torch.randn([1] + list(shape[1:]), device=device, dtype=dtype)
+            start_info = dict(x_info, xt=xt.expand(list(shape)))
         x, timesteps = self._initial_latent(shape, start_info, dtype, device)
         x_info['x'] = x
         scale = float(c_infos[0]['unconditional_guidance_scale'])
@@ -173,6 +183,8 @@ class DDIMSampler(object):
             mask_per_item = self._inpaint_state(st, x0_in, mask_in, seed, total_steps, x if full_walk else None, bs, device)
         if inv_blend:
             mask_per_item = self._inversion_blend_state(st, inv, inv_mask, device)
+        if pe is not None:
+            pe_state = self._prompt_edit_state(st, pe, c_infos[pe_ctx], ctxs, pe_ctx, cfg, H, W, total_steps, device)
         if cfg:
             st['x_in'][bs:].copy_(st['x_in'][:bs])
         st['coef'][:total_steps].copy_(coef)
@@ -192,6 +204,9 @@ class DDIMSampler(object):
             if inv_blend:
                 ops.inversion_blend(st['x_in'][:bs], st['traj'], st['mask'] if mask_per_item else st['mask'][:1], st['idx'],
                                     x_dup=st['x_in'][bs:] if cfg else None)
+            if pe is not None and pe_state.blend:
+                ops.local_blend(st['x_in'][:bs], pe_state.map, pe_state.flags, st['idx'], pe_state.h4, pe_state.w4,
+                                pe_state.threshold, x_dup=st['x_in'][bs:] if cfg else None)
             ops.add_int(st['idx'], -1)
 
         intermediates = {'pred_xt': [], 'pred_x0': []}
@@ -219,6 +234,8 @@ class DDIMSampler(object):
                 key += (('inpaint', mask_per_item),)
             if inv_blend:
                 key += (('inversion', mask_per_item),)
+            if pe is not None:
+                key += (('prompt_edit', pe.n, pe.has_beta, pe.blend is not None, pe_state.threshold),)
             n = self._walk(key, '_graphs', step, total_steps, st, c_types, ctxs, lambda i: log(total_steps - i - 1))
             if n is not None:
                 self.last_step_launches = n
@@ -419,6 +436,25 @@ class DDIMSampler(object):
         st['mask'][:mask.shape[0]].copy_(mask.view(mask.shape[0], H * W))
         return int(mask.shape[0] != 1)
 
+    def _prompt_edit_state(self, st, ed, ci, ctxs, i, cfg, H, W, total_steps, device):
+        """Swap context i for its persistent extended buffer [context rows; edited contexts] and refill the edit's device state
+        in st in place, so a cached step graph replays on new prompts and tables -> the prompt_edit.EditState (also carried
+        by the context).  lib/model_zoo/prompt_edit.py specifies the semantics."""
+        from .attention import PaddedContext
+        from .prompt_edit import EditState, quarter
+        c = ci['c']
+        ext = torch.cat([c.float(), ed.edited_contexts(ci['conditioning']).to(c.device)])
+        buf = self._ctx_buffer(('prompt_edit', i), ext)
+        es = st.get('prompt_edit')
+        want = (ed.n, 2 * ed.n if cfg else ed.n, ext.shape[0], ed.has_beta, ed.blend is not None, quarter(H), quarter(W))
+        if es is None or es.key() != want:
+            es = EditState(ed.n, cfg, ext.shape[0], ed.has_beta, ed.blend is not None, quarter(H), quarter(W), device)
+            st['prompt_edit'] = es
+            self._graphs = {}           # a cached graph reads the old buffers
+        es.fill(ed, total_steps, cfg, st['idx'])
+        ctxs[i] = PaddedContext(buf, c.shape[1], edit=es)
+        return es
+
     def _inpaint_state(self, st, x0, mask, seed, total_steps, x_T, bs, device):
         """Refill the inpainting buffers of st in place, so a cached step graph replays on a new image, mask and seed ->
         whether the mask is per item.  With x_T (the full walk) the kept region of x_in[:bs] becomes x0 noised to t_top with
@@ -462,6 +498,9 @@ class DDIMSampler(object):
 
     def _p_sample(self, x_info, c_infos, multi, t, index, repeat_noise, use_original_steps, noise_dropout, temperature):
         """One eager DDIM step with the reference's argument conventions (ddim.py:129-171, 244-298)."""
+        if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
+            raise NotImplementedError("a prompt edit spans the walk (its windows and word maps): use sample / "
+                                      "sample_multicontext (lib/model_zoo/prompt_edit.py)")
         ops = _ops()
         model = self.model
         x = x_info['x']

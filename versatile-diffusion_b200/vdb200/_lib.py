@@ -35,6 +35,7 @@ SIGNATURES = {
     "vdb_latent_store_slot_f32": (i, [p, p, i, p, i, ll, p]),
     "vdb_inversion_blend_f32": (i, [p, p, p, i, p, i, p, i, ll, i, p]),
     "vdb_diffedit_mask_f32": (i, [p, p, f, p, p, f, i, i, ll, i, f, p, p]),
+    "vdb_local_blend_f32": (i, [p, p, p, p, p, i, i, i, i, i, i, f, p]),
     "vdb_axpby_f32": (i, [p, p, f, f, p, ll, p]),
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),
@@ -47,6 +48,8 @@ SIGNATURES = {
     "vdb_attention_dv_pad": (i, [i]),
     "vdb_attention_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p]),
     "vdb_attention_varlen_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p, p]),
+    "vdb_attention_indexed_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, i, i, p, p, i, p]),
+    "vdb_xattn_word_map_f32": (i, [p, ll, p, ll, p, p, i, i, i, i, i, i, i, f, p]),
     "vdb_groupnorm_nsplit": (i, [i, i]),
     "vdb_groupnorm_scratch_floats": (ll, [i, i]),
     "vdb_groupnorm_nhwc": (i, [p, i, p, i, i, i, i, p, p, f, i, p, p, p]),

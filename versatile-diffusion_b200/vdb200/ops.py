@@ -495,6 +495,57 @@ def attention(q, k, vt, out, B, H, Nq, Nk, d_head, scale=None, q_col0=0, k_col0=
     return out
 
 
+def attention_indexed(q, k, vt, out, B, H, Nq, Nk, d_head, Bq, Bkv, items, step_idx, scale=None, q_col0=0, k_col0=0,
+                      q_bstride=0, kv_bstride=0, accumulate=False):
+    """Flash attention with the operands of each output item chosen by a device table (vdb_attention_indexed_bf16,
+    lib/model_zoo/prompt_edit.py): output item b reads Q / K / V^T from items items[r, 0..2, b], r = step_idx[0]; items int32
+    [rows, 3, B] with entries in [0, Bq) / [0, Bkv), a negative V item skips b.  accumulate: out += the attention (bf16)."""
+    _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(vt, BF16, "vt", True); _need(out, BF16, "out", True)
+    _need(items, torch.int32, "items"); _need(step_idx, torch.int32, "step_idx")
+    if items.dim() != 3 or items.shape[1] != 3 or items.shape[2] != B:
+        raise ValueError(f"items: expected [rows, 3, {B}], got {tuple(items.shape)}")
+    if scale is None:
+        scale = d_head ** -0.5
+    with _Span("attention", 4.0 * B * H * Nq * Nk * d_head, 2.0 * B * H * d_head * (2 * Nq + 2 * Nk)):
+        check(lib.vdb_attention_indexed_bf16(_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt),
+                                             vt.stride(0), _ptr(out), out.stride(0), B, H, Nq, Nk, int(q_bstride), int(kv_bstride),
+                                             d_head, float(scale), 0, int(Bq), int(Bkv), _ptr(items), _ptr(step_idx),
+                                             1 if accumulate else 0, _stream()), "attention_indexed_bf16")
+    return out
+
+
+def xattn_word_map(q, k, w, out, row0, H, N, L, d_head, kv_bstride=0, scale=None):
+    """Prompt-to-Prompt's word maps (vdb_xattn_word_map_f32): out[r, p] += sum_h sum_j w[r, j] softmax(scale q k^T)[h, p, j] for
+    the n = w.shape[0] items row0 .. row0 + n - 1 of a cross-attention call's q [B*N, >= H*dk] and k [Bkv*kv_bstride, >= H*dk]."""
+    _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(w, torch.float32, "w"); _need(out, torch.float32, "out")
+    n = w.shape[0]
+    if w.dim() != 2 or w.shape[1] != L:
+        raise ValueError(f"w: expected [n, {L}], got {tuple(w.shape)}")
+    if out.numel() != n * N:
+        raise ValueError(f"out: expected {n * N} elements ([{n}, {N}]), got {tuple(out.shape)}")
+    if scale is None:
+        scale = d_head ** -0.5
+    check(lib.vdb_xattn_word_map_f32(_ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(w), _ptr(out), n, int(row0), H, N, L,
+                                     int(kv_bstride), d_head, float(scale), _stream()), "xattn_word_map")
+    return out
+
+
+def local_blend(x, wmap, flags, step_idx, h, w, threshold, x_dup=None):
+    """Prompt-to-Prompt's local blend after a step (vdb_local_blend_f32), in place on x fp32 NHWC [n, H, W, C] (row 0 the
+    source): wmap fp32 [n, h*w] word maps, flags int32 device table read at step_idx[0]."""
+    for name, t in (("x", x), ("wmap", wmap), ("x_dup", x_dup)):
+        _need(t, torch.float32, name)
+    _need(flags, torch.int32, "flags"); _need(step_idx, torch.int32, "step_idx")
+    n, H, W, C = x.shape
+    if x_dup is not None and x_dup.shape != x.shape:
+        raise ValueError(f"x_dup: expected {tuple(x.shape)}, got {tuple(x_dup.shape)}")
+    if wmap.numel() != n * h * w:
+        raise ValueError(f"wmap: expected {n * h * w} elements ([{n}, {h}, {w}]), got {tuple(wmap.shape)}")
+    check(lib.vdb_local_blend_f32(_ptr(x), _ptr(x_dup), _ptr(wmap), _ptr(flags), _ptr(step_idx), n, H, W, C, int(h), int(w),
+                                  float(threshold), _stream()), "local_blend")
+    return x
+
+
 def groupnorm(x1, gamma, beta, eps, act=ACT_NONE, x2=None, out=None, groups=32):
     """GN32(+SiLU) over NHWC bf16 [B,H,W,C1] (+ concat x2 [B,H,W,C2]) -> [B,H,W,C1+C2]."""
     _need(x1, BF16, "x1"); _need(x2, BF16, "x2"); _need(gamma, torch.float32, "gamma"); _need(beta, torch.float32, "beta")
