@@ -113,6 +113,29 @@ int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_sr
  * x_dup and map overlapping. */
 int vdb_local_blend_f32(float* x, float* x_dup, const float* map, const int* flags, const int* step_idx, int n, int H, int W, int C,
                         int h, int w, float threshold, void* stream);
+/* ---- panoramas: MultiDiffusion window fusion — lib/model_zoo/panorama.py (an addition: the reference has no panorama mode; the
+ * layout and the merge are specified in that module's docstring) -------------------------------------------------------------------
+ * The canvas is fp32 NHWC [bs, H, W, C].  The layout has ny x nx windows of h x w; window g = iy*nx + ix reads rows oy[iy] + r
+ * (r < h) and columns (ox[ix] + j) mod W (j < w); oy / ox are device int32 tables, and only a circular layout has columns that
+ * wrap.  Both entry points take a range [first, first + k) of windows, one UNet chunk.
+ * vdb_window_gather_f32: out [k*bs, h, w, C], row j*bs + b = window first + j of image b, an exact copy; out_dup (may be NULL)
+ * receives a second copy (the CFG half).  VDB_ERR_INVALID before any launch: a null x / out / table, a size <= 0, a window larger
+ * than the canvas, a range outside the ny*nx windows, x / out / out_dup not 16-byte aligned or tables not 4-byte aligned, or any
+ * two of x, out and out_dup overlapping.
+ * vdb_window_merge_f32: eps [halves*k*bs, h, w, C] (halves 1, or 2 for [u rows; c rows] under CFG; row s*k*bs + j*bs + b is
+ * window first + j of image b) -> out [halves*bs, H, W, C].  cover_y int32 [H, 2]: the windows covering row y are iy in
+ * [cover_y[2y], cover_y[2y+1]); cover_x int32 [W, 4]: those covering column x are ix in [cover_x[4x], cover_x[4x+1]) then
+ * [cover_x[4x+2], cover_x[4x+3]), ascending.  Per element, over its covering windows in ascending window index, fp32 with
+ * round-to-nearest: the first sets out, each later one is added, and the call whose range holds the last one divides by their
+ * count.  Elements with no covering window in the range are not touched.  So calls over consecutive ranges compute exactly what
+ * one call over all windows does, and an element with one covering window gets that window's eps bit for bit.  No atomics: the
+ * result is bit-reproducible.  VDB_ERR_INVALID before any launch: as the gather, plus a null cover table, halves not 1 or 2,
+ * eps / out / cover_x not 16-byte aligned, or eps overlapping out. */
+int vdb_window_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
+                          int first, int k, float* out, float* out_dup, void* stream);
+int vdb_window_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox,
+                         const int* cover_y, const int* cover_x, int ny, int nx, int h, int w, int first, int k, float* out,
+                         void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */

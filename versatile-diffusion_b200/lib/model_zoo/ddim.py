@@ -117,6 +117,11 @@ class DDIMSampler(object):
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         model = self.model
         device = torch.device(model.device)
+        # window fusion (lib/model_zoo/panorama.py): refuse unsupported inputs before any device work
+        win = None
+        if x_info.get('windows', None) is not None:
+            from .panorama import check_sample_inputs
+            win = check_sample_inputs(x_info, shape, c_infos)
         # Prompt-to-Prompt (lib/model_zoo/prompt_edit.py): refuse unsupported inputs before any device work
         pe_ctx = pe = None
         if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
@@ -185,15 +190,41 @@ class DDIMSampler(object):
             mask_per_item = self._inversion_blend_state(st, inv, inv_mask, device)
         if pe is not None:
             pe_state = self._prompt_edit_state(st, pe, c_infos[pe_ctx], ctxs, pe_ctx, cfg, H, W, total_steps, device)
+        sig_types, sig_ctxs = c_types, ctxs
+        if win is not None:
+            from . import panorama
+            per = panorama.WINDOWS_PER_CHUNK
+            chunks = win.chunks(per)
+            ws = self._window_state(st, win, per, bs, cfg, shape[1], device)
+            wctxs = {k: self._contexts(c_infos, cfg, x_type, multi, buffer_tag=('windows', k), repeat=k)[0]
+                     for k in sorted({k for _, k in chunks})}
+            sig_types = [ct for _ in wctxs for ct in c_types]
+            sig_ctxs = [c for k in wctxs for c in wctxs[k]]
         if cfg:
             st['x_in'][bs:].copy_(st['x_in'][:bs])
         st['coef'][:total_steps].copy_(coef)
         st['ts'][:total_steps].copy_(ts_table)
         st['idx'].fill_(total_steps - 1)
 
+        def windowed_eps():
+            """gather -> UNet -> merge per chunk of windows, into the canvas eps [e_u; e_c]"""
+            t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=ws.xw.shape[0])
+            for first, k in chunks:
+                rows = k * bs
+                xw = ws.xw[:B // bs * rows]
+                ops.window_gather(st['x_in'][:bs], ws.oy, ws.ox, win.h, win.w, first, k, out=xw[:rows],
+                                  out_dup=xw[rows:] if cfg else None)
+                e = model.eps_nhwc(xw, x_type, t_emb[:xw.shape[0]], c_types, wctxs[k], ratios, time_from)
+                ops.window_merge(e, ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, ws.eps, halves=B // bs)
+            return ws.eps
+
         def step(noise=None):
-            t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=B)
-            eps = model.eps_nhwc(st['x_in'].view(B, -1) if flat else st['x_in'], x_type, t_emb, c_types, ctxs, ratios, time_from)
+            if win is not None:
+                eps = windowed_eps()
+            else:
+                t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=B)
+                eps = model.eps_nhwc(st['x_in'].view(B, -1) if flat else st['x_in'], x_type, t_emb, c_types, ctxs, ratios,
+                                     time_from)
             if flat:
                 eps = eps.view(B, 1, 1, -1)
             e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
@@ -236,7 +267,9 @@ class DDIMSampler(object):
                 key += (('inversion', mask_per_item),)
             if pe is not None:
                 key += (('prompt_edit', pe.n, pe.has_beta, pe.blend is not None, pe_state.threshold),)
-            n = self._walk(key, '_graphs', step, total_steps, st, c_types, ctxs, lambda i: log(total_steps - i - 1))
+            if win is not None:
+                key += (('windows', win.key(), per, tuple((c.data.data_ptr(), tuple(c.data.shape)) for c in sig_ctxs)),)
+            n = self._walk(key, '_graphs', step, total_steps, st, sig_types, sig_ctxs, lambda i: log(total_steps - i - 1))
             if n is not None:
                 self.last_step_launches = n
 
@@ -247,14 +280,18 @@ class DDIMSampler(object):
         x_info['x'] = pred_xt
         return pred_xt, intermediates
 
-    def _contexts(self, c_infos, cfg, x_type, multi, buffer_tag=None):
+    def _contexts(self, c_infos, cfg, x_type, multi, buffer_tag=None, repeat=1):
         """[uncond ; cond] of every context, built once (the reference re-concatenates every step, ddim.py:146), in persistent
-        padded buffers (per buffer_tag, so the inversion keeps its own) -> (contexts, c_types, ratios, time_from, model_channels)"""
+        padded buffers (per buffer_tag, so the inversion and the window chunks keep their own) -> (contexts, c_types, ratios,
+        time_from, model_channels).  repeat = k: each half's rows repeated k times, [u; u; ...; c; c; ...], the contexts of a
+        chunk of k windows (lib/model_zoo/panorama.py)."""
         from .attention import PaddedContext
         ctxs = []
         for i, ci in enumerate(c_infos):
             c = torch.cat([ci['unconditional_conditioning'], ci['conditioning']]) if cfg else ci['conditioning']
             ci['c'] = c
+            if repeat != 1:
+                c = torch.cat([h.repeat(repeat, 1, 1) for h in c.chunk(2 if cfg else 1)])
             ctxs.append(PaddedContext(self._ctx_buffer(i if buffer_tag is None else (buffer_tag, i), c), c.shape[1]))
         c_types = [ci['type'] for ci in c_infos]
         ratios = [float(ci.get('ratio', 1.0)) for ci in c_infos]
@@ -455,6 +492,18 @@ class DDIMSampler(object):
         ctxs[i] = PaddedContext(buf, c.shape[1], edit=es)
         return es
 
+    def _window_state(self, st, lay, per, bs, cfg, C, device):
+        """The persistent device state of a windowed walk in st (panorama.WindowState), its layout tables refilled in place, so a
+        cached step graph replays on new prompts or a new x_T.  lib/model_zoo/panorama.py specifies the semantics."""
+        from .panorama import WindowState
+        ws = st.get('windows')
+        if ws is None or ws.key != WindowState.key_for(lay, per, bs, cfg, C):
+            ws = WindowState(lay, per, bs, cfg, C, device)
+            st['windows'] = ws
+            self._graphs = {}           # a cached graph reads the old buffers
+        ws.fill(lay)
+        return ws
+
     def _inpaint_state(self, st, x0, mask, seed, total_steps, x_T, bs, device):
         """Refill the inpainting buffers of st in place, so a cached step graph replays on a new image, mask and seed ->
         whether the mask is per item.  With x_T (the full walk) the kept region of x_in[:bs] becomes x0 noised to t_top with
@@ -501,6 +550,9 @@ class DDIMSampler(object):
         if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
             raise NotImplementedError("a prompt edit spans the walk (its windows and word maps): use sample / "
                                       "sample_multicontext (lib/model_zoo/prompt_edit.py)")
+        if x_info.get('windows', None) is not None:
+            raise NotImplementedError("window fusion runs inside the sampler's walk: use sample / sample_multicontext "
+                                      "(lib/model_zoo/panorama.py)")
         ops = _ops()
         model = self.model
         x = x_info['x']

@@ -46,6 +46,9 @@ class PLMSSampler(DDIMSampler):
         if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
             raise NotImplementedError("PLMSSampler has no prompt editing: use DDIMSampler or DPMSolverSampler "
                                       "(lib/model_zoo/prompt_edit.py)")
+        if x_info.get('windows', None) is not None:
+            raise NotImplementedError("PLMSSampler has no window fusion: use DDIMSampler or DPMSolverSampler "
+                                      "(lib/model_zoo/panorama.py)")
         if x_info.get('inversion', None) is not None:
             raise NotImplementedError("PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
                                       "(lib/model_zoo/edit.py)")

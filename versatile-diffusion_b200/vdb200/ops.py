@@ -546,6 +546,47 @@ def local_blend(x, wmap, flags, step_idx, h, w, threshold, x_dup=None):
     return x
 
 
+def window_gather(x, oy, ox, h, w, first, k, out=None, out_dup=None):
+    """Windows [first, first + k) of the canvas x fp32 NHWC [bs, H, W, C] -> out [k*bs, h, w, C] (row j*bs + b: window first + j
+    of image b), and a copy into out_dup when given (lib/model_zoo/panorama.py).  oy / ox: int32 device origin tables."""
+    for name, t in (("x", x), ("out", out), ("out_dup", out_dup)):
+        _need(t, torch.float32, name)
+    _need(oy, torch.int32, "oy"); _need(ox, torch.int32, "ox")
+    bs, H, W, C = x.shape
+    shape = (k * bs, h, w, C)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    for name, t in (("out", out), ("out_dup", out_dup)):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError(f"{name}: expected {shape}, got {tuple(t.shape)}")
+    check(lib.vdb_window_gather_f32(_ptr(x), bs, H, W, C, _ptr(oy), _ptr(ox), oy.numel(), ox.numel(), int(h), int(w), int(first),
+                                    int(k), _ptr(out), _ptr(out_dup), _stream()), "window_gather")
+    return out
+
+
+def window_merge(eps, oy, ox, cover_y, cover_x, first, k, out, halves=1):
+    """Merge windows [first, first + k) of eps fp32 [halves*k*bs, h, w, C] into the canvas out [halves*bs, H, W, C] (lib/model_zoo/
+    panorama.py): the running fp32 sum over each element's covering windows in ascending window index, divided by their count
+    at the element's last one.  oy / ox / cover_y [H, 2] / cover_x [W, 4]: int32 device tables.  halves = 2 under CFG: eps is
+    [u rows; c rows] and out [e_u; e_c]."""
+    for name, t in (("eps", eps), ("out", out)):
+        _need(t, torch.float32, name)
+    for name, t in (("oy", oy), ("ox", ox), ("cover_y", cover_y), ("cover_x", cover_x)):
+        _need(t, torch.int32, name)
+    n, H, W, C = out.shape
+    if halves not in (1, 2) or n % halves:
+        raise ValueError(f"halves must be 1 or 2 and divide the {n} rows of out, got {halves}")
+    bs = n // halves
+    if eps.dim() != 4 or eps.shape[0] != k * n or eps.shape[3] != C:
+        raise ValueError(f"eps: expected [{k * n}, h, w, {C}] for out {tuple(out.shape)}, got {tuple(eps.shape)}")
+    _, h, w, _ = eps.shape
+    if cover_y.numel() != 2 * H or cover_x.numel() != 4 * W:
+        raise ValueError(f"cover tables: expected {2 * H} and {4 * W} entries, got {cover_y.numel()} and {cover_x.numel()}")
+    check(lib.vdb_window_merge_f32(_ptr(eps), halves, bs, H, W, C, _ptr(oy), _ptr(ox), _ptr(cover_y), _ptr(cover_x), oy.numel(),
+                                   ox.numel(), int(h), int(w), int(first), int(k), _ptr(out), _stream()), "window_merge")
+    return out
+
+
 def groupnorm(x1, gamma, beta, eps, act=ACT_NONE, x2=None, out=None, groups=32):
     """GN32(+SiLU) over NHWC bf16 [B,H,W,C1] (+ concat x2 [B,H,W,C2]) -> [B,H,W,C1+C2]."""
     _need(x1, BF16, "x1"); _need(x2, BF16, "x2"); _need(gamma, torch.float32, "gamma"); _need(beta, torch.float32, "beta")
