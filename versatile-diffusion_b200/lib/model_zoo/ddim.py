@@ -8,15 +8,113 @@ live in device tables indexed by a device-side step counter; the 50-step loop is
 no host<->device traffic (the reference does ~15 tiny kernels + 4 H2D fills per step, ddim.py:159-171).
 The latent stays fp32 NHWC between steps; NCHW conversion happens only at the API boundary.
 """
+from types import SimpleNamespace
+
 import numpy as np
 import torch
 
-from .diffusion_utils import make_ddim_sampling_parameters, make_ddim_timesteps, noise_like, require_cuda
+from .diffusion_utils import (make_ddim_sampling_parameters, make_ddim_timesteps, noise_like, pack_epoch, require_cuda,
+                              to_numpy)
 
 
 def _ops():
     from vdb200 import ops
     return ops
+
+
+# ------------------------------------------------------------------ sampling modes and how they combine
+# A mode is selected by an optional input: x_info['windows'] (lib/model_zoo/panorama.py), a context's 'prompt_edit'
+# (prompt_edit.py), x_info['inversion'] (edit.py) and x_info['inpaint_mask'] (inpaint.py).  The start inputs x_info['x0'] (with
+# 'x0_forward_timesteps') and x_info['xt'] select no mode, but some modes refuse them.
+#
+# REFUSES: who -> {input given: (exception type, message)}, checked in this order.
+#   - Entry points, before anything else: 'sample' (DDIMSampler's and DPMSolverSampler's sample / sample_multicontext), 'plms'
+#     (PLMSSampler's) and 'p_sample' (p_sample_ddim(_multicontext), which ignores the inputs it does not list).
+#   - Modes, for the pairs that refuse each other: each mode checks its row after the type of its own input and before its
+#     other checks, modes in the order of DDIMSampler._modes.
+REFUSES = {
+    'sample': {},
+    'plms': {k: (NotImplementedError, msg) for k, msg in (
+        ('inpaint_mask', "PLMSSampler has no inpainting: use DDIMSampler or DPMSolverSampler (lib/model_zoo/inpaint.py)"),
+        ('prompt_edit', "PLMSSampler has no prompt editing: use DDIMSampler or DPMSolverSampler (lib/model_zoo/prompt_edit.py)"),
+        ('windows', "PLMSSampler has no window fusion: use DDIMSampler or DPMSolverSampler (lib/model_zoo/panorama.py)"),
+        ('inversion', "PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
+                      "(lib/model_zoo/edit.py)"))},
+    'p_sample': {
+        'prompt_edit': (NotImplementedError, "a prompt edit spans the walk (its windows and word maps): use sample / "
+                                             "sample_multicontext (lib/model_zoo/prompt_edit.py)"),
+        'windows': (NotImplementedError, "window fusion runs inside the sampler's walk: use sample / sample_multicontext "
+                                         "(lib/model_zoo/panorama.py)")},
+    'windows': {
+        'prompt_edit': (NotImplementedError, "windows with prompt_edit: the edit's item tables index prompts, not windows "
+                                             "(lib/model_zoo/panorama.py)"),
+        'inversion': (NotImplementedError, "windows cannot sample from an inversion (lib/model_zoo/panorama.py)")},
+    'prompt_edit': {k: (ValueError, f"'prompt_edit' does not combine with {k!r}") for k in ('x0', 'inpaint_mask', 'inversion')},
+    'inversion': {k: (ValueError, f"x_info['{k}'] cannot be given with 'inversion': the walk starts from the inversion")
+                  for k in ('xt', 'x0', 'x0_forward_timesteps')},
+}
+
+# Pairs that change meaning: mode -> inputs it takes over, which then select no mode of their own.  An inpaint_mask given with an
+# inversion is the mask of the inversion's trajectory blend, not inpainting.
+TAKES = {'inversion': ('inpaint_mask',)}
+
+
+def given_inputs(x_info, c_infos):
+    """The optional inputs given (not None) to a call."""
+    given = {k for k in ('x0', 'xt', 'x0_forward_timesteps', 'inpaint_mask', 'inversion', 'windows')
+             if x_info.get(k, None) is not None}
+    if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
+        given.add('prompt_edit')
+    return given
+
+
+def refuse(who, x_info, c_infos):
+    """Raise what REFUSES says `who` (an entry point or a mode) raises for the inputs given."""
+    given = given_inputs(x_info, c_infos)
+    for k, (exc, msg) in REFUSES[who].items():
+        if k in given:
+            raise exc(msg)
+
+
+def buffers_key(*bufs):
+    """The identity (address and shape) of the device buffers a captured step graph reads, for its key."""
+    return tuple((b.data_ptr(), tuple(b.shape)) for b in bufs if b is not None)
+
+
+class SamplerMode(object):
+    """A mode's part in DDIMSampler's walk.  The constructor checks the mode's inputs on the host, before any device work; the
+    mode keeps its persistent device state in the walk record (run.walk, under the mode's own names), refilled in place so a
+    cached step graph replays.  `run` is the call's record (DDIMSampler._run): the walk record, the batch and latent shape, the contexts, and
+    run.x / run.x_dup, the latent [bs, H, W, C] and its CFG duplicate (or None)."""
+
+    def start(self, sampler, x_info, shape, dtype, device):
+        """-> (x_T NCHW, the grid points to walk) when the mode changes the start latent, else None."""
+        return None
+
+    def prepare(self, sampler, run):
+        """Refill the device state for this call (a mode may also swap the contexts the step reads) -> its part of the graph
+        key, which covers every buffer the mode's launches read."""
+        raise NotImplementedError
+
+    def eps(self, sampler, run):
+        """-> the step's eps [run.B, H, W, C] when the mode replaces the UNet call on the latent, else None."""
+        return None
+
+    def after_update(self, run):
+        """The mode's launches after the step's update, before the step counter moves."""
+
+
+class _Walk(dict):
+    """The persistent device buffers of one kind of walk by name (sampling or inversion, so neither evicts the other's graph),
+    with the device state its modes add, and `graphs`, its one captured step graph as {key: (CUDAGraph, K / V^T signature)}
+    (one live graph: its private pool holds the activations).  The graph reads these buffers, so it lives and dies with the
+    record."""
+
+    def __init__(self, key, bs, B, H, W, C, cols, rings, device):
+        z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=device)
+        super().__init__(x_in=z(B, H, W, C), pred_x0=z(bs, H, W, C), coef=z(1000, cols), ts=z(1000, dtype=torch.int64),
+                         idx=z(1, dtype=torch.int32), **{name: z(*s) for name, s in rings.items()})
+        self.key, self.graphs = key, {}
 
 
 class DDIMSampler(object):
@@ -26,8 +124,6 @@ class DDIMSampler(object):
         self.ddpm_num_timesteps = model.num_timesteps
         self.schedule = schedule
         self.use_cuda_graph = kwargs.get("use_cuda_graph", True)
-        self._graphs = {}
-        self._inv_graphs = {}
 
     def register_buffer(self, name, attr):
         # the reference forces .to('cuda') here (ddim.py:17-21); follow the model's device instead
@@ -96,13 +192,9 @@ class DDIMSampler(object):
 
     # ------------------------------------------------------------------ the loop
     def _initial_latent(self, shape, x_info, dtype, device):
-        """ddim.py:94-105: injected x_T ('xt'), img2img start (x0 + q_sample) or fresh noise; or slot k of an inversion and the
-        first k grid points (lib/model_zoo/edit.py)."""
+        """ddim.py:94-105: injected x_T ('xt'), img2img start (x0 + q_sample) or fresh noise."""
         timesteps = self.ddim_timesteps
-        if x_info.get('inversion', None) is not None:
-            inv = x_info['inversion']
-            x, timesteps = inv.xt.to(dtype).to(device), timesteps[:inv.k]
-        elif x_info.get('xt', None) is not None:
+        if x_info.get('xt', None) is not None:
             x = x_info['xt'].to(dtype).to(device)       # (the reference's `.astype` here is a bug, ddim.py:95)
         elif x_info.get('x0', None) is not None:
             x0 = x_info['x0'].type(dtype).to(device)
@@ -114,49 +206,32 @@ class DDIMSampler(object):
             x = torch.randn(shape, device=device, dtype=dtype)
         return x, timesteps
 
+    def _modes(self, entry, x_info, shape, c_infos):
+        """Refuse what entry point `entry` does not take, then build the active modes in the order they check their inputs
+        (the order in which refusals win) -> [SamplerMode].  Host work only: every refusal comes before any device work."""
+        from .edit import FromInversion
+        from .inpaint import Inpainting
+        from .panorama import WindowFusion
+        from .prompt_edit import PromptEditing
+        refuse(entry, x_info, c_infos)
+        given = given_inputs(x_info, c_infos)
+        taken = {k for m in given for k in TAKES.get(m, ())}
+        return [cls(self, x_info, shape, c_infos) for name, cls in (('windows', WindowFusion), ('prompt_edit', PromptEditing),
+                                                                      ('inversion', FromInversion), ('inpaint_mask', Inpainting))
+                if name in given and name not in taken]
+
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
         model = self.model
         device = torch.device(model.device)
-        # window fusion (lib/model_zoo/panorama.py): refuse unsupported inputs before any device work
-        win = None
-        if x_info.get('windows', None) is not None:
-            from .panorama import check_sample_inputs
-            win = check_sample_inputs(x_info, shape, c_infos)
-        # Prompt-to-Prompt (lib/model_zoo/prompt_edit.py): refuse unsupported inputs before any device work
-        pe_ctx = pe = None
-        if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
-            from .prompt_edit import check_sample_inputs
-            pe_ctx, pe = check_sample_inputs(x_info, shape, c_infos)
-        # a walk from an inversion (lib/model_zoo/edit.py): its mask blends against the trajectory, with no draws
-        from_inv = x_info.get('inversion', None) is not None
-        if from_inv:
-            from .edit import check_sample_inputs
-            inv, inv_mask = check_sample_inputs(x_info, shape, self.ddim_timesteps)
-        inv_blend = from_inv and inv_mask is not None
-        # inpainting (lib/model_zoo/inpaint.py): refuse bad inputs before any device work; the Philox key comes from torch's CPU
-        # generator, drawn only when a mask is given
-        inpaint = x_info.get('inpaint_mask', None) is not None and not from_inv
-        if inpaint:
-            from .inpaint import check_inputs
-            x0_in, mask_in = check_inputs(x_info, shape)
-            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64)
+        modes = self._modes('sample', x_info, shape, c_infos)
         if device.type != 'cuda':
             raise RuntimeError("DDIMSampler: the H100 build has no CPU path (model.to('cuda') first)")
         ops = _ops()
         dtype = c_infos[0]['conditioning'].dtype
         bs = shape[0]
-        full_walk = inpaint and x_info.get('x0_forward_timesteps', None) is None
-        start_info = x_info
-        if full_walk:       # a masked full walk starts from x_T as an unmasked one does, never from the img2img start
-            start_info = {k: v for k, v in x_info.items() if k != 'x0'}
-        elif inpaint:       # the img2img start noises x0 row by row: a batch-1 x0 is noised once per item
-            start_info = dict(x_info, x0=x0_in.expand(bs, *x0_in.shape[1:]))
-        elif pe is not None:    # every prompt starts from the same noise: one draw, or the given x_T, expanded to the n rows
-            xt = x_info.get('xt', None)
-            if xt is None:
-                xt = torch.randn([1] + list(shape[1:]), device=device, dtype=dtype)
-            start_info = dict(x_info, xt=xt.expand(list(shape)))
-        x, timesteps = self._initial_latent(shape, start_info, dtype, device)
+        starts = [s for s in (m.start(self, x_info, shape, dtype, device) for m in modes) if s is not None]
+        # REFUSES and TAKES leave at most one mode that changes the start
+        x, timesteps = starts[0] if starts else self._initial_latent(shape, x_info, dtype, device)
         x_info['x'] = x
         scale = float(c_infos[0]['unconditional_guidance_scale'])
         cfg = scale != 1.
@@ -165,7 +240,7 @@ class DDIMSampler(object):
             # x0_forward_timesteps == 0 leaves no step to run: the reference's loop never executes and it raises on the unbound
             # result (ddim.py:105-127); here the device tables would be indexed at -1
             raise ValueError(f"DDIM walk of {total_steps} steps: need 1..1000 (x0_forward_timesteps must be >= 1)")
-        sigmas = np.asarray(self.ddim_sigmas.cpu() if isinstance(self.ddim_sigmas, torch.Tensor) else self.ddim_sigmas)
+        sigmas = to_numpy(self.ddim_sigmas)
         fast = self.use_cuda_graph and noise_dropout == 0. and not np.any(sigmas[:total_steps] != 0)
 
         x_type = x_info['type']
@@ -182,98 +257,50 @@ class DDIMSampler(object):
         coef = torch.tensor(self._coef_table(timesteps, sigmas), dtype=torch.float32, device=device).contiguous()
         ts_table = torch.tensor(np.asarray(timesteps, dtype=np.int64), device=device)
 
-        st = self._state(bs, B, H, W, shape[1], device)
-        ops.nchw_to_nhwc(x.float().contiguous(), out=st['x_in'][:bs])
-        if inpaint:
-            mask_per_item = self._inpaint_state(st, x0_in, mask_in, seed, total_steps, x if full_walk else None, bs, device)
-        if inv_blend:
-            mask_per_item = self._inversion_blend_state(st, inv, inv_mask, device)
-        if pe is not None:
-            pe_state = self._prompt_edit_state(st, pe, c_infos[pe_ctx], ctxs, pe_ctx, cfg, H, W, total_steps, device)
-        sig_types, sig_ctxs = c_types, ctxs
-        if win is not None:
-            from . import panorama
-            per = panorama.WINDOWS_PER_CHUNK
-            chunks = win.chunks(per)
-            ws = self._window_state(st, win, per, bs, cfg, shape[1], device)
-            wctxs = {k: self._contexts(c_infos, cfg, x_type, multi, buffer_tag=('windows', k), repeat=k)[0]
-                     for k in sorted({k for _, k in chunks})}
-            sig_types = [ct for _ in wctxs for ct in c_types]
-            sig_ctxs = [c for k in wctxs for c in wctxs[k]]
+        w = self._walk_record('_st', bs, B, H, W, shape[1], self._coef_cols, device, self._rings(bs, H, W, shape[1]))
+        ops.nchw_to_nhwc(x.float().contiguous(), out=w['x_in'][:bs])
+        run = SimpleNamespace(walk=w, modes=modes, bs=bs, B=B, H=H, W=W, C=shape[1], cfg=cfg, scale=scale, flat=flat,
+                              total=total_steps, device=device, x_type=x_type, multi=multi, c_infos=c_infos, c_types=c_types,
+                              ctxs=ctxs, ratios=ratios, time_from=time_from, mch=mch, kv_types=c_types, kv_ctxs=ctxs,
+                              x=w['x_in'][:bs], x_dup=w['x_in'][bs:] if cfg else None)
+        mode_keys = tuple(m.prepare(self, run) for m in modes)
         if cfg:
-            st['x_in'][bs:].copy_(st['x_in'][:bs])
-        st['coef'][:total_steps].copy_(coef)
-        st['ts'][:total_steps].copy_(ts_table)
-        st['idx'].fill_(total_steps - 1)
-
-        def windowed_eps():
-            """gather -> UNet -> merge per chunk of windows, into the canvas eps [e_u; e_c]"""
-            t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=ws.xw.shape[0])
-            for first, k in chunks:
-                rows = k * bs
-                xw = ws.xw[:B // bs * rows]
-                ops.window_gather(st['x_in'][:bs], ws.oy, ws.ox, win.h, win.w, first, k, out=xw[:rows],
-                                  out_dup=xw[rows:] if cfg else None)
-                e = model.eps_nhwc(xw, x_type, t_emb[:xw.shape[0]], c_types, wctxs[k], ratios, time_from)
-                ops.window_merge(e, ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, ws.eps, halves=B // bs)
-            return ws.eps
+            w['x_in'][bs:].copy_(w['x_in'][:bs])
+        w['coef'][:total_steps].copy_(coef)
+        w['ts'][:total_steps].copy_(ts_table)
+        w['idx'].fill_(total_steps - 1)
 
         def step(noise=None):
-            if win is not None:
-                eps = windowed_eps()
-            else:
-                t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=B)
-                eps = model.eps_nhwc(st['x_in'].view(B, -1) if flat else st['x_in'], x_type, t_emb, c_types, ctxs, ratios,
-                                     time_from)
-            if flat:
-                eps = eps.view(B, 1, 1, -1)
-            e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
-            self._update(st, e_u, e_c, scale, bs, cfg, noise, temperature)
-            if inpaint:
-                ops.inpaint_blend(st['x_in'][:bs], st['x0'], st['mask'] if mask_per_item else st['mask'][:1], st['blend'],
-                                  st['idx'], seed=st['seed'], x_dup=st['x_in'][bs:] if cfg else None)
-            if inv_blend:
-                ops.inversion_blend(st['x_in'][:bs], st['traj'], st['mask'] if mask_per_item else st['mask'][:1], st['idx'],
-                                    x_dup=st['x_in'][bs:] if cfg else None)
-            if pe is not None and pe_state.blend:
-                ops.local_blend(st['x_in'][:bs], pe_state.map, pe_state.flags, st['idx'], pe_state.h4, pe_state.w4,
-                                pe_state.threshold, x_dup=st['x_in'][bs:] if cfg else None)
-            ops.add_int(st['idx'], -1)
+            e_u, e_c = self._eps(run)
+            self._update(w, e_u, e_c, scale, bs, cfg, noise, temperature)
+            for m in modes:
+                m.after_update(run)
+            ops.add_int(w['idx'], -1)
 
         intermediates = {'pred_xt': [], 'pred_x0': []}
 
         def log(index):
             if index % log_every_t == 0 or index == total_steps - 1:
-                intermediates['pred_xt'].append(ops.nhwc_to_nchw(st['x_in'][:bs].contiguous()).to(dtype))
-                intermediates['pred_x0'].append(ops.nhwc_to_nchw(st['pred_x0']).to(dtype))
+                intermediates['pred_xt'].append(ops.nhwc_to_nchw(w['x_in'][:bs].contiguous()).to(dtype))
+                intermediates['pred_x0'].append(ops.nhwc_to_nchw(w['pred_x0']).to(dtype))
 
         if not fast:
             for i in range(total_steps):
                 index = total_steps - i - 1
                 noise = None
                 if sigmas[index] != 0:
-                    noise = noise_like(st['x_in'][:bs], False)
+                    noise = noise_like(w['x_in'][:bs], False)
                     if noise_dropout > 0.:
                         noise = torch.nn.functional.dropout(noise, p=noise_dropout)
                 step(noise)
                 log(index)
         else:
-            from .diffusion_utils import pack_epoch
-            key = (pack_epoch(), bs, B, H, W, x_type, tuple(c_types), tuple(ratios), scale, float(temperature), time_from,
-                   tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs)) + self._graph_tag()
-            if inpaint:
-                key += (('inpaint', mask_per_item),)
-            if inv_blend:
-                key += (('inversion', mask_per_item),)
-            if pe is not None:
-                key += (('prompt_edit', pe.n, pe.has_beta, pe.blend is not None, pe_state.threshold),)
-            if win is not None:
-                key += (('windows', win.key(), per, tuple((c.data.data_ptr(), tuple(c.data.shape)) for c in sig_ctxs)),)
-            n = self._walk(key, '_graphs', step, total_steps, st, sig_types, sig_ctxs, lambda i: log(total_steps - i - 1))
+            n = self._walk(run, (float(temperature),) + self._graph_tag() + mode_keys, step, total_steps,
+                           lambda i: log(total_steps - i - 1))
             if n is not None:
                 self.last_step_launches = n
 
-        pred_xt = ops.nhwc_to_nchw(st['x_in'][:bs].contiguous()).to(dtype)
+        pred_xt = ops.nhwc_to_nchw(w['x_in'][:bs].contiguous()).to(dtype)
         if flat:
             pred_xt = pred_xt.reshape(bs, -1)
             intermediates = {k: [v.reshape(bs, -1) for v in vs] for k, vs in intermediates.items()}
@@ -298,12 +325,31 @@ class DDIMSampler(object):
         time_from = self.model.time_source(x_type, multi)
         return ctxs, c_types, ratios, time_from, self.model.diffuser[time_from].model_channels
 
-    def _walk(self, key, graphs_attr, step, total_steps, st, c_types, ctxs, log):
-        """Run total_steps steps of `step` on a captured step graph kept in self.<graphs_attr>; log(i) after walk position i.
-        -> the launches of one step, or None when a cached graph replayed every step."""
-        model, ops = self.model, _ops()
-        ent = getattr(self, graphs_attr).get(key)
-        if ent is not None and ent[1] == model.context_kv_signature(c_types, ctxs):
+    def _eps(self, run):
+        """The step's eps at the walk's timestep, as its CFG halves (e_u or None, e_c): the UNet on the latent, or the eps of a
+        mode that replaces that call."""
+        w = run.walk
+        for m in run.modes:
+            eps = m.eps(self, run)
+            if eps is not None:
+                break
+        else:
+            t_emb = _ops().timestep_embedding(w['ts'], run.mch, step_idx=w['idx'], batch=run.B)
+            eps = self.model.eps_nhwc(w['x_in'].view(run.B, -1) if run.flat else w['x_in'], run.x_type, t_emb, run.c_types,
+                                      run.ctxs, run.ratios, run.time_from)
+        if run.flat:
+            eps = eps.view(run.B, 1, 1, -1)
+        return (eps[:run.bs], eps[run.bs:]) if run.cfg else (None, eps)
+
+    def _walk(self, run, tag, step, total_steps, log):
+        """Run total_steps steps of `step` on the captured step graph kept in run.walk; log(i) after walk position i.  The key
+        covers the shapes, the contexts the step reads and `tag`.  -> the launches of one step, or None when a cached graph
+        replayed every step."""
+        model, ops, w = self.model, _ops(), run.walk
+        key = (pack_epoch(), run.bs, run.B, run.H, run.W, run.x_type, tuple(run.kv_types), tuple(run.ratios), run.scale,
+               run.time_from, tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in run.kv_ctxs)) + tag
+        ent = w.graphs.get(key)
+        if ent is not None and ent[1] == model.context_kv_signature(run.kv_types, run.kv_ctxs):
             # steady state: the context projections were just refreshed in place; every step is a graph replay
             for i in range(total_steps):
                 ent[0].replay()
@@ -317,19 +363,33 @@ class DDIMSampler(object):
         if total_steps > 1:
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
-            idx_before = st['idx'].clone()
-            x_before = st['x_in'].clone()
+            idx_before = w['idx'].clone()
+            x_before = w['x_in'].clone()
             with torch.cuda.graph(g):
                 step()
             # capture does not execute; make sure state is exactly what the eager step left
-            st['idx'].copy_(idx_before)
-            st['x_in'].copy_(x_before)
+            w['idx'].copy_(idx_before)
+            w['x_in'].copy_(x_before)
             # keep one live graph (its private pool holds the activations) + the K / V^T buffers it reads
-            setattr(self, graphs_attr, {key: (g, model.context_kv_signature(c_types, ctxs))})
+            w.graphs = {key: (g, model.context_kv_signature(run.kv_types, run.kv_ctxs))}
         for i in range(1, total_steps):
             g.replay()
             log(i)
         return launches
+
+    def _walk_record(self, attr, bs, B, H, W, C, cols, device, rings):
+        """The persistent _Walk in self.<attr> ('_st' samples, '_inv_st' inverts), rebuilt (dropping its graph) when its buffers
+        change shape."""
+        key = (bs, B, H, W, C, cols, tuple(rings.items()), str(device))
+        w = getattr(self, attr, None)
+        if w is None or w.key != key:
+            w = _Walk(key, bs, B, H, W, C, cols, rings, device)
+            setattr(self, attr, w)
+        return w
+
+    # the cached step graph of the sampling walk and of the inversion walk, {key: (CUDAGraph, K / V^T signature)}
+    _graphs = property(lambda self: self._st.graphs if hasattr(self, '_st') else {})
+    _inv_graphs = property(lambda self: self._inv_st.graphs if hasattr(self, '_inv_st') else {})
 
     # ------------------------------------------------------------------ DDIM inversion (lib/model_zoo/edit.py)
     @torch.no_grad()
@@ -347,8 +407,7 @@ class DDIMSampler(object):
 
     def _invert(self, steps, x0, c_infos, multi, k, verbose):
         from .edit import Inversion, check_invert_inputs, context_batch, inversion_rows
-        model = self.model
-        device = torch.device(model.device)
+        device = torch.device(self.model.device)
         self.make_schedule(ddim_num_steps=steps, ddim_eta=0., verbose=verbose)
         timesteps = self.ddim_timesteps
         bs = context_batch(c_infos, float(c_infos[0]['unconditional_guidance_scale']))
@@ -361,32 +420,30 @@ class DDIMSampler(object):
         cfg = scale != 1.
         B = 2 * bs if cfg else bs
         ctxs, c_types, ratios, time_from, mch = self._contexts(c_infos, cfg, 'image', multi, buffer_tag='invert')
-        st = self._inv_state(bs, B, H, W, C, len(timesteps) + 1, device)
-        ring = st['ring']
+        w = self._walk_record('_inv_st', bs, B, H, W, C, 4, device, {'ring': (len(timesteps) + 1, bs, H, W, C)})
+        ring = w['ring']
         ring[0].copy_(ops.nchw_to_nhwc(x0.to(device=device, dtype=torch.float32).expand(bs, C, H, W).contiguous()))
-        st['x_in'][:bs].copy_(ring[0])
+        w['x_in'][:bs].copy_(ring[0])
         if cfg:
-            st['x_in'][bs:].copy_(ring[0])
-        st['coef'][:k].copy_(torch.from_numpy(inversion_rows(self.ddim_alphas, self.ddim_alphas_prev, k)))
-        st['ts'][:len(timesteps)].copy_(torch.tensor(np.asarray(timesteps, dtype=np.int64)))
-        st['idx'].fill_(0)
+            w['x_in'][bs:].copy_(ring[0])
+        w['coef'][:k].copy_(torch.from_numpy(inversion_rows(self.ddim_alphas, self.ddim_alphas_prev, k)))
+        w['ts'][:len(timesteps)].copy_(torch.tensor(np.asarray(timesteps, dtype=np.int64)))
+        w['idx'].fill_(0)
+        run = SimpleNamespace(walk=w, modes=[], bs=bs, B=B, H=H, W=W, cfg=cfg, scale=scale, flat=False, x_type='image',
+                              c_types=c_types, ctxs=ctxs, ratios=ratios, time_from=time_from, mch=mch, kv_types=c_types,
+                              kv_ctxs=ctxs)
 
         def step():
-            t_emb = ops.timestep_embedding(st['ts'], mch, step_idx=st['idx'], batch=B)
-            eps = model.eps_nhwc(st['x_in'], 'image', t_emb, c_types, ctxs, ratios, time_from)
-            e_u, e_c = (eps[:bs], eps[bs:]) if cfg else (None, eps)
-            DDIMSampler._update(self, st, e_u, e_c, scale, bs, cfg, None, 1.0)
-            ops.latent_store_slot(st['x_in'][:bs], ring, st['idx'], 1)
-            ops.add_int(st['idx'], 1)
+            e_u, e_c = self._eps(run)
+            DDIMSampler._update(self, w, e_u, e_c, scale, bs, cfg, None, 1.0)
+            ops.latent_store_slot(w['x_in'][:bs], ring, w['idx'], 1)
+            ops.add_int(w['idx'], 1)
 
         if not self.use_cuda_graph:
             for _ in range(k):
                 step()
         else:
-            from .diffusion_utils import pack_epoch
-            key = (pack_epoch(), bs, B, H, W, tuple(c_types), tuple(ratios), scale, time_from,
-                   tuple((c.data.data_ptr(), tuple(c.data.shape), c.length) for c in ctxs), 'invert')
-            n = self._walk(key, '_inv_graphs', step, k, st, c_types, ctxs, lambda i: None)
+            n = self._walk(run, (), step, k, lambda i: None)
             if n is not None:
                 self.last_invert_step_launches = n
         return Inversion(ring[:k + 1].clone(), steps, k, timesteps, (bs, C, H, W))
@@ -397,16 +454,20 @@ class DDIMSampler(object):
     def _coef_table(self, timesteps, sigmas):
         """fp32 [len(timesteps), 4] rows {a_t, a_prev, sigma_t, sqrt(1 - a_t)} of the walk, indexed by the DDIM index."""
         total_steps = timesteps.shape[0]
-        return np.stack([np.asarray(self.ddim_alphas.cpu() if isinstance(self.ddim_alphas, torch.Tensor) else self.ddim_alphas, dtype=np.float32)[:total_steps],
+        return np.stack([to_numpy(self.ddim_alphas, np.float32)[:total_steps],
                          np.asarray(self.ddim_alphas_prev, dtype=np.float32)[:total_steps],
                          sigmas.astype(np.float32)[:total_steps],
-                         np.asarray(self.ddim_sqrt_one_minus_alphas.cpu() if isinstance(self.ddim_sqrt_one_minus_alphas, torch.Tensor) else self.ddim_sqrt_one_minus_alphas, dtype=np.float32)[:total_steps]], axis=1)
+                         to_numpy(self.ddim_sqrt_one_minus_alphas, np.float32)[:total_steps]], axis=1)
 
-    def _update(self, st, e_u, e_c, scale, bs, cfg, noise, temperature):
-        """CFG mix + x_{t-1} from row st['idx'] of st['coef']: x_in[:bs] in place, its copy into x_in[bs:], pred_x0."""
-        _ops().ddim_cfg_step(e_u, e_c, st['x_in'][:bs], st['coef'], scale, x_prev=st['x_in'][:bs],
-                             x_prev_dup=st['x_in'][bs:] if cfg else None, pred_x0=st['pred_x0'], noise=noise,
-                             temperature=temperature, step_idx=st['idx'])
+    def _rings(self, bs, H, W, C):
+        """name -> shape of the sampling walk's extra persistent buffers (DPMSolverSampler's history ring)."""
+        return {}
+
+    def _update(self, w, e_u, e_c, scale, bs, cfg, noise, temperature):
+        """CFG mix + x_{t-1} from row w['idx'] of w['coef']: x_in[:bs] in place, its copy into x_in[bs:], pred_x0."""
+        _ops().ddim_cfg_step(e_u, e_c, w['x_in'][:bs], w['coef'], scale, x_prev=w['x_in'][:bs],
+                             x_prev_dup=w['x_in'][bs:] if cfg else None, pred_x0=w['pred_x0'], noise=noise, temperature=temperature,
+                             step_idx=w['idx'])
 
     def _graph_tag(self):
         """What else, besides the shapes and contexts, the captured step graph depends on."""
@@ -424,114 +485,6 @@ class DDIMSampler(object):
         buf[:, :L].copy_(c)
         return buf
 
-    def _state(self, bs, B, H, W, C, device):
-        key = (bs, B, H, W, C, str(device))
-        st = getattr(self, '_st', None)
-        if st is None or st['key'] != key:
-            st = {'key': key,
-                  'x_in': torch.zeros(B, H, W, C, dtype=torch.float32, device=device),
-                  'pred_x0': torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
-                  'coef': torch.zeros(1000, self._coef_cols, dtype=torch.float32, device=device),
-                  'ts': torch.zeros(1000, dtype=torch.int64, device=device),
-                  'idx': torch.zeros(1, dtype=torch.int32, device=device)}
-            self._st = st
-            self._graphs = {}
-        return st
-
-    def _inv_state(self, bs, B, H, W, C, slots, device):
-        """The inversion walk's own persistent buffers (so it never evicts the sampling graph) and its trajectory ring."""
-        key = (bs, B, H, W, C, slots, str(device))
-        st = getattr(self, '_inv_st', None)
-        if st is None or st['key'] != key:
-            st = {'key': key,
-                  'x_in': torch.zeros(B, H, W, C, dtype=torch.float32, device=device),
-                  'pred_x0': torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
-                  'coef': torch.zeros(1000, 4, dtype=torch.float32, device=device),
-                  'ts': torch.zeros(1000, dtype=torch.int64, device=device),
-                  'idx': torch.zeros(1, dtype=torch.int32, device=device),
-                  'ring': torch.zeros(slots, bs, H, W, C, dtype=torch.float32, device=device)}
-            self._inv_st = st
-            self._inv_graphs = {}
-        return st
-
-    def _inversion_blend_state(self, st, inv, mask, device):
-        """Refill the trajectory and mask buffers of st in place, so a cached step graph replays on a new inversion and mask ->
-        whether the mask is per item.  lib/model_zoo/edit.py specifies the semantics."""
-        ops = _ops()
-        bs, H, W = inv.bs, inv.shape[2], inv.shape[3]
-        traj = st.get('traj')
-        if traj is None or traj.shape[0] < inv.k or tuple(traj.shape[1:]) != tuple(inv.trajectory.shape[1:]):
-            st['traj'] = torch.zeros((max(inv.k, len(self.ddim_timesteps)),) + tuple(inv.trajectory.shape[1:]),
-                                     dtype=torch.float32, device=device)
-            self._graphs = {}           # a cached graph reads the old buffer
-        st['traj'][:inv.k].copy_(inv.trajectory[:inv.k])
-        if 'mask' not in st:
-            st['mask'] = torch.zeros(bs, H * W, dtype=torch.float32, device=device)
-        mask = mask.to(device=device, dtype=torch.float32).contiguous()
-        if mask.shape[-1] != W:
-            mask = ops.mask_to_latent(mask)
-        st['mask'][:mask.shape[0]].copy_(mask.view(mask.shape[0], H * W))
-        return int(mask.shape[0] != 1)
-
-    def _prompt_edit_state(self, st, ed, ci, ctxs, i, cfg, H, W, total_steps, device):
-        """Swap context i for its persistent extended buffer [context rows; edited contexts] and refill the edit's device state
-        in st in place, so a cached step graph replays on new prompts and tables -> the prompt_edit.EditState (also carried
-        by the context).  lib/model_zoo/prompt_edit.py specifies the semantics."""
-        from .attention import PaddedContext
-        from .prompt_edit import EditState, quarter
-        c = ci['c']
-        ext = torch.cat([c.float(), ed.edited_contexts(ci['conditioning']).to(c.device)])
-        buf = self._ctx_buffer(('prompt_edit', i), ext)
-        es = st.get('prompt_edit')
-        want = (ed.n, 2 * ed.n if cfg else ed.n, ext.shape[0], ed.has_beta, ed.blend is not None, quarter(H), quarter(W))
-        if es is None or es.key() != want:
-            es = EditState(ed.n, cfg, ext.shape[0], ed.has_beta, ed.blend is not None, quarter(H), quarter(W), device)
-            st['prompt_edit'] = es
-            self._graphs = {}           # a cached graph reads the old buffers
-        es.fill(ed, total_steps, cfg, st['idx'])
-        ctxs[i] = PaddedContext(buf, c.shape[1], edit=es)
-        return es
-
-    def _window_state(self, st, lay, per, bs, cfg, C, device):
-        """The persistent device state of a windowed walk in st (panorama.WindowState), its layout tables refilled in place, so a
-        cached step graph replays on new prompts or a new x_T.  lib/model_zoo/panorama.py specifies the semantics."""
-        from .panorama import WindowState
-        ws = st.get('windows')
-        if ws is None or ws.key != WindowState.key_for(lay, per, bs, cfg, C):
-            ws = WindowState(lay, per, bs, cfg, C, device)
-            st['windows'] = ws
-            self._graphs = {}           # a cached graph reads the old buffers
-        ws.fill(lay)
-        return ws
-
-    def _inpaint_state(self, st, x0, mask, seed, total_steps, x_T, bs, device):
-        """Refill the inpainting buffers of st in place, so a cached step graph replays on a new image, mask and seed ->
-        whether the mask is per item.  With x_T (the full walk) the kept region of x_in[:bs] becomes x0 noised to t_top with
-        x_T's own draw.  lib/model_zoo/inpaint.py specifies the semantics."""
-        from .inpaint import blend_table
-        ops = _ops()
-        _, H, W, C = st['x_in'].shape
-        if 'x0' not in st:
-            st.update(x0=torch.zeros(bs, H, W, C, dtype=torch.float32, device=device),
-                      mask=torch.zeros(bs, H * W, dtype=torch.float32, device=device),
-                      blend=torch.zeros(1000, 2, dtype=torch.float32, device=device),
-                      seed=torch.zeros(1, dtype=torch.int64, device=device))
-        st['x0'].copy_(ops.nchw_to_nhwc(x0.to(device=device, dtype=torch.float32).contiguous()))   # broadcasts a [1] batch
-        mask = mask.to(device=device, dtype=torch.float32).contiguous()
-        if mask.shape[-1] != W:
-            mask = ops.mask_to_latent(mask)
-        st['mask'][:mask.shape[0]].copy_(mask.view(mask.shape[0], H * W))
-        st['blend'][:total_steps].copy_(torch.from_numpy(blend_table(self.ddim_alphas_prev[:total_steps])))
-        st['seed'].copy_(seed)
-        mask_per_item = int(mask.shape[0] != 1)
-        if x_T is not None:
-            a_top = float(self.ddim_alphas[total_steps - 1])
-            row = torch.tensor([[np.sqrt(a_top), np.sqrt(1.0 - a_top)]], dtype=torch.float32, device=device)
-            ops.inpaint_blend(st['x_in'][:bs], st['x0'], st['mask'] if mask_per_item else st['mask'][:1], row,
-                              torch.zeros(1, dtype=torch.int32, device=device),
-                              noise=ops.nchw_to_nhwc(x_T.float().contiguous()))
-        return mask_per_item
-
     # ------------------------------------------------------------------ single-step API (reference parity)
     @torch.no_grad()
     def p_sample_ddim(self, x_info, c_info, t, index, repeat_noise=False, use_original_steps=False,
@@ -547,12 +500,7 @@ class DDIMSampler(object):
 
     def _p_sample(self, x_info, c_infos, multi, t, index, repeat_noise, use_original_steps, noise_dropout, temperature):
         """One eager DDIM step with the reference's argument conventions (ddim.py:129-171, 244-298)."""
-        if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
-            raise NotImplementedError("a prompt edit spans the walk (its windows and word maps): use sample / "
-                                      "sample_multicontext (lib/model_zoo/prompt_edit.py)")
-        if x_info.get('windows', None) is not None:
-            raise NotImplementedError("window fusion runs inside the sampler's walk: use sample / sample_multicontext "
-                                      "(lib/model_zoo/panorama.py)")
+        refuse('p_sample', x_info, c_infos)
         ops = _ops()
         model = self.model
         x = x_info['x']

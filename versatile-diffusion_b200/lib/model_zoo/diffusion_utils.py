@@ -53,6 +53,11 @@ def make_ddim_sampling_parameters(alphacums, ddim_timesteps, eta, verbose=True):
     return sigmas, alphas, alphas_prev
 
 
+def to_numpy(x, dtype=None):
+    """A tensor on any device, or anything np.asarray takes -> ndarray (of dtype when given)."""
+    return np.asarray(x.cpu() if isinstance(x, torch.Tensor) else x, dtype=dtype)
+
+
 def extract_into_tensor(a, t, x_shape):
     b, *_ = t.shape
     out = a.gather(-1, t)

@@ -34,9 +34,9 @@ Differences from DDIMSampler: eta != 0 raises ValueError (no stochastic variant)
 single-step form).  order in {1, 2, 3}; the default 2 is the paper's recommendation for guided sampling.
 """
 import numpy as np
-import torch
 
 from .ddim import DDIMSampler
+from .diffusion_utils import to_numpy
 
 
 def _ops():
@@ -57,8 +57,7 @@ def dpmpp_table(alphas_cumprod, timesteps, order):
     (the grid points actually visited: DDIM's ddim_timesteps, shortened by an img2img start)."""
     if order not in (1, 2, 3):
         raise ValueError(f"order must be 1, 2 or 3, got {order!r}")
-    ac = np.asarray(alphas_cumprod.cpu() if isinstance(alphas_cumprod, torch.Tensor) else alphas_cumprod,
-                    dtype=np.float32).astype(np.float64)
+    ac = to_numpy(alphas_cumprod, np.float32).astype(np.float64)
     ts = np.asarray(timesteps)
     n = ts.shape[0]
     alpha, sigma = np.sqrt(ac[ts]), np.sqrt(1.0 - ac[ts])
@@ -108,15 +107,12 @@ class DPMSolverSampler(DDIMSampler):
     def _coef_table(self, timesteps, sigmas):
         return dpmpp_table(self.model.alphas_cumprod, timesteps, self.order)
 
-    def _state(self, bs, B, H, W, C, device):
-        st = super()._state(bs, B, H, W, C, device)
-        if 'hist' not in st:
-            st['hist'] = torch.zeros(3 * bs * H * W * C, dtype=torch.float32, device=device)
-        return st
+    def _rings(self, bs, H, W, C):
+        return {'hist': (3 * bs * H * W * C,)}
 
-    def _update(self, st, e_u, e_c, scale, bs, cfg, noise, temperature):
-        _ops().dpmpp_cfg_step(e_u, e_c, st['x_in'][:bs], st['coef'], st['idx'], scale, st['hist'], x_next=st['x_in'][:bs],
-                              x_next_dup=st['x_in'][bs:] if cfg else None, pred_x0=st['pred_x0'])
+    def _update(self, w, e_u, e_c, scale, bs, cfg, noise, temperature):
+        _ops().dpmpp_cfg_step(e_u, e_c, w['x_in'][:bs], w['coef'], w['idx'], scale, w['hist'], x_next=w['x_in'][:bs],
+                              x_next_dup=w['x_in'][bs:] if cfg else None, pred_x0=w['pred_x0'])
 
     def _graph_tag(self):
         return ('dpmpp', self.order)

@@ -49,7 +49,8 @@ pure inversion-anchored regeneration), sample under tgt (a list: multi-context, 
 import numpy as np
 import torch
 
-from .diffusion_utils import make_ddim_timesteps
+from .ddim import SamplerMode, buffers_key, refuse
+from .diffusion_utils import make_ddim_timesteps, to_numpy
 
 
 def _ops():
@@ -74,8 +75,7 @@ class Inversion(object):
 
 def inversion_rows(alphas, alphas_prev, k):
     """fp32 [k, 4] rows {a'_i, a_i, 0, sqrt(1 - a'_i)} of inversion steps 0 ... k-1, built in fp64."""
-    a = np.asarray(alphas.cpu() if isinstance(alphas, torch.Tensor) else alphas, dtype=np.float64)[:k]
-    ap = np.asarray(alphas_prev.cpu() if isinstance(alphas_prev, torch.Tensor) else alphas_prev, dtype=np.float64)[:k]
+    a, ap = to_numpy(alphas, np.float64)[:k], to_numpy(alphas_prev, np.float64)[:k]
     return np.stack([ap, a, np.zeros_like(a), np.sqrt(1.0 - ap)], axis=1).astype(np.float32)
 
 
@@ -91,25 +91,46 @@ def check_invert_inputs(x0, bs, k, n):
     return k
 
 
-def check_sample_inputs(x_info, shape, timesteps):
-    """The host-side refusals of a sampling call from an inversion -> (inversion, mask or None).  Runs before any device work."""
-    inv = x_info['inversion']
-    if not isinstance(inv, Inversion):
-        raise ValueError(f"x_info['inversion']: expected an Inversion (DDIMSampler.invert), got {type(inv).__name__}")
-    for key in ('xt', 'x0', 'x0_forward_timesteps'):
-        if x_info.get(key, None) is not None:
-            raise ValueError(f"x_info['{key}'] cannot be given with 'inversion': the walk starts from the inversion")
-    if not np.array_equal(np.asarray(timesteps), inv.timesteps):
-        raise ValueError(f"the inversion was made with steps={inv.steps}: sample with the same steps")
-    if tuple(shape) != inv.shape:
-        raise ValueError(f"shape {list(shape)} differs from the inversion's {list(inv.shape)}")
-    mask = x_info.get('inpaint_mask', None)
-    if mask is not None:
-        from .inpaint import mask_resolution
-        mask_resolution(mask.shape, *inv.shape[:1], *inv.shape[2:])
-        if not bool(((mask >= 0) & (mask <= 1)).all()):
-            raise ValueError("inpaint_mask: values must lie in [0, 1]")
-    return inv, mask
+class FromInversion(SamplerMode):
+    """x_info['inversion'] in the sampler's walk: the start at slot k, and with an inpaint_mask the trajectory blend after every
+    step."""
+
+    def __init__(self, sampler, x_info, shape, c_infos):
+        """The host-side refusals of a sampling call from an inversion, before any device work."""
+        inv = self.inv = x_info['inversion']
+        if not isinstance(inv, Inversion):
+            raise ValueError(f"x_info['inversion']: expected an Inversion (DDIMSampler.invert), got {type(inv).__name__}")
+        refuse('inversion', x_info, c_infos)
+        if not np.array_equal(np.asarray(sampler.ddim_timesteps), inv.timesteps):
+            raise ValueError(f"the inversion was made with steps={inv.steps}: sample with the same steps")
+        if tuple(shape) != inv.shape:
+            raise ValueError(f"shape {list(shape)} differs from the inversion's {list(inv.shape)}")
+        self.mask = x_info.get('inpaint_mask', None)
+        if self.mask is not None:
+            from .inpaint import check_mask
+            check_mask(self.mask, *inv.shape[:1], *inv.shape[2:])
+
+    def start(self, sampler, x_info, shape, dtype, device):
+        return self.inv.xt.to(dtype).to(device), sampler.ddim_timesteps[:self.inv.k]
+
+    def prepare(self, sampler, run):
+        if self.mask is None:
+            return ()
+        from .inpaint import load_mask
+        inv = self.inv
+        st = run.walk
+        if 'traj' not in st or st['traj'].shape[0] < inv.k or st['traj'].shape[1:] != inv.trajectory.shape[1:]:
+            st['traj'] = torch.zeros((max(inv.k, len(sampler.ddim_timesteps)),) + tuple(inv.trajectory.shape[1:]),
+                                     dtype=torch.float32, device=run.device)
+        if 'mask' not in st:
+            st['mask'] = torch.zeros(run.bs, run.H * run.W, dtype=torch.float32, device=run.device)
+        st['traj'][:inv.k].copy_(inv.trajectory[:inv.k])
+        self.traj, self.mask_rows = st['traj'], load_mask(st['mask'], self.mask, run.W)
+        return ('inversion',) + buffers_key(self.traj, self.mask_rows)
+
+    def after_update(self, run):
+        if self.mask is not None:
+            _ops().inversion_blend(run.x, self.traj, self.mask_rows, run.walk['idx'], x_dup=run.x_dup)
 
 
 def context_batch(c_infos, scale):

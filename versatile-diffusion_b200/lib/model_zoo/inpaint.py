@@ -38,6 +38,9 @@ nothing changes: the same launches, the same bits, the same graph key.
 import numpy as np
 import torch
 
+from .ddim import SamplerMode, buffers_key
+from .diffusion_utils import to_numpy
+
 
 def _ops():
     from vdb200 import ops
@@ -56,29 +59,79 @@ def mask_resolution(mask_shape, bs, H, W):
                      f"got {s}")
 
 
-def check_inputs(x_info, shape):
-    """The host-side refusals of a masked call -> (x0, mask).  Runs before any device work."""
-    mask = x_info['inpaint_mask']
-    if len(shape) != 4:
-        raise ValueError(f"inpainting needs an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
-    x0 = x_info.get('x0', None)
-    if x0 is None:
-        raise ValueError("inpaint_mask needs x_info['x0'], the latent of the image to keep")
-    bs, C, H, W = shape
-    if x0.dim() != 4 or x0.shape[0] not in (1, bs) or tuple(x0.shape[1:]) != (C, H, W):
-        raise ValueError(f"x0: expected [{bs} or 1, {C}, {H}, {W}], got {tuple(x0.shape)}")
+def check_mask(mask, bs, H, W):
+    """The refusals of an inpaint_mask (also the mask of a walk from an inversion, lib/model_zoo/edit.py)."""
     mask_resolution(mask.shape, bs, H, W)
     if not bool(((mask >= 0) & (mask <= 1)).all()):
         raise ValueError("inpaint_mask: values must lie in [0, 1]")
-    return x0, mask
 
 
 def blend_table(alphas_prev):
     """fp32 [n, 2] rows {sqrt(a'), sqrt(1 - a')} in fp64 -> fp32, indexed by the grid index; row 0 is {1, 0}."""
-    a = np.asarray(alphas_prev.cpu() if isinstance(alphas_prev, torch.Tensor) else alphas_prev, dtype=np.float64)
+    a = to_numpy(alphas_prev, np.float64)
     t = np.stack([np.sqrt(a), np.sqrt(1.0 - a)], axis=1).astype(np.float32)
     t[0] = (1.0, 0.0)
     return t
+
+
+def load_mask(dst, mask, W):
+    """Copy a latent or pixel mask [n, 1, ., .] into rows 0 .. n-1 of the device buffer dst [bs, H * W] -> the rows a blend
+    reads: dst, or dst[:1] for one mask shared by every item."""
+    mask = mask.to(device=dst.device, dtype=torch.float32).contiguous()
+    if mask.shape[-1] != W:
+        mask = _ops().mask_to_latent(mask)
+    dst[:mask.shape[0]].copy_(mask.view(mask.shape[0], dst.shape[1]))
+    return dst if mask.shape[0] != 1 else dst[:1]
+
+
+class Inpainting(SamplerMode):
+    """x_info['inpaint_mask'] in the sampler's walk: the start of a full walk, and the blend after every step."""
+
+    def __init__(self, sampler, x_info, shape, c_infos):
+        """The host-side refusals of a masked call, before any device work."""
+        self.mask = x_info['inpaint_mask']
+        if len(shape) != 4:
+            raise ValueError(f"inpainting needs an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
+        self.x0 = x_info.get('x0', None)
+        if self.x0 is None:
+            raise ValueError("inpaint_mask needs x_info['x0'], the latent of the image to keep")
+        bs, C, H, W = shape
+        if self.x0.dim() != 4 or self.x0.shape[0] not in (1, bs) or tuple(self.x0.shape[1:]) != (C, H, W):
+            raise ValueError(f"x0: expected [{bs} or 1, {C}, {H}, {W}], got {tuple(self.x0.shape)}")
+        check_mask(self.mask, bs, H, W)
+        self.full_walk = x_info.get('x0_forward_timesteps', None) is None
+        # the Philox key, from torch's CPU generator; drawn only when a mask is given, after every refusal
+        self.seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64)
+
+    def start(self, sampler, x_info, shape, dtype, device):
+        if self.full_walk:      # a masked full walk starts from x_T as an unmasked one does, never from the img2img start
+            self.x_T, ts = sampler._initial_latent(shape, {k: v for k, v in x_info.items() if k != 'x0'}, dtype, device)
+            return self.x_T, ts
+        # the img2img start noises x0 row by row: a batch-1 x0 is noised once per item
+        return sampler._initial_latent(shape, dict(x_info, x0=self.x0.expand(shape[0], *self.x0.shape[1:])), dtype, device)
+
+    def prepare(self, sampler, run):
+        """With x_T (the full walk) the kept region of the latent becomes x0 noised to t_top with x_T's own draw."""
+        ops = _ops()
+        z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=run.device)
+        st = run.walk
+        if 'x0' not in st:
+            st.update(x0=z(run.bs, run.H, run.W, run.C), mask=z(run.bs, run.H * run.W), blend=z(1000, 2),
+                      seed=z(1, dtype=torch.int64))
+        st['x0'].copy_(ops.nchw_to_nhwc(self.x0.to(device=run.device, dtype=torch.float32).contiguous()))   # broadcasts [1]
+        self.mask_rows = load_mask(st['mask'], self.mask, run.W)
+        st['blend'][:run.total].copy_(torch.from_numpy(blend_table(sampler.ddim_alphas_prev[:run.total])))
+        st['seed'].copy_(self.seed)
+        if self.full_walk:
+            a_top = float(sampler.ddim_alphas[run.total - 1])
+            row = torch.tensor([[np.sqrt(a_top), np.sqrt(1.0 - a_top)]], dtype=torch.float32, device=run.device)
+            ops.inpaint_blend(run.x, st['x0'], self.mask_rows, row, torch.zeros(1, dtype=torch.int32, device=run.device),
+                              noise=ops.nchw_to_nhwc(self.x_T.float().contiguous()))
+        return ('inpaint',) + buffers_key(st['x0'], self.mask_rows, st['blend'], st['seed'])
+
+    def after_update(self, run):
+        w = run.walk
+        _ops().inpaint_blend(run.x, w['x0'], self.mask_rows, w['blend'], w['idx'], seed=w['seed'], x_dup=run.x_dup)
 
 
 def latent_mask(pixel_mask):

@@ -48,6 +48,14 @@ a 64x256 latent, and it grows quadratically with wider canvases.
 import numpy as np
 import torch
 
+from .ddim import SamplerMode, buffers_key, refuse
+
+
+def _ops():
+    from vdb200 import ops
+    return ops
+
+
 # Windows per UNet call.  A chunk's UNet batch is 2 * WINDOWS_PER_CHUNK * n under CFG; larger chunks amortise the per-call launch
 # overhead, smaller ones bound the activation memory on large canvases.  tools/panorama_bench.py, DPM-Solver++ 20 at 512x2048 and
 # stride 8 (25 windows), one NVIDIA H100 80GB HBM3 at a 700 W power limit: chunks of 1 / 4 / 8 / 13 / 25 windows take 149.3 /
@@ -146,27 +154,12 @@ def layout(windows, H, W):
     return Layout(windows, H, W)
 
 
-def check_sample_inputs(x_info, shape, c_infos):
-    """The host-side refusals of a windowed call -> Layout.  Runs before any device work."""
-    windows = x_info['windows']
-    if not isinstance(windows, Windows):
-        raise ValueError(f"x_info['windows'] must be a panorama.Windows, got {type(windows).__name__}")
-    if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
-        raise NotImplementedError("windows with prompt_edit: the edit's item tables index prompts, not windows "
-                                  "(lib/model_zoo/panorama.py)")
-    if x_info.get('inversion', None) is not None:
-        raise NotImplementedError("windows cannot sample from an inversion (lib/model_zoo/panorama.py)")
-    if len(shape) != 4:
-        raise ValueError(f"windows need an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
-    return layout(windows, shape[2], shape[3])
-
-
 class WindowState(object):
     """The device side of a windowed walk, persistent across calls so a captured step graph replays: the layout tables, the
     window batch of a full chunk ([u rows; c rows]) and the canvas eps [e_u; e_c]."""
 
     def __init__(self, lay, per, bs, cfg, C, device):
-        self.key = self.key_for(lay, per, bs, cfg, C)
+        self.key = lay.key() + (per, bs, cfg, C)
         tab, offs = lay.table()
         self.tables = torch.zeros(tab.size, dtype=torch.int32, device=device)
         for name, (o, n) in offs.items():
@@ -175,13 +168,52 @@ class WindowState(object):
         self.xw = torch.zeros(halves * min(per, lay.nwin) * bs, lay.h, lay.w, C, dtype=torch.float32, device=device)
         self.eps = torch.zeros(halves * bs, lay.H, lay.W, C, dtype=torch.float32, device=device)
 
-    @staticmethod
-    def key_for(lay, per, bs, cfg, C):
-        return lay.key() + (per, bs, cfg, C)
-
     def fill(self, lay):
         """refill the layout tables in place"""
         self.tables.copy_(torch.from_numpy(lay.table()[0]))
+
+
+class WindowFusion(SamplerMode):
+    """x_info['windows'] in the sampler's walk: the windowed eps in place of the UNet call on the canvas."""
+
+    def __init__(self, sampler, x_info, shape, c_infos):
+        """The host-side refusals of a windowed call, before any device work."""
+        if not isinstance(x_info['windows'], Windows):
+            raise ValueError(f"x_info['windows'] must be a panorama.Windows, got {type(x_info['windows']).__name__}")
+        refuse('windows', x_info, c_infos)
+        if len(shape) != 4:
+            raise ValueError(f"windows need an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
+        self.lay = layout(x_info['windows'], shape[2], shape[3])
+        self.per = WINDOWS_PER_CHUNK
+        self.chunks = self.lay.chunks(self.per)
+
+    def prepare(self, sampler, run):
+        """Refill the WindowState in place and the window contexts (each context row repeated per window), which become the
+        contexts whose K / V^T the step reads."""
+        lay, per = self.lay, self.per
+        ws = run.walk.get('windows')
+        if ws is None or ws.key != lay.key() + (per, run.bs, run.cfg, run.C):
+            ws = run.walk['windows'] = WindowState(lay, per, run.bs, run.cfg, run.C, run.device)
+        ws.fill(lay)
+        self.ws = ws
+        self.ctxs = {k: sampler._contexts(run.c_infos, run.cfg, run.x_type, run.multi, buffer_tag=('windows', k), repeat=k)[0]
+                     for k in sorted({k for _, k in self.chunks})}
+        run.kv_types = [ct for _ in self.ctxs for ct in run.c_types]
+        run.kv_ctxs = [c for k in self.ctxs for c in self.ctxs[k]]
+        return ('windows', lay.key(), per) + buffers_key(ws.tables, ws.xw, ws.eps)
+
+    def eps(self, sampler, run):
+        """gather -> UNet -> merge per chunk of windows, into the canvas eps [e_u; e_c]"""
+        ops, ws, lay, bs = _ops(), self.ws, self.lay, run.bs
+        halves = run.B // bs
+        t_emb = ops.timestep_embedding(run.walk['ts'], run.mch, step_idx=run.walk['idx'], batch=ws.xw.shape[0])
+        for first, k in self.chunks:
+            rows = k * bs
+            xw = ws.xw[:halves * rows]
+            ops.window_gather(run.x, ws.oy, ws.ox, lay.h, lay.w, first, k, out=xw[:rows], out_dup=xw[rows:] if run.cfg else None)
+            e = sampler.model.eps_nhwc(xw, run.x_type, t_emb[:xw.shape[0]], run.c_types, self.ctxs[k], run.ratios, run.time_from)
+            ops.window_merge(e, ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, ws.eps, halves=halves)
+        return ws.eps
 
 
 @torch.no_grad()

@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from .ddim import DDIMSampler
+from .diffusion_utils import to_numpy
 
 
 def _ops():
@@ -40,47 +41,22 @@ class PLMSSampler(DDIMSampler):
         self.invert()
 
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):
-        if x_info.get('inpaint_mask', None) is not None:
-            raise NotImplementedError("PLMSSampler has no inpainting: use DDIMSampler or DPMSolverSampler "
-                                      "(lib/model_zoo/inpaint.py)")
-        if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
-            raise NotImplementedError("PLMSSampler has no prompt editing: use DDIMSampler or DPMSolverSampler "
-                                      "(lib/model_zoo/prompt_edit.py)")
-        if x_info.get('windows', None) is not None:
-            raise NotImplementedError("PLMSSampler has no window fusion: use DDIMSampler or DPMSolverSampler "
-                                      "(lib/model_zoo/panorama.py)")
-        if x_info.get('inversion', None) is not None:
-            raise NotImplementedError("PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
-                                      "(lib/model_zoo/edit.py)")
+        self._modes('plms', x_info, shape, c_infos)
         ops = _ops()
         model = self.model
         device = torch.device(model.device)
         if device.type != 'cuda':
             raise RuntimeError("PLMSSampler: the H100 build has no CPU path (model.to('cuda') first)")
-        from .attention import PaddedContext
         dtype = c_infos[0]['conditioning'].dtype
         bs = shape[0]
         x, timesteps = self._initial_latent(shape, x_info, dtype, device)
         scale = float(c_infos[0]['unconditional_guidance_scale'])
         cfg = scale != 1.
         total = timesteps.shape[0]
-        ctxs = []
-        for i, ci in enumerate(c_infos):
-            c = torch.cat([ci['unconditional_conditioning'], ci['conditioning']]) if cfg else ci['conditioning']
-            ci['c'] = c
-            ctxs.append(PaddedContext(self._ctx_buffer(i, c), c.shape[1]))
-        c_types = [ci['type'] for ci in c_infos]
-        ratios = [float(ci.get('ratio', 1.0)) for ci in c_infos]
         x_type = x_info['type']
-        time_from = model.time_source(x_type, multi)
-        mch = model.diffuser[time_from].model_channels
+        ctxs, c_types, ratios, time_from, mch = self._contexts(c_infos, cfg, x_type, multi)
         B = 2 * bs if cfg else bs
-        alphas = np.asarray(self.ddim_alphas.cpu() if isinstance(self.ddim_alphas, torch.Tensor) else self.ddim_alphas, dtype=np.float32)
-        alphas_prev = np.asarray(self.ddim_alphas_prev, dtype=np.float32)
-        s1m = np.asarray(self.ddim_sqrt_one_minus_alphas.cpu() if isinstance(self.ddim_sqrt_one_minus_alphas, torch.Tensor)
-                         else self.ddim_sqrt_one_minus_alphas, dtype=np.float32)
-        coef = torch.tensor(np.stack([alphas, alphas_prev, np.zeros_like(alphas), s1m], 1)[:total], dtype=torch.float32,
-                            device=device).contiguous()
+        coef = torch.tensor(self._coef_table(timesteps, to_numpy(self.ddim_sigmas)), dtype=torch.float32, device=device)
         # identity coefficients turn vdb_ddim_cfg_step into a pure CFG mix: a_t = 1, a_prev = 1, sigma = 0,
         # sqrt(1-a_t) = -1  =>  pred_x0 = x + e  with x = 0, i.e. pred_x0 = e_u + s (e_c - e_u)
         ident = torch.tensor([[1.0, 1.0, 0.0, -1.0]], dtype=torch.float32, device=device)

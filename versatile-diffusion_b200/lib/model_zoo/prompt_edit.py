@@ -72,7 +72,14 @@ import math
 import numpy as np
 import torch
 
+from .ddim import SamplerMode, buffers_key, refuse
+
 L_MAX = 77
+
+
+def _ops():
+    from vdb200 import ops
+    return ops
 
 
 # ---------------------------------------------------------------------------------------------------- tokens and words
@@ -308,36 +315,6 @@ def reweight(tok, prompts, words, values, cross_steps=0.8, self_steps=0.4, blend
 
 
 # ---------------------------------------------------------------------------------------------------- sampler side
-def check_sample_inputs(x_info, shape, c_infos):
-    """Refuse what the edit does not support, before any device work -> (index of the context carrying the edit, PromptEdit)."""
-    carriers = [i for i, ci in enumerate(c_infos) if ci.get('prompt_edit', None) is not None]
-    if len(carriers) != 1:
-        raise ValueError(f"one context may carry 'prompt_edit', got {len(carriers)}")
-    i = carriers[0]
-    ed = c_infos[i]['prompt_edit']
-    if not isinstance(ed, PromptEdit):
-        raise ValueError(f"'prompt_edit' must be a PromptEdit, got {type(ed).__name__}")
-    for k in ('x0', 'inpaint_mask', 'inversion'):
-        if x_info.get(k, None) is not None:
-            raise ValueError(f"'prompt_edit' does not combine with {k!r}")
-    if len(shape) != 4 or x_info.get('type', 'image') != 'image':
-        raise ValueError("'prompt_edit' edits image latents [n, C, H, W]; a text latent cannot be edited")
-    if c_infos[i].get('type') != 'text':
-        raise ValueError(f"'prompt_edit' must ride on a text context, got {c_infos[i].get('type')!r}")
-    for ci in c_infos:
-        for k in ('conditioning', 'unconditional_conditioning'):
-            if ci.get(k, None) is not None and ci[k].shape[0] != ed.n:
-                raise ValueError(f"'prompt_edit' of {ed.n} prompts needs a {k} batch of {ed.n}, got {ci[k].shape[0]}")
-    if c_infos[i]['conditioning'].shape[1] != ed.L:
-        raise ValueError(f"'prompt_edit' tables of {ed.L} positions, the context has {c_infos[i]['conditioning'].shape[1]}")
-    if shape[0] != ed.n:
-        raise ValueError(f"'prompt_edit' of {ed.n} prompts needs a batch of {ed.n}, got {shape[0]}")
-    xt = x_info.get('xt', None)
-    if xt is not None and (xt.dim() != 4 or xt.shape[0] not in (1, ed.n) or tuple(xt.shape[1:]) != tuple(shape[1:])):
-        raise ValueError(f"'xt' must be [1 or {ed.n}, {', '.join(map(str, shape[1:]))}], got {tuple(xt.shape)}")
-    return i, ed
-
-
 def quarter(side):
     """The token side of the UNet level at 1/4 of the latent side (two stride-2 convolutions, each rounding up)."""
     return ((side + 1) // 2 + 1) // 2
@@ -348,6 +325,7 @@ class EditState(object):
     item tables, the step counter, the word weights and maps.  The sampler keeps it and refills it in place."""
 
     def __init__(self, n, cfg, ctx_batch, has_beta, blend, h4, w4, device):
+        self.args = (n, cfg, ctx_batch, has_beta, blend, h4, w4)
         self.n, self.c0, self.B = n, (n if cfg else 0), (2 * n if cfg else n)
         self.ctx_batch, self.has_beta, self.blend, self.h4, self.w4 = ctx_batch, has_beta, blend, h4, w4
         z = lambda *s: torch.zeros(*s, dtype=torch.int32, device=device)
@@ -356,9 +334,6 @@ class EditState(object):
         self.w = torch.zeros(n, L_MAX, dtype=torch.float32, device=device) if blend else None
         self.map = torch.zeros(n, h4 * w4, dtype=torch.float32, device=device) if blend else None
         self.idx, self.threshold = None, 0.3
-
-    def key(self):
-        return (self.n, self.B, self.ctx_batch, self.has_beta, self.blend, self.h4, self.w4)
 
     def fill(self, ed, T, cfg, idx):
         tabs = ed.tables(T, cfg)
@@ -378,3 +353,64 @@ class EditState(object):
 
     def maps_at(self, N):
         return self.blend and N == self.h4 * self.w4
+
+
+class PromptEditing(SamplerMode):
+    """A context's 'prompt_edit' in the sampler's walk: one start noise for every prompt, the edited context with its EditState,
+    and the local blend after every step."""
+
+    def __init__(self, sampler, x_info, shape, c_infos):
+        """Refuse what the edit does not support, before any device work."""
+        carriers = [i for i, ci in enumerate(c_infos) if ci.get('prompt_edit', None) is not None]
+        if len(carriers) != 1:
+            raise ValueError(f"one context may carry 'prompt_edit', got {len(carriers)}")
+        i = self.i = carriers[0]
+        ed = self.ed = c_infos[i]['prompt_edit']
+        if not isinstance(ed, PromptEdit):
+            raise ValueError(f"'prompt_edit' must be a PromptEdit, got {type(ed).__name__}")
+        refuse('prompt_edit', x_info, c_infos)
+        if len(shape) != 4 or x_info.get('type', 'image') != 'image':
+            raise ValueError("'prompt_edit' edits image latents [n, C, H, W]; a text latent cannot be edited")
+        if c_infos[i].get('type') != 'text':
+            raise ValueError(f"'prompt_edit' must ride on a text context, got {c_infos[i].get('type')!r}")
+        for ci in c_infos:
+            for k in ('conditioning', 'unconditional_conditioning'):
+                if ci.get(k, None) is not None and ci[k].shape[0] != ed.n:
+                    raise ValueError(f"'prompt_edit' of {ed.n} prompts needs a {k} batch of {ed.n}, got {ci[k].shape[0]}")
+        if c_infos[i]['conditioning'].shape[1] != ed.L:
+            raise ValueError(f"'prompt_edit' tables of {ed.L} positions, the context has {c_infos[i]['conditioning'].shape[1]}")
+        if shape[0] != ed.n:
+            raise ValueError(f"'prompt_edit' of {ed.n} prompts needs a batch of {ed.n}, got {shape[0]}")
+        xt = x_info.get('xt', None)
+        if xt is not None and (xt.dim() != 4 or xt.shape[0] not in (1, ed.n) or tuple(xt.shape[1:]) != tuple(shape[1:])):
+            raise ValueError(f"'xt' must be [1 or {ed.n}, {', '.join(map(str, shape[1:]))}], got {tuple(xt.shape)}")
+
+    def start(self, sampler, x_info, shape, dtype, device):
+        """every prompt starts from the same noise: one draw, or the given x_T, expanded to the n rows"""
+        xt = x_info.get('xt', None)
+        if xt is None:
+            xt = torch.randn([1] + list(shape[1:]), device=device, dtype=dtype)
+        return sampler._initial_latent(shape, dict(x_info, xt=xt.expand(list(shape))), dtype, device)
+
+    def prepare(self, sampler, run):
+        """Swap the edited context for its persistent extended buffer [context rows; edited contexts], which carries the
+        EditState, and refill that state in place."""
+        from .attention import PaddedContext
+        ed, i, cfg = self.ed, self.i, run.cfg
+        c = run.c_infos[i]['c']
+        ext = torch.cat([c.float(), ed.edited_contexts(run.c_infos[i]['conditioning']).to(c.device)])
+        buf = sampler._ctx_buffer(('prompt_edit', i), ext)
+        es = run.walk.get('prompt_edit')
+        args = (ed.n, cfg, ext.shape[0], ed.has_beta, ed.blend is not None, quarter(run.H), quarter(run.W))
+        if es is None or es.args != args:
+            es = run.walk['prompt_edit'] = EditState(*args, run.device)
+        es.fill(ed, run.total, cfg, run.walk['idx'])
+        run.ctxs[i] = PaddedContext(buf, c.shape[1], edit=es)
+        self.es = es
+        return ('prompt_edit', ed.n, ed.has_beta, es.blend, es.threshold) + buffers_key(es.cross, es.selfm, es.cross2, es.flags,
+                                                                                         es.w, es.map)
+
+    def after_update(self, run):
+        es = self.es
+        if es.blend:
+            _ops().local_blend(run.x, es.map, es.flags, run.walk['idx'], es.h4, es.w4, es.threshold, x_dup=run.x_dup)
