@@ -166,6 +166,9 @@ int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const 
 int vdb_igemm_last_plan(int* out, int n);
 /* The tile height BM (128 or 256 rows) of that same launch; 0 before the first one. */
 int vdb_igemm_last_bm(void);
+/* The order in which that same launch walked its output tiles: 0 = M tile index fastest, 1 = N tile index fastest (a single-pass
+ * launch with several N tiles whose A operand outweighs W, so that a wave reads each band of A rows once). */
+int vdb_igemm_last_n_fast(void);
 
 /* ---- the same GEMM with a LayerNorm folded in — BasicTransformerBlock norm1/2/3, attention.py:206-208,214-218 -------------
  * CONSUMER (ln_stats != NULL):  out = act( LN(x) W0^T + b0 )  computed from the RAW x without ever forming LN(x):

@@ -40,6 +40,11 @@ VDB_DEVINL void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2
   asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
                : "memory");
 }
+// ldmatrix: the inverse of stmatrix_x4 at the same addresses (four 8x8 b16 matrices into the accumulator-fragment layout)
+VDB_DEVINL void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr)
+               : "memory");
+}
 
 VDB_DEVINL uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));

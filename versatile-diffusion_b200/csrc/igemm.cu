@@ -46,6 +46,7 @@ struct alignas(64) IgemmParams {
   CUtensorMap tmA[kMaxA];  // 4D (C, W, H, B) bf16, box (64, TW, TH, TB), SWIZZLE_128B
   CUtensorMap tmB;         // 2D (Ktot, N) bf16, box (64, BN), SWIZZLE_128B
   CUtensorMap tmO;         // TMA-store epilogues: 4D (N, Wo, Ho, Bo) bf16 output, box (32, bw, bh, bb) = one warp's 16-row x 32-column chunk, SWIZZLE_64B
+  CUtensorMap tmR;         // modes 3 / 7 with a residual: tmO's geometry over resid / ldr (loaded into the staging boxes)
   ASeg seg[kMaxSeg];
   int nseg;
   int kb_total;      // total k-blocks over all segments
@@ -54,6 +55,7 @@ struct alignas(64) IgemmParams {
   int TW, TH, TB;    // M tile = TW*TH*TB = BM output pixels
   int Wo, Ho, Bo;    // output pixel grid (GEMM view: Wo = M, Ho = Bo = 1)
   int tilesW, tilesH, tilesB, tilesN;
+  int n_fast;        // tile walk: 0 = M tile index fastest, 1 = N tile index fastest (run_igemm decides; see igemm_kernel)
   int N;             // valid output columns (GEGLU: packed columns, output has N/2)
   // epilogue
   const float* bias;          // [bias_rows, N] fp32 or null
@@ -157,12 +159,18 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
   uint64_t* empty_bar = full_bar + STAGES;
   float* sbias = reinterpret_cast<float*>(empty_bar + STAGES);  // [BN] bias of the current output tile
   float* slnx = sbias + BN;                                   // [BN] LN modes: colsum s (on_cols 0) / column mean (on_cols 1)
+  uint64_t* rbar = reinterpret_cast<uint64_t*>(slnx + (kLnIn ? BN : 0));   // modes 3 / 7: [kNumEpiWarps][kBoxes] residual loads
   const uint32_t sbias_s = smem_u32(sbias), slnx_s = smem_u32(slnx);   // (shared-space addresses: LDS, not generic LD)
   (void)slnx_s;
   if constexpr (kLnIn) {
     if (reinterpret_cast<uint8_t*>(slnx + BN) > smem_raw + p.smem_bytes) __trap();
   }
   auto epi_bar_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNumEpiThreads) : "memory"); };   // the consumer warps only
+  // modes 3 / 7 TMA-load the residual of a chunk into the staging box the chunk is stored from (tmR); mode 0 reads it from
+  // global memory into registers (its accumulator leaves no registers for the box protocol), and split-K adds it in
+  // splitk_reduce_kernel
+  constexpr bool kResidTma = MODE == 3 || MODE == 7;
+  const bool resid_tma = kResidTma && p.resid != nullptr;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -171,20 +179,26 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
     for (int i = 0; i < kMaxA; ++i) tma_prefetch_desc(&p.tmA[i]);
     tma_prefetch_desc(&p.tmB);
     if (MODE != 0 || (!p.out_f32 && p.ksplit == 1)) tma_prefetch_desc(&p.tmO);   // (mode 0 builds it for bf16 output only)
+    if (resid_tma) tma_prefetch_desc(&p.tmR);
   }
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], kNumEpiWarps);
     }
+    if constexpr (kResidTma)
+      for (int i = 0; i < kNumEpiWarps * kBoxes; ++i) mbar_init(&rbar[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
 
   const int tilesM = p.tilesW * p.tilesH * p.tilesB;
-  const int unitsM = tilesM;
-  const int num_tiles = unitsM * p.tilesN * p.ksplit;
-  // Tile walk of this CTA (both roles use the same bounds): tiles c, c + grid, ..., with M as the fast tile index.
+  const int num_tiles = tilesM * p.tilesN * p.ksplit;
+  // Tile walk of this CTA (both roles use the same bounds and the same incremental arithmetic): tiles c, c + grid, ..., tile t =
+  // unit_f + units_f * unit_s.  M-fast (n_fast 0): unit_f = M tile, unit_s = N tile + tilesN * k-split.  N-fast (n_fast 1,
+  // ksplit 1 only): unit_f = N tile, unit_s = M tile, so a wave reads each band of A rows once, for all its N tiles together.
+  const int units_f = p.n_fast ? p.tilesN : tilesM;
+  const int step_f = gridDim.x % units_f, step_s = gridDim.x / units_f;
   const int t_first = blockIdx.x, t_step = gridDim.x, t_end = num_tiles;
 
   if (warp >= kNumEpiWarps) {
@@ -193,12 +207,11 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
     if (warp == kNumEpiWarps && lane == 0) {
       uint32_t stage = 0, phase = 0;
       const bool flat = (p.tilesH == 1) && (p.tilesB == 1);
-      const int step_m = t_step % unitsM, step_r = t_step / unitsM;
-      int unit_m = t_first % unitsM, rest = t_first / unitsM;
+      int unit_f = t_first % units_f, unit_s = t_first / units_f;
       for (int t = t_first; t < t_end; t += t_step) {
-        const int m_idx = unit_m;
-        int n_idx = rest, ks = 0;
-        if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
+        const int m_idx = p.n_fast ? unit_s : unit_f;
+        int n_idx = p.n_fast ? unit_f : unit_s, ks = 0;
+        if (p.ksplit > 1) { n_idx = unit_s % p.tilesN; ks = unit_s / p.tilesN; }
         int wt = m_idx, ht = 0, bt = 0;
         if (!flat) {
           wt = m_idx % p.tilesW;
@@ -206,8 +219,8 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
           ht = q % p.tilesH;
           bt = q / p.tilesH;
         }
-        unit_m += step_m; rest += step_r;
-        if (unit_m >= unitsM) { unit_m -= unitsM; ++rest; }
+        unit_f += step_f; unit_s += step_s;
+        if (unit_f >= units_f) { unit_f -= units_f; ++unit_s; }
         const int w0 = wt * p.TW, h0 = ht * p.TH, b0 = bt * p.TB;
         const int n0 = n_idx * BN;
         const int kb_begin = ks * p.kb_per_split;
@@ -237,7 +250,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
     // hb sits 8 KB after block hb - 1 in the stage)
     uint32_t ml_stage = 0, ml_phase = 0;
     float acc[kMB][BN / 2];
-    auto mainloop = [&](int kb_begin, int kb_end) {
+    auto mainloop = [&](int kb_begin, int kb_end, auto&& after_first_kblock) {
       const int g = warp >> 2;
 #pragma unroll
       for (int hb = 0; hb < kMB; ++hb)
@@ -257,6 +270,7 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
 #pragma unroll
           for (int hb = 0; hb < kMB; ++hb) wgmma_ss<BN>(acc[hb], adesc[hb] + 2 * k, bdesc + 2 * k, (kb > kb_begin || k > 0) ? 1u : 0u);
         wgmma_commit();
+        if (kb == kb_begin) after_first_kblock();
         if (kb > kb_begin) {            // the previous k-block's MMAs have read their stage: hand it back to the producer
           wgmma_wait<1>();
           __syncwarp();
@@ -272,12 +286,12 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
       if (lane == 0 && kb_end > kb_begin) mbar_arrive(&empty_bar[prev]);
     };
     int st_buf = 0;                     // which of this warp's kBoxes staging boxes is written next
+    uint32_t rphase = 0;                // modes 3 / 7, bit b: parity of the next residual load into box b
     const float* sbias_src = nullptr;   // which bias row/offset currently sits in sbias
     // The per-tile bookkeeping sits on the critical path of epilogue-bound GEMMs: the tile index advances incrementally (no
     // divisions in the GEMM view), row indices are 32-bit, and everything that depends only on the thread is hoisted.
     const bool flat = (p.tilesH == 1) && (p.tilesB == 1);   // GEMM view: M tiles along W only
-    const int step_m = t_step % unitsM, step_r = t_step / unitsM;
-    int unit_m = t_first % unitsM, rest = t_first / unitsM;
+    int unit_f = t_first % units_f, unit_s = t_first / units_f;
     // the accumulator stays in the wgmma fragment layout, so in each 64-row block hb of its warpgroup warp w
     // owns the 16 tile rows from e_row0 + 64 hb on (warpgroup w / 4, quarter w % 4) and this thread rows + lane / 4 and
     // + lane / 4 + 8 of them, at columns 8 j + 2 (lane % 4) + {0, 1}
@@ -306,12 +320,12 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
       }
     };
     if constexpr (kLnIn) {
-      if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t_first < t_end) ln_prefetch((t_first % unitsM) * kBlockM + e_row0 + (lane & 15));
+      if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t_first < t_end) ln_prefetch((p.n_fast ? unit_s : unit_f) * kBlockM + e_row0 + (lane & 15));
     }
     for (int t = t_first; t < t_end; t += t_step) {
-      const int m_idx = unit_m;
-      int n_idx = rest, ks = 0;
-      if (p.ksplit > 1) { n_idx = rest % p.tilesN; ks = rest / p.tilesN; }
+      const int m_idx = p.n_fast ? unit_s : unit_f;
+      int n_idx = p.n_fast ? unit_f : unit_s, ks = 0;
+      if (p.ksplit > 1) { n_idx = unit_s % p.tilesN; ks = unit_s / p.tilesN; }
       int wt = m_idx, ht = 0, bt = 0;
       if (!flat) {
         wt = m_idx % p.tilesW;
@@ -319,8 +333,8 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
         ht = q % p.tilesH;
         bt = q / p.tilesH;
       }
-      unit_m += step_m; rest += step_r;
-      if (unit_m >= unitsM) { unit_m -= unitsM; ++rest; }
+      unit_f += step_f; unit_s += step_s;
+      if (unit_f >= units_f) { unit_f -= units_f; ++unit_s; }
       const int gp_first = ((bt * p.TB) * p.Ho + ht * p.TH) * p.Wo + wt * p.TW;
       const int n0 = n_idx * BN;
 
@@ -362,8 +376,8 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
           sbias_src = key;
         }
       } else if (bias_uniform) {
-        // consecutive tiles of a CTA usually share the N tile (M is the fast tile index): reload only on change,
-        // otherwise the ~0.7 us global-load latency + two barriers sit between every two tiles
+        // consecutive tiles of a CTA often share the N tile (M-fast walks; N-fast ones whose grid is a multiple of tilesN):
+        // reload only on change, otherwise the ~0.7 us global-load latency + two barriers sit between every two tiles
         const float* brow = p.bias + (p.bias_bstride ? static_cast<long long>(gp_first / p.rows_per_batch) * p.bias_bstride : 0) + n0;
         if (brow != sbias_src) {              // uniform across the epilogue threads
           epi_bar_sync();                     // previous tile's readers are done with sbias
@@ -426,10 +440,34 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
             ln_a1[h] = __shfl_sync(0xffffffffu, rs, (lane >> 2) + 8 * h);
           }
         }
-        // request the next tile's row partials (GEMM view, M-fast order: unit_m already points at the next tile)
-        if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t + t_step < t_end) ln_prefetch(unit_m * kBlockM + e_row0 + (lane & 15));
+        // request the next tile's row partials (GEMM view: unit_f / unit_s already point at the next tile)
+        if (!p.ln_on_cols && p.ln_parts <= 2 * kLnPre && t + t_step < t_end)
+          ln_prefetch((p.n_fast ? unit_s : unit_f) * kBlockM + e_row0 + (lane & 15));
       }
-      mainloop(ks * p.kb_per_split, min(p.kb_total, ks * p.kb_per_split + p.kb_per_split));
+      // residual (modes 3 / 7, lane 0): chunk j = ochunks hb + c of this warp's chunks of the tile -> staging box `box`,
+      // completing on the box's mbarrier.  Rows and columns past the output are zero-filled.
+      auto resid_chunks = [&] { return min(BN / 32, (p.N - n_idx * BN + 31) / 32); };
+      auto req_resid = [&](int j, int box) {
+        const int och = resid_chunks();
+        const int hb = (kMB > 1 && j >= och) ? 1 : 0, c = j - hb * och;
+        const int b_row0 = e_row0 + 64 * hb;
+        uint64_t* bar = rbar + warp * kBoxes + box;
+        mbar_arrive_expect_tx(bar, 1024);
+        tma_load_4d(sstage + warp * kStgWarp + box * 1024, &p.tmR, bar, n_idx * BN + c * 32, wt * p.TW + (b_row0 % p.TW),
+                    ht * p.TH + ((b_row0 / p.TW) % p.TH), bt * p.TB + b_row0 / (p.TW * p.TH));
+      };
+      // the tile's first kBoxes boxes are requested under its mainloop, once the first k-block's products are issued, and once
+      // the stores of the previous tile have read them
+      mainloop(ks * p.kb_per_split, min(p.kb_total, ks * p.kb_per_split + p.kb_per_split), [&] {
+        if constexpr (kResidTma) {
+          if (resid_tma && lane == 0) {
+            bulk_wait_read<0>();
+            const int n = min(kBoxes, kMB * resid_chunks());
+            for (int j = 0; j < n; ++j) req_resid(j, (st_buf + j) & (kBoxes - 1));
+          }
+          __syncwarp();
+        }
+      });
 
       // ---- the epilogue, straight from the wgmma registers (no barrier between the warpgroups).  Each warp walks the 32-column
       // chunks of its 16 rows: per-element fp32 arithmetic on the thread's 2 rows x 8 columns of the chunk, bf16 pack, two
@@ -450,9 +488,13 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
       const int nvalid = (geglu ? p.N / 2 : p.N) - ocol0;               // output columns of this tile inside the output
       const int ochunks = geglu ? BN / 64 : min(BN / 32, (nvalid + 31) / 32);
       const int tq2 = 2 * (lane & 3);                                    // this thread's first column of every 8-column group
-      // residual (modes 0 / 3 / 7): the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each (mode 0:
-      // one 2-byte load for a pair that ends at N, none past it), requested a chunk ahead
-      const bool do_resid = (MODE == 3 || MODE == 7 || (MODE == 0 && !split && !geglu)) && p.resid != nullptr;
+      // residual, mode 0: the thread's 2 bf16 of row h and 8-column group jj of a chunk, one 4-byte load each (one 2-byte load
+      // for a pair that ends at N, none past it), requested a chunk ahead
+      const bool do_resid = MODE == 0 && !split && !geglu && p.resid != nullptr;
+      // stmatrix / ldmatrix x4 per 16 columns u of a box: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l
+      // addresses row l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
+      const int x4_row = ((lane >> 3) & 1) * 8 + (lane & 7);
+      auto x4_addr = [&](uint32_t box, int u) { return box + x4_row * 64 + (((2 * u + (lane >> 4)) ^ ((x4_row >> 1) & 3)) << 4); };
       const bool row_bias = MODE == 0 && p.bias && !bias_uniform && !split;   // a tile that one bias row does not cover
 #pragma unroll
       for (int hb = 0; hb < kMB; ++hb) {
@@ -570,7 +612,22 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
             alpha_act8(&o[0][0][0], p.alpha, p.act);
             alpha_act8(&o[2][0][0], p.alpha, p.act);
           }
-          if (do_resid) {
+          if (resid_tma) {
+            // the residual box of this chunk, read at the addresses the stmatrix below writes: it arrives in the fragment layout
+            mbar_wait(&rbar[warp * kBoxes + st_buf], (rphase >> st_buf) & 1u);
+            rphase ^= 1u << st_buf;
+            uint32_t rb[2][4];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) ldmatrix_x4(x4_addr(stg_s + st_buf * 1024, u), rb[0][2 * u], rb[1][2 * u], rb[0][2 * u + 1], rb[1][2 * u + 1]);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const float2 x = unpack_bf16x2(rb[h][jj]);
+                o[jj][h][0] = __fadd_rn(o[jj][h][0], x.x);
+                o[jj][h][1] = __fadd_rn(o[jj][h][1], x.y);
+              }
+          } else if (do_resid) {
             uint32_t rn[2][4];
             const bool more = c + 1 < ochunks;
             if (more) load_resid(c + 1, rn);
@@ -623,22 +680,23 @@ __global__ void __launch_bounds__(igemm_threads(BM, BN), 1) igemm_kernel(const _
             }
             continue;
           }
-          // the box about to be rewritten was handed to the TMA unit kBoxes - 1 chunks ago: wait until it has been read
-          if (lane == 0) bulk_wait_read<kBoxes - 1>();
+          if (resid_tma) {
+            // this box was refilled only once its previous store had read it.  The box of the previous chunk j - 1 takes the
+            // residual of chunk j - 1 + kBoxes, once the store of chunk j - 1 has read it
+            const int j = hb * ochunks + c;
+            if (lane == 0 && j >= 1 && j - 1 + kBoxes < kMB * ochunks) {
+              bulk_wait_read<0>();
+              req_resid(j - 1 + kBoxes, (st_buf + kBoxes - 1) & (kBoxes - 1));
+            }
+          } else if (lane == 0) {
+            bulk_wait_read<kBoxes - 1>();  // the box about to be rewritten was handed to the TMA unit kBoxes - 1 chunks ago
+          }
           __syncwarp();
           const uint32_t box = stg_s + st_buf * 1024;
-          {
-            // stmatrix x4 per 16 columns: matrix i = rows (i & 1) * 8 + 0..7 of 16-byte unit 2 u + i / 2; lane l addresses row
-            // l % 8 of matrix l / 8.  SWIZZLE_64B: unit q of box row rr sits at unit q ^ ((rr / 2) % 4)
-            const int mi = lane >> 3, brow = (mi & 1) * 8 + (lane & 7);
 #pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int unit = 2 * u + (mi >> 1);
-              stmatrix_x4(box + brow * 64 + ((unit ^ ((brow >> 1) & 3)) << 4),
-                          pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
-                          pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
-            }
-          }
+          for (int u = 0; u < 2; ++u)
+            stmatrix_x4(x4_addr(box, u), pack_bf16x2(o[2 * u][0][0], o[2 * u][0][1]), pack_bf16x2(o[2 * u][1][0], o[2 * u][1][1]),
+                        pack_bf16x2(o[2 * u + 1][0][0], o[2 * u + 1][0][1]), pack_bf16x2(o[2 * u + 1][1][0], o[2 * u + 1][1][1]));
           fence_proxy_async_smem();      // every writer: generic-proxy stores -> visible to the TMA (async proxy) read
           __syncwarp();
           if (lane == 0) {
@@ -710,7 +768,9 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, int kspl
 template <int BM, int BN, int STAGES, int MODE>
 static int launch_igemm(const IgemmParams& p0, int num_units, void* stream) {
   constexpr bool kLn = MODE == 5 || MODE == 6;       // one more [BN] fp32 table (colsum / column mean)
-  constexpr size_t need = STAGES * (BM + BN) * kBlockK * 2 + 2 * STAGES * 8 + BN * 4 + (kLn ? BN * 4 : 0) + kNumEpiWarps * igemm_boxes(BM) * 1024;   // (see igemm_kernel)
+  constexpr bool kResid = MODE == 3 || MODE == 7;     // one residual mbarrier per staging box
+  constexpr size_t need = STAGES * (BM + BN) * kBlockK * 2 + 2 * STAGES * 8 + BN * 4 + (kLn ? BN * 4 : 0) +
+                          kNumEpiWarps * igemm_boxes(BM) * (1024 + (kResid ? 8 : 0));   // (see igemm_kernel)
   // + up to 1024 bytes of slack for the 1024-byte alignment of the operand ring (the LN modes at BN 256 may get less: the dynamic
   // window starts 1024-aligned in practice, and the kernel traps if its carve-up would not fit)
   constexpr size_t smem = (need + 1024 <= 227 * 1024) ? need + 1024 : 227 * 1024;
@@ -745,6 +805,7 @@ static int pick_bn(int N, int act, int forced) {
 constexpr int kPlanFields = 7;
 static thread_local int g_last_plan[kPlanFields] = {0};
 static thread_local int g_last_bm = 0;
+static thread_local int g_last_n_fast = 0;     // and its tile walk (vdb_igemm_last_n_fast)
 
 // bf16 output leaves through a TMA output map (16-byte aligned base and row stride), the split-K reduction stores fp32 rows as
 // float4 and the fp32 epilogue column pairs as float2, so out / resid must be 16-byte aligned.  Checked before any tensor map is
@@ -911,6 +972,21 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
                         static_cast<uint64_t>(ldw) * 2, kBlockK, BN);
   if (rc) return rc;
   const int num_tiles = mn_tiles * p.ksplit;
+  // Tile walk.  M-fast, the CTAs of a wave share a few N tiles and read a band of A rows per N tile; when A is the larger
+  // operand that band has usually left the L2 before the next N tile of the same rows comes round (ff-down at 64x64: 84 MB of A,
+  // two N tiles two waves apart), so A is read from HBM once per N tile.  N-fast, a wave takes every N tile of its rows together
+  // and A is read once; W, the smaller operand, is the one re-read.  A's bytes: output pixels times the channels of every A map
+  // (the pixels of a stride-2 conv's four parity maps add up to the input's).
+  {
+    long long a_chan = 0;
+    for (int m = 0; m < kMaxA; ++m) {
+      int c = 0;
+      for (int s = 0; s < p.nseg; ++s)
+        if (p.seg[s].tmap == m) c = std::max(c, p.seg[s].c0 + p.seg[s].nkb * kBlockK);
+      a_chan += c;
+    }
+    p.n_fast = p.ksplit == 1 && p.tilesN > 1 && M * a_chan > N * Ktot;
+  }
   // epilogue specialisation (see igemm_kernel): 3 = plain bf16 fast path, 4 = GEGLU, 0 = everything else
   int mode = 0;
   if (p.ksplit == 1 && !e.out_f32 && one_bias_row(p, BM, e)) {
@@ -947,6 +1023,15 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     if (ln_in && mode == 4 && e.ln_on_cols) return set_error(VDB_ERR_UNSUPPORTED, "igemm: GEGLU with column statistics");
     mode = st_out ? 7 : mode + 2;
   }
+  if (e.resid && (mode == 3 || mode == 7)) {
+    // the residual enters through the staging boxes: the output map's geometry over resid / ldr (the interleaved-output upsample
+    // modes take no residual)
+    const int bw = std::min(p.TW, 16), bh = std::min(p.TH, 16 / bw), bb = 16 / (bw * bh);
+    rc = make_tmap_4d_sw64(&p.tmR, e.resid, static_cast<uint64_t>(N), static_cast<uint64_t>(p.Wo), static_cast<uint64_t>(p.Ho),
+                           static_cast<uint64_t>(p.Bo), static_cast<uint64_t>(e.ldr) * 2, static_cast<uint64_t>(p.Wo) * e.ldr * 2,
+                           static_cast<uint64_t>(p.Ho) * p.Wo * e.ldr * 2, 32, bw, bh, bb);
+    if (rc) return rc;
+  }
   if (BM == 256 && mode != 3 && mode != 7)
     return set_error(VDB_ERR_UNSUPPORTED, "igemm: the 256-row tile needs the plain TMA-store epilogue (bf16 out, no activation, alpha 1, "
                                           "N %% 32 == 0, one bias row per tile, no split-K, no LayerNorm input)");
@@ -955,6 +1040,7 @@ static int run_igemm(IgemmParams& p, const void* Wt, long long N, long long Ktot
     const int plan[kPlanFields] = {BN, stages, mode, p.ksplit, std::min(num_tiles, num_sms()), tilesM, p.tilesN};
     for (int i = 0; i < kPlanFields; ++i) g_last_plan[i] = plan[i];
     g_last_bm = BM;
+    g_last_n_fast = p.n_fast;
   }
   if (BM == 256) {
     rc = mode == 7 ? launch_igemm<256, 160, 4, 7>(p, num_tiles, stream) : launch_igemm<256, 160, 4, 3>(p, num_tiles, stream);
@@ -1016,6 +1102,9 @@ int vdb_igemm_last_plan(int* out, int n) {
 
 // see include/vdb200.h
 int vdb_igemm_last_bm(void) { return g_last_bm; }
+
+// see include/vdb200.h
+int vdb_igemm_last_n_fast(void) { return g_last_n_fast; }
 
 // out[M,N] = act(alpha * ([A | A2] @ W^T + bias)) + resid     (see include/vdb200.h)
 int vdb_gemm_bf16(const void* A, long long M, long long K, long long lda, const void* A2, long long K2,

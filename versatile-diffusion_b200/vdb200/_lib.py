@@ -44,6 +44,7 @@ SIGNATURES = {
     "vdb_gemm_bf16": (i, [p, ll, ll, ll, p, ll, ll, p, ll, ll, p, ll, ll, p, ll, p, ll, i, i, f, i, i, p, sz, p]),
     "vdb_igemm_last_plan": (i, [C.POINTER(i), i]),
     "vdb_igemm_last_bm": (i, []),
+    "vdb_igemm_last_n_fast": (i, []),
     "vdb_gemm_ln_bf16":(i, [p, ll, ll, ll, p, ll, ll, p, p, ll, p, ll, i, p, ll, i, i, f, p, i, p, p, p, i, p]),
     "vdb_conv3x3_bf16": (i, [p, i, i, i, i, i, p, i, ll, p, i, p, i, p, ll, p, ll, p, ll, i, i, i, i, p, sz, p]),
     "vdb_attention_dk_pad": (i, [i]),

@@ -377,17 +377,17 @@ def gemm(a, w, bias=None, resid=None, out=None, act=ACT_NONE, a2=None, out_dtype
     return out
 
 
-IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n", "bm")   # (bm: vdb_igemm_last_bm)
+IGEMM_PLAN_FIELDS = ("bn", "stages", "mode", "ksplit", "grid", "tiles_m", "tiles_n", "bm", "n_fast")   # (bm, n_fast: their own accessors)
 BM256 = 0x1000      # VDB_IGEMM_BM256: bn=160 | BM256 forces the 256-row tile of gemm / gemm_ln / conv3x3
 
 
 def igemm_last_plan():
     """The tiling of the last gemm / gemm_ln / conv3x3 launch on this thread (vdb_igemm_last_plan): which kernel instantiation
-    (BM, BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile counts."""
-    buf = (ctypes.c_int * (len(IGEMM_PLAN_FIELDS) - 1))()
+    (BM, BN, STAGES, epilogue MODE) ran, with its split-K factor, grid and tile counts, and whether it walked its tiles N-fast."""
+    buf = (ctypes.c_int * (len(IGEMM_PLAN_FIELDS) - 2))()
     n = lib.vdb_igemm_last_plan(buf, len(buf))
     assert n == len(buf), n
-    return dict(zip(IGEMM_PLAN_FIELDS, list(buf) + [lib.vdb_igemm_last_bm()]))
+    return dict(zip(IGEMM_PLAN_FIELDS, list(buf) + [lib.vdb_igemm_last_bm(), lib.vdb_igemm_last_n_fast()]))
 
 
 class LnFold(object):
