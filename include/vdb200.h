@@ -136,6 +136,38 @@ int vdb_window_gather_f32(const float* x, int bs, int H, int W, int C, const int
 int vdb_window_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox,
                          const int* cover_y, const int* cover_x, int ny, int nx, int h, int w, int first, int k, float* out,
                          void* stream);
+/* ---- region prompts: MultiDiffusion region-based generation — lib/model_zoo/regions.py (an addition: the reference has no region
+ * mode; the weights, the merge and the bootstrapping are specified in that module's docstring) ---------------------------------------
+ * On the window layout and tables of the panorama entry points (one window equal to the canvas when no windows are asked for).
+ * masks: fp32 [R, bs, H, W] on the canvas, region r = 1..R at row r - 1, values in [0, 1]; 1 <= R <= 8.  Region 0 is the
+ * background, of weight m_0 = max(0, 1 - S) with S = m_1 + ... + m_R summed in ascending r, and D = m_0 + S (fp32, rounded).
+ * vdb_region_gather_f32: out = u_blocks + R + 1 blocks of [k*bs, h, w, C], u_blocks in {0, 1, R + 1}; block blk is region
+ * blk - u_blocks of the c half, region 0 for the single u block, region blk for one of R + 1 u blocks; row j*bs + b of a block is
+ * window first + j of image b.  Every block is an exact copy of the window (as vdb_window_gather_f32) unless rows is non-NULL and
+ * row *step_idx of rows (fp32 {on, a, b, 0}) has on != 0: then region r >= 1 reads, per element of mask value m,
+ * m == 1 ? x : m == 0 ? k : m*x + (1 - m)*k  with  k = a*bg + b*z  (fp32, round-to-nearest), bg = row floor(w*nb / 2^32) of the
+ * backgrounds bg fp32 [nb, C], w the first word of Philox4x32-10 at counter ((r*bs + b), *step_idx, 0x72676e73 "rgns", 1) under the
+ * key *seed, and z = noise (fp32 NHWC canvas) when non-NULL, else the canvas element's normal at counter (element quad, *step_idx,
+ * "rgns", 0) by the Box-Muller of vdb_inpaint_blend_f32.  VDB_ERR_INVALID before any launch: the window gather's refusals, R
+ * outside [1, 8], u_blocks not 0, 1 or R + 1, rows without masks / step_idx / seed / nb > 0 backgrounds, x / out / noise not
+ * 16-byte aligned, masks / rows / bg / step_idx not 4-byte, seed not 8-byte, or out overlapping x, masks, noise or bg.
+ * vdb_region_noise_f32: the gather's draws of step *step_idx: z [n] for canvas elements [0, n), picks int32 [R*bs], entry
+ * (r - 1)*bs + b the background row of region r, image b.
+ * vdb_region_merge_f32: eps [halves*(R+1)*k*bs, h, w, C], block s*(R+1) + r (halves 1, or 2 for [u blocks; c blocks]) -> out
+ * [halves*bs, H, W, C].  Per element, over its covering windows in ascending window index and r = 0..R inside each, fp32 with
+ * round-to-nearest: each term m_r*e of nonzero weight (a zero weight is skipped) is one product; the first sets out, later ones
+ * are added, and the call whose range holds the last window divides by n*D (n covering windows, the product rounded).  Elements
+ * with no covering window in the range are not touched, so calls over consecutive ranges equal one call; a hard mask selects its
+ * region's eps bit for bit.  No atomics.  VDB_ERR_INVALID before any launch: the window merge's refusals, a null masks, R outside
+ * [1, 8], masks not 4-byte aligned, or eps or masks overlapping out. */
+int vdb_region_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
+                          int first, int k, int R, int u_blocks, const float* masks, const float* rows, const int* step_idx,
+                          const unsigned long long* seed, const float* bg, int nb, const float* noise, float* out, void* stream);
+int vdb_region_noise_f32(const unsigned long long* seed, const int* step_idx, long long n, int R, int bs, int nb, float* z, int* picks,
+                         void* stream);
+int vdb_region_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox, const int* cover_y,
+                         const int* cover_x, int ny, int nx, int h, int w, int first, int k, int R, const float* masks, float* out,
+                         void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */

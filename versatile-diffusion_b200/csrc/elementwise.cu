@@ -164,10 +164,10 @@ __device__ __forceinline__ float mask_blend(float m, float x, float k) {
   return m == 1.f ? x : m == 0.f ? k : __fadd_rn(__fmul_rn(m, x), __fmul_rn(__fsub_rn(1.f, m), k));
 }
 
-// Four standard normals of counter (quad, step, "inpt", 0) under a 64-bit key: two Box-Muller pairs, u = (b + 0.5) 2^-32 in
+// Four standard normals of counter (quad, step, tag, 0) under a 64-bit key: two Box-Muller pairs, u = (b + 0.5) 2^-32 in
 // fp64 (never 0 or 1), (r cos 2 pi u', r sin 2 pi u') with r = sqrt(-2 ln u), rounded to fp32.
-__device__ __forceinline__ void inpaint_normals(unsigned long long key, unsigned quad, int step, float z[4]) {
-  const uint4 b = curand_Philox4x32_10(make_uint4(quad, static_cast<unsigned>(step), kInpaintTag, 0u),
+__device__ __forceinline__ void philox_normals(unsigned long long key, unsigned quad, int step, unsigned tag, float z[4]) {
+  const uint4 b = curand_Philox4x32_10(make_uint4(quad, static_cast<unsigned>(step), tag, 0u),
                                        make_uint2(static_cast<unsigned>(key), static_cast<unsigned>(key >> 32)));
   const unsigned w[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -180,6 +180,10 @@ __device__ __forceinline__ void inpaint_normals(unsigned long long key, unsigned
     z[2 * p] = static_cast<float>(r * c);
     z[2 * p + 1] = static_cast<float>(r * s);
   }
+}
+
+__device__ __forceinline__ void inpaint_normals(unsigned long long key, unsigned quad, int step, float z[4]) {
+  philox_normals(key, quad, step, kInpaintTag, z);
 }
 
 // x, x0, noise: fp32 NHWC [bs, hw, c] flattened to n = bs*hw*c; mask [bs | 1, hw], broadcast over c.  Element quad i/4 draws
@@ -532,6 +536,185 @@ __global__ void window_merge_kernel(const float* __restrict__ eps, int bs, int H
       const float n = static_cast<float>((y1 - y0) * ((cx.y - cx.x) + (cx.w - cx.z)));
 #pragma unroll
       for (int q = 0; q < VW; ++q) acc[q] = __fdiv_rn(acc[q], n);
+    }
+    if (VW == 4) *reinterpret_cast<float4*>(o) = *reinterpret_cast<float4*>(acc);
+    else o[0] = acc[0];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// MultiDiffusion region prompts (lib/model_zoo/regions.py), on the window layout above.  masks fp32 [R, bs, H, W] on the canvas,
+// region r >= 1 at row r - 1; region 0 is the background, of weight m_0 = max(0, 1 - S), S = m_1 + ... + m_R.  A chunk's UNet
+// batch is ub + R + 1 blocks of [k*bs, h, w, C]: ub u blocks (0; 1, region 0's; or R + 1, one per region), then the R + 1 c
+// blocks, region r at c block r.  Row j*bs + b of a block is window first + j of image b.
+// ---------------------------------------------------------------------------------------------
+constexpr unsigned kRegionTag = 0x72676e73u;   // "rgns"
+constexpr int kRegionsMax = 8;
+
+// the background entry of region r >= 1, image b at step `step`: floor(w nb / 2^32), w the first word at counter
+// (r*bs + b, step, "rgns", 1)
+__device__ __forceinline__ int region_pick(unsigned long long key, int r, int b, int bs, int step, int nb) {
+  const uint4 v = curand_Philox4x32_10(make_uint4(static_cast<unsigned>(r * bs + b), static_cast<unsigned>(step), kRegionTag, 1u),
+                                       make_uint2(static_cast<unsigned>(key), static_cast<unsigned>(key >> 32)));
+  return static_cast<int>((static_cast<unsigned long long>(v.x) * static_cast<unsigned>(nb)) >> 32);
+}
+
+// canvas x -> the chunk's batch out.  Block 0 of each half, and every block while the step's flag is off (or rows is NULL), is an
+// exact copy.  While it is on (row *step_idx of rows {on, a, b, 0}), region r >= 1 reads m x + (1 - m) (a bg + b z): the exact
+// selects of mask_blend, k = a*bg + b*z rounded as the inpainting blend's.  z: noise (canvas NHWC) when given, else four normals
+// per canvas element quad at counter (quad, step, "rgns", 0); bg: row region_pick of the backgrounds [nb, C].
+template <int VW>
+__global__ void region_gather_kernel(const float* __restrict__ x, int bs, int H, int W, int C, const int* __restrict__ oy,
+                                     const int* __restrict__ ox, int nx, int h, int w, int first, int k, int ub,
+                                     const float* __restrict__ masks, const float* __restrict__ rows,
+                                     const int* __restrict__ step_idx, const unsigned long long* __restrict__ seed,
+                                     const float* __restrict__ bg, int nb, const float* __restrict__ noise, long long total,
+                                     float* __restrict__ out) {
+  int idx = 0;
+  bool on = false;
+  float a = 0.f, bz = 0.f;
+  if (rows) {
+    idx = *step_idx;
+    on = rows[4 * idx] != 0.f;
+    a = rows[4 * idx + 1];
+    bz = rows[4 * idx + 2];
+  }
+  const unsigned long long key = on ? *seed : 0ull;
+  const int cv = C / VW;
+  const int kb = k * bs;
+  const long long plane = static_cast<long long>(bs) * H * W;
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(e % cv) * VW;
+    long long p = e / cv;
+    const int wx = static_cast<int>(p % w);
+    p /= w;
+    const int wy = static_cast<int>(p % h);
+    const long long row = p / h;
+    const int blk = static_cast<int>(row / kb), rb = static_cast<int>(row % kb);
+    const int b = rb % bs, g = first + rb / bs;
+    const int r = blk < ub ? (ub == 1 ? 0 : blk) : blk - ub;
+    int sx = ox[g % nx] + wx;
+    if (sx >= W) sx -= W;
+    const long long pix = (static_cast<long long>(b) * H + oy[g / nx] + wy) * W + sx;
+    const long long src = pix * C + c;
+    float v[VW];
+    if (VW == 4) *reinterpret_cast<float4*>(v) = __ldg(reinterpret_cast<const float4*>(x + src));
+    else v[0] = __ldg(x + src);
+    if (on && r > 0) {
+      const float m = __ldg(masks + (r - 1) * plane + pix);
+      if (m != 1.f) {
+        const float* bgr = bg + static_cast<long long>(region_pick(key, r, b, bs, idx, nb)) * C + c;
+        float z[4];
+        if (noise) {
+          if (VW == 4) *reinterpret_cast<float4*>(z) = __ldg(reinterpret_cast<const float4*>(noise + src));
+          else z[0] = __ldg(noise + src);
+        } else {
+          philox_normals(key, static_cast<unsigned>(src >> 2), idx, kRegionTag, z);
+          if (VW == 1) {    // the element's lane of its quad, selected without indexing the array by a runtime value
+            const int lane = static_cast<int>(src & 3);
+            z[0] = lane == 0 ? z[0] : lane == 1 ? z[1] : lane == 2 ? z[2] : z[3];
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < VW; ++q) {       // VW == 4: src is a multiple of 4, so lane q is element src + q
+          const float kq = __fadd_rn(__fmul_rn(a, __ldg(bgr + q)), __fmul_rn(bz, z[q]));
+          v[q] = mask_blend(m, v[q], kq);
+        }
+      }
+    }
+    if (VW == 4) *reinterpret_cast<float4*>(out + e * 4) = *reinterpret_cast<float4*>(v);
+    else out[e] = v[0];
+  }
+}
+
+// the gather's draws of step *step_idx: z for canvas elements [0, n), and picks[(r - 1)*bs + b] for r = 1..R
+__global__ void region_noise_kernel(const unsigned long long* __restrict__ seed, const int* __restrict__ step_idx, long long n,
+                                    int R, int bs, int nb, float* __restrict__ z, int* __restrict__ picks) {
+  const unsigned long long key = *seed;
+  const int idx = *step_idx;
+  const long long quads = (n + 3) / 4;
+  const long long total = quads > static_cast<long long>(R) * bs ? quads : static_cast<long long>(R) * bs;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    if (i < quads) {
+      float v[4];
+      philox_normals(key, static_cast<unsigned>(i), idx, kRegionTag, v);
+      for (int q = 0; q < 4; ++q)
+        if (4 * i + q < n) z[4 * i + q] = v[q];
+    }
+    if (i < static_cast<long long>(R) * bs)
+      picks[i] = region_pick(key, static_cast<int>(i / bs) + 1, static_cast<int>(i % bs), bs, idx, nb);
+  }
+}
+
+// The weighted merge of windows [first, first+k): eps [halves*(R+1)*k*bs, h, w, C], block s*(R+1) + r; out [halves*bs, H, W, C].
+// Per element p: S = m_1 + ... + m_R (ascending, rounded), m_0 = max(0, 1 - S), D = m_0 + S.  Over its covering windows in
+// ascending index, and r = 0..R inside each, every term m_r e_{j,r} of nonzero weight is one rounded product: the first sets out,
+// later ones are added; the launch holding the last window divides once by n D.  As window_merge_kernel, calls over consecutive
+// ranges make the same operations as one call.  Some weight is nonzero at every element (D >= 1 - 2^-24), so every covering window
+// adds at least one term.
+template <int VW>
+__global__ void region_merge_kernel(const float* __restrict__ eps, int bs, int H, int W, int C, const int* __restrict__ oy,
+                                    const int* __restrict__ ox, const int* __restrict__ cover_y, const int* __restrict__ cover_x,
+                                    int nx, int h, int w, int first, int k, int R, const float* __restrict__ masks, long long total,
+                                    float* __restrict__ out) {
+  const int cv = C / VW;
+  const int last = first + k;
+  const long long plane = static_cast<long long>(h) * w * C, mplane = static_cast<long long>(bs) * H * W;
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
+       e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(e % cv) * VW;
+    long long p = e / cv;
+    const int x = static_cast<int>(p % W);
+    p /= W;
+    const int y = static_cast<int>(p % H);
+    const long long ob = p / H;                               // output row s*bs + b
+    const int s = static_cast<int>(ob / bs), b = static_cast<int>(ob % bs);
+    const int y0 = cover_y[2 * y], y1 = cover_y[2 * y + 1];
+    const int4 cx = *reinterpret_cast<const int4*>(cover_x + 4 * x);
+    const int xlo = cx.y > cx.x ? cx.x : cx.z, xhi = cx.w > cx.z ? cx.w - 1 : cx.y - 1;
+    const int g_first = y0 * nx + xlo, g_last = (y1 - 1) * nx + xhi;
+    if (g_last < first || g_first >= last) continue;          // no covering window in this range
+    const float* mp = masks + (static_cast<long long>(b) * H + y) * W + x;
+    float S = __ldg(mp);
+    for (int r = 2; r <= R; ++r) S = __fadd_rn(S, __ldg(mp + (r - 1) * mplane));
+    const float m0 = fmaxf(0.f, __fsub_rn(1.f, S));
+    float acc[VW];
+    float* o = out + ((ob * H + y) * W + x) * C + c;
+    bool started = g_first < first;
+    if (started) {
+      if (VW == 4) *reinterpret_cast<float4*>(acc) = *reinterpret_cast<const float4*>(o);
+      else acc[0] = o[0];
+    }
+    for (int iy = y0; iy < y1; ++iy) {
+      const int wy = y - oy[iy];
+      for (int part = 0; part < 2; ++part) {
+        const int a0 = part ? cx.z : cx.x, a1 = part ? cx.w : cx.y;
+        for (int ix = a0; ix < a1; ++ix) {
+          const int g = iy * nx + ix;
+          if (g < first || g >= last) continue;
+          int wx = x - ox[ix];
+          if (wx < 0) wx += W;
+          const float* src = eps + ((static_cast<long long>(s) * (R + 1) * k + (g - first)) * bs + b) * plane +
+                             (static_cast<long long>(wy) * w + wx) * C + c;
+          for (int r = 0; r <= R; ++r, src += k * bs * plane) {
+            const float m = r == 0 ? m0 : __ldg(mp + (r - 1) * mplane);
+            if (m == 0.f) continue;
+            float v[VW];
+            if (VW == 4) *reinterpret_cast<float4*>(v) = __ldg(reinterpret_cast<const float4*>(src));
+            else v[0] = __ldg(src);
+#pragma unroll
+            for (int q = 0; q < VW; ++q) acc[q] = started ? __fadd_rn(acc[q], __fmul_rn(m, v[q])) : __fmul_rn(m, v[q]);
+            started = true;
+          }
+        }
+      }
+    }
+    if (g_last < last) {
+      const float dn = __fmul_rn(static_cast<float>((y1 - y0) * ((cx.y - cx.x) + (cx.w - cx.z))), __fadd_rn(m0, S));
+#pragma unroll
+      for (int q = 0; q < VW; ++q) acc[q] = __fdiv_rn(acc[q], dn);
     }
     if (VW == 4) *reinterpret_cast<float4*>(o) = *reinterpret_cast<float4*>(acc);
     else o[0] = acc[0];
@@ -1981,6 +2164,64 @@ int vdb_window_merge_f32(const float* eps, int halves, int bs, int H, int W, int
                   h, w, first, k, nout / 4, out);
   return launch(window_merge_kernel<1>, ew_blocks(nout, 256), 256, 0, stream, eps, bs, H, W, C, oy, ox, cover_y, cover_x, nx, h, w,
                 first, k, nout, out);
+}
+
+int vdb_region_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
+                          int first, int k, int R, int u_blocks, const float* masks, const float* rows, const int* step_idx,
+                          const unsigned long long* seed, const float* bg, int nb, const float* noise, float* out, void* stream) {
+  if (!out) return set_error(VDB_ERR_INVALID, "region_gather: null/empty argument");
+  if (int st = window_args("region_gather", x, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
+  if (R < 1 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_gather: R must be in [1, %d], got %d", kRegionsMax, R);
+  if (u_blocks != 0 && u_blocks != 1 && u_blocks != R + 1)
+    return set_error(VDB_ERR_INVALID, "region_gather: u_blocks must be 0, 1 or R + 1 = %d, got %d", R + 1, u_blocks);
+  if (rows && (!masks || !step_idx || !seed || !bg || nb <= 0))
+    return set_error(VDB_ERR_INVALID, "region_gather: null/empty argument (rows needs masks, step_idx, seed and nb > 0 backgrounds)");
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(noise)) & 15 ||
+      (reinterpret_cast<uintptr_t>(masks) | reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(bg) |
+       reinterpret_cast<uintptr_t>(step_idx)) & 3 || reinterpret_cast<uintptr_t>(seed) & 7)
+    return set_error(VDB_ERR_INVALID, "region_gather: x, out and noise must be 16-byte aligned, masks, rows, bg and step_idx 4-byte, "
+                                      "seed 8-byte");
+  const long long nin = static_cast<long long>(bs) * H * W * C;
+  const long long nout = static_cast<long long>(u_blocks + R + 1) * k * bs * h * w * C;
+  // the batch is written while everything else is read through the read-only path: no byte may be shared
+  if (overlaps(out, nout, x, nin) || (rows && (overlaps(out, nout, masks, static_cast<long long>(R) * bs * H * W) ||
+                                                overlaps(out, nout, noise, nin) || overlaps(out, nout, bg, static_cast<long long>(nb) * C))))
+    return set_error(VDB_ERR_INVALID, "region_gather: out overlaps x, masks, noise or bg");
+  if ((C & 3) == 0)
+    return launch(region_gather_kernel<4>, ew_blocks(nout / 4, 256), 256, 0, stream, x, bs, H, W, C, oy, ox, nx, h, w, first, k,
+                  u_blocks, masks, rows, step_idx, seed, bg, nb, noise, nout / 4, out);
+  return launch(region_gather_kernel<1>, ew_blocks(nout, 256), 256, 0, stream, x, bs, H, W, C, oy, ox, nx, h, w, first, k, u_blocks,
+                masks, rows, step_idx, seed, bg, nb, noise, nout, out);
+}
+
+int vdb_region_noise_f32(const unsigned long long* seed, const int* step_idx, long long n, int R, int bs, int nb, float* z, int* picks,
+                         void* stream) {
+  if (!seed || !step_idx || !z || !picks || n <= 0 || bs <= 0 || nb <= 0)
+    return set_error(VDB_ERR_INVALID, "region_noise: null/empty argument");
+  if (R < 1 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_noise: R must be in [1, %d], got %d", kRegionsMax, R);
+  const long long quads = (n + 3) / 4, total = quads > static_cast<long long>(R) * bs ? quads : static_cast<long long>(R) * bs;
+  return launch(region_noise_kernel, ew_blocks(total, 256), 256, 0, stream, seed, step_idx, n, R, bs, nb, z, picks);
+}
+
+int vdb_region_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox, const int* cover_y,
+                         const int* cover_x, int ny, int nx, int h, int w, int first, int k, int R, const float* masks, float* out,
+                         void* stream) {
+  if (!out || !cover_y || !cover_x || !masks || (halves != 1 && halves != 2))
+    return set_error(VDB_ERR_INVALID, "region_merge: null/empty argument (halves 1 or 2)");
+  if (int st = window_args("region_merge", eps, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
+  if (R < 1 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_merge: R must be in [1, %d], got %d", kRegionsMax, R);
+  if ((reinterpret_cast<uintptr_t>(eps) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(cover_x)) & 15 ||
+      (reinterpret_cast<uintptr_t>(cover_y) | reinterpret_cast<uintptr_t>(masks)) & 3)
+    return set_error(VDB_ERR_INVALID, "region_merge: eps, out and cover_x must be 16-byte aligned, cover_y and masks 4-byte");
+  const long long nout = static_cast<long long>(halves) * bs * H * W * C;
+  if (overlaps(out, nout, eps, static_cast<long long>(halves) * (R + 1) * k * bs * h * w * C) ||
+      overlaps(out, nout, masks, static_cast<long long>(R) * bs * H * W))
+    return set_error(VDB_ERR_INVALID, "region_merge: eps or masks overlaps out");
+  if ((C & 3) == 0)
+    return launch(region_merge_kernel<4>, ew_blocks(nout / 4, 256), 256, 0, stream, eps, bs, H, W, C, oy, ox, cover_y, cover_x, nx,
+                  h, w, first, k, R, masks, nout / 4, out);
+  return launch(region_merge_kernel<1>, ew_blocks(nout, 256), 256, 0, stream, eps, bs, H, W, C, oy, ox, cover_y, cover_x, nx, h, w,
+                first, k, R, masks, nout, out);
 }
 
 int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_src, const float* e_tgt_u, const float* e_tgt_c,

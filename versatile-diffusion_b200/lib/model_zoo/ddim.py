@@ -23,7 +23,8 @@ def _ops():
 
 
 # ------------------------------------------------------------------ sampling modes and how they combine
-# A mode is selected by an optional input: x_info['windows'] (lib/model_zoo/panorama.py), a context's 'prompt_edit'
+# A mode is selected by an optional input: x_info['regions'] (lib/model_zoo/regions.py), x_info['windows'] (lib/model_zoo/
+# panorama.py), a context's 'prompt_edit'
 # (prompt_edit.py), x_info['inversion'] (edit.py) and x_info['inpaint_mask'] (inpaint.py).  The start inputs x_info['x0'] (with
 # 'x0_forward_timesteps') and x_info['xt'] select no mode, but some modes refuse them.
 #
@@ -38,13 +39,20 @@ REFUSES = {
         ('inpaint_mask', "PLMSSampler has no inpainting: use DDIMSampler or DPMSolverSampler (lib/model_zoo/inpaint.py)"),
         ('prompt_edit', "PLMSSampler has no prompt editing: use DDIMSampler or DPMSolverSampler (lib/model_zoo/prompt_edit.py)"),
         ('windows', "PLMSSampler has no window fusion: use DDIMSampler or DPMSolverSampler (lib/model_zoo/panorama.py)"),
+        ('regions', "PLMSSampler has no region prompts: use DDIMSampler or DPMSolverSampler (lib/model_zoo/regions.py)"),
         ('inversion', "PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
                       "(lib/model_zoo/edit.py)"))},
     'p_sample': {
         'prompt_edit': (NotImplementedError, "a prompt edit spans the walk (its windows and word maps): use sample / "
                                              "sample_multicontext (lib/model_zoo/prompt_edit.py)"),
         'windows': (NotImplementedError, "window fusion runs inside the sampler's walk: use sample / sample_multicontext "
-                                         "(lib/model_zoo/panorama.py)")},
+                                         "(lib/model_zoo/panorama.py)"),
+        'regions': (NotImplementedError, "region prompts run inside the sampler's walk: use sample / sample_multicontext "
+                                         "(lib/model_zoo/regions.py)")},
+    'regions': {
+        'prompt_edit': (NotImplementedError, "regions with prompt_edit: the edit's item tables index prompts, not regions "
+                                             "(lib/model_zoo/regions.py)"),
+        'inversion': (NotImplementedError, "regions cannot sample from an inversion (lib/model_zoo/regions.py)")},
     'windows': {
         'prompt_edit': (NotImplementedError, "windows with prompt_edit: the edit's item tables index prompts, not windows "
                                              "(lib/model_zoo/panorama.py)"),
@@ -55,13 +63,14 @@ REFUSES = {
 }
 
 # Pairs that change meaning: mode -> inputs it takes over, which then select no mode of their own.  An inpaint_mask given with an
-# inversion is the mask of the inversion's trajectory blend, not inpainting.
-TAKES = {'inversion': ('inpaint_mask',)}
+# inversion is the mask of the inversion's trajectory blend, not inpainting.  Windows given with regions are the region walk's
+# window layout, not a walk of their own.
+TAKES = {'inversion': ('inpaint_mask',), 'regions': ('windows',)}
 
 
 def given_inputs(x_info, c_infos):
     """The optional inputs given (not None) to a call."""
-    given = {k for k in ('x0', 'xt', 'x0_forward_timesteps', 'inpaint_mask', 'inversion', 'windows')
+    given = {k for k in ('x0', 'xt', 'x0_forward_timesteps', 'inpaint_mask', 'inversion', 'windows', 'regions')
              if x_info.get(k, None) is not None}
     if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
         given.add('prompt_edit')
@@ -213,11 +222,13 @@ class DDIMSampler(object):
         from .inpaint import Inpainting
         from .panorama import WindowFusion
         from .prompt_edit import PromptEditing
+        from .regions import RegionPrompts
         refuse(entry, x_info, c_infos)
         given = given_inputs(x_info, c_infos)
         taken = {k for m in given for k in TAKES.get(m, ())}
-        return [cls(self, x_info, shape, c_infos) for name, cls in (('windows', WindowFusion), ('prompt_edit', PromptEditing),
-                                                                      ('inversion', FromInversion), ('inpaint_mask', Inpainting))
+        return [cls(self, x_info, shape, c_infos) for name, cls in (('regions', RegionPrompts), ('windows', WindowFusion),
+                                                                      ('prompt_edit', PromptEditing), ('inversion', FromInversion),
+                                                                      ('inpaint_mask', Inpainting))
                 if name in given and name not in taken]
 
     def _run(self, shape, x_info, c_infos, multi, noise_dropout, temperature, log_every_t):

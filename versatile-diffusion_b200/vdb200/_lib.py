@@ -38,6 +38,9 @@ SIGNATURES = {
     "vdb_local_blend_f32": (i, [p, p, p, p, p, i, i, i, i, i, i, f, p]),
     "vdb_window_gather_f32": (i, [p, i, i, i, i, p, p, i, i, i, i, i, i, p, p, p]),
     "vdb_window_merge_f32": (i, [p, i, i, i, i, i, p, p, p, p, i, i, i, i, i, i, p, p]),
+    "vdb_region_gather_f32": (i, [p, i, i, i, i, p, p, i, i, i, i, i, i, i, i, p, p, p, p, p, i, p, p, p]),
+    "vdb_region_noise_f32": (i, [p, p, ll, i, i, i, p, p, p]),
+    "vdb_region_merge_f32": (i, [p, i, i, i, i, i, p, p, p, p, i, i, i, i, i, i, i, p, p, p]),
     "vdb_axpby_f32": (i, [p, p, f, f, p, ll, p]),
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),

@@ -587,6 +587,76 @@ def window_merge(eps, oy, ox, cover_y, cover_x, first, k, out, halves=1):
     return out
 
 
+def _region_masks(masks, R, bs, H, W):
+    if masks is not None and masks.numel() != R * bs * H * W:
+        raise ValueError(f"masks: expected [{R}, {bs}, {H}, {W}], got {tuple(masks.shape)}")
+
+
+def region_gather(x, oy, ox, h, w, first, k, R, u_blocks, out=None, masks=None, rows=None, step_idx=None, seed=None, bg=None,
+                  noise=None):
+    """Windows [first, first + k) of the canvas x fp32 NHWC [bs, H, W, C] -> the chunk batch out [(u_blocks + R + 1)*k*bs, h, w, C]
+    of a region walk (lib/model_zoo/regions.py): u_blocks (0, 1 or R + 1) u blocks, then the R + 1 c blocks.  Exact copies unless
+    rows (fp32 [., 4] {on, a, b, 0} device rows, row step_idx[0]) is on: then region r >= 1 reads m x + (1 - m) (a bg + b z) with
+    masks fp32 [R, bs, H, W], bg fp32 [nb, C] picked by the Philox stream keyed by seed (int64 device word), and z = noise (fp32
+    like x) when given, else that stream's normals."""
+    for name, t in (("x", x), ("out", out), ("masks", masks), ("rows", rows), ("bg", bg), ("noise", noise)):
+        _need(t, torch.float32, name)
+    _need(oy, torch.int32, "oy"); _need(ox, torch.int32, "ox"); _need(step_idx, torch.int32, "step_idx")
+    _need(seed, torch.int64, "seed")
+    bs, H, W, C = x.shape
+    shape = ((u_blocks + R + 1) * k * bs, h, w, C)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    if tuple(out.shape) != shape:
+        raise ValueError(f"out: expected {shape}, got {tuple(out.shape)}")
+    _region_masks(masks, R, bs, H, W)
+    if noise is not None and noise.shape != x.shape:
+        raise ValueError(f"noise: expected {tuple(x.shape)}, got {tuple(noise.shape)}")
+    if bg is not None and (bg.dim() != 2 or bg.shape[1] != C):
+        raise ValueError(f"bg: expected [nb, {C}], got {tuple(bg.shape)}")
+    if rows is not None and (rows.dim() != 2 or rows.shape[1] != 4):
+        raise ValueError(f"rows: expected [., 4], got {tuple(rows.shape)}")
+    check(lib.vdb_region_gather_f32(_ptr(x), bs, H, W, C, _ptr(oy), _ptr(ox), oy.numel(), ox.numel(), int(h), int(w), int(first),
+                                    int(k), int(R), int(u_blocks), _ptr(masks), _ptr(rows), _ptr(step_idx), _ptr(seed), _ptr(bg),
+                                    0 if bg is None else bg.shape[0], _ptr(noise), _ptr(out), _stream()), "region_gather")
+    return out
+
+
+def region_noise(seed, step_idx, n, R, bs, nb):
+    """The region gather's draws at step step_idx[0] -> (z fp32 [n] for the first n canvas elements, picks int32 [R, bs]: the
+    background row of region r + 1, image b)."""
+    _need(seed, torch.int64, "seed")
+    _need(step_idx, torch.int32, "step_idx")
+    z = torch.empty(n, dtype=torch.float32, device=seed.device)
+    picks = torch.empty(R, bs, dtype=torch.int32, device=seed.device)
+    check(lib.vdb_region_noise_f32(_ptr(seed), _ptr(step_idx), int(n), int(R), int(bs), int(nb), _ptr(z), _ptr(picks), _stream()),
+          "region_noise")
+    return z, picks
+
+
+def region_merge(eps, oy, ox, cover_y, cover_x, first, k, R, masks, out, halves=1):
+    """The mask-weighted merge of windows [first, first + k) of eps fp32 [halves*(R+1)*k*bs, h, w, C] (block s*(R+1) + r) into the
+    canvas out [halves*bs, H, W, C] (lib/model_zoo/regions.py).  masks fp32 [R, bs, H, W]; the tables are window_merge's."""
+    for name, t in (("eps", eps), ("out", out), ("masks", masks)):
+        _need(t, torch.float32, name)
+    for name, t in (("oy", oy), ("ox", ox), ("cover_y", cover_y), ("cover_x", cover_x)):
+        _need(t, torch.int32, name)
+    n, H, W, C = out.shape
+    if halves not in (1, 2) or n % halves:
+        raise ValueError(f"halves must be 1 or 2 and divide the {n} rows of out, got {halves}")
+    bs = n // halves
+    if eps.dim() != 4 or eps.shape[0] != (R + 1) * k * n or eps.shape[3] != C:
+        raise ValueError(f"eps: expected [{(R + 1) * k * n}, h, w, {C}] for out {tuple(out.shape)}, got {tuple(eps.shape)}")
+    _, h, w, _ = eps.shape
+    _region_masks(masks, R, bs, H, W)
+    if cover_y.numel() != 2 * H or cover_x.numel() != 4 * W:
+        raise ValueError(f"cover tables: expected {2 * H} and {4 * W} entries, got {cover_y.numel()} and {cover_x.numel()}")
+    check(lib.vdb_region_merge_f32(_ptr(eps), halves, bs, H, W, C, _ptr(oy), _ptr(ox), _ptr(cover_y), _ptr(cover_x), oy.numel(),
+                                   ox.numel(), int(h), int(w), int(first), int(k), int(R), _ptr(masks), _ptr(out), _stream()),
+          "region_merge")
+    return out
+
+
 def groupnorm(x1, gamma, beta, eps, act=ACT_NONE, x2=None, out=None, groups=32):
     """GN32(+SiLU) over NHWC bf16 [B,H,W,C1] (+ concat x2 [B,H,W,C2]) -> [B,H,W,C1+C2]."""
     _need(x1, BF16, "x1"); _need(x2, BF16, "x2"); _need(gamma, torch.float32, "gamma"); _need(beta, torch.float32, "beta")
