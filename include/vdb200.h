@@ -113,53 +113,41 @@ int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_sr
  * x_dup and map overlapping. */
 int vdb_local_blend_f32(float* x, float* x_dup, const float* map, const int* flags, const int* step_idx, int n, int H, int W, int C,
                         int h, int w, float threshold, void* stream);
-/* ---- panoramas: MultiDiffusion window fusion — lib/model_zoo/panorama.py (an addition: the reference has no panorama mode; the
- * layout and the merge are specified in that module's docstring) -------------------------------------------------------------------
- * The canvas is fp32 NHWC [bs, H, W, C].  The layout has ny x nx windows of h x w; window g = iy*nx + ix reads rows oy[iy] + r
- * (r < h) and columns (ox[ix] + j) mod W (j < w); oy / ox are device int32 tables, and only a circular layout has columns that
- * wrap.  Both entry points take a range [first, first + k) of windows, one UNet chunk.
- * vdb_window_gather_f32: out [k*bs, h, w, C], row j*bs + b = window first + j of image b, an exact copy; out_dup (may be NULL)
- * receives a second copy (the CFG half).  VDB_ERR_INVALID before any launch: a null x / out / table, a size <= 0, a window larger
- * than the canvas, a range outside the ny*nx windows, x / out / out_dup not 16-byte aligned or tables not 4-byte aligned, or any
- * two of x, out and out_dup overlapping.
- * vdb_window_merge_f32: eps [halves*k*bs, h, w, C] (halves 1, or 2 for [u rows; c rows] under CFG; row s*k*bs + j*bs + b is
- * window first + j of image b) -> out [halves*bs, H, W, C].  cover_y int32 [H, 2]: the windows covering row y are iy in
- * [cover_y[2y], cover_y[2y+1]); cover_x int32 [W, 4]: those covering column x are ix in [cover_x[4x], cover_x[4x+1]) then
- * [cover_x[4x+2], cover_x[4x+3]), ascending.  Per element, over its covering windows in ascending window index, fp32 with
- * round-to-nearest: the first sets out, each later one is added, and the call whose range holds the last one divides by their
- * count.  Elements with no covering window in the range are not touched.  So calls over consecutive ranges compute exactly what
- * one call over all windows does, and an element with one covering window gets that window's eps bit for bit.  No atomics: the
- * result is bit-reproducible.  VDB_ERR_INVALID before any launch: as the gather, plus a null cover table, halves not 1 or 2,
- * eps / out / cover_x not 16-byte aligned, or eps overlapping out. */
-int vdb_window_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
-                          int first, int k, float* out, float* out_dup, void* stream);
-int vdb_window_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox,
-                         const int* cover_y, const int* cover_x, int ny, int nx, int h, int w, int first, int k, float* out,
-                         void* stream);
-/* ---- region prompts: MultiDiffusion region-based generation — lib/model_zoo/regions.py (an addition: the reference has no region
- * mode; the weights, the merge and the bootstrapping are specified in that module's docstring) ---------------------------------------
- * On the window layout and tables of the panorama entry points (one window equal to the canvas when no windows are asked for).
- * masks: fp32 [R, bs, H, W] on the canvas, region r = 1..R at row r - 1, values in [0, 1]; 1 <= R <= 8.  Region 0 is the
- * background, of weight m_0 = max(0, 1 - S) with S = m_1 + ... + m_R summed in ascending r, and D = m_0 + S (fp32, rounded).
+/* ---- region prompts and panoramas: MultiDiffusion on a window layout — lib/model_zoo/regions.py and lib/model_zoo/panorama.py
+ * (additions: the reference has no region or panorama mode; the layout, the weights, the merge and the bootstrapping are specified
+ * in those modules' docstrings) -------------------------------------------------------------------------------------------------
+ * A panorama's window fusion is the walk with no regions, R = 0.  The canvas is fp32 NHWC [bs, H, W, C].  The layout has ny x nx
+ * windows of h x w; window g = iy*nx + ix reads rows oy[iy] + r (r < h) and columns (ox[ix] + j) mod W (j < w); oy / ox are device
+ * int32 tables, and only a circular layout has columns that wrap.  Region prompts without windows use one window equal to the
+ * canvas.  The gather and the merge take a range [first, first + k) of windows, one UNet chunk.
+ * masks: fp32 [R, bs, H, W] on the canvas, region r = 1..R at row r - 1, values in [0, 1]; 0 <= R <= 8.  Region 0 is the
+ * background, of weight m_0 = max(0, 1 - S) with S = m_1 + ... + m_R summed in ascending r (S = 0 when R = 0), and D = m_0 + S
+ * (fp32, rounded).
  * vdb_region_gather_f32: out = u_blocks + R + 1 blocks of [k*bs, h, w, C], u_blocks in {0, 1, R + 1}; block blk is region
  * blk - u_blocks of the c half, region 0 for the single u block, region blk for one of R + 1 u blocks; row j*bs + b of a block is
- * window first + j of image b.  Every block is an exact copy of the window (as vdb_window_gather_f32) unless rows is non-NULL and
+ * window first + j of image b.  Every block is an exact copy of the window unless rows is non-NULL and
  * row *step_idx of rows (fp32 {on, a, b, 0}) has on != 0: then region r >= 1 reads, per element of mask value m,
  * m == 1 ? x : m == 0 ? k : m*x + (1 - m)*k  with  k = a*bg + b*z  (fp32, round-to-nearest), bg = row floor(w*nb / 2^32) of the
  * backgrounds bg fp32 [nb, C], w the first word of Philox4x32-10 at counter ((r*bs + b), *step_idx, 0x72676e73 "rgns", 1) under the
  * key *seed, and z = noise (fp32 NHWC canvas) when non-NULL, else the canvas element's normal at counter (element quad, *step_idx,
- * "rgns", 0) by the Box-Muller of vdb_inpaint_blend_f32.  VDB_ERR_INVALID before any launch: the window gather's refusals, R
- * outside [1, 8], u_blocks not 0, 1 or R + 1, rows without masks / step_idx / seed / nb > 0 backgrounds, x / out / noise not
- * 16-byte aligned, masks / rows / bg / step_idx not 4-byte, seed not 8-byte, or out overlapping x, masks, noise or bg.
+ * "rgns", 0) by the Box-Muller of vdb_inpaint_blend_f32.  VDB_ERR_INVALID before any launch: a null x / out / table, a size <= 0,
+ * a window larger than the canvas, a range outside the ny*nx windows, tables not 4-byte aligned, R outside [0, 8], u_blocks not
+ * 0, 1 or R + 1, rows without step_idx / seed / nb > 0 backgrounds (or without masks when R >= 1), x / out / noise not 16-byte
+ * aligned, masks / rows / bg / step_idx not 4-byte, seed not 8-byte, or out overlapping x, masks, noise or bg.
  * vdb_region_noise_f32: the gather's draws of step *step_idx: z [n] for canvas elements [0, n), picks int32 [R*bs], entry
- * (r - 1)*bs + b the background row of region r, image b.
+ * (r - 1)*bs + b the background row of region r, image b; 1 <= R <= 8.
  * vdb_region_merge_f32: eps [halves*(R+1)*k*bs, h, w, C], block s*(R+1) + r (halves 1, or 2 for [u blocks; c blocks]) -> out
- * [halves*bs, H, W, C].  Per element, over its covering windows in ascending window index and r = 0..R inside each, fp32 with
- * round-to-nearest: each term m_r*e of nonzero weight (a zero weight is skipped) is one product; the first sets out, later ones
- * are added, and the call whose range holds the last window divides by n*D (n covering windows, the product rounded).  Elements
- * with no covering window in the range are not touched, so calls over consecutive ranges equal one call; a hard mask selects its
- * region's eps bit for bit.  No atomics.  VDB_ERR_INVALID before any launch: the window merge's refusals, a null masks, R outside
- * [1, 8], masks not 4-byte aligned, or eps or masks overlapping out. */
+ * [halves*bs, H, W, C].  cover_y int32 [H, 2]: the windows covering row y are iy in [cover_y[2y], cover_y[2y+1]); cover_x int32
+ * [W, 4]: those covering column x are ix in [cover_x[4x], cover_x[4x+1]) then [cover_x[4x+2], cover_x[4x+3]), ascending.  Per
+ * element, over its covering windows in ascending window index and r = 0..R inside each, fp32 with round-to-nearest: each term
+ * m_r*e of nonzero weight (a zero weight is skipped) is one product; the first sets out, later ones are added, and the call whose
+ * range holds the last window divides by n*D (n covering windows, the product rounded).  Elements with no covering window in the
+ * range are not touched, so calls over consecutive ranges compute exactly what one call over all windows does; a hard mask selects
+ * its region's eps bit for bit.  With R = 0 (masks may be NULL) every product is 1*e = e and n*D = n, so the merge is the plain
+ * window average and an element with one covering window gets that window's eps bit for bit.  No atomics: the result is
+ * bit-reproducible.  VDB_ERR_INVALID before any launch: the gather's size, range and table refusals, a null cover table, a null
+ * masks when R >= 1, halves not 1 or 2, R outside [0, 8], eps / out / cover_x not 16-byte aligned, cover_y / masks not 4-byte, or
+ * eps or masks overlapping out. */
 int vdb_region_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
                           int first, int k, int R, int u_blocks, const float* masks, const float* rows, const int* step_idx,
                           const unsigned long long* seed, const float* bg, int nb, const float* noise, float* out, void* stream);

@@ -1,6 +1,7 @@
-"""Panoramas, CPU side (lib/model_zoo/panorama.py): the window layout and its cover tables, every refusal of the samplers, the
-argument checks of the C entry points, and the oracle (oracle/panorama_oracle.py): its paper-form DDIM average against the eps
-average on an analytic eps function in fp64, and a one-window layout reducing its walk to the plain walk."""
+"""Panoramas, CPU side (lib/model_zoo/panorama.py): the window layout and its cover tables, every refusal of the samplers, and the
+oracle (oracle/panorama_oracle.py): its paper-form DDIM average against the eps average on an analytic eps function in fp64, and a
+one-window layout reducing its walk to the plain walk.  The C entry points a panorama runs are the region ones at R = 0, whose
+argument checks tests/test_regions.py covers."""
 import types
 
 import numpy as np
@@ -161,58 +162,6 @@ def test_panorama_helper_refuses_odd_sizes():
     from lib.model_zoo.panorama import panorama
     with pytest.raises(ValueError, match="multiples of 8"):
         panorama(None, None, _cinfo(), height=500, width=2048)
-
-
-def test_entry_points_reject_bad_arguments_without_gpu():
-    """vdb_window_gather_f32 and vdb_window_merge_f32 refuse null, misaligned, empty, out-of-range and overlapping arguments
-    before any launch (the fake addresses below are never dereferenced: every call fails its checks)."""
-    from vdb200._lib import lib
-    bs, H, W, C, h, w, ny, nx = 2, 16, 40, 4, 16, 16, 1, 4
-    nin, nout = bs * H * W * C, nx * bs * h * w * C
-    ok = dict(x=0x1000000, bs=bs, H=H, W=W, C=C, oy=0x2000000, ox=0x2100000, ny=ny, nx=nx, h=h, w=w, first=0, k=nx,
-              out=0x3000000, dup=0x4000000, cy=0x2200000, cx=0x2300000, halves=2)
-
-    def gather(**kw):
-        a = dict(ok, **kw)
-        return lib.vdb_window_gather_f32(a["x"], a["bs"], a["H"], a["W"], a["C"], a["oy"], a["ox"], a["ny"], a["nx"], a["h"],
-                                         a["w"], a["first"], a["k"], a["out"], a["dup"], None)
-
-    def merge(**kw):
-        a = dict(ok, **kw)
-        return lib.vdb_window_merge_f32(a["x"], a["halves"], a["bs"], a["H"], a["W"], a["C"], a["oy"], a["ox"], a["cy"], a["cx"],
-                                        a["ny"], a["nx"], a["h"], a["w"], a["first"], a["k"], a["out"], None)
-
-    before = lib.vdb_launch_count()
-    for fn, what in ((gather, b"window_gather"), (merge, b"window_merge")):
-        nulls = ("x", "oy", "ox", "out") + (("cy", "cx") if fn is merge else ())
-        for key in nulls:
-            assert fn(**{key: None}) == 1 and what + b": null" in lib.vdb_last_error(), key
-        for key in ("bs", "H", "W", "C", "ny", "nx", "h", "w", "k"):
-            for v in (0, -1):
-                assert fn(**{key: v}) == 1 and b"empty" in lib.vdb_last_error(), (key, v)
-        assert fn(h=H + 1) == 1 and b"larger than the canvas" in lib.vdb_last_error()
-        assert fn(w=W + 8) == 1 and b"larger than the canvas" in lib.vdb_last_error()
-        for first, k in ((-1, 2), (3, 2), (0, 5), (4, 1)):
-            assert fn(first=first, k=k) == 1 and b"outside the layout" in lib.vdb_last_error(), (first, k)
-        for key in ("oy", "ox"):
-            assert fn(**{key: ok[key] + 2}) == 1 and b"4-byte aligned" in lib.vdb_last_error(), key
-    for key in ("x", "out", "dup"):
-        assert gather(**{key: ok[key] + 4}) == 1 and b"16-byte aligned" in lib.vdb_last_error(), key
-    for key in ("x", "out", "cx"):
-        assert merge(**{key: ok[key] + 4}) == 1 and b"16-byte aligned" in lib.vdb_last_error(), key
-    assert merge(cy=ok["cy"] + 2) == 1 and b"4-byte" in lib.vdb_last_error()
-    for v in (0, 3):
-        assert merge(halves=v) == 1 and b"halves" in lib.vdb_last_error(), v
-    # overlaps: first and last shared float of the window batch (out, out_dup) and the canvas
-    x = ok["x"]
-    for addr in (x, x + 4 * (nin - 4), x - 4 * (nout - 4)):
-        assert gather(out=addr) == 1 and b"must not overlap" in lib.vdb_last_error(), addr
-        assert gather(dup=addr) == 1 and b"must not overlap" in lib.vdb_last_error(), addr
-    assert gather(dup=ok["out"] + 4 * (nout - 4)) == 1 and b"must not overlap" in lib.vdb_last_error()
-    m_in, m_out = 2 * nx * bs * h * w * C, 2 * bs * H * W * C          # merge: eps is x here
-    for addr in (x, x + 4 * (m_in - 4), x - 4 * (m_out - 4)):
-        assert merge(out=addr) == 1 and b"overlaps out" in lib.vdb_last_error(), addr
-    assert lib.vdb_launch_count() == before
 
 
 # ---- the oracle on an analytic eps function ---------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
-"""Panoramas on the GPU (lib/model_zoo/panorama.py): vdb_window_gather_f32 bitwise against a numpy copy, vdb_window_merge_f32
-bitwise against its fp32 restatement in the same order and within 1e-6 of fp64, chunked merges equal to one merge; the
+"""Panoramas on the GPU (lib/model_zoo/panorama.py): vdb_region_gather_f32 at R = 0 bitwise against a numpy copy,
+vdb_region_merge_f32 at R = 0 bitwise against the window average's fp32 restatement in the same order and within 1e-6 of fp64,
+chunked merges equal to one merge; the
 windowed DDIM and DPM-Solver++ samplers on the mini UNet against the MultiDiffusion oracle (oracle/panorama_oracle.py); the
 invariants (a window equal to the canvas gives the unwindowed result bit for bit, graph equals eager, a cached graph replays on
 new prompts, other chunk sizes agree); and a wide latent through the mini VAE."""
@@ -21,10 +22,8 @@ def _dev(a):
 
 
 def _tables(lay):
-    from lib.model_zoo.panorama import WindowState
-    ws = WindowState(lay, lay.nwin, 1, False, 4, DEV)
-    ws.fill(lay)
-    return ws
+    from lib.model_zoo.panorama import LayoutTables
+    return LayoutTables(lay, DEV)
 
 
 def _crop_nhwc(x, oy, ox, h, w):
@@ -38,7 +37,7 @@ LAYOUTS = [(16, 40, 16, 8, False), (24, 20, 16, 7, False), (32, 32, 16, 8, False
 
 @pytest.mark.parametrize("H,W,size,stride,circular", LAYOUTS)
 @pytest.mark.parametrize("bs,C", [(1, 4), (3, 4), (2, 3)])
-def test_gather_bitwise(H, W, size, stride, circular, bs, C):
+def test_gather_with_no_regions_bitwise(H, W, size, stride, circular, bs, C):
     from lib.model_zoo.panorama import Windows, layout
     from vdb200 import ops
     lay = layout(Windows(size, stride, circular), H, W)
@@ -47,17 +46,19 @@ def test_gather_bitwise(H, W, size, stride, circular, bs, C):
     dx = _dev(x)
     wins = [(int(oy), int(ox)) for oy in lay.oy for ox in lay.ox]
     for first, k in lay.chunks(3) + [(0, lay.nwin)]:
-        out = torch.full((k * bs, lay.h, lay.w, C), float("nan"), device=DEV)
-        dup = torch.full_like(out, float("nan")) if first % 2 == 0 else None
-        ops.window_gather(dx, ws.oy, ws.ox, lay.h, lay.w, first, k, out=out, out_dup=dup)
+        ub = 1 if first % 2 == 0 else 0          # with a u block (CFG), the c block is a second copy
+        out = torch.full(((ub + 1) * k * bs, lay.h, lay.w, C), float("nan"), device=DEV)
+        ops.region_gather(dx, ws.oy, ws.ox, lay.h, lay.w, first, k, 0, ub, out=out)
         want = np.concatenate([_crop_nhwc(x, *wins[g], lay.h, lay.w) for g in range(first, first + k)])
-        assert np.array_equal(out.cpu().numpy(), want), (first, k)
-        if dup is not None:
-            assert np.array_equal(dup.cpu().numpy(), want)
+        got = out.cpu().numpy()
+        assert np.array_equal(got[:k * bs], want), (first, k)
+        if ub:
+            assert np.array_equal(got[k * bs:], want)
 
 
 def merge_restated(eps, lay, wins, bs, halves, C):
-    """vdb_window_merge_f32 in numpy fp32: ascending window index, first sets, later ones add (rounded), one division"""
+    """The window average (vdb_region_merge_f32 at R = 0) in numpy fp32: ascending window index, first sets, later ones add
+    (rounded), one division by the count"""
     H, W, h, w = lay.H, lay.W, lay.h, lay.w
     n = len(wins)
     e = eps.reshape(halves, n, bs, h, w, C)
@@ -84,7 +85,7 @@ def merge_fp64(eps, lay, wins, bs, halves, C):
 
 @pytest.mark.parametrize("H,W,size,stride,circular", LAYOUTS)
 @pytest.mark.parametrize("bs,halves,C", [(1, 2, 4), (2, 1, 4), (3, 2, 4), (2, 2, 5)])
-def test_merge_bitwise_and_against_fp64(H, W, size, stride, circular, bs, halves, C):
+def test_merge_with_no_regions_bitwise_and_against_fp64(H, W, size, stride, circular, bs, halves, C):
     from lib.model_zoo.panorama import Windows, layout
     from vdb200 import ops
     lay = layout(Windows(size, stride, circular), H, W)
@@ -102,7 +103,7 @@ def test_merge_bitwise_and_against_fp64(H, W, size, stride, circular, bs, halves
         out = torch.full((halves * bs, H, W, C), float("nan"), device=DEV)
         for first, k in lay.chunks(per):
             e = np.ascontiguousarray(per_window[:, first:first + k]).reshape(halves * k * bs, lay.h, lay.w, C)
-            ops.window_merge(_dev(e), ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, out, halves=halves)
+            ops.region_merge(_dev(e), ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, 0, None, out, halves=halves)
         outs.append(out.cpu().numpy())
     got = outs[0]
     assert np.array_equal(got, want), np.abs(got - want).max()

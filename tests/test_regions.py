@@ -143,9 +143,10 @@ def test_plms_and_the_single_step_api_refuse_regions():
 
 
 def test_regions_take_the_windows():
-    """Windows given with regions select no window walk of their own: the region mode reads the layout."""
+    """Windows given with regions select no window walk of their own: the region mode reads the layout.  Windows alone select the
+    same mode with no regions (R = 0), in chunks of WINDOWS_PER_CHUNK windows."""
     from lib.model_zoo.ddim import TAKES, DDIMSampler
-    from lib.model_zoo.panorama import Windows
+    from lib.model_zoo.panorama import WINDOWS_PER_CHUNK, Windows
     from lib.model_zoo.regions import RegionPrompts
     assert TAKES["regions"] == ("windows",)
     S = DDIMSampler(_fake_model())
@@ -156,6 +157,11 @@ def test_regions_take_the_windows():
     assert m.lay.nwin == 4 and m.per == 2 and m.chunks == [(0, 2), (2, 2)], "8 // (R + 1) windows per chunk"
     m = S._modes("sample", {"type": "image", "regions": _regions(R=8)}, [1, 4, 16, 24], [_cinfo()])[0]
     assert (m.lay.h, m.lay.w, m.lay.nwin, m.per) == (16, 24, 1, 1), "no windows: one window, the canvas"
+    modes = S._modes("sample", {"type": "image", "windows": Windows(64, 8)}, [1, 4, 64, 256], [_cinfo()])
+    assert [type(m) for m in modes] == [RegionPrompts]
+    m = modes[0]
+    assert m.R == 0 and not m.boot and m.per == WINDOWS_PER_CHUNK == 8
+    assert m.lay.nwin == 25 and m.chunks == [(0, 8), (8, 8), (16, 8), (24, 1)]
 
 
 def test_the_weight_rule_on_a_dense_grid():
@@ -205,9 +211,10 @@ def test_step_rows(kind, steps, k, boot):
     assert [bool(rows[i, 0]) for i in walked] == [n < boot for n in range(total)]
 
 
-def test_entry_points_reject_bad_arguments_without_gpu():
+def test_entry_points_reject_bad_arguments_at_every_R_without_gpu():
     """vdb_region_gather_f32, vdb_region_merge_f32 and vdb_region_noise_f32 refuse null, misaligned, empty, out-of-range and
-    overlapping arguments before any launch (the fake addresses are never dereferenced: every call fails its checks)."""
+    overlapping arguments before any launch (the fake addresses are never dereferenced: every call fails its checks).  R = 0, a
+    panorama's walk, needs no masks."""
     from vdb200._lib import lib
     bs, H, W, C, h, w, ny, nx, R = 2, 16, 40, 4, 16, 16, 1, 4, 2
     nin = bs * H * W * C
@@ -239,14 +246,19 @@ def test_entry_points_reject_bad_arguments_without_gpu():
             for v in (0, -1):
                 assert fn(**{key: v}) == 1 and b"empty" in err(), (key, v)
         assert fn(h=H + 1) == 1 and b"larger than the canvas" in err()
+        assert fn(w=W + 8) == 1 and b"larger than the canvas" in err()
         for first, k in ((-1, 2), (3, 2), (0, 5), (4, 1)):
             assert fn(first=first, k=k) == 1 and b"outside the layout" in err(), (first, k)
         for key in ("oy", "ox"):
             assert fn(**{key: ok[key] + 2}) == 1 and b"4-byte aligned" in err(), key
-        for bad in (0, -1, 9, 100):
-            assert fn(R=bad) == 1 and b"R must be in [1, 8]" in err(), bad
+        for bad in (-1, 9, 100):
+            assert fn(R=bad) == 1 and b"R must be in [0, 8]" in err(), bad
+        # R = 0 without masks passes the null checks and fails on the next refusal
+        assert fn(R=0, masks=None, out=ok["out"] + 4) == 1 and b"16-byte aligned" in err()
     for ub in (2, -1, R + 2):
         assert gather(ub=ub) == 1 and b"u_blocks" in err(), ub
+    for ub in (2, -1):
+        assert gather(R=0, masks=None, ub=ub) == 1 and b"u_blocks must be 0, 1 or R + 1 = 1" in err(), ub
     for key in ("masks", "idx", "seed", "bg"):
         assert gather(**{key: None}) == 1 and b"rows needs" in err(), key
     assert gather(nb=0) == 1 and b"rows needs" in err()
@@ -276,7 +288,8 @@ def test_entry_points_reject_bad_arguments_without_gpu():
         assert noise(**{key: None}) == 1 and b"region_noise: null" in err(), key
     for key in ("n", "bs", "nb"):
         assert noise(**{key: 0}) == 1 and b"empty" in err(), key
-    assert noise(R=9) == 1 and b"R must be in [1, 8]" in err()
+    for bad in (0, 9):
+        assert noise(R=bad) == 1 and b"R must be in [1, 8]" in err(), bad
     assert lib.vdb_launch_count() == before
 
 

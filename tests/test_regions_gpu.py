@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from oracle import regions_oracle as G
+from test_panorama_gpu import merge_restated as window_average_restated
 from test_parity_gpu import _cmp, build_net
 
 pytestmark = pytest.mark.gpu
@@ -25,10 +26,8 @@ def _idx(i):
 
 
 def _tables(lay):
-    from lib.model_zoo.panorama import WindowState
-    ws = WindowState(lay, lay.nwin, 1, False, 4, DEV)
-    ws.fill(lay)
-    return ws
+    from lib.model_zoo.panorama import LayoutTables
+    return LayoutTables(lay, DEV)
 
 
 def _masks(kind, R, bs, H, W, seed):
@@ -71,7 +70,7 @@ def gather_restated(x, wins, h, w, first, k, R, ub, masks, on, a, b, bg, picks, 
 
 @pytest.mark.parametrize("H,W,size,stride,circular", LAYOUTS)
 @pytest.mark.parametrize("bs,C,R", [(1, 4, 1), (3, 4, 3), (2, 3, 2), (1, 4, 8)])
-def test_gather_bitwise(H, W, size, stride, circular, bs, C, R):
+def test_gather_bitwise_against_numpy(H, W, size, stride, circular, bs, C, R):
     from lib.model_zoo.panorama import Windows, layout
     from vdb200 import ops
     lay = layout(Windows(size, stride, circular), H, W)
@@ -102,12 +101,14 @@ def test_gather_bitwise(H, W, size, stride, circular, bs, C, R):
                     ops.region_gather(dx, ws.oy, ws.ox, lay.h, lay.w, first, k, R, ub, out=fed, masks=dm, rows=drows,
                                       step_idx=_idx(step), seed=seed, bg=dbg, noise=z)
                     assert torch.equal(fed, out), "the Philox path equals the noise path"
-                    if step == 0:       # flag off, and no rows at all: exact copies, as the window gather
+                    if step == 0:       # flag off, and no rows at all: exact copies of the windows in every block
                         plain = torch.full(shape, float("nan"), device=DEV)
                         ops.region_gather(dx, ws.oy, ws.ox, lay.h, lay.w, first, k, R, ub, out=plain)
                         assert torch.equal(plain, out)
-                        win = ops.window_gather(dx, ws.oy, ws.ox, lay.h, lay.w, first, k)
-                        assert torch.equal(plain.view(ub + R + 1, *win.shape), win.expand(ub + R + 1, *win.shape))
+                        win = np.concatenate([x[:, oy:oy + lay.h][:, :, (ox + np.arange(lay.w)) % W]
+                                              for oy, ox in wins[first:first + k]])
+                        assert np.array_equal(plain.cpu().numpy().reshape(ub + R + 1, *win.shape),
+                                              np.broadcast_to(win, (ub + R + 1,) + win.shape))
 
 
 def merge_restated(eps, wins, lay, bs, halves, R, masks, C):
@@ -141,7 +142,7 @@ def merge_restated(eps, wins, lay, bs, halves, R, masks, C):
 
 @pytest.mark.parametrize("H,W,size,stride,circular", LAYOUTS)
 @pytest.mark.parametrize("bs,halves,C,R", [(1, 2, 4, 2), (2, 1, 4, 1), (3, 2, 4, 3), (2, 2, 5, 2), (1, 1, 4, 8)])
-def test_merge_bitwise_and_against_fp64(H, W, size, stride, circular, bs, halves, C, R):
+def test_merge_bitwise_against_numpy_and_fp64(H, W, size, stride, circular, bs, halves, C, R):
     from lib.model_zoo.panorama import Windows, layout
     from vdb200 import ops
     lay = layout(Windows(size, stride, circular), H, W)
@@ -193,10 +194,9 @@ def test_merge_bitwise_and_against_fp64(H, W, size, stride, circular, bs, halves
         ex = np.broadcast_to(exact[None, ..., None], picked.shape)
         assert np.array_equal(got.reshape(picked.shape)[ex], picked[ex]), kind
         if kind == "zero":
-            win = torch.full((halves * bs, H, W, C), float("nan"), device=DEV)
             bg_only = np.ascontiguousarray(per_window[:, 0]).reshape(halves * n * bs, lay.h, lay.w, C)
-            ops.window_merge(_dev(bg_only), ws.oy, ws.ox, ws.cover_y, ws.cover_x, 0, n, win, halves=halves)
-            assert np.array_equal(got, win.cpu().numpy()), "all-zero masks: the background's window average bit for bit"
+            avg, _ = window_average_restated(bg_only, lay, wins, bs, halves, C)
+            assert np.array_equal(got, avg), "all-zero masks: the background's window average bit for bit"
         if kind == "hard":
             assert exact[:, cnt == 1].all()
         print(f"[regions] merge {H}x{W} size {size} stride {stride} circular {circular} bs {bs} halves {halves} R {R} {kind}: "

@@ -160,16 +160,15 @@ with torch.no_grad():
         # gather + merge alone, at this chunk size: one step's worth captured in a graph and replayed
         if per == default_chunk:
             st = s._st
-            ws = st["windows"]
+            ws = st["regions"]                     # a panorama is the region walk with no regions
             lay = panorama.layout(panorama.Windows(64, 8), H, W)
             eps_in = torch.randn_like(ws.xw)
 
             def gm():
                 for first, k in lay.chunks(per):
-                    rows = k
-                    ops.window_gather(st["x_in"][:1], ws.oy, ws.ox, lay.h, lay.w, first, k, out=ws.xw[:rows],
-                                      out_dup=ws.xw[rows:2 * rows])
-                    ops.window_merge(eps_in[:2 * rows], ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, ws.eps, halves=2)
+                    rows = 2 * k                       # [u block; c block] of n = 1
+                    ops.region_gather(st["x_in"][:1], ws.oy, ws.ox, lay.h, lay.w, first, k, 0, 1, out=ws.xw[:rows])
+                    ops.region_merge(eps_in[:rows], ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, 0, None, ws.eps, halves=2)
 
             gm()
             torch.cuda.synchronize()

@@ -445,108 +445,13 @@ __global__ void __launch_bounds__(kBlendThreads) local_blend_kernel(float* x, fl
 }
 
 // ---------------------------------------------------------------------------------------------
-// MultiDiffusion window fusion (lib/model_zoo/panorama.py).  The canvas is fp32 NHWC [bs, H, W, C]; window g = iy*nx + ix covers
-// rows oy[iy] .. oy[iy]+h-1 and columns (ox[ix] + j) mod W, j < w, so a circular layout reads across the W seam and every other
-// layout never wraps.  VW = 4 moves whole float4s (C % 4 == 0, the latent's 4 channels); VW = 1 moves one float at a time.
-// ---------------------------------------------------------------------------------------------
-// windows [first, first+k) of x -> out [k*bs, h, w, C], row j*bs + b = window first+j of image b; out_dup (may be NULL) gets a copy
-template <int VW>
-__global__ void window_gather_kernel(const float* __restrict__ x, int bs, int H, int W, int C, const int* __restrict__ oy,
-                                     const int* __restrict__ ox, int nx, int h, int w, int first, long long total,
-                                     float* __restrict__ out, float* __restrict__ out_dup) {
-  const int cv = C / VW;
-  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
-       e += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(e % cv) * VW;
-    long long p = e / cv;
-    const int wx = static_cast<int>(p % w);
-    p /= w;
-    const int wy = static_cast<int>(p % h);
-    const long long row = p / h;
-    const int b = static_cast<int>(row % bs), g = first + static_cast<int>(row / bs);
-    int sx = ox[g % nx] + wx;
-    if (sx >= W) sx -= W;
-    const long long src = ((static_cast<long long>(b) * H + oy[g / nx] + wy) * W + sx) * C + c;
-    const long long dst = ((row * h + wy) * w + wx) * C + c;
-    if (VW == 4) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(x + src));
-      *reinterpret_cast<float4*>(out + dst) = v;
-      if (out_dup) *reinterpret_cast<float4*>(out_dup + dst) = v;
-    } else {
-      const float v = __ldg(x + src);
-      out[dst] = v;
-      if (out_dup) out_dup[dst] = v;
-    }
-  }
-}
-
-// The merge of windows [first, first+k): eps [halves*k*bs, h, w, C], half s at rows s*k*bs + j*bs + b; out [halves*bs, H, W, C].
-// The windows covering row y are iy in [cover_y[2y], cover_y[2y+1]); those covering column x are ix in [cover_x[4x], cover_x[4x+1])
-// then [cover_x[4x+2], cover_x[4x+3]), in ascending order.  Per element, over its covering windows in ascending window index: the
-// first one sets out, every later one adds to it (fp32, rounded to nearest), and the launch that holds the last one divides by
-// the count.  Calls over consecutive ranges therefore make the same operations in the same order as one call over all windows:
-// the result does not depend on the chunking, and with one covering window it is that window's eps bit for bit.
-template <int VW>
-__global__ void window_merge_kernel(const float* __restrict__ eps, int bs, int H, int W, int C, const int* __restrict__ oy,
-                                    const int* __restrict__ ox, const int* __restrict__ cover_y, const int* __restrict__ cover_x,
-                                    int nx, int h, int w, int first, int k, long long total, float* __restrict__ out) {
-  const int cv = C / VW;
-  const int last = first + k;
-  const long long plane = static_cast<long long>(h) * w * C;
-  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
-       e += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int c = static_cast<int>(e % cv) * VW;
-    long long p = e / cv;
-    const int x = static_cast<int>(p % W);
-    p /= W;
-    const int y = static_cast<int>(p % H);
-    const long long ob = p / H;                               // output row s*bs + b
-    const int s = static_cast<int>(ob / bs), b = static_cast<int>(ob % bs);
-    const int y0 = cover_y[2 * y], y1 = cover_y[2 * y + 1];
-    const int4 cx = *reinterpret_cast<const int4*>(cover_x + 4 * x);
-    const int xlo = cx.y > cx.x ? cx.x : cx.z, xhi = cx.w > cx.z ? cx.w - 1 : cx.y - 1;
-    const int g_first = y0 * nx + xlo, g_last = (y1 - 1) * nx + xhi;
-    if (g_last < first || g_first >= last) continue;          // no covering window in this range
-    float acc[VW];
-    float* o = out + ((ob * H + y) * W + x) * C + c;
-    if (g_first < first) {
-      if (VW == 4) *reinterpret_cast<float4*>(acc) = *reinterpret_cast<const float4*>(o);
-      else acc[0] = o[0];
-    }
-    for (int iy = y0; iy < y1; ++iy) {
-      const int wy = y - oy[iy];
-      for (int part = 0; part < 2; ++part) {
-        const int a0 = part ? cx.z : cx.x, a1 = part ? cx.w : cx.y;
-        for (int ix = a0; ix < a1; ++ix) {
-          const int g = iy * nx + ix;
-          if (g < first || g >= last) continue;
-          int wx = x - ox[ix];
-          if (wx < 0) wx += W;
-          const float* src = eps + (static_cast<long long>(s) * k + (g - first)) * bs * plane + b * plane +
-                             (static_cast<long long>(wy) * w + wx) * C + c;
-          float v[VW];
-          if (VW == 4) *reinterpret_cast<float4*>(v) = __ldg(reinterpret_cast<const float4*>(src));
-          else v[0] = __ldg(src);
-#pragma unroll
-          for (int q = 0; q < VW; ++q) acc[q] = g == g_first ? v[q] : __fadd_rn(acc[q], v[q]);
-        }
-      }
-    }
-    if (g_last < last) {
-      const float n = static_cast<float>((y1 - y0) * ((cx.y - cx.x) + (cx.w - cx.z)));
-#pragma unroll
-      for (int q = 0; q < VW; ++q) acc[q] = __fdiv_rn(acc[q], n);
-    }
-    if (VW == 4) *reinterpret_cast<float4*>(o) = *reinterpret_cast<float4*>(acc);
-    else o[0] = acc[0];
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// MultiDiffusion region prompts (lib/model_zoo/regions.py), on the window layout above.  masks fp32 [R, bs, H, W] on the canvas,
-// region r >= 1 at row r - 1; region 0 is the background, of weight m_0 = max(0, 1 - S), S = m_1 + ... + m_R.  A chunk's UNet
-// batch is ub + R + 1 blocks of [k*bs, h, w, C]: ub u blocks (0; 1, region 0's; or R + 1, one per region), then the R + 1 c
-// blocks, region r at c block r.  Row j*bs + b of a block is window first + j of image b.
+// MultiDiffusion region prompts (lib/model_zoo/regions.py) on a window layout; a panorama's window fusion (lib/model_zoo/
+// panorama.py) is the walk with no regions, R = 0.  The canvas is fp32 NHWC [bs, H, W, C]; window g = iy*nx + ix covers rows
+// oy[iy] .. oy[iy]+h-1 and columns (ox[ix] + j) mod W, j < w, so a circular layout reads across the W seam and every other layout
+// never wraps.  VW = 4 moves whole float4s (C % 4 == 0, the latent's 4 channels); VW = 1 moves one float at a time.
+// masks fp32 [R, bs, H, W] on the canvas, region r >= 1 at row r - 1; region 0 is the background, of weight m_0 = max(0, 1 - S),
+// S = m_1 + ... + m_R.  A chunk's UNet batch is ub + R + 1 blocks of [k*bs, h, w, C]: ub u blocks (0; 1, region 0's; or R + 1, one
+// per region), then the R + 1 c blocks, region r at c block r.  Row j*bs + b of a block is window first + j of image b.
 // ---------------------------------------------------------------------------------------------
 constexpr unsigned kRegionTag = 0x72676e73u;   // "rgns"
 constexpr int kRegionsMax = 8;
@@ -649,11 +554,17 @@ __global__ void region_noise_kernel(const unsigned long long* __restrict__ seed,
 }
 
 // The weighted merge of windows [first, first+k): eps [halves*(R+1)*k*bs, h, w, C], block s*(R+1) + r; out [halves*bs, H, W, C].
-// Per element p: S = m_1 + ... + m_R (ascending, rounded), m_0 = max(0, 1 - S), D = m_0 + S.  Over its covering windows in
-// ascending index, and r = 0..R inside each, every term m_r e_{j,r} of nonzero weight is one rounded product: the first sets out,
-// later ones are added; the launch holding the last window divides once by n D.  As window_merge_kernel, calls over consecutive
-// ranges make the same operations as one call.  Some weight is nonzero at every element (D >= 1 - 2^-24), so every covering window
-// adds at least one term.
+// The windows covering row y are iy in [cover_y[2y], cover_y[2y+1]); those covering column x are ix in [cover_x[4x], cover_x[4x+1])
+// then [cover_x[4x+2], cover_x[4x+3]), in ascending order.  Per element p: S = m_1 + ... + m_R (ascending, rounded; the first mask
+// sets S, and S = 0 when R = 0), m_0 = max(0, 1 - S), D = m_0 + S.  Over its covering windows in ascending index, and r = 0..R
+// inside each, every term m_r e_{j,r} of nonzero weight is one rounded product: the first sets out, later ones are added; the
+// launch holding the last window divides once by n D.  Calls over consecutive ranges therefore make the same operations in the
+// same order as one call over all windows: the result does not depend on the chunking.  Some weight is nonzero at every element
+// (D >= 1 - 2^-24), so every covering window adds at least one term.
+// With no regions (R = 0, masks unused) this is the uniform window average bit for bit: m_0 = max(0, 1 - 0) = 1, each term
+// 1 * e_j is e_j exactly for every finite or infinite value, so the first window's eps sets out and each later one is added with
+// one rounding; and n D = n * (1 + 0) is n exactly, so the last launch divides once by the count.  An element with one covering
+// window therefore gets that window's eps bit for bit.
 template <int VW>
 __global__ void region_merge_kernel(const float* __restrict__ eps, int bs, int H, int W, int C, const int* __restrict__ oy,
                                     const int* __restrict__ ox, const int* __restrict__ cover_y, const int* __restrict__ cover_x,
@@ -677,7 +588,7 @@ __global__ void region_merge_kernel(const float* __restrict__ eps, int bs, int H
     const int g_first = y0 * nx + xlo, g_last = (y1 - 1) * nx + xhi;
     if (g_last < first || g_first >= last) continue;          // no covering window in this range
     const float* mp = masks + (static_cast<long long>(b) * H + y) * W + x;
-    float S = __ldg(mp);
+    float S = R ? __ldg(mp) : 0.f;
     for (int r = 2; r <= R; ++r) S = __fadd_rn(S, __ldg(mp + (r - 1) * mplane));
     const float m0 = fmaxf(0.f, __fsub_rn(1.f, S));
     float acc[VW];
@@ -2117,7 +2028,7 @@ int vdb_local_blend_f32(float* x, float* x_dup, const float* map, const int* fla
   return launch(local_blend_kernel, n - 1, kBlendThreads, 0, stream, x, x_dup, map, flags, step_idx, H, W, C, h, w, threshold);
 }
 
-// the refusals shared by the two window entry points: sizes, the window range and the tables' alignment
+// the refusals shared by the region gather and merge: sizes, the window range and the tables' alignment
 static int window_args(const char* what, const void* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx,
                        int h, int w, int first, int k) {
   if (!x || !oy || !ox || bs <= 0 || H <= 0 || W <= 0 || C <= 0 || ny <= 0 || nx <= 0 || h <= 0 || w <= 0 || k <= 0)
@@ -2130,51 +2041,15 @@ static int window_args(const char* what, const void* x, int bs, int H, int W, in
   return 0;
 }
 
-int vdb_window_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
-                          int first, int k, float* out, float* out_dup, void* stream) {
-  if (!out) return set_error(VDB_ERR_INVALID, "window_gather: null/empty argument");
-  if (int st = window_args("window_gather", x, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(out_dup)) & 15)
-    return set_error(VDB_ERR_INVALID, "window_gather: pointers must be 16-byte aligned");
-  const long long nin = static_cast<long long>(bs) * H * W * C, nout = static_cast<long long>(k) * bs * h * w * C;
-  // the window batch is written while the canvas is read through the read-only path: no byte may be shared
-  if (overlaps(out, nout, x, nin) || overlaps(out_dup, nout, x, nin) || overlaps(out, nout, out_dup, nout))
-    return set_error(VDB_ERR_INVALID, "window_gather: x, out and out_dup must not overlap");
-  if ((C & 3) == 0)
-    return launch(window_gather_kernel<4>, ew_blocks(nout / 4, 256), 256, 0, stream, x, bs, H, W, C, oy, ox, nx, h, w, first,
-                  nout / 4, out, out_dup);
-  return launch(window_gather_kernel<1>, ew_blocks(nout, 256), 256, 0, stream, x, bs, H, W, C, oy, ox, nx, h, w, first, nout, out,
-                out_dup);
-}
-
-int vdb_window_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox,
-                         const int* cover_y, const int* cover_x, int ny, int nx, int h, int w, int first, int k, float* out,
-                         void* stream) {
-  if (!out || !cover_y || !cover_x || (halves != 1 && halves != 2))
-    return set_error(VDB_ERR_INVALID, "window_merge: null/empty argument (halves 1 or 2)");
-  if (int st = window_args("window_merge", eps, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
-  if ((reinterpret_cast<uintptr_t>(eps) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(cover_x)) & 15 ||
-      reinterpret_cast<uintptr_t>(cover_y) & 3)
-    return set_error(VDB_ERR_INVALID, "window_merge: eps, out and cover_x must be 16-byte aligned, cover_y 4-byte");
-  const long long nout = static_cast<long long>(halves) * bs * H * W * C;
-  if (overlaps(out, nout, eps, static_cast<long long>(halves) * k * bs * h * w * C))
-    return set_error(VDB_ERR_INVALID, "window_merge: eps overlaps out");
-  if ((C & 3) == 0)
-    return launch(window_merge_kernel<4>, ew_blocks(nout / 4, 256), 256, 0, stream, eps, bs, H, W, C, oy, ox, cover_y, cover_x, nx,
-                  h, w, first, k, nout / 4, out);
-  return launch(window_merge_kernel<1>, ew_blocks(nout, 256), 256, 0, stream, eps, bs, H, W, C, oy, ox, cover_y, cover_x, nx, h, w,
-                first, k, nout, out);
-}
-
 int vdb_region_gather_f32(const float* x, int bs, int H, int W, int C, const int* oy, const int* ox, int ny, int nx, int h, int w,
                           int first, int k, int R, int u_blocks, const float* masks, const float* rows, const int* step_idx,
                           const unsigned long long* seed, const float* bg, int nb, const float* noise, float* out, void* stream) {
   if (!out) return set_error(VDB_ERR_INVALID, "region_gather: null/empty argument");
   if (int st = window_args("region_gather", x, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
-  if (R < 1 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_gather: R must be in [1, %d], got %d", kRegionsMax, R);
+  if (R < 0 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_gather: R must be in [0, %d], got %d", kRegionsMax, R);
   if (u_blocks != 0 && u_blocks != 1 && u_blocks != R + 1)
     return set_error(VDB_ERR_INVALID, "region_gather: u_blocks must be 0, 1 or R + 1 = %d, got %d", R + 1, u_blocks);
-  if (rows && (!masks || !step_idx || !seed || !bg || nb <= 0))
+  if (rows && ((R > 0 && !masks) || !step_idx || !seed || !bg || nb <= 0))
     return set_error(VDB_ERR_INVALID, "region_gather: null/empty argument (rows needs masks, step_idx, seed and nb > 0 backgrounds)");
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(noise)) & 15 ||
       (reinterpret_cast<uintptr_t>(masks) | reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(bg) |
@@ -2206,10 +2081,10 @@ int vdb_region_noise_f32(const unsigned long long* seed, const int* step_idx, lo
 int vdb_region_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox, const int* cover_y,
                          const int* cover_x, int ny, int nx, int h, int w, int first, int k, int R, const float* masks, float* out,
                          void* stream) {
-  if (!out || !cover_y || !cover_x || !masks || (halves != 1 && halves != 2))
+  if (!out || !cover_y || !cover_x || (R > 0 && !masks) || (halves != 1 && halves != 2))
     return set_error(VDB_ERR_INVALID, "region_merge: null/empty argument (halves 1 or 2)");
   if (int st = window_args("region_merge", eps, bs, H, W, C, oy, ox, ny, nx, h, w, first, k)) return st;
-  if (R < 1 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_merge: R must be in [1, %d], got %d", kRegionsMax, R);
+  if (R < 0 || R > kRegionsMax) return set_error(VDB_ERR_INVALID, "region_merge: R must be in [0, %d], got %d", kRegionsMax, R);
   if ((reinterpret_cast<uintptr_t>(eps) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(cover_x)) & 15 ||
       (reinterpret_cast<uintptr_t>(cover_y) | reinterpret_cast<uintptr_t>(masks)) & 3)
     return set_error(VDB_ERR_INVALID, "region_merge: eps, out and cover_x must be 16-byte aligned, cover_y and masks 4-byte");

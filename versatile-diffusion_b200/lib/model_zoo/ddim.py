@@ -24,7 +24,7 @@ def _ops():
 
 # ------------------------------------------------------------------ sampling modes and how they combine
 # A mode is selected by an optional input: x_info['regions'] (lib/model_zoo/regions.py), x_info['windows'] (lib/model_zoo/
-# panorama.py), a context's 'prompt_edit'
+# panorama.py: the region walk with no regions), a context's 'prompt_edit'
 # (prompt_edit.py), x_info['inversion'] (edit.py) and x_info['inpaint_mask'] (inpaint.py).  The start inputs x_info['x0'] (with
 # 'x0_forward_timesteps') and x_info['xt'] select no mode, but some modes refuse them.
 #
@@ -220,13 +220,12 @@ class DDIMSampler(object):
         (the order in which refusals win) -> [SamplerMode].  Host work only: every refusal comes before any device work."""
         from .edit import FromInversion
         from .inpaint import Inpainting
-        from .panorama import WindowFusion
         from .prompt_edit import PromptEditing
         from .regions import RegionPrompts
         refuse(entry, x_info, c_infos)
         given = given_inputs(x_info, c_infos)
         taken = {k for m in given for k in TAKES.get(m, ())}
-        return [cls(self, x_info, shape, c_infos) for name, cls in (('regions', RegionPrompts), ('windows', WindowFusion),
+        return [cls(self, x_info, shape, c_infos) for name, cls in (('regions', RegionPrompts), ('windows', RegionPrompts),
                                                                       ('prompt_edit', PromptEditing), ('inversion', FromInversion),
                                                                       ('inpaint_mask', Inpainting))
                 if name in given and name not in taken]
@@ -318,18 +317,15 @@ class DDIMSampler(object):
         x_info['x'] = pred_xt
         return pred_xt, intermediates
 
-    def _contexts(self, c_infos, cfg, x_type, multi, buffer_tag=None, repeat=1):
+    def _contexts(self, c_infos, cfg, x_type, multi, buffer_tag=None):
         """[uncond ; cond] of every context, built once (the reference re-concatenates every step, ddim.py:146), in persistent
-        padded buffers (per buffer_tag, so the inversion and the window chunks keep their own) -> (contexts, c_types, ratios,
-        time_from, model_channels).  repeat = k: each half's rows repeated k times, [u; u; ...; c; c; ...], the contexts of a
-        chunk of k windows (lib/model_zoo/panorama.py)."""
+        padded buffers (per buffer_tag, so the inversion keeps its own) -> (contexts, c_types, ratios, time_from,
+        model_channels)."""
         from .attention import PaddedContext
         ctxs = []
         for i, ci in enumerate(c_infos):
             c = torch.cat([ci['unconditional_conditioning'], ci['conditioning']]) if cfg else ci['conditioning']
             ci['c'] = c
-            if repeat != 1:
-                c = torch.cat([h.repeat(repeat, 1, 1) for h in c.chunk(2 if cfg else 1)])
             ctxs.append(PaddedContext(self._ctx_buffer(i if buffer_tag is None else (buffer_tag, i), c), c.shape[1]))
         c_types = [ci['type'] for ci in c_infos]
         ratios = [float(ci.get('ratio', 1.0)) for ci in c_infos]

@@ -22,13 +22,14 @@ the same a and b for every window), the CFG mix, and DPM-Solver++'s data predict
 averaging the per-window eps into a canvas eps and running the unchanged update on the whole canvas.  Under CFG the unconditional
 and conditional halves are averaged separately, then mixed by vdb_ddim_cfg_step / vdb_dpmpp_cfg_step.
 
-Step.  Inside the sampler's step, the UNet call on the canvas becomes, for each chunk of at most WINDOWS_PER_CHUNK windows in
-window order: vdb_window_gather_f32 (canvas -> [u rows of the chunk's windows; c rows], an exact copy), the UNet on that batch
-with window contexts (each context row repeated per window, in persistent buffers of their own), and vdb_window_merge_f32 into a
-persistent canvas eps [e_u; e_c].  Everything after it is untouched: the update, the inpainting blend, the DPM-Solver++ history
-ring (which holds the canvas).
+Step.  A panorama is the region walk of lib/model_zoo/regions.py with no regions (R = 0).  Inside the sampler's step, the UNet
+call on the canvas becomes, for each chunk of at most WINDOWS_PER_CHUNK windows in window order: vdb_region_gather_f32 at R = 0
+(canvas -> [u rows of the chunk's windows; c rows], exact copies), the UNet on that batch with window contexts (each context row
+repeated per window, in persistent buffers of their own), and vdb_region_merge_f32 at R = 0 into a persistent canvas eps
+[e_u; e_c].  Everything after it is untouched: the update, the inpainting blend, the DPM-Solver++ history ring (which holds the
+canvas).
 
-Merge.  Uniform weights, as in the paper.  Each canvas element is the fp32 sum of the eps of its covering windows, taken in
+Merge.  Uniform weights, as in the paper (at R = 0 every weight of the region merge is 1 and its D is 1, exactly).  Each canvas element is the fp32 sum of the eps of its covering windows, taken in
 ascending window index, divided by the integer count: the first window sets the sum, each later one is added with
 round-to-nearest, and the division is one round-to-nearest.  Each output element loops over its covering windows (gather form):
 no atomics, so the result is bit-reproducible and the graph path equals the eager path.  Merges over consecutive chunks make the
@@ -47,13 +48,6 @@ a 64x256 latent, and it grows quadratically with wider canvases.
 """
 import numpy as np
 import torch
-
-from .ddim import SamplerMode, buffers_key, refuse
-
-
-def _ops():
-    from vdb200 import ops
-    return ops
 
 
 # Windows per UNet call.  A chunk's UNet batch is 2 * WINDOWS_PER_CHUNK * n under CFG; larger chunks amortise the per-call launch
@@ -154,66 +148,15 @@ def layout(windows, H, W):
     return Layout(windows, H, W)
 
 
-class WindowState(object):
-    """The device side of a windowed walk, persistent across calls so a captured step graph replays: the layout tables, the
-    window batch of a full chunk ([u rows; c rows]) and the canvas eps [e_u; e_c]."""
+class LayoutTables(object):
+    """A layout's int32 tables on the device, in one buffer (`tables`) read through the views cover_x, cover_y, oy and ox.  They
+    depend on the layout's key alone, so state kept under that key never needs them refilled."""
 
-    def __init__(self, lay, per, bs, cfg, C, device):
-        self.key = lay.key() + (per, bs, cfg, C)
+    def __init__(self, lay, device):
         tab, offs = lay.table()
-        self.tables = torch.zeros(tab.size, dtype=torch.int32, device=device)
+        self.tables = torch.from_numpy(tab).to(device)
         for name, (o, n) in offs.items():
             setattr(self, name, self.tables[o:o + n])
-        halves = 2 if cfg else 1
-        self.xw = torch.zeros(halves * min(per, lay.nwin) * bs, lay.h, lay.w, C, dtype=torch.float32, device=device)
-        self.eps = torch.zeros(halves * bs, lay.H, lay.W, C, dtype=torch.float32, device=device)
-
-    def fill(self, lay):
-        """refill the layout tables in place"""
-        self.tables.copy_(torch.from_numpy(lay.table()[0]))
-
-
-class WindowFusion(SamplerMode):
-    """x_info['windows'] in the sampler's walk: the windowed eps in place of the UNet call on the canvas."""
-
-    def __init__(self, sampler, x_info, shape, c_infos):
-        """The host-side refusals of a windowed call, before any device work."""
-        if not isinstance(x_info['windows'], Windows):
-            raise ValueError(f"x_info['windows'] must be a panorama.Windows, got {type(x_info['windows']).__name__}")
-        refuse('windows', x_info, c_infos)
-        if len(shape) != 4:
-            raise ValueError(f"windows need an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
-        self.lay = layout(x_info['windows'], shape[2], shape[3])
-        self.per = WINDOWS_PER_CHUNK
-        self.chunks = self.lay.chunks(self.per)
-
-    def prepare(self, sampler, run):
-        """Refill the WindowState in place and the window contexts (each context row repeated per window), which become the
-        contexts whose K / V^T the step reads."""
-        lay, per = self.lay, self.per
-        ws = run.walk.get('windows')
-        if ws is None or ws.key != lay.key() + (per, run.bs, run.cfg, run.C):
-            ws = run.walk['windows'] = WindowState(lay, per, run.bs, run.cfg, run.C, run.device)
-        ws.fill(lay)
-        self.ws = ws
-        self.ctxs = {k: sampler._contexts(run.c_infos, run.cfg, run.x_type, run.multi, buffer_tag=('windows', k), repeat=k)[0]
-                     for k in sorted({k for _, k in self.chunks})}
-        run.kv_types = [ct for _ in self.ctxs for ct in run.c_types]
-        run.kv_ctxs = [c for k in self.ctxs for c in self.ctxs[k]]
-        return ('windows', lay.key(), per) + buffers_key(ws.tables, ws.xw, ws.eps)
-
-    def eps(self, sampler, run):
-        """gather -> UNet -> merge per chunk of windows, into the canvas eps [e_u; e_c]"""
-        ops, ws, lay, bs = _ops(), self.ws, self.lay, run.bs
-        halves = run.B // bs
-        t_emb = ops.timestep_embedding(run.walk['ts'], run.mch, step_idx=run.walk['idx'], batch=ws.xw.shape[0])
-        for first, k in self.chunks:
-            rows = k * bs
-            xw = ws.xw[:halves * rows]
-            ops.window_gather(run.x, ws.oy, ws.ox, lay.h, lay.w, first, k, out=xw[:rows], out_dup=xw[rows:] if run.cfg else None)
-            e = sampler.model.eps_nhwc(xw, run.x_type, t_emb[:xw.shape[0]], run.c_types, self.ctxs[k], run.ratios, run.time_from)
-            ops.window_merge(e, ws.oy, ws.ox, ws.cover_y, ws.cover_x, first, k, ws.eps, halves=halves)
-        return ws.eps
 
 
 @torch.no_grad()

@@ -4,8 +4,9 @@ The reference has no region mode; this is an addition, and its semantics are spe
 applies: "a red car on the left, a pine forest on the right, a snowy sky above".  The method is the region-based mode of
 MultiDiffusion (Bar-Tal et al., "MultiDiffusion: Fusing Diffusion Paths for Controlled Image Generation", ICML 2023, section 4.2):
 every step runs one UNet pass per region, each with its own context, and every latent element takes the mask-weighted average of
-the regions' predictions.  It needs no retraining, and it combines with the window fusion of lib/model_zoo/panorama.py.  A region's
-context may be a CLIP image context, so one region can follow a reference photo while another follows text.
+the regions' predictions.  It needs no retraining, and it combines with the window fusion of lib/model_zoo/panorama.py, which is
+this walk with no regions (R = 0).  A region's context may be a CLIP image context, so one region can follow a reference photo
+while another follows text.
 
 API.  x_info['regions'] = Regions([Region(mask, conditioning), ...], bootstrap_steps=0, backgrounds=None) on DDIMSampler.sample /
 sample_multicontext and DPMSolverSampler (same methods).
@@ -38,10 +39,9 @@ a x + b e: averaging eps and running the unchanged update on the canvas is the s
 DPM-Solver++'s data predictions, and the img2img start, the inpainting blend and the DPM-Solver++ history ring run unchanged.  With
 soft masks and bootstrapping the per-region inputs differ where 0 < m_r < 1, and the mask-weighted eps average is the definition.
 
-CFG layout.  A chunk's batch is [u blocks; c blocks]; within a block, row j bs + b is window first + j of image b, as the window
-gather writes it.
-  - Without bootstrapping the unconditional half is one block, region 0's context on the plain latent, averaged over windows by
-    vdb_window_merge_f32 (halves = 1) as a panorama's.  The c blocks go through vdb_region_merge_f32.
+CFG layout.  A chunk's batch is [u blocks; c blocks]; within a block, row j bs + b is window first + j of image b.
+  - Without bootstrapping the unconditional half is one block, region 0's context on the plain latent, averaged over windows as a
+    panorama's (vdb_region_merge_f32 at R = 0, halves = 1).  The c blocks go through vdb_region_merge_f32 at R.
   - With bootstrapping each region's input differs from the canvas, so each block has its own unconditional row (R + 1 u blocks)
     and both halves go through the weighted merge.  Then e_u + s (e_c - e_u) = sum_r m_r (u_r + s (c_r - u_r)) / D, the paper's
     per-region guided eps.
@@ -61,8 +61,9 @@ which pins its object inside the mask.
 Step.  Inside the sampler's step, for each chunk of max(1, WINDOWS_PER_CHUNK // (R + 1)) windows (so a UNet call holds about as
 many items as a panorama chunk): vdb_region_gather_f32 (canvas -> the chunk's batch, every block in one launch), the UNet on the
 batch with the region contexts ([u...; c_0...; c_R...], each row repeated per window, in persistent buffers of their own), and the
-merges into a persistent canvas eps [e_u; e_c].  The walk's state (RegionState: the layout tables, masks, step rows, backgrounds
-and key, the chunk batch and the canvas eps) is refilled in place, so a cached step graph replays on new prompts and masks.
+merges into a persistent canvas eps [e_u; e_c].  The walk's state (RegionState: the layout tables, the masks, the step rows,
+backgrounds and key while bootstrapping, the chunk batch and the canvas eps) is refilled in place, so a cached step graph replays
+on new prompts and masks.
 
 Refusals, before any device work.  ValueError: x_info['regions'] not a Regions; a text latent; a mask or conditioning of the wrong
 type or shape; mask values outside [0, 1] or NaN; R outside [1, 8]; bootstrap_steps outside [0, steps]; bootstrapping without
@@ -84,7 +85,7 @@ import torch
 
 from .ddim import SamplerMode, buffers_key, refuse
 from .diffusion_utils import to_numpy
-from .panorama import Windows, layout
+from .panorama import LayoutTables, Windows, layout
 
 REGIONS_MAX = 8
 
@@ -161,19 +162,17 @@ def latent_masks(regs, bs, H, W, device):
     return out
 
 
-class RegionState(object):
+class RegionState(LayoutTables):
     """The device side of a region walk, persistent across calls so a captured step graph replays: the layout tables, the masks
-    [R, bs, H, W], the step rows, the backgrounds, the key, the chunk batch and the canvas eps [e_u; e_c]."""
+    [R, bs, H, W] (R >= 1), the step rows, the backgrounds and the key (while bootstrapping: nb > 0), the chunk batch and the
+    canvas eps [e_u; e_c].  What the walk does not use is None."""
 
     def __init__(self, key, lay, per, bs, cfg, C, R, ub, nb, device):
+        super().__init__(lay, device)
         self.key = key
-        tab, offs = lay.table()
-        self.tables = torch.zeros(tab.size, dtype=torch.int32, device=device)
-        for name, (o, n) in offs.items():
-            setattr(self, name, self.tables[o:o + n])
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=device)
-        self.masks, self.rows, self.seed = z(R, bs, lay.H, lay.W), z(1000, 4), z(1, dtype=torch.int64)
-        self.bg = z(nb, C) if nb else None
+        self.masks = z(R, bs, lay.H, lay.W) if R else None
+        self.rows, self.seed, self.bg = (z(1000, 4), z(1, dtype=torch.int64), z(nb, C)) if nb else (None, None, None)
         self.xw = z((ub + R + 1) * min(per, lay.nwin) * bs, lay.h, lay.w, C)
         self.eps = z((2 if cfg else 1) * bs, lay.H, lay.W, C)
 
@@ -182,18 +181,23 @@ class RegionState(object):
 
 
 class RegionPrompts(SamplerMode):
-    """x_info['regions'] in the sampler's walk: the mask-weighted eps of the regions in place of the UNet call on the canvas."""
+    """x_info['regions'] in the sampler's walk: the mask-weighted eps of the regions in place of the UNet call on the canvas.  With
+    x_info['windows'] alone it is a panorama's window fusion: the walk with no regions (R = 0)."""
 
     def __init__(self, sampler, x_info, shape, c_infos):
-        """The host-side refusals of a region call, before any device work."""
-        regs = x_info['regions']
-        if not isinstance(regs, Regions):
+        """The host-side refusals of a region or panorama call, before any device work."""
+        regs, win = x_info.get('regions', None), x_info.get('windows', None)
+        who = 'windows' if regs is None else 'regions'
+        if regs is None:
+            _check_windows(win)
+        elif not isinstance(regs, Regions):
             raise ValueError(f"x_info['regions'] must be a regions.Regions, got {type(regs).__name__}")
-        refuse('regions', x_info, c_infos)
+        refuse(who, x_info, c_infos)
         if len(shape) != 4:
-            raise ValueError(f"regions need an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
+            raise ValueError(f"{who} need an image latent [bs, C, H, W], got shape {list(shape)} (a text latent?)")
         bs, C, H, W = shape
-        for r, reg in enumerate(regs.regions, 1):
+        self.regions = [] if regs is None else regs.regions
+        for r, reg in enumerate(self.regions, 1):
             m = reg.mask
             if m.dim() != 3 or m.shape[0] not in (1, bs) or tuple(m.shape[1:]) not in ((H, W), (8 * H, 8 * W)):
                 raise ValueError(f"region {r}: mask expected [{bs} or 1, {H}, {W}] (latent) or [{bs} or 1, {8 * H}, {8 * W}] "
@@ -206,18 +210,18 @@ class RegionPrompts(SamplerMode):
                 if tuple(c.shape) != tuple(ci['conditioning'].shape):
                     raise ValueError(f"region {r}: conditioning {i} expected {tuple(ci['conditioning'].shape)} (as the call's), "
                                      f"got {tuple(c.shape)}")
-        steps = len(sampler.ddim_timesteps)
-        if regs.bootstrap_steps > steps:
-            raise ValueError(f"Regions: bootstrap_steps must lie in [0, {steps}] (the steps), got {regs.bootstrap_steps}")
-        if regs.backgrounds is not None and regs.backgrounds.shape[1] != C:
-            raise ValueError(f"Regions: backgrounds expected [nb, {C}], got {tuple(regs.backgrounds.shape)}")
-        win = x_info.get('windows', None)
+        if regs is not None:
+            steps = len(sampler.ddim_timesteps)
+            if regs.bootstrap_steps > steps:
+                raise ValueError(f"Regions: bootstrap_steps must lie in [0, {steps}] (the steps), got {regs.bootstrap_steps}")
+            if regs.backgrounds is not None and regs.backgrounds.shape[1] != C:
+                raise ValueError(f"Regions: backgrounds expected [nb, {C}], got {tuple(regs.backgrounds.shape)}")
         if win is None:
             side = max(H, W, 8)
             win = Windows(side, side)
-        elif not isinstance(win, Windows):
-            raise ValueError(f"x_info['windows'] must be a panorama.Windows, got {type(win).__name__}")
-        self.regs, self.R, self.boot = regs, len(regs), regs.bootstrap_steps > 0
+        else:
+            _check_windows(win)
+        self.regs, self.R, self.boot = regs, len(self.regions), regs is not None and regs.bootstrap_steps > 0
         self.lay = layout(win, H, W)
         from . import panorama
         self.per = max(1, panorama.WINDOWS_PER_CHUNK // (self.R + 1))
@@ -237,14 +241,14 @@ class RegionPrompts(SamplerMode):
         st = run.walk.get('regions')
         if st is None or st.key != key:
             st = run.walk['regions'] = RegionState(key, lay, per, run.bs, run.cfg, run.C, R, self.ub, nb, run.device)
-        st.tables.copy_(torch.from_numpy(lay.table()[0]))
-        st.masks.copy_(latent_masks(regs, run.bs, lay.H, lay.W, run.device))
+        if R:
+            st.masks.copy_(latent_masks(regs, run.bs, lay.H, lay.W, run.device))
         if self.boot:
             st.rows[:run.total].copy_(torch.from_numpy(step_rows(sampler.ddim_alphas, run.total, regs.bootstrap_steps)))
             st.bg.copy_(regs.backgrounds.to(device=run.device, dtype=torch.float32))
             st.seed.copy_(self.seed)
         self.st = st
-        self.ctxs = {k: region_contexts(sampler, run, regs, k, self.ub) for k in sorted({k for _, k in self.chunks})}
+        self.ctxs = {k: region_contexts(sampler, run, self.regions, k, self.ub) for k in sorted({k for _, k in self.chunks})}
         run.kv_types = [ct for _ in self.ctxs for ct in run.c_types]
         run.kv_ctxs = [c for k in self.ctxs for c in self.ctxs[k]]
         return ('regions', lay.key(), per, R, self.ub, nb) + buffers_key(*st.buffers())
@@ -260,22 +264,28 @@ class RegionPrompts(SamplerMode):
             ops.region_gather(run.x, st.oy, st.ox, lay.h, lay.w, first, k, R, ub, out=xw, masks=st.masks, **boot)
             e = sampler.model.eps_nhwc(xw, run.x_type, t_emb[:xw.shape[0]], run.c_types, self.ctxs[k], run.ratios, run.time_from)
             tabs = (st.oy, st.ox, st.cover_y, st.cover_x, first, k)
-            if ub == 1:         # one u block on the plain latent: the window average; the c blocks: the weighted merge
-                ops.window_merge(e[:rows], *tabs, st.eps[:bs], halves=1)
+            if ub == 1 and R:   # one u block on the plain latent: the window average (R = 0); the c blocks: the weighted merge
+                ops.region_merge(e[:rows], *tabs, 0, None, st.eps[:bs], halves=1)
                 ops.region_merge(e[rows:], *tabs, R, st.masks, st.eps[bs:], halves=1)
             else:
                 ops.region_merge(e, *tabs, R, st.masks, st.eps, halves=2 if ub else 1)
         return st.eps
 
 
-def region_contexts(sampler, run, regs, k, ub):
+def _check_windows(win):
+    if not isinstance(win, Windows):
+        raise ValueError(f"x_info['windows'] must be a panorama.Windows, got {type(win).__name__}")
+
+
+def region_contexts(sampler, run, regions, k, ub):
     """The contexts of a chunk of k windows, one per c_info, in persistent buffers of their own: blocks [u x ub; c_0; c_1 ..
-    c_R], each block's bs rows repeated k times (row j bs + b is image b)."""
+    c_R] (c_1 .. c_R from the Region list `regions`, none for a panorama), each block's bs rows repeated k times (row j bs + b is
+    image b)."""
     from .attention import PaddedContext
     ctxs = []
     for i, ci in enumerate(run.c_infos):
         c0 = ci['conditioning']
-        blocks = [ci['unconditional_conditioning']] * ub + [c0] + [reg.conds[i] for reg in regs.regions]
+        blocks = [ci['unconditional_conditioning']] * ub + [c0] + [reg.conds[i] for reg in regions]
         c = torch.cat([b.to(device=c0.device, dtype=c0.dtype).repeat(k, 1, 1) for b in blocks])
         ctxs.append(PaddedContext(sampler._ctx_buffer((('regions', k), i), c), c.shape[1]))
     return ctxs

@@ -36,8 +36,6 @@ SIGNATURES = {
     "vdb_inversion_blend_f32": (i, [p, p, p, i, p, i, p, i, ll, i, p]),
     "vdb_diffedit_mask_f32": (i, [p, p, f, p, p, f, i, i, ll, i, f, p, p]),
     "vdb_local_blend_f32": (i, [p, p, p, p, p, i, i, i, i, i, i, f, p]),
-    "vdb_window_gather_f32": (i, [p, i, i, i, i, p, p, i, i, i, i, i, i, p, p, p]),
-    "vdb_window_merge_f32": (i, [p, i, i, i, i, i, p, p, p, p, i, i, i, i, i, i, p, p]),
     "vdb_region_gather_f32": (i, [p, i, i, i, i, p, p, i, i, i, i, i, i, i, i, p, p, p, p, p, i, p, p, p]),
     "vdb_region_noise_f32": (i, [p, p, ll, i, i, i, p, p, p]),
     "vdb_region_merge_f32": (i, [p, i, i, i, i, i, p, p, p, p, i, i, i, i, i, i, i, p, p, p]),

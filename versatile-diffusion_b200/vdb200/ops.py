@@ -546,47 +546,6 @@ def local_blend(x, wmap, flags, step_idx, h, w, threshold, x_dup=None):
     return x
 
 
-def window_gather(x, oy, ox, h, w, first, k, out=None, out_dup=None):
-    """Windows [first, first + k) of the canvas x fp32 NHWC [bs, H, W, C] -> out [k*bs, h, w, C] (row j*bs + b: window first + j
-    of image b), and a copy into out_dup when given (lib/model_zoo/panorama.py).  oy / ox: int32 device origin tables."""
-    for name, t in (("x", x), ("out", out), ("out_dup", out_dup)):
-        _need(t, torch.float32, name)
-    _need(oy, torch.int32, "oy"); _need(ox, torch.int32, "ox")
-    bs, H, W, C = x.shape
-    shape = (k * bs, h, w, C)
-    if out is None:
-        out = torch.empty(shape, dtype=torch.float32, device=x.device)
-    for name, t in (("out", out), ("out_dup", out_dup)):
-        if t is not None and tuple(t.shape) != shape:
-            raise ValueError(f"{name}: expected {shape}, got {tuple(t.shape)}")
-    check(lib.vdb_window_gather_f32(_ptr(x), bs, H, W, C, _ptr(oy), _ptr(ox), oy.numel(), ox.numel(), int(h), int(w), int(first),
-                                    int(k), _ptr(out), _ptr(out_dup), _stream()), "window_gather")
-    return out
-
-
-def window_merge(eps, oy, ox, cover_y, cover_x, first, k, out, halves=1):
-    """Merge windows [first, first + k) of eps fp32 [halves*k*bs, h, w, C] into the canvas out [halves*bs, H, W, C] (lib/model_zoo/
-    panorama.py): the running fp32 sum over each element's covering windows in ascending window index, divided by their count
-    at the element's last one.  oy / ox / cover_y [H, 2] / cover_x [W, 4]: int32 device tables.  halves = 2 under CFG: eps is
-    [u rows; c rows] and out [e_u; e_c]."""
-    for name, t in (("eps", eps), ("out", out)):
-        _need(t, torch.float32, name)
-    for name, t in (("oy", oy), ("ox", ox), ("cover_y", cover_y), ("cover_x", cover_x)):
-        _need(t, torch.int32, name)
-    n, H, W, C = out.shape
-    if halves not in (1, 2) or n % halves:
-        raise ValueError(f"halves must be 1 or 2 and divide the {n} rows of out, got {halves}")
-    bs = n // halves
-    if eps.dim() != 4 or eps.shape[0] != k * n or eps.shape[3] != C:
-        raise ValueError(f"eps: expected [{k * n}, h, w, {C}] for out {tuple(out.shape)}, got {tuple(eps.shape)}")
-    _, h, w, _ = eps.shape
-    if cover_y.numel() != 2 * H or cover_x.numel() != 4 * W:
-        raise ValueError(f"cover tables: expected {2 * H} and {4 * W} entries, got {cover_y.numel()} and {cover_x.numel()}")
-    check(lib.vdb_window_merge_f32(_ptr(eps), halves, bs, H, W, C, _ptr(oy), _ptr(ox), _ptr(cover_y), _ptr(cover_x), oy.numel(),
-                                   ox.numel(), int(h), int(w), int(first), int(k), _ptr(out), _stream()), "window_merge")
-    return out
-
-
 def _region_masks(masks, R, bs, H, W):
     if masks is not None and masks.numel() != R * bs * H * W:
         raise ValueError(f"masks: expected [{R}, {bs}, {H}, {W}], got {tuple(masks.shape)}")
@@ -595,10 +554,11 @@ def _region_masks(masks, R, bs, H, W):
 def region_gather(x, oy, ox, h, w, first, k, R, u_blocks, out=None, masks=None, rows=None, step_idx=None, seed=None, bg=None,
                   noise=None):
     """Windows [first, first + k) of the canvas x fp32 NHWC [bs, H, W, C] -> the chunk batch out [(u_blocks + R + 1)*k*bs, h, w, C]
-    of a region walk (lib/model_zoo/regions.py): u_blocks (0, 1 or R + 1) u blocks, then the R + 1 c blocks.  Exact copies unless
-    rows (fp32 [., 4] {on, a, b, 0} device rows, row step_idx[0]) is on: then region r >= 1 reads m x + (1 - m) (a bg + b z) with
-    masks fp32 [R, bs, H, W], bg fp32 [nb, C] picked by the Philox stream keyed by seed (int64 device word), and z = noise (fp32
-    like x) when given, else that stream's normals."""
+    of a region walk (lib/model_zoo/regions.py; R = 0 is a panorama's): u_blocks (0, 1 or R + 1) u blocks, then the R + 1 c blocks
+    (row j*bs + b of a block: window first + j of image b).  oy / ox: int32 device origin tables.  Exact copies unless rows (fp32
+    [., 4] {on, a, b, 0} device rows, row step_idx[0]) is on: then region r >= 1 reads m x + (1 - m) (a bg + b z) with masks fp32
+    [R, bs, H, W], bg fp32 [nb, C] picked by the Philox stream keyed by seed (int64 device word), and z = noise (fp32 like x) when
+    given, else that stream's normals."""
     for name, t in (("x", x), ("out", out), ("masks", masks), ("rows", rows), ("bg", bg), ("noise", noise)):
         _need(t, torch.float32, name)
     _need(oy, torch.int32, "oy"); _need(ox, torch.int32, "ox"); _need(step_idx, torch.int32, "step_idx")
@@ -636,7 +596,10 @@ def region_noise(seed, step_idx, n, R, bs, nb):
 
 def region_merge(eps, oy, ox, cover_y, cover_x, first, k, R, masks, out, halves=1):
     """The mask-weighted merge of windows [first, first + k) of eps fp32 [halves*(R+1)*k*bs, h, w, C] (block s*(R+1) + r) into the
-    canvas out [halves*bs, H, W, C] (lib/model_zoo/regions.py).  masks fp32 [R, bs, H, W]; the tables are window_merge's."""
+    canvas out [halves*bs, H, W, C] (lib/model_zoo/regions.py): the running fp32 sum over each element's covering windows in
+    ascending window index, divided at the element's last one.  masks fp32 [R, bs, H, W], None when R = 0: then the merge is the
+    plain window average of a panorama.  oy / ox / cover_y [H, 2] / cover_x [W, 4]: int32 device tables.  halves = 2 under CFG:
+    eps is [u blocks; c blocks] and out [e_u; e_c]."""
     for name, t in (("eps", eps), ("out", out), ("masks", masks)):
         _need(t, torch.float32, name)
     for name, t in (("oy", oy), ("ox", ox), ("cover_y", cover_y), ("cover_x", cover_x)):
