@@ -396,24 +396,25 @@ int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const fl
                      void* stream);
 /* Attention.forward for the one new query of each row (optimus_gpt2.py:205-227, _attn :152-175), d_head 64.  qkv [R, ldq] holds
  * c_attn's q | k | v (H*64 each); this step's k / v are appended at slot *step of kcache / vcache ([R][H][T][64] fp32, this
- * layer); the keys are the layer's latent slice mem[r, h*64 ..] (key == value, position 0) then slots 0 .. *step.  out [R, H*64]. */
-int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache, int R,
-                          int H, int T, const int* step, float scale, float* out, long long ldo, void* stream);
+ * layer); the keys are the layer's latent slice mem[r, h*64 ..] (key == value, position 0) then slots 0 .. *step.  out [R, H*64].
+ * src (may be NULL; beam search): cache slot j < *step of row r is read from physical row src[r * T + j] (int32 [R, T], every
+ * entry in [0, R)) instead of row r; this step's k / v are still written at row r, slot *step.  A physical (row, slot) is written
+ * once, at step == slot, so permuting beams permutes src rows and never moves the cache.  With src[r, j] = r the output equals
+ * src == NULL's bitwise.  src is checked for 4-byte alignment when given; the other argument checks do not depend on it. */
+int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
+                          const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo, void* stream);
 /* h[r, :] = wte[tokens[r, s]] + wpe[s + pos_offset] + emb[r, :], s = *step: the embedding sum of GPT2Model_XX.forward
  * (optimus_gpt2.py:941-948) with emb = linear_emb(z); pos_offset 1 (the latent is position 0).  fp32 wte [V, D], wpe [P, D]. */
 int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* wte, int V, const float* wpe, int P, int pos_offset,
                       const float* emb, int R, int D, float* h, void* stream);
-/* torch.multinomial(softmax(logits / temperature)) of sample_single_sequence_conditional (top_k 0, top_p 1: no filtering), by
- * inverse CDF of u in [0, 1): u = uniforms[r * ldu + s] when uniforms != NULL, else a Philox4x32-10 draw keyed by *seed (device
- * u64) at counter (r, s).  forced != NULL takes token s+1 from forced[r * ldf + s + 1] instead (teacher forcing).  Writes
- * tokens[r * ldt + s + 1]; == eos sets done[r] = 1 and lengths[r] = s + 2; when s + 1 == max_len - 2 a non-eos row also gets eos at
- * s + 2 (the reference overwrites the max_len-th token, so its last draw is skipped).  Rows with done[r] != 0 are left frozen.
- * record (may be NULL) receives the step's logits at record[(s * R + r) * V ..]. */
-int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
-                       const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
-                       const int* step, int eos, int max_len, float* record, void* stream);
-/* vdb_textdec_sample with the top-k / nucleus cuts of top_k_top_p_filtering (reference optimus.py:690-719), as
- * sample_single_sequence_conditional applies them (optimus.py:662-688).  Per row, l = logits / temperature (fp32):
+/* torch.multinomial(softmax(logits / temperature)) of sample_single_sequence_conditional (optimus.py:662-688), by inverse CDF of
+ * u in [0, 1): u = uniforms[r * ldu + s] when uniforms != NULL, else a Philox4x32-10 draw keyed by *seed (device u64) at counter
+ * (r, s).  forced != NULL takes token s+1 from forced[r * ldf + s + 1] instead (teacher forcing).  Writes tokens[r * ldt + s + 1];
+ * == eos sets done[r] = 1 and lengths[r] = s + 2; when s + 1 == max_len - 2 a non-eos row also gets eos at s + 2 (the reference
+ * overwrites the max_len-th token, so its last draw is skipped).  Rows with done[r] != 0 are left frozen.  record (may be NULL)
+ * receives the step's logits at record[(s * R + r) * V ..].
+ * The top-k / nucleus cuts of top_k_top_p_filtering (reference optimus.py:690-719) restrict the draw.  Per row, l = logits /
+ * temperature (fp32):
  *   top_k > 0: k = min(top_k, V); every token with l < (the k-th largest l) is removed.  Ties with the k-th value are kept, so
  *     more than k tokens can survive.
  *   then, when 0 < top_p < 1: the survivors' softmax, ordered by descending l; a survivor is kept when the probability mass
@@ -422,26 +423,18 @@ int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float t
  *     first min(#ties, 1 + floor((top_p - M(>v)) / q)) ties are kept.  (The reference's torch.sort is not stable, so this is the
  *     one case its order leaves open.)  Masses are exp(l - max) / Z with Z the survivors' fp64 sum, compared as 64-bit fixed-point
  *     integers (units of 2^-62), so the cut is exact and repeatable.
- * top_k == 0 (or >= V) turns the top-k cut off, top_p == 0 or 1 the nucleus cut; with both off (or with forced tokens) this is
- * vdb_textdec_sample exactly.  top_k = 1 is greedy decoding.  The draw is vdb_textdec_sample's inverse CDF over the kept tokens
- * only, in vocabulary order, their mass renormalised, with the same u.  The filter stages the row in shared memory: with a cut on,
- * V <= 53248.  top_k < 0 or top_p NaN or outside [0, 1] return VDB_ERR_INVALID before any launch, as do vdb_textdec_sample's
- * argument errors. */
-int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
-                                const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
-                                int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
-                                void* stream);
-/* vdb_textdec_attention for beam search: cache slot j < *step of row r is read from physical row src[r * T + j] (int32 [R, T],
- * every entry in [0, R)) instead of row r; this step's k / v are still written at row r, slot *step.  A physical (row, slot) is
- * written once, at step == slot, so permuting beams permutes src rows and never moves the cache.  Same argument checks as
- * vdb_textdec_attention, plus a non-null, 4-byte aligned src.  With src[r, j] = r the output equals vdb_textdec_attention's bitwise. */
-int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
-                                  const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo,
-                                  void* stream);
+ * top_k == 0 (or >= V) turns the top-k cut off, top_p == 0 or 1 the nucleus cut; with both off, or with forced tokens, the full
+ * softmax is sampled (reference top_k 0, top_p 1: no filtering).  top_k = 1 is greedy decoding.  With a cut on, the draw is the
+ * inverse CDF over the kept tokens only, in vocabulary order, their mass renormalised, with the same u; the filter stages the row
+ * in shared memory, so V <= 53248.  top_k < 0 or top_p NaN or outside [0, 1] return VDB_ERR_INVALID before any launch, as do
+ * the other argument errors. */
+int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
+                       const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt,
+                       int* done, int* lengths, const int* step, int eos, int max_len, float* record, void* stream);
 /* One beam-search step, s = *step.  It stands in for the reference's optimus_vae.decode(z, strategy='beam', K)
  * (optimus.py:196-213), whose beam_search_decode does not exist in the reference's GPT-2, so this definition is the specification.
  * Rows r = latent * K + beam, R = n * K <= 16, 1 <= K <= 16.  Per beam: tokens [R, ldt] (token 0 = <BOS>), src [R, lds] (the
- * slot-to-row table of vdb_textdec_attention_indexed), scores fp64 [R], done [R], lengths [R].  Before step 0 the caller sets
+ * slot-to-row table of vdb_textdec_attention), scores fp64 [R], done [R], lengths [R].  Before step 0 the caller sets
  * every score to -inf except beam 0's (0), so the first step does not produce K copies of one hypothesis.
  *   logp_r(v) = log softmax(logits[r] / temperature)(v), all in fp64 from the fp32 logits (the division, max, exp, sum and log).
  *   Candidates: each live beam b crossed with each token v, score S_b + logp_b(v); each finished beam b as itself, score S_b.
@@ -451,7 +444,7 @@ int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* 
  *   is appended at s + 2 unscored and it finishes (lengths = s + 3).  A finished beam keeps its score and length.
  * A latent is finished when all K beams are; live scores only decrease, so no live beam could have beaten them.  A beam's
  * scored-token count is min(lengths - 1, max_len - 2) (a chosen <eos> counts, a forced one does not).  Two launches: one CTA per
- * row (K best tokens via the top-k radix select of vdb_textdec_sample_filtered, ties in vocabulary order; at most K of one
+ * row (K best tokens via the top-k radix select of vdb_textdec_sample, ties in vocabulary order; at most K of one
  * row's tokens can enter the K best), then one CTA per latent.  The per-row pick orders a row's tokens by their fp32 logit
  * (ties to the lower token id), which is the order of S_b + logp_b(v) except where the fp64 rounding of l / temperature - lse or
  * of S_b + logp makes two different logits score equal: there the larger logit is kept, where the rule above would keep the
@@ -465,7 +458,7 @@ int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* 
 int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, float temperature, int K, int* tokens, int ldt, int* src,
                           int lds, double* scores, int* done, int* lengths, const int* step, int eos, int max_len, int* cand_tok,
                           double* cand_logp, float* record, double* trace, void* stream);
-/* The repetition logits processors, in place on the fp32 logits [R, ldl] of one token step, before vdb_textdec_sample(_filtered)
+/* The repetition logits processors, in place on the fp32 logits [R, ldl] of one token step, before vdb_textdec_sample
  * or vdb_textdec_beam_step reads them (so those see, and `record` holds, the edited logits).  Row r's history is
  * h = tokens[r, 0 .. s], s = *step: <BOS>, then every token so far, including this step's input token.
  *   Repetition penalty p (finite, > 0; 1 = off), as HF's RepetitionPenaltyLogitsProcessor: for each DISTINCT id v of h with

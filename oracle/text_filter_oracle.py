@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY. fp64 restatement of the text sampler's top-k / nucleus cuts (top_k_top_p_filtering, reference
 lib/model_zoo/optimus.py:690-719, as sample_single_sequence_conditional applies it at :662-688) and of the inverse-CDF pick over
-the tokens they keep (vdb_textdec_sample_filtered).
+the tokens they keep (vdb_textdec_sample with top_k / top_p).
 """
 import numpy as np
 import torch

@@ -111,7 +111,7 @@ def test_oracle_forced_eos_is_not_scored():
     assert score == lp[0] + lp[1] and norm == score / 2
 
 
-def test_beam_entry_points_check_arguments_before_launch():
+def test_beam_step_and_attention_src_check_arguments_before_launch():
     """bad arguments return VDB_ERR_INVALID with a message (the fake addresses are never touched)."""
     from vdb200._lib import lib
     x, out, step = 0x10000, 0x30000, 0x40000
@@ -127,11 +127,13 @@ def test_beam_entry_points_check_arguments_before_launch():
                     (dict(tokens=out + 2), b"4-byte aligned"), (dict(src=out + 1), b"4-byte aligned"),
                     (dict(logits=x + 2), b"4-byte aligned")):
         assert beam(**kw) == 1 and msg in lib.vdb_last_error(), (kw, lib.vdb_last_error())
-    att = lambda R=4, src=out: lib.vdb_textdec_attention_indexed(x, 2304, x, 768, out, out, src, R, 12, 32, step, 0.125, out, 768,
-                                                                 None)
+    att = lambda R=4, src=out, qkv=x: lib.vdb_textdec_attention(qkv, 2304, x, 768, out, out, src, R, 12, 32, step, 0.125, out, 768,
+                                                                None)
     assert att(R=17) == 1 and b"R <= 16" in lib.vdb_last_error()
-    assert att(src=None) == 1 and b"null" in lib.vdb_last_error()
+    assert att(qkv=None) == 1 and b"null" in lib.vdb_last_error()
     assert att(src=out + 2) == 1 and b"aligned" in lib.vdb_last_error()
+    # src = NULL is the plain path: it passes the null-pointer check, so the row count is what is refused
+    assert att(src=None, R=17) == 1 and b"R <= 16" in lib.vdb_last_error()
 
 
 def test_decode_rejects_bad_beam_arguments():

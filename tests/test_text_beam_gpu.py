@@ -1,6 +1,6 @@
 """Text decoder beam search on the GPU: vdb_textdec_beam_step against the fp64 oracle (oracle/text_beam_oracle.py) on a grid of
-row layouts, vocabularies, temperatures, steps, finished beams, exact ties and -1e30 logits; the indexed KV-cache attention
-against the plain one on a physically gathered cache; a full-size decode replayed step by step through the oracle on its own
+row layouts, vocabularies, temperatures, steps, finished beams, exact ties and -1e30 logits; the KV-cache attention through a
+src table against the plain one on a physically gathered cache; a full-size decode replayed step by step through the oracle on its own
 recorded logits; returned scores re-scored from teacher-forced and fp64-oracle logits; width 1 against greedy decoding; graph
 replay, repeatability and the group split; and net.vae_decode(x, 'text', num_beams=4).
 
@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import torch
 
+from lib.model_zoo.optimus import decode_plan
 from oracle.text_beam_oracle import BeamState, beam_step, log_softmax64, place, rank_final
 
 pytestmark = pytest.mark.gpu
@@ -109,7 +110,7 @@ def test_beam_step_matches_oracle(n, K, V, temperature, s):
 
 
 @pytest.mark.parametrize("s", [0, 1, 17, 30, 31])
-def test_indexed_attention_equals_attention_on_a_gathered_cache(s):
+def test_attention_src_equals_attention_on_a_gathered_cache(s):
     from vdb200 import ops
     R, H, T = 16, 12, 32
     D = H * 64
@@ -123,7 +124,7 @@ def test_indexed_attention_equals_attention_on_a_gathered_cache(s):
     for name, src in tables.items():
         src = src.to(torch.int32).contiguous().to(DEV)
         k1, v1, o1 = kc.clone(), vc.clone(), torch.empty(R, D, device=DEV)
-        ops.textdec_attention_indexed(qkv, mem, k1, v1, src, step, o1)
+        ops.textdec_attention(qkv, mem, k1, v1, step, o1, src=src)
         idx = src.long()[:, None, :, None].expand(R, H, T, 64)
         kg, vg = torch.gather(kc, 0, idx).contiguous(), torch.gather(vc, 0, idx).contiguous()
         o2 = torch.empty(R, D, device=DEV)
@@ -146,11 +147,11 @@ def latents(n, seed):
 
 
 @pytest.mark.parametrize("temperature", [1.0, 0.7])
-def test_full_decode_follows_the_oracle_step_by_step(full, temperature):
+def test_full_beam_plan_decode_follows_the_oracle_step_by_step(full, temperature):
     m, _ = full
     n, K = 4, 4
     z = latents(n, 21)
-    out, st, ran = m._beam_group(z.to(DEV), K, temperature, 1.0, EOS, 1.0, record=True)
+    out, st, ran = m._beam_group(z.to(DEV), decode_plan("beam", temperature, EOS, record=True, num_beams=K), 1.0, 1.0)
     rec, trace = st.record[:ran].cpu().numpy(), st.trace[:ran].cpu().numpy()
     ost = BeamState.start(n, K, BOS, EOS)
     exempt = 0

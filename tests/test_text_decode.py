@@ -2,6 +2,7 @@
 GPT2Tokenizer, the C ABI's argument checks and the VDB_TEXT_FLOWS configuration."""
 import contextlib
 import json
+import math
 import os
 import sys
 
@@ -106,7 +107,7 @@ def test_detokenizer_on_a_synthetic_vocabulary(tmp_path):
         GPT2Detokenizer(str(tmp_path / "missing" / "gpt2-vocab.json")).sentence([BOS_ID, 0, EOS_ID])
 
 
-def test_text_decoder_entry_points_check_arguments_before_launch():
+def test_text_decoder_entry_points_with_cuts_and_src_check_arguments_before_launch():
     """null, oversize and misaligned arguments return VDB_ERR_INVALID with a message (the fake addresses are never touched)."""
     from vdb200._lib import lib
     x, w, out, bad = 0x10000, 0x20000, 0x30000, 0x20008
@@ -119,20 +120,22 @@ def test_text_decoder_entry_points_check_arguments_before_launch():
     assert lib.vdb_textdec_gemv(x, 4, 768, 768, x + 4096, None, 1e-5, w, 64, 768, None, 0, 0, out, 64, None) == 1
     assert lib.vdb_textdec_gemv(x, 4, 768, 768, None, None, 0.0, w, 64, 768, None, 2, 0, out, 64, None) == 1
     step = 0x40000
-    assert lib.vdb_textdec_attention(None, 2304, x, 768, out, out, 4, 12, 32, step, 0.125, out, 768, None) == 1
-    assert lib.vdb_textdec_attention(x, 2304, x, 768, out, out, 17, 12, 32, step, 0.125, out, 768, None) == 1
-    assert lib.vdb_textdec_attention(x, 2304, x, 768, out + 2, out, 4, 12, 32, step, 0.125, out, 768, None) == 1
+    assert lib.vdb_textdec_attention(None, 2304, x, 768, out, out, None, 4, 12, 32, step, 0.125, out, 768, None) == 1
+    assert lib.vdb_textdec_attention(x, 2304, x, 768, out, out, None, 17, 12, 32, step, 0.125, out, 768, None) == 1
+    assert lib.vdb_textdec_attention(x, 2304, x, 768, out + 2, out, None, 4, 12, 32, step, 0.125, out, 768, None) == 1
     assert b"aligned" in lib.vdb_last_error()
     assert lib.vdb_textdec_embed(None, 33, step, x, 50260, x, 1024, 1, x, 4, 768, out, None) == 1
     assert lib.vdb_textdec_embed(x, 33, step, x, 50260, x, 1024, 1, x, 32, 768, out, None) == 1
-    sample = lambda R=4, temp=1.0, seed=x, uniforms=None: lib.vdb_textdec_sample(
-        x, R, 50260, 50260, temp, seed, uniforms, 32, None, 0, out, 33, out, out, step, 50259, 30, None, None)
-    assert sample(R=17) == 1 and b"R <= 16" in lib.vdb_last_error()
-    assert sample(temp=0.0) == 1 and b"temperature" in lib.vdb_last_error()
-    assert sample(seed=None) == 1 and b"seed" in lib.vdb_last_error()
-    assert sample(seed=x + 4) == 1 and b"8-byte aligned" in lib.vdb_last_error()
-    assert lib.vdb_textdec_sample(None, 4, 50260, 50260, 1.0, x, None, 0, None, 0, out, 33, out, out, step, 50259, 30, None,
-                                  None) == 1
+    # the sampler with the cuts off (top_k 0, top_p 0) and on (40, 0.9)
+    sample = lambda R=4, V=50260, temp=1.0, top_k=0, top_p=0.0, seed=x, logits=x: lib.vdb_textdec_sample(
+        logits, R, V, V, temp, top_k, top_p, seed, None, 32, None, 0, out, 33, out, out, step, 50259, 30, None, None)
+    for cuts in (dict(), dict(top_k=40, top_p=0.9)):
+        for kw, msg in ((dict(R=17), b"R <= 16"), (dict(temp=0.0), b"temperature"), (dict(seed=None), b"seed"),
+                        (dict(seed=x + 4), b"8-byte aligned"), (dict(logits=None), b"null")):
+            assert sample(**cuts, **kw) == 1 and msg in lib.vdb_last_error(), (cuts, kw, lib.vdb_last_error())
+    for kw, msg in ((dict(top_k=-1), b"top_k"), (dict(top_p=math.nan), b"top_p"), (dict(top_p=-0.1), b"top_p"),
+                    (dict(top_p=1.5), b"top_p"), (dict(top_p=math.inf), b"top_p"), (dict(V=60000), b"53248")):
+        assert sample(**{"top_k": 40, "top_p": 0.9, **kw}) == 1 and msg in lib.vdb_last_error(), (kw, lib.vdb_last_error())
 
 
 def test_text_flows_config_carries_the_text_vae(monkeypatch):

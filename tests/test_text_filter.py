@@ -1,6 +1,6 @@
 """Top-k / nucleus cuts of the text sampler, CPU side: the fp64 restatement (oracle/text_filter_oracle.py) against what the
-reference's top_k_top_p_filtering kept (tests/golden/text_filter.npz), and the argument checks of vdb_textdec_sample_filtered
-and optimus_vae_next.decode_ids, which must reject bad cuts before any launch."""
+reference's top_k_top_p_filtering kept (tests/golden/text_filter.npz), and the checks of optimus_vae_next.decode_ids, which must
+reject bad cuts before any launch (the C entry point's are in test_text_decode)."""
 import math
 import os
 
@@ -53,21 +53,6 @@ def test_top_k_ties_and_a_dominant_token_in_the_fixture():
     assert (gold["kept"][4, k40, TOP_P.index(0.0)] == 44).all() and (gold["ties_kept"][4, k40, TOP_P.index(0.0)] == 8).all()
     assert (gold["kept"][4, k1, TOP_P.index(0.0)] == 2).all()
     assert (gold["kept"][6, :, 1:] == 1).all()
-
-
-def test_filtered_entry_point_checks_arguments_before_launch():
-    """Every call here is refused before a launch (the fake addresses are never touched)."""
-    from vdb200._lib import lib
-    x, out, step = 0x10000, 0x30000, 0x40000
-
-    def sample(R=4, V=50260, temp=1.0, top_k=40, top_p=0.9, seed=x, logits=x):
-        return lib.vdb_textdec_sample_filtered(logits, R, V, V, temp, top_k, top_p, seed, None, 32, None, 0, out, 33, out, out, step,
-                                               50259, 30, None, None)
-    for kw, msg in ((dict(top_k=-1), b"top_k"), (dict(top_p=math.nan), b"top_p"), (dict(top_p=-0.1), b"top_p"),
-                    (dict(top_p=1.5), b"top_p"), (dict(top_p=math.inf), b"top_p"), (dict(R=17), b"R <= 16"),
-                    (dict(temp=0.0), b"temperature"), (dict(seed=None), b"seed"), (dict(seed=x + 4), b"8-byte aligned"),
-                    (dict(logits=None), b"null"), (dict(V=60000), b"53248")):
-        assert sample(**kw) == 1 and msg in lib.vdb_last_error(), (kw, lib.vdb_last_error())
 
 
 def test_decode_ids_rejects_bad_cuts_before_launch():

@@ -1,7 +1,7 @@
-"""Top-k / nucleus cuts of the text sampler on the GPU (vdb_textdec_sample_filtered): picks against the fp64 oracle
+"""Top-k / nucleus cuts of the text sampler on the GPU (vdb_textdec_sample's top_k / top_p): picks against the fp64 oracle
 (oracle/text_filter_oracle.py) over the fixture's grid, the exact kept set and the Philox distribution on a small vocabulary,
-greedy decoding, bitwise equality with vdb_textdec_sample when the cuts are off, a full-size filtered decode checked step by step,
-and net.vae_decode(x, 'text', top_p=...) through the public surface.
+greedy decoding, every spelling of the cuts off bitwise equal to top_k 0, top_p 0, a full-size filtered decode checked step by
+step, and net.vae_decode(x, 'text', top_p=...) through the public surface.
 
 Exemption at the nucleus boundary: the kernel sums fixed-point masses exactly, the oracle in fp64.  A pick that differs from the
 oracle's is excused (counted and printed) when it is the oracle's pick with top_p moved by 1e-5 either way, or when u lies within
@@ -25,8 +25,8 @@ def _ptr(t):
 
 
 def _sample(logits, temperature=1.0, top_k=0, top_p=0.0, uniforms=None, seed=None, steps=1, entry="ops"):
-    """Token s+1 of every row for s < steps -> int64 [R, steps].  entry: 'ops' (ops.textdec_sample), or 'filtered' / 'plain' for
-    the C entry points vdb_textdec_sample_filtered / vdb_textdec_sample called directly."""
+    """Token s+1 of every row for s < steps -> int64 [R, steps].  entry: 'ops' (ops.textdec_sample), or 'c' for the C entry point
+    vdb_textdec_sample called directly."""
     from vdb200 import ops
     from vdb200._lib import lib, check
     R, Vr = logits.shape
@@ -40,12 +40,9 @@ def _sample(logits, temperature=1.0, top_k=0, top_p=0.0, uniforms=None, seed=Non
             ops.textdec_sample(dl, tokens, done, lengths, step, temperature=temperature, uniforms=uniforms, seed=seed, eos=-1,
                                max_len=1 << 30, top_k=top_k, top_p=top_p)
         else:
-            tail = (_ptr(seed), _ptr(uniforms), uniforms.stride(0) if uniforms is not None else 0, None, 0, _ptr(tokens), 33,
-                    _ptr(done), _ptr(lengths), _ptr(step), -1, 1 << 30, None, None)
-            if entry == "filtered":
-                check(lib.vdb_textdec_sample_filtered(_ptr(dl), R, Vr, Vr, float(temperature), int(top_k), float(top_p), *tail))
-            else:
-                check(lib.vdb_textdec_sample(_ptr(dl), R, Vr, Vr, float(temperature), *tail))
+            check(lib.vdb_textdec_sample(_ptr(dl), R, Vr, Vr, float(temperature), int(top_k), float(top_p), _ptr(seed), _ptr(uniforms),
+                                         uniforms.stride(0) if uniforms is not None else 0, None, 0, _ptr(tokens), 33, _ptr(done),
+                                         _ptr(lengths), _ptr(step), -1, 1 << 30, None, None))
         out.append(tokens[:, s + 1].clone())
     return torch.stack(out, 1).cpu().long()
 
@@ -124,17 +121,19 @@ def test_greedy_is_the_argmax():
                            want[:, :8])
 
 
-def test_cuts_off_are_bitwise_the_plain_sampler():
+def test_every_cuts_off_spelling_is_bitwise_the_uncut_sampler():
+    """Every spelling of "no cut" draws the tokens of top_k 0, top_p 0 bit for bit, through the C entry point and through ops."""
     g = torch.Generator().manual_seed(13)
     logits = torch.randn(16, V, generator=g) * 3
     u = torch.rand(16, 32, generator=g, dtype=torch.float64).to(DEV)
     seed = torch.tensor([4321], dtype=torch.int64, device=DEV)
     for temp in (0.7, 1.0):
-        plain_u = _sample(logits, temp, uniforms=u, steps=32, entry="plain")
-        plain_s = _sample(logits, temp, seed=seed, steps=32, entry="plain")
-        for k, p in ((0, 0.0), (0, 1.0), (V, 0.0), (60000, 1.0)):
-            assert torch.equal(_sample(logits, temp, k, p, uniforms=u, steps=32, entry="filtered"), plain_u), (temp, k, p)
-            assert torch.equal(_sample(logits, temp, k, p, seed=seed, steps=32, entry="filtered"), plain_s), (temp, k, p)
+        plain_u = _sample(logits, temp, uniforms=u, steps=32, entry="c")
+        plain_s = _sample(logits, temp, seed=seed, steps=32, entry="c")
+        for entry in ("c", "ops"):
+            for k, p in ((0, 0.0), (0, 1.0), (V, 0.0), (60000, 1.0)):
+                assert torch.equal(_sample(logits, temp, k, p, uniforms=u, steps=32, entry=entry), plain_u), (temp, k, p, entry)
+                assert torch.equal(_sample(logits, temp, k, p, seed=seed, steps=32, entry=entry), plain_s), (temp, k, p, entry)
 
 
 @pytest.fixture(scope="module")

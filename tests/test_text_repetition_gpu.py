@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import torch
 
+from lib.model_zoo.optimus import decode_plan
 from oracle.text_beam_oracle import BeamState, log_softmax64
 from oracle.text_repetition_oracle import has_repeated_ngram, process, processed_beam_search, processed_pick
 
@@ -91,7 +92,7 @@ def _same_beams(a, b):
                                                              for p, q in zip(x, y)) for x, y in zip(a, b))
 
 
-def test_off_is_the_existing_path(full):
+def test_processors_off_are_the_existing_path(full):
     from vdb200 import ops
     m, _ = full
     z = latents(4, 31).to(DEV)
@@ -107,13 +108,13 @@ def test_off_is_the_existing_path(full):
         assert _same_beams(m.decode_beams(z, 4), m.decode_beams(z, 4, **kw)), kw
     # launches: per step 64 (sampling) / 65 (beams) with both off, one more with either on; a whole eager decode likewise
     p = m.packed()
-    for mode, K, R, off in (("seed", 0, 4, 64), ("beam", 4, 16, 65)):
+    for draw, K, R, off in (("seed", 0, 4, 64), ("beam", 4, 16, 65)):
         st = m._state(R, z.device)
         for (rp, nr), want in (((1.0, 0), off), ((1.3, 0), off + 1), ((1.0, 2), off + 1), ((1.3, 2), off + 1)):
             st.step.zero_()
             n0 = ops.launch_count()
-            m._step(st, p, 1.0, EOS, MAX_LEN, mode, False, 0, 0.0, K, rp, nr)
-            assert ops.launch_count() - n0 == want, (mode, rp, nr)
+            m._step(st, p, decode_plan(draw, 1.0, EOS, MAX_LEN, num_beams=K, repetition_penalty=rp, no_repeat_ngram_size=nr))
+            assert ops.launch_count() - n0 == want, (draw, rp, nr)
     counts = []
     for kw in ({}, dict(repetition_penalty=1.0, no_repeat_ngram_size=0), dict(repetition_penalty=1.3, no_repeat_ngram_size=2)):
         n0 = ops.launch_count()
@@ -167,12 +168,12 @@ def test_full_size_decode_follows_the_oracle(full, top_k, top_p, temperature):
 
 
 @pytest.mark.parametrize("rp,nr", [(1.0, 2), (1.2, 3)])
-def test_beam_search_follows_the_oracle(full, rp, nr):
+def test_beam_plan_search_follows_the_oracle(full, rp, nr):
     m, _ = full
     n, K, temperature = 4, 4, 1.0
     z = latents(n, 25)
-    out, st, ran = m._beam_group(z.to(DEV), K, temperature, 1.0, EOS, 1.0, record=True, repetition_penalty=rp,
-                                 no_repeat_ngram_size=nr)
+    plan = decode_plan("beam", temperature, EOS, record=True, num_beams=K, repetition_penalty=rp, no_repeat_ngram_size=nr)
+    out, st, ran = m._beam_group(z.to(DEV), plan, 1.0, 1.0)
     rec, trace = st.record[:ran].cpu().numpy(), st.trace[:ran].cpu().numpy()
     zr = z.repeat_interleave(K, 0).to(DEV)
     raw = {}

@@ -25,7 +25,7 @@ import torch  # noqa: E402
 from lib.cfg_helper import model_cfg_bank  # noqa: E402
 from lib.model_zoo import get_model  # noqa: E402
 from lib.model_zoo.ddim import DDIMSampler  # noqa: E402
-from lib.model_zoo.optimus import STEPS_PER_CHECK  # noqa: E402
+from lib.model_zoo.optimus import STEPS_PER_CHECK, decode_plan  # noqa: E402
 from vdb200 import ops  # noqa: E402
 
 ap = argparse.ArgumentParser()
@@ -67,9 +67,10 @@ with torch.no_grad():
         vae.decode_ids(z, eos_token=-1)                      # warm-up: packs weights, captures the step-chunk graph
     p = vae.packed()
     st = vae._state(R, dev)
-    graph = st.graphs[(1.0, -1, 30, "seed", False, 0, 0.0, 0, 1.0, 0)]
+    plan = decode_plan("seed", eos=-1)
+    graph = st.graphs[plan]
     n0 = ops.launch_count()
-    vae._step(st, p, 1.0, -1, 30, "seed", False)
+    vae._step(st, p, plan)
     launches = ops.launch_count() - n0
     torch.cuda.synchronize()
     reps = 20
@@ -111,14 +112,15 @@ def step_ms_off_and_on(R, top_k, top_p, rounds=5, reps=10):
         for name, (k, p) in cuts.items():
             for _ in range(2):
                 vae.decode_ids(zr, eos_token=-1, top_k=k, top_p=p)
+            plan = decode_plan("seed", eos=-1, top_k=k, top_p=p)
             n0 = ops.launch_count()
-            vae._step(st, vae.packed(), 1.0, -1, 30, "seed", False, k, p)
-            out[name] = dict(launches_per_step=ops.launch_count() - n0, ms=[])
+            vae._step(st, vae.packed(), plan)
+            out[name] = dict(plan=plan, launches_per_step=ops.launch_count() - n0, ms=[])
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
-            for name, (k, p) in cuts.items():
-                g = st.graphs[(1.0, -1, 30, "seed", False, k, p, 0, 1.0, 0)]
+            for name in cuts:
+                g = st.graphs[out[name]["plan"]]
                 e0.record()
                 for _ in range(reps):
                     st.step.zero_()
@@ -154,9 +156,10 @@ def sampling_and_beams(K, n=4, rounds=5, reps=10):
             for _ in range(2):
                 call()
             st = vae._state(rows, dev)
+            plan = decode_plan(mode, eos=-1, num_beams=k)
             n0 = ops.launch_count()
-            vae._step(st, vae.packed(), 1.0, -1, 30, mode, False, 0, 0.0, k)
-            out[name] = dict(rows=rows, graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, k, 1.0, 0)], st=st,
+            vae._step(st, vae.packed(), plan)
+            out[name] = dict(rows=rows, graph=st.graphs[plan], st=st,
                              launches_per_step=ops.launch_count() - n0, ms=[], ms_decode=[])
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
@@ -210,10 +213,10 @@ def repetition_off_and_on(n, K, penalty, ngram, rounds=5, reps=10):
                 else:
                     vae.decode_ids(zr, eos_token=-1, repetition_penalty=rp, no_repeat_ngram_size=nr)
             st.step.zero_()
+            plan = decode_plan(mode, eos=-1, num_beams=K, repetition_penalty=rp, no_repeat_ngram_size=nr)
             n0 = ops.launch_count()
-            vae._step(st, vae.packed(), 1.0, -1, 30, mode, False, 0, 0.0, K, rp, nr)
-            out[name] = dict(launches_per_step=ops.launch_count() - n0, ms=[],
-                             graph=st.graphs[(1.0, -1, 30, mode, False, 0, 0.0, K, rp, nr)])
+            vae._step(st, vae.packed(), plan)
+            out[name] = dict(launches_per_step=ops.launch_count() - n0, ms=[], graph=st.graphs[plan])
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         for _ in range(rounds):
             for name in knobs:

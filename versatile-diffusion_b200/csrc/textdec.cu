@@ -330,7 +330,7 @@ VDB_DEVINL Selected radix_select(const uint32_t* keys, int V, uint32_t lo, unsig
 // forced (teacher forcing) replaces the draw.  A finished row (done[r] != 0) is left untouched.  After writing token s+1:
 // == eos ends the row; otherwise when s+1 == max_len - 2 the row gets eos at s+2 (optimus.py:682-688 overwrites the 30th
 // token, so that last draw is skipped).  record (may be NULL) receives this step's raw logits at [s][r][:].
-// kFilter: the same pick over the tokens the top-k / nucleus cuts keep (vdb_textdec_sample_filtered), removed tokens weigh 0.
+// kFilter: the same pick over the tokens the top-k / nucleus cuts keep (vdb_textdec_sample's top_k / top_p), removed tokens weigh 0.
 // The kept set is every key > bound plus the first `cap` keys == bound in vocabulary order.
 // ---------------------------------------------------------------------------------------------------------------------------
 template <bool kFilter>
@@ -756,37 +756,19 @@ int vdb_textdec_gemv(const float* x, int R, long long K, long long ldx, const fl
                 reinterpret_cast<const __nv_bfloat16*>(W), n, ldw, bias, act, accumulate, out, ldo, ks, ldxs);
 }
 
-int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache, int R,
-                          int H, int T, const int* step, float scale, float* out, long long ldo, void* stream) {
+int vdb_textdec_attention(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
+                          const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo, void* stream) {
   if (!qkv || !mem || !kcache || !vcache || !step || !out) return set_error(VDB_ERR_INVALID, "textdec_attention: null pointer");
   if (R < 1 || R > kGvMaxRows || H < 1 || H > 64 || T < 1 || T > 1024)
     return set_error(VDB_ERR_INVALID, "textdec_attention: need 1 <= R <= 16, 1 <= H <= 64, 1 <= T <= 1024");
   const long long D = static_cast<long long>(H) * kHeadDim;
   if (ldq < 3 * D || ldm < D || ldo < D) return set_error(VDB_ERR_INVALID, "textdec_attention: leading dimensions smaller than the rows");
   if ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(mem) | reinterpret_cast<uintptr_t>(out) |
-       reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache)) & 3)
-    return set_error(VDB_ERR_INVALID, "textdec_attention: fp32 buffers must be 4-byte aligned");
-  const int warps = R * H;
-  return launch(textdec_attention_kernel<false>, (warps + 3) / 4, 128, 0, stream, qkv, ldq, mem, ldm, kcache, vcache, R, H, T,
-                step, scale, out, ldo, nullptr);
-}
-
-int vdb_textdec_attention_indexed(const float* qkv, long long ldq, const float* mem, long long ldm, float* kcache, float* vcache,
-                                  const int* src, int R, int H, int T, const int* step, float scale, float* out, long long ldo,
-                                  void* stream) {
-  if (!qkv || !mem || !kcache || !vcache || !src || !step || !out)
-    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: null pointer");
-  if (R < 1 || R > kGvMaxRows || H < 1 || H > 64 || T < 1 || T > 1024)
-    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: need 1 <= R <= 16, 1 <= H <= 64, 1 <= T <= 1024");
-  const long long D = static_cast<long long>(H) * kHeadDim;
-  if (ldq < 3 * D || ldm < D || ldo < D)
-    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: leading dimensions smaller than the rows");
-  if ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(mem) | reinterpret_cast<uintptr_t>(out) |
        reinterpret_cast<uintptr_t>(kcache) | reinterpret_cast<uintptr_t>(vcache) | reinterpret_cast<uintptr_t>(src)) & 3)
-    return set_error(VDB_ERR_INVALID, "textdec_attention_indexed: buffers must be 4-byte aligned");
+    return set_error(VDB_ERR_INVALID, "textdec_attention: buffers must be 4-byte aligned");
   const int warps = R * H;
-  return launch(textdec_attention_kernel<true>, (warps + 3) / 4, 128, 0, stream, qkv, ldq, mem, ldm, kcache, vcache, R, H, T,
-                step, scale, out, ldo, src);
+  return launch(src == nullptr ? textdec_attention_kernel<false> : textdec_attention_kernel<true>, (warps + 3) / 4, 128, 0, stream,
+                qkv, ldq, mem, ldm, kcache, vcache, R, H, T, step, scale, out, ldo, src);
 }
 
 int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* wte, int V, const float* wpe, int P, int pos_offset,
@@ -797,10 +779,12 @@ int vdb_textdec_embed(const int* tokens, int ldt, const int* step, const float* 
   return launch(textdec_embed_kernel, R, 256, 0, stream, tokens, ldt, step, wte, V, wpe, P, pos_offset, emb, D, h);
 }
 
-static int textdec_sample_launch(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
-                                 const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
-                                 int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
-                                 void* stream) {
+int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
+                       const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt,
+                       int* done, int* lengths, const int* step, int eos, int max_len, float* record, void* stream) {
+  if (top_k < 0) return set_error(VDB_ERR_INVALID, "textdec_sample: top_k must be >= 0, got %d", top_k);
+  if (!(top_p >= 0.0f && top_p <= 1.0f))
+    return set_error(VDB_ERR_INVALID, "textdec_sample: top_p must be in [0, 1], got %g", static_cast<double>(top_p));
   if (!logits || !tokens || !done || !lengths || !step) return set_error(VDB_ERR_INVALID, "textdec_sample: null pointer");
   if (!forced && !uniforms && !seed) return set_error(VDB_ERR_INVALID, "textdec_sample: need a seed, uniforms or forced tokens");
   if (R < 1 || R > kGvMaxRows || V < 1 || ldl < V) return set_error(VDB_ERR_INVALID, "textdec_sample: need 1 <= R <= 16, ldl >= V >= 1");
@@ -815,8 +799,7 @@ static int textdec_sample_launch(const float* logits, int R, int V, long long ld
     return launch(textdec_sample_kernel<false>, R, kSampleThreads, 0, stream, logits, R, V, ldl, temperature, seed, uniforms, ldu,
                   forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record, 0, 0.0f);
   if (V > kFilterMaxV)
-    return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top-k / top-p stage at most %d logits per row, got V = %d",
-                     kFilterMaxV, V);
+    return set_error(VDB_ERR_INVALID, "textdec_sample: top-k / top-p stage at most %d logits per row, got V = %d", kFilterMaxV, V);
   const size_t smem = kFilterHistBytes + static_cast<size_t>(V) * sizeof(uint32_t);
   static bool configured = false;
   if (!configured) {
@@ -826,24 +809,6 @@ static int textdec_sample_launch(const float* logits, int R, int V, long long ld
   }
   return launch(textdec_sample_kernel<true>, R, kSampleThreads, smem, stream, logits, R, V, ldl, temperature, seed, uniforms, ldu,
                 forced, ldf, tokens, ldt, done, lengths, step, eos, max_len, record, top_k, top_p);
-}
-
-int vdb_textdec_sample(const float* logits, int R, int V, long long ldl, float temperature, const unsigned long long* seed,
-                       const double* uniforms, int ldu, const int* forced, int ldf, int* tokens, int ldt, int* done, int* lengths,
-                       const int* step, int eos, int max_len, float* record, void* stream) {
-  return textdec_sample_launch(logits, R, V, ldl, temperature, 0, 0.0f, seed, uniforms, ldu, forced, ldf, tokens, ldt, done, lengths,
-                               step, eos, max_len, record, stream);
-}
-
-int vdb_textdec_sample_filtered(const float* logits, int R, int V, long long ldl, float temperature, int top_k, float top_p,
-                                const unsigned long long* seed, const double* uniforms, int ldu, const int* forced, int ldf,
-                                int* tokens, int ldt, int* done, int* lengths, const int* step, int eos, int max_len, float* record,
-                                void* stream) {
-  if (top_k < 0) return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top_k must be >= 0, got %d", top_k);
-  if (!(top_p >= 0.0f && top_p <= 1.0f))
-    return set_error(VDB_ERR_INVALID, "textdec_sample_filtered: top_p must be in [0, 1], got %g", static_cast<double>(top_p));
-  return textdec_sample_launch(logits, R, V, ldl, temperature, top_k, top_p, seed, uniforms, ldu, forced, ldf, tokens, ldt, done,
-                               lengths, step, eos, max_len, record, stream);
 }
 
 int vdb_textdec_beam_step(const float* logits, int R, int V, long long ldl, float temperature, int K, int* tokens, int ldt, int* src,

@@ -35,7 +35,7 @@ Differences from the reference, all deliberate:
   - decode(z, top_k=..., top_p=...) applies the reference's top-k and nucleus cuts (optimus.py:690-719) in the sampling kernel,
     inside the captured step graph; top_k=1 is greedy decoding.  The probabilities the nucleus cut sums are fp64-exact fixed-point
     integers rather than an fp32 cumsum, and tied tokens at the nucleus boundary are taken in vocabulary order (the reference's
-    unstable sort leaves their order open); see vdb_textdec_sample_filtered;
+    unstable sort leaves their order open); see vdb_textdec_sample;
   - the reference's 29th forward pass, whose draw is always overwritten with <EOS>, is skipped;
   - weights are bf16 (packed at load); the residual stream, attention, logits and the sampler's sums are fp32 / fp64.
 
@@ -54,10 +54,10 @@ Beam search: decode(z, num_beams=K) (and decode_ids, decode_beams) stands in for
   - final ranking by S / n ** length_penalty, n the scored tokens (a chosen <EOS> counts, a forced one does not; length_penalty 0
     ranks by the raw sum), ties to the lower beam index.  K = 1 picks the argmax, the lowest token id among equal maxima: the
     tokens of greedy decoding (top_k=1), which differs only at an exact tie for the maximum, where it draws among the tied tokens.
-The KV cache is not moved when beams are reordered: each physical (row, slot) is written once, and the indexed attention reads
-slot j of beam r from row src[r, j], a table the beam step permutes with the token rows.  A step streams the weights once for all
-n * K rows (the GEMV is one 16-row tile), so n * K <= 16 rows run together; more latents are split into groups of 16 // K,
-decoded one after the other, each group re-streaming the weights.
+The KV cache is not moved when beams are reordered: each physical (row, slot) is written once, and the attention reads slot j of
+beam r from row src[r, j] (vdb_textdec_attention's src), a table the beam step permutes with the token rows.  A step streams the
+weights once for all n * K rows (the GEMV is one 16-row tile), so n * K <= 16 rows run together; more latents are split into
+groups of 16 // K, decoded one after the other, each group re-streaming the weights.
 
 Repetition: decode / decode_ids / decode_beams(..., repetition_penalty=p, no_repeat_ngram_size=n) apply the two logits processors
 of Hugging Face generation (RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor) in one kernel inside the captured step
@@ -74,12 +74,16 @@ ban renormalises the beam's distribution; HF edits log-probabilities instead and
 working beam path, so this definition stands.  A banned token is never drawn nor extends a beam while a row keeps a finite logit
 (K of them for beams), which a 50260-token vocabulary and at most 30 history tokens always leave.  teacher_forced_logits takes no
 processors.  With both off no launch is added and every output is bitwise what it is without the arguments.
+
+Each entry point checks its options once, in decode_plan; the DecodePlan it returns drives the token walk (_run, _step) and is the
+key of the walk's captured step graphs.
 """
 import json
 import math
 import numbers
 import os
 import unicodedata
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -107,38 +111,55 @@ def _ops():
     return ops
 
 
-def _check_cuts(top_k, top_p):
-    """-> (int top_k, float top_p) of the sampler's top-k / nucleus cuts, or ValueError."""
-    if isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral) or top_k < 0:
-        raise ValueError(f"optimus_vae_next: top_k must be an int >= 0 (0: no top-k cut), got {top_k!r}")
-    if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real) or not math.isfinite(top_p) or not 0.0 <= top_p <= 1.0:
-        raise ValueError(f"optimus_vae_next: top_p must be a finite float in [0, 1] (0 or 1: no nucleus cut), got {top_p!r}")
-    return int(top_k), float(top_p)
-
-
 MAX_BEAMS = 16                                    # the rows of one token step (vdb_textdec_beam_step's K limit)
 
 
-def _check_beams(num_beams, length_penalty, top_k, top_p):
-    """-> (int num_beams, float length_penalty), or ValueError; beam search takes no top-k / nucleus cut."""
-    if isinstance(num_beams, bool) or not isinstance(num_beams, numbers.Integral) or not 0 <= num_beams <= MAX_BEAMS:
-        raise ValueError(f"optimus_vae_next: num_beams must be an int in [0, {MAX_BEAMS}] (0: sampling), got {num_beams!r}")
-    if isinstance(length_penalty, bool) or not isinstance(length_penalty, numbers.Real) or not math.isfinite(length_penalty):
-        raise ValueError(f"optimus_vae_next: length_penalty must be a finite float, got {length_penalty!r}")
-    if num_beams and (top_k != 0 or top_p != 0.0):
-        raise ValueError("optimus_vae_next: beam search (num_beams >= 1) takes no top_k / top_p cut")
-    return int(num_beams), float(length_penalty)
+class DecodePlan(NamedTuple):
+    """The options of one token walk, checked (decode_plan).  It is also the key of the walk's captured step graphs: two walks
+    with equal plans launch the same step.  draw: 'seed' (Philox, seeded from torch's CPU generator), 'uniforms' (given draws),
+    'forced' (teacher forcing) or 'beam' (beam search with num_beams >= 1; the cuts are then 0, 0.0)."""
+    draw: str
+    temperature: float
+    eos: int
+    max_len: int
+    record: bool
+    top_k: int
+    top_p: float
+    num_beams: int
+    repetition_penalty: float
+    no_repeat_ngram_size: int
 
 
-def _check_repetition(repetition_penalty, no_repeat_ngram_size):
-    """-> (float repetition_penalty, int no_repeat_ngram_size) of the repetition logits processors, or ValueError."""
+def decode_plan(draw, temperature=1.0, eos=EOS_ID, max_len=MAX_LENGTH, record=False, top_k=0, top_p=0.0, num_beams=0,
+                length_penalty=1.0, repetition_penalty=1.0, no_repeat_ngram_size=0):
+    """-> the DecodePlan of a walk, or ValueError.  draw 'seed' / 'uniforms' with num_beams >= 1 is decode_ids' beam search, which
+    takes no cuts, uniforms or logits; draw 'beam' is decode_beams', which needs num_beams >= 1.  length_penalty is only checked:
+    it ranks finished beams on the host and is no part of the walk.  The order of the checks decides which refusal a call with
+    several bad options gets (tests/test_text_decode_plan.py pins it)."""
     p, n = repetition_penalty, no_repeat_ngram_size
     if (isinstance(p, bool) or not isinstance(p, numbers.Real) or not math.isfinite(p) or not p > 0
             or not 0.0 < float(torch.tensor(float(p), dtype=torch.float32)) < math.inf):     # the kernel takes it as fp32
         raise ValueError(f"optimus_vae_next: repetition_penalty must be a finite float > 0 (1: off), got {p!r}")
     if isinstance(n, bool) or not isinstance(n, numbers.Integral) or not 0 <= n <= MAX_LENGTH:
         raise ValueError(f"optimus_vae_next: no_repeat_ngram_size must be an int in [0, {MAX_LENGTH}] (0: off), got {n!r}")
-    return float(p), int(n)
+    if isinstance(num_beams, bool) or not isinstance(num_beams, numbers.Integral) or not 0 <= num_beams <= MAX_BEAMS:
+        raise ValueError(f"optimus_vae_next: num_beams must be an int in [0, {MAX_BEAMS}] (0: sampling), got {num_beams!r}")
+    if isinstance(length_penalty, bool) or not isinstance(length_penalty, numbers.Real) or not math.isfinite(length_penalty):
+        raise ValueError(f"optimus_vae_next: length_penalty must be a finite float, got {length_penalty!r}")
+    if num_beams and (top_k != 0 or top_p != 0.0):
+        raise ValueError("optimus_vae_next: beam search (num_beams >= 1) takes no top_k / top_p cut")
+    if draw == "beam" and num_beams < 1:
+        raise ValueError(f"optimus_vae_next.decode_beams: num_beams must be >= 1, got {int(num_beams)}")
+    if num_beams:
+        if draw == "uniforms" or (draw != "beam" and record):
+            raise ValueError("optimus_vae_next: beam search takes no uniforms and returns no logits")
+        draw, top_k, top_p = "beam", 0, 0.0
+    if isinstance(top_k, bool) or not isinstance(top_k, numbers.Integral) or top_k < 0:
+        raise ValueError(f"optimus_vae_next: top_k must be an int >= 0 (0: no top-k cut), got {top_k!r}")
+    if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real) or not math.isfinite(top_p) or not 0.0 <= top_p <= 1.0:
+        raise ValueError(f"optimus_vae_next: top_p must be a finite float in [0, 1] (0 or 1: no nucleus cut), got {top_p!r}")
+    return DecodePlan(draw, float(temperature), int(eos), int(max_len), bool(record), int(top_k), float(top_p), int(num_beams),
+                      float(p), int(n))
 
 
 class VocabularyMissingError(RuntimeError):
@@ -658,46 +679,41 @@ class optimus_vae_next(PackedModule):
         self.__dict__['_states'] = {}        # captured graphs hold the old weight addresses
 
     # ------------------------------------------------------------------ one token step (5 launches per layer + 4)
-    def _step(self, st, p, temperature, eos, max_len, mode, record, top_k=0, top_p=0.0, num_beams=0, repetition_penalty=1.0,
-              no_repeat_ngram_size=0):
+    def _step(self, st, p, plan):
         ops = _ops()
         dec = self.decoder
         D = dec.n_embd
         ops.textdec_embed(st.tokens, st.step, p["wte32"], p["wpe32"], st.emb, st.h, pos_offset=1)
         for i, L in enumerate(p["layers"]):
             ops.textdec_gemv(st.h, L["w_attn"], st.qkv, bias=L["b_attn"], ln=L["ln1"])
-            if num_beams:
-                ops.textdec_attention_indexed(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.src, st.step, st.a,
-                                              scale=0.125)
-            else:
-                ops.textdec_attention(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.step, st.a, scale=0.125)
+            ops.textdec_attention(st.qkv, st.mem[:, i * D:(i + 1) * D], st.kc[i], st.vc[i], st.step, st.a, scale=0.125,
+                                  src=st.src if plan.num_beams else None)
             ops.textdec_gemv(st.a, L["w_aproj"], st.h, bias=L["b_aproj"], accumulate=True)
             ops.textdec_gemv(st.h, L["w_fc"], st.m, bias=L["b_fc"], ln=L["ln2"], act=ops.ACT_GELU_TANH)
             ops.textdec_gemv(st.m, L["w_mproj"], st.h, bias=L["b_mproj"], accumulate=True)
         ops.textdec_gemv(st.h, p["lm_head"], st.logits, ln=p["lnf"])
-        if mode != "forced" and (repetition_penalty != 1.0 or no_repeat_ngram_size):
-            ops.textdec_repetition(st.logits, st.tokens, st.done, st.step, repetition_penalty, no_repeat_ngram_size)
-        if num_beams:
-            ops.textdec_beam_step(st.logits, num_beams, st.tokens, st.src, st.scores, st.done, st.lengths, st.step, st.cand_tok,
-                                  st.cand_logp, temperature=temperature, eos=eos, max_len=max_len,
-                                  record=st.record if record else None, trace=st.trace if record else None)
+        if plan.repetition_penalty != 1.0 or plan.no_repeat_ngram_size:
+            ops.textdec_repetition(st.logits, st.tokens, st.done, st.step, plan.repetition_penalty, plan.no_repeat_ngram_size)
+        if plan.num_beams:
+            ops.textdec_beam_step(st.logits, plan.num_beams, st.tokens, st.src, st.scores, st.done, st.lengths, st.step, st.cand_tok,
+                                  st.cand_logp, temperature=plan.temperature, eos=plan.eos, max_len=plan.max_len,
+                                  record=st.record if plan.record else None, trace=st.trace if plan.record else None)
         else:
-            ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=temperature,
-                               seed=st.seed if mode == "seed" else None, uniforms=st.uniforms if mode == "uniforms" else None,
-                               forced=st.forced if mode == "forced" else None, eos=eos, max_len=max_len,
-                               record=st.record if record else None, top_k=top_k, top_p=top_p)
+            ops.textdec_sample(st.logits, st.tokens, st.done, st.lengths, st.step, temperature=plan.temperature,
+                               seed=st.seed if plan.draw == "seed" else None,
+                               uniforms=st.uniforms if plan.draw == "uniforms" else None,
+                               forced=st.forced if plan.draw == "forced" else None, eos=plan.eos, max_len=plan.max_len,
+                               record=st.record if plan.record else None, top_k=plan.top_k, top_p=plan.top_p)
         ops.add_int(st.step, 1)
 
     @torch.no_grad()
-    def _run(self, z, temperature, eos, pre_scale=1.0, max_len=MAX_LENGTH, nsteps=None, mode="seed", uniforms=None, forced=None,
-             record=False, graph=True, top_k=0, top_p=0.0, num_beams=0, repetition_penalty=1.0, no_repeat_ngram_size=0):
-        """mode "beam" (num_beams >= 1) decodes the n latents of z as rows latent * num_beams + beam, n * num_beams <= 16."""
-        top_k, top_p = _check_cuts(top_k, top_p)
-        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
+    def _run(self, z, plan, pre_scale=1.0, nsteps=None, uniforms=None, forced=None, graph=True):
+        """Runs the walk of a checked plan.  A beam plan decodes the n latents of z as rows latent * num_beams + beam,
+        n * num_beams <= 16."""
         require_cuda(z, "optimus_vae_next.decode")
         if z.dim() != 2 or z.shape[1] != self.nz:
             raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
-        K = int(num_beams) if mode == "beam" else 0
+        K = plan.num_beams
         R = z.shape[0] * max(K, 1)
         if not 1 <= R <= 16:
             raise ValueError(f"optimus_vae_next: decodes 1 to 16 latents per call, got {R}" if not K else
@@ -705,7 +721,7 @@ class optimus_vae_next(PackedModule):
         ops = _ops()
         p = self.packed()
         st = self._state(R, z.device)
-        nsteps = max_len - 2 if nsteps is None else nsteps
+        nsteps = plan.max_len - 2 if nsteps is None else nsteps
         if nsteps > CACHE_SLOTS:
             raise ValueError(f"optimus_vae_next: at most {CACHE_SLOTS} steps")
         # per-call state: latent projections (the memory slices and the embedding offset), tokens, flags, seed
@@ -713,20 +729,20 @@ class optimus_vae_next(PackedModule):
         zs = (zs.repeat_interleave(K, 0) if K else zs).contiguous()
         ops.textdec_gemv(zs, p["w_emb"], st.emb)
         ops.textdec_gemv(zs, p["w_lin"], st.mem)
-        init = torch.full((R, CACHE_SLOTS + 1), eos, dtype=torch.int32)
+        init = torch.full((R, CACHE_SLOTS + 1), plan.eos, dtype=torch.int32)
         init[:, 0] = BOS_ID
-        if mode == "forced":
+        if plan.draw == "forced":
             init[:, :forced.shape[1]] = forced.cpu()
         st.tokens.copy_(init)
         st.done.zero_()
         st.lengths.fill_(nsteps + 1)
         st.step.zero_()
-        if mode == "seed":
+        if plan.draw == "seed":
             st.seed.copy_(torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64))
-        elif mode == "uniforms":
+        elif plan.draw == "uniforms":
             st.uniforms.zero_()
             st.uniforms[:, :uniforms.shape[1]].copy_(uniforms)
-        elif mode == "beam":
+        elif plan.draw == "beam":
             scores = torch.full((R,), -math.inf, dtype=torch.float64)
             scores[::K] = 0.0                     # only beam 0 of each latent is live at step 0
             st.scores.copy_(scores)
@@ -734,47 +750,55 @@ class optimus_vae_next(PackedModule):
         else:
             st.forced.zero_()
             st.forced[:, :forced.shape[1]].copy_(forced)
-        key = (float(temperature), int(eos), int(max_len), mode, bool(record), top_k, top_p, K, rp, nr)
         s = 0
         while s < nsteps:
             n = min(STEPS_PER_CHECK, nsteps - s)
-            g = st.graphs.get(key) if graph and n == STEPS_PER_CHECK else None
+            g = st.graphs.get(plan) if graph and n == STEPS_PER_CHECK else None
             if g is not None:
                 g.replay()
             else:
                 for _ in range(n):
-                    self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K, rp, nr)
-                if graph and n == STEPS_PER_CHECK and key not in st.graphs:
+                    self._step(st, p, plan)
+                if graph and n == STEPS_PER_CHECK and plan not in st.graphs:
                     # the chunk just ran eagerly (kernels configured, caches warm); capture one for the later chunks
                     torch.cuda.current_stream().synchronize()
                     step_before = st.step.clone()
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
                         for _ in range(n):
-                            self._step(st, p, temperature, eos, max_len, mode, record, top_k, top_p, K, rp, nr)
+                            self._step(st, p, plan)
                     st.step.copy_(step_before)        # capture does not execute, but keep the counter exactly as the eager chunk left it
-                    st.graphs[key] = g
+                    st.graphs[plan] = g
             s += n
-            if mode != "forced" and bool(st.done.cpu().all()):
+            if plan.draw != "forced" and bool(st.done.cpu().all()):
                 break
         return st, s
 
-    def _beam_group(self, z, num_beams, temperature, pre_scale, eos, length_penalty, record=False, graph=True,
-                    repetition_penalty=1.0, no_repeat_ngram_size=0):
+    def _beam_group(self, z, plan, pre_scale, length_penalty, graph=True):
         """Beam search of n latents with n * num_beams <= 16 -> (per latent, its num_beams (ids, score, normalized score) best
         first; the state; the steps run)."""
-        st, ran = self._run(z, temperature, eos, pre_scale=pre_scale, mode="beam", record=record, graph=graph, num_beams=num_beams,
-                            repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+        st, ran = self._run(z, plan, pre_scale=pre_scale, graph=graph)
+        K = plan.num_beams
         tokens, lengths, scores = st.tokens.cpu(), st.lengths.cpu().tolist(), st.scores.cpu().tolist()
         out = []
         for i in range(z.shape[0]):
             beams = []
-            for j in range(num_beams):
-                r = i * num_beams + j
+            for j in range(K):
+                r = i * K + j
                 n = min(lengths[r] - 1, MAX_LENGTH - 2)   # scored tokens: a forced final <EOS> has none
                 beams.append((tokens[r, :lengths[r]].long(), scores[r], scores[r] / n ** length_penalty))
-            out.append([beams[j] for j in sorted(range(num_beams), key=lambda j: (-beams[j][2], j))])
+            out.append([beams[j] for j in sorted(range(K), key=lambda j: (-beams[j][2], j))])
         return out, st, ran
+
+    def _beams(self, z, plan, pre_scale, length_penalty, graph):
+        require_cuda(z, "optimus_vae_next.decode")
+        if z.dim() != 2 or z.shape[0] < 1:
+            raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
+        per = MAX_BEAMS // plan.num_beams
+        out = []
+        for i0 in range(0, z.shape[0], per):
+            out += self._beam_group(z[i0:i0 + per], plan, pre_scale, length_penalty, graph=graph)[0]
+        return out
 
     @torch.no_grad()
     def decode_beams(self, z, num_beams, temperature=1.0, pre_scale=1.0, length_penalty=1.0, eos_token=EOS_ID, graph=True,
@@ -784,19 +808,9 @@ class optimus_vae_next(PackedModule):
         num_beams latents' worth of rows run per token step, at most 16: more latents are decoded in groups of 16 // num_beams,
         one after the other, each re-streaming the weights.  repetition_penalty / no_repeat_ngram_size edit each beam's logits
         before its log-softmax (see the module docstring); the scores are then log-probabilities of the edited logits."""
-        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
-        num_beams, length_penalty = _check_beams(num_beams, length_penalty, 0, 0.0)
-        if num_beams < 1:
-            raise ValueError(f"optimus_vae_next.decode_beams: num_beams must be >= 1, got {num_beams}")
-        require_cuda(z, "optimus_vae_next.decode")
-        if z.dim() != 2 or z.shape[0] < 1:
-            raise ValueError(f"optimus_vae_next: expected latents [n, {self.nz}], got {tuple(z.shape)}")
-        per = MAX_BEAMS // num_beams
-        out = []
-        for i0 in range(0, z.shape[0], per):
-            out += self._beam_group(z[i0:i0 + per], num_beams, temperature, pre_scale, int(eos_token), length_penalty,
-                                    graph=graph, repetition_penalty=rp, no_repeat_ngram_size=nr)[0]
-        return out
+        plan = decode_plan("beam", temperature, eos_token, num_beams=num_beams, length_penalty=length_penalty,
+                           repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+        return self._beams(z, plan, pre_scale, float(length_penalty), graph)
 
     @torch.no_grad()
     def decode_ids(self, z, temperature=1.0, eos_token=EOS_ID, pre_scale=1.0, uniforms=None, return_logits=False, graph=True,
@@ -808,17 +822,12 @@ class optimus_vae_next(PackedModule):
         repetition_penalty != 1 / no_repeat_ngram_size > 0 edit the logits before the draw (see the module docstring); the
         returned logits are the edited ones.
         num_beams >= 1: each latent's best beam-search hypothesis instead (decode_beams; no cuts, uniforms or logits)."""
-        rp, nr = _check_repetition(repetition_penalty, no_repeat_ngram_size)
-        num_beams, length_penalty = _check_beams(num_beams, length_penalty, top_k, top_p)
-        if num_beams:
-            if uniforms is not None or return_logits:
-                raise ValueError("optimus_vae_next: beam search takes no uniforms and returns no logits")
-            return [b[0][0] for b in self.decode_beams(z, num_beams, temperature=temperature, pre_scale=pre_scale,
-                                                       length_penalty=length_penalty, eos_token=eos_token, graph=graph,
-                                                       repetition_penalty=rp, no_repeat_ngram_size=nr)]
-        st, ran = self._run(z, temperature, int(eos_token), pre_scale=pre_scale, mode="uniforms" if uniforms is not None else "seed",
-                            uniforms=uniforms, record=return_logits, graph=graph, top_k=top_k, top_p=top_p, repetition_penalty=rp,
-                            no_repeat_ngram_size=nr)
+        plan = decode_plan("uniforms" if uniforms is not None else "seed", temperature, eos_token, record=return_logits, top_k=top_k,
+                           top_p=top_p, num_beams=num_beams, length_penalty=length_penalty,
+                           repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+        if plan.num_beams:
+            return [b[0][0] for b in self._beams(z, plan, pre_scale, float(length_penalty), graph)]
+        st, ran = self._run(z, plan, pre_scale=pre_scale, uniforms=uniforms, graph=graph)
         tokens, lengths = st.tokens.cpu(), st.lengths.cpu()
         rows = [tokens[r, :int(lengths[r])].long() for r in range(st.R)]
         if return_logits:
@@ -831,8 +840,8 @@ class optimus_vae_next(PackedModule):
         step by step over the KV cache with the tokens forced instead of sampled."""
         ids = torch.as_tensor(ids)
         R, L = ids.shape
-        st, ran = self._run(z, 1.0, -1, max_len=1 << 30, nsteps=L, mode="forced", forced=ids.to(torch.int32).to(z.device),
-                            record=True, graph=graph)
+        st, ran = self._run(z, decode_plan("forced", 1.0, -1, max_len=1 << 30, record=True), nsteps=L,
+                            forced=ids.to(torch.int32).to(z.device), graph=graph)
         return st.record[:L].permute(1, 0, 2).contiguous()
 
     @torch.no_grad()

@@ -81,11 +81,9 @@ SIGNATURES = {
     "vdb_pack_geglu": (i, [p, p, i, i, p, p, p]),
     "vdb_pad_heads": (i, [p, i, i, i, i, p, p]),
     "vdb_textdec_gemv": (i, [p, i, ll, ll, p, p, f, p, ll, ll, p, i, i, p, ll, p]),
-    "vdb_textdec_attention": (i, [p, ll, p, ll, p, p, i, i, i, p, f, p, ll, p]),
+    "vdb_textdec_attention": (i, [p, ll, p, ll, p, p, p, i, i, i, p, f, p, ll, p]),
     "vdb_textdec_embed": (i, [p, i, p, p, i, p, i, i, p, i, i, p, p]),
-    "vdb_textdec_sample": (i, [p, i, i, ll, f, p, p, i, p, i, p, i, p, p, p, i, i, p, p]),
-    "vdb_textdec_sample_filtered": (i, [p, i, i, ll, f, i, f, p, p, i, p, i, p, i, p, p, p, i, i, p, p]),
-    "vdb_textdec_attention_indexed": (i, [p, ll, p, ll, p, p, p, i, i, i, p, f, p, ll, p]),
+    "vdb_textdec_sample": (i, [p, i, i, ll, f, i, f, p, p, i, p, i, p, i, p, p, p, i, i, p, p]),
     "vdb_textdec_beam_step": (i, [p, i, i, ll, f, i, p, i, p, i, p, p, p, p, i, i, p, p, p, p, p]),
     "vdb_textdec_repetition": (i, [p, i, i, ll, p, i, p, p, f, i, p]),
     "vdb_rank_adjust_f32": (i, [p, i, i, i, p, i, i, p, i, p, p, p, p, p]),

@@ -928,14 +928,18 @@ def textdec_gemv(x, w, out, bias=None, ln=None, act=ACT_NONE, accumulate=False):
     return out
 
 
-def textdec_attention(qkv, mem, kcache, vcache, step, out, scale=0.125):
-    """qkv fp32 [R, 3*H*64], mem fp32 [R, >=H*64] (this layer's latent slice), caches fp32 [R, H, T, 64], step int32 [1]."""
+def textdec_attention(qkv, mem, kcache, vcache, step, out, scale=0.125, src=None):
+    """qkv fp32 [R, 3*H*64], mem fp32 [R, >=H*64] (this layer's latent slice), caches fp32 [R, H, T, 64], step int32 [1].
+    src int32 [R, T] (beam search): cache slot j of row r is read from physical row src[r, j] (see vdb_textdec_attention)."""
     for n, t in (("qkv", qkv), ("mem", mem), ("out", out)):
         _need(t, torch.float32, n, rows_ok=True)
     _need(kcache, torch.float32, "kcache"); _need(vcache, torch.float32, "vcache"); _need(step, torch.int32, "step")
+    _need(src, torch.int32, "src")
     R, H, T, _ = kcache.shape
-    check(lib.vdb_textdec_attention(_ptr(qkv), qkv.stride(0), _ptr(mem), mem.stride(0), _ptr(kcache), _ptr(vcache), R, H, T,
-                                    _ptr(step), float(scale), _ptr(out), out.stride(0), _stream()), "textdec_attention")
+    if src is not None and tuple(src.shape) != (R, T):
+        raise ValueError(f"textdec_attention: src must be [{R}, {T}], got {list(src.shape)}")
+    check(lib.vdb_textdec_attention(_ptr(qkv), qkv.stride(0), _ptr(mem), mem.stride(0), _ptr(kcache), _ptr(vcache), _ptr(src), R, H,
+                                    T, _ptr(step), float(scale), _ptr(out), out.stride(0), _stream()), "textdec_attention")
     return out
 
 
@@ -954,36 +958,16 @@ def textdec_sample(logits, tokens, done, lengths, step, temperature=1.0, seed=No
                    max_len=30, record=None, top_k=0, top_p=0.0):
     """Token *step+1 of every unfinished row ~ softmax(logits / temperature) (see vdb_textdec_sample).  seed: device uint64 [1]
     (as int64), uniforms: fp64 [R, >=steps] given draws, forced: int32 [R, L] teacher-forced tokens, record: fp32 [steps, R, V].
-    top_k > 0 or 0 < top_p < 1 draw from the tokens those cuts keep instead (vdb_textdec_sample_filtered)."""
+    top_k > 0 or 0 < top_p < 1 draw from the tokens those cuts keep instead."""
     _need(logits, torch.float32, "logits", rows_ok=True)
     _need(tokens, torch.int32, "tokens"); _need(done, torch.int32, "done"); _need(lengths, torch.int32, "lengths")
     _need(step, torch.int32, "step"); _need(seed, torch.int64, "seed"); _need(uniforms, torch.float64, "uniforms")
     _need(forced, torch.int32, "forced"); _need(record, torch.float32, "record")
     R, V = logits.shape
-    args = (_ptr(seed), _ptr(uniforms), uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
-            forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done), _ptr(lengths), _ptr(step),
-            int(eos), int(max_len), _ptr(record), _stream())
-    if top_k == 0 and top_p in (0.0, 1.0):
-        check(lib.vdb_textdec_sample(_ptr(logits), R, V, logits.stride(0), float(temperature), *args), "textdec_sample")
-    else:
-        check(lib.vdb_textdec_sample_filtered(_ptr(logits), R, V, logits.stride(0), float(temperature), int(top_k), float(top_p),
-                                              *args), "textdec_sample_filtered")
-
-
-def textdec_attention_indexed(qkv, mem, kcache, vcache, src, step, out, scale=0.125):
-    """textdec_attention with cache slot j of row r read from physical row src[r, j] (int32 [R, T]; see
-    vdb_textdec_attention_indexed)."""
-    for n, t in (("qkv", qkv), ("mem", mem), ("out", out)):
-        _need(t, torch.float32, n, rows_ok=True)
-    _need(kcache, torch.float32, "kcache"); _need(vcache, torch.float32, "vcache"); _need(step, torch.int32, "step")
-    _need(src, torch.int32, "src")
-    R, H, T, _ = kcache.shape
-    if tuple(src.shape) != (R, T):
-        raise ValueError(f"textdec_attention_indexed: src must be [{R}, {T}], got {list(src.shape)}")
-    check(lib.vdb_textdec_attention_indexed(_ptr(qkv), qkv.stride(0), _ptr(mem), mem.stride(0), _ptr(kcache), _ptr(vcache),
-                                            _ptr(src), R, H, T, _ptr(step), float(scale), _ptr(out), out.stride(0), _stream()),
-          "textdec_attention_indexed")
-    return out
+    check(lib.vdb_textdec_sample(_ptr(logits), R, V, logits.stride(0), float(temperature), int(top_k), float(top_p), _ptr(seed),
+                                 _ptr(uniforms), uniforms.stride(0) if uniforms is not None else 0, _ptr(forced),
+                                 forced.stride(0) if forced is not None else 0, _ptr(tokens), tokens.stride(0), _ptr(done),
+                                 _ptr(lengths), _ptr(step), int(eos), int(max_len), _ptr(record), _stream()), "textdec_sample")
 
 
 def textdec_beam_step(logits, num_beams, tokens, src, scores, done, lengths, step, cand_tok, cand_logp, temperature=1.0,
