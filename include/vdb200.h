@@ -240,33 +240,31 @@ int vdb_conv3x3_bf16(const void* X, int B, int H, int W, int C, int mode, const 
  * May hold any finite values: the pad keys (K rows / Vt columns b*kv_bstride + [Nk, kv_bstride)), the pad
  * query rows b*q_bstride + [Nq, q_bstride) of Q, and everything outside the given slices (other columns of
  * Q / K / Vt, Vt columns past B*kv_bstride).  Only rows b*q_bstride + [0, Nq), columns [0, H*d_head) of out
- * are written. */
+ * are written.
+ * Three forms, picked by kv_len and items (both non-NULL: VDB_ERR_UNSUPPORTED, no such kernel):
+ * - plain (kv_len and items NULL; Bq, Bkv, step_idx and accumulate 0 / NULL): the above.
+ * - kv_len != NULL: a key count per batch item — BertSelfAttention.forward, optimus_bert.py:200-233, under the padding mask of
+ *   BertForLatentConnector_XX.forward (:1404-1412): key j of item b is visible iff j < kv_len[b] (kv_len: device int32 [B],
+ *   clamped to [0, Nk]).  The reference adds -10000 to the masked scores; exp of that underflows to exactly 0 in fp32 next to any
+ *   visible key, so the hard mask computes the same function.  An item with kv_len[b] <= 0 gets zero output rows.  Masked K / V
+ *   rows are never weighted (they may hold any finite values).  d_head 64 only (VDB_ERR_UNSUPPORTED otherwise); causal != 0 or a
+ *   misaligned kv_len return VDB_ERR_INVALID.
+ * - items != NULL: the operands of each output item chosen by a device table — Prompt-to-Prompt's attention injection,
+ *   lib/model_zoo/prompt_edit.py.  items: device int32 [rows][3][B]; output item b reads Q from item bq = items[r][0][b], K from
+ *   item bk = items[r][1][b] and V^T from item bv = items[r][2][b] of row r = *step_idx (device int), and writes item b of out.
+ *   Entries must lie in [0, Bq) (bq) and [0, Bkv) (bk, bv), where Q holds Bq items and K / V^T hold Bkv items (the tensor maps are
+ *   sized by them); bv < 0 skips item b: nothing is read or written for it.  accumulate != 0: out = bf16(float(out) + O).  With
+ *   items[r][.][b] = b and accumulate 0 the output equals the plain form's bitwise.  A null or misaligned items / step_idx, or
+ *   Bq / Bkv <= 0, return VDB_ERR_INVALID; so does any of Bq, Bkv, step_idx, accumulate given without items.
+ * Refusals in order: the form's own (for the table: items / step_idx, then kv_len, then Bq / Bkv), then the checks common to all
+ * three, then a d_head without a kernel (VDB_ERR_UNSUPPORTED). */
 int vdb_attention_dk_pad(int d_head);
 int vdb_attention_dv_pad(int d_head);
 int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
                        const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                       int q_bstride, int kv_bstride, int d_head, float scale, int causal, void* stream);
-/* The same attention with a key count per batch item — BertSelfAttention.forward, optimus_bert.py:200-233, under the padding mask
- * of BertForLatentConnector_XX.forward (:1404-1412): key j of item b is visible iff j < kv_len[b] (kv_len: device int32 [B],
- * clamped to [0, Nk]).  The reference adds -10000 to the masked scores; exp of that underflows to exactly 0 in fp32 next to any
- * visible key, so the hard mask computes the same function.  An item with kv_len[b] <= 0 gets zero output rows.  Masked K / V
- * rows are never weighted (they may hold any finite values).  d_head 64 only (VDB_ERR_UNSUPPORTED otherwise); causal != 0 and a
- * NULL or misaligned kv_len return VDB_ERR_INVALID.  The other arguments are those of vdb_attention_bf16. */
-int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                              const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                              int q_bstride, int kv_bstride, int d_head, float scale, int causal, const int* kv_len,
-                              void* stream);
-/* The same attention with the operands of each output item chosen by a device table — Prompt-to-Prompt's attention injection,
- * lib/model_zoo/prompt_edit.py.  items: device int32 [rows][3][B]; output item b reads Q from item bq = items[r][0][b], K from item
- * bk = items[r][1][b] and V^T from item bv = items[r][2][b] of row r = *step_idx (device int), and writes item b of out.  Entries must
- * lie in [0, Bq) (bq) and [0, Bkv) (bk, bv), where Q holds Bq items and K / V^T hold Bkv items (the tensor maps are sized by them);
- * bv < 0 skips item b: nothing is read or written for it.  accumulate != 0: out = bf16(float(out) + O).  With items[r][.][b] = b and
- * accumulate 0 the output equals vdb_attention_bf16's bitwise.  A null or misaligned items / step_idx, or Bq / Bkv <= 0, return
- * VDB_ERR_INVALID.  The other arguments are those of vdb_attention_bf16. */
-int vdb_attention_indexed_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                               const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                               int q_bstride, int kv_bstride, int d_head, float scale, int causal, int Bq, int Bkv,
-                               const int* items, const int* step_idx, int accumulate, void* stream);
+                       int q_bstride, int kv_bstride, int d_head, float scale, int causal,
+                       const int* kv_len, int Bq, int Bkv, const int* items, const int* step_idx, int accumulate,
+                       void* stream);
 /* Prompt-to-Prompt's word maps from the operands of a cross-attention call, fp32 math: for r in [0, n) and query p in [0, N),
  *   map[r, p] += sum over heads h of sum over keys j < L of w[r, j] * softmax_j(scale * q . k)
  * with q = Q row (row0 + r) * N + p, k = K row (row0 + r) * kv_bstride + j, both at columns h*DK .. h*DK + d_head (DK =

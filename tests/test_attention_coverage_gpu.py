@@ -8,7 +8,7 @@ restates it and each case asserts that the pads agree:
     56-64     64   64   128  2       consumer-issued TMA
     72-80     128  80   64   3       consumer-issued TMA
     136-160   192  160  64   2       producer warp
-    64        64   64   128  2       varlen (vdb_attention_varlen_bf16)
+    64        64   64   128  2       varlen (vdb_attention_bf16 with kv_len)
 d_head 88-128 and > 160 are refused (test_cabi pins that).  Key tile t sits in ring stage t % stages and waits for phase
 (t / stages) & 1, so a batch item with n keys runs T = ceil(n / BKV) tiles and wraps its rings (T - 1) // stages times.  Each
 case is tagged with the instantiation, T, the wraps, the keys in its last tile, whether the last 128-row query tile is partial
@@ -73,7 +73,7 @@ about +-60), against softmax(float32(scale) q k^T) v in fp64 with the bound e ab
 UNet step (B 8, H 8: self-attention through the fused q | k buffer at N 4096 / 1024 / 256 / 64 with d_head 40 / 80 / 160 / 160,
 cross-attention over 77 and 257 context tokens stored in 80 / 264 rows per item at each level), the ragged self-attention path
 (kv_bstride = Np > N), CLIP's text (77 of 80 rows, causal, d 64, H 12) and image (257 of 264, d 64, H 16) encoders, a small
-case at every supported d_head, causal masks at d_head 40, 80 and 160, and the varlen entry with kv_len 0, 1, 127, 128,
+case at every supported d_head, causal masks at d_head 40, 80 and 160, and the varlen form with kv_len 0, 1, 127, 128,
 129, 248, Nk, > Nk (clamped) and negative (an item without visible keys must get zero rows).
 
 Layout and write safety, every case: Q and K sit in wider buffers (NaN in the columns outside the heads; ldq != ldk; in the

@@ -252,23 +252,27 @@ def test_refusals_before_any_device_work():
         S.p_sample_ddim_multicontext(x_info, [_cinfo(ed=ed)], torch.zeros(3, dtype=torch.long), 4)
 
 
-def test_entry_points_reject_bad_arguments_without_gpu():
-    """vdb_attention_indexed_bf16, vdb_xattn_word_map_f32 and vdb_local_blend_f32 refuse bad arguments before any launch (the
-    fake addresses are never dereferenced)."""
+def test_items_attention_word_map_and_blend_reject_bad_arguments_without_gpu():
+    """vdb_attention_bf16 with an item table, vdb_xattn_word_map_f32 and vdb_local_blend_f32 refuse bad arguments before any
+    launch (the fake addresses are never dereferenced)."""
     from vdb200._lib import lib
     before = lib.vdb_launch_count()
-    at = dict(q=0x100000, k=0x200000, vt=0x300000, out=0x400000, items=0x500000, idx=0x600000, Bq=4, Bkv=6, d=40)
+    at = dict(q=0x100000, k=0x200000, vt=0x300000, out=0x400000, items=0x500000, idx=0x600000, Bq=4, Bkv=6, acc=1, d=40)
 
     def attn(**kw):
         a = dict(at, **kw)
-        return lib.vdb_attention_indexed_bf16(a["q"], 1280, 0, a["k"], 1280, 0, a["vt"], 512, a["out"], 1280, 4, 8, 64, 77, 0, 80,
-                                              a["d"], 0.125, 0, a["Bq"], a["Bkv"], a["items"], a["idx"], 1, None)
+        return lib.vdb_attention_bf16(a["q"], 1280, 0, a["k"], 1280, 0, a["vt"], 512, a["out"], 1280, 4, 8, 64, 77, 0, 80,
+                                      a["d"], 0.125, 0, None, a["Bq"], a["Bkv"], a["items"], a["idx"], a["acc"], None)
 
     for k in ("items", "idx"):
-        assert attn(**{k: None}) == 1 and b"attention_indexed: items and step_idx" in lib.vdb_last_error(), k
+        assert attn(**{k: None}) == 1 and b"attention: items and step_idx" in lib.vdb_last_error(), k
         assert attn(**{k: at[k] + 2}) == 1 and b"4-byte aligned" in lib.vdb_last_error(), k
     for k in ("Bq", "Bkv"):
         assert attn(**{k: 0}) == 1 and b"Bq and Bkv" in lib.vdb_last_error(), k
+    # Bq, Bkv, step_idx and accumulate belong to the table: each one alone, without items, is refused
+    none = dict(items=None, idx=None, Bq=0, Bkv=0, acc=0)
+    for k in ("Bq", "Bkv", "idx", "acc"):
+        assert attn(**dict(none, **{k: at[k]})) == 1 and b"items and step_idx" in lib.vdb_last_error(), k
     for k in ("q", "k", "vt", "out"):
         assert attn(**{k: None}) == 1 and b"attention: null" in lib.vdb_last_error(), k
     assert attn(d=44) == 1 and b"multiples of 8" in lib.vdb_last_error()

@@ -1,5 +1,5 @@
-"""Prompt-to-Prompt on the GPU (lib/model_zoo/prompt_edit.py): vdb_attention_indexed_bf16 per element against fp64 at every
-instantiation (with random tables, skips and accumulation) and bitwise against vdb_attention_bf16 under the identity table,
+"""Prompt-to-Prompt on the GPU (lib/model_zoo/prompt_edit.py): vdb_attention_bf16 with an item table per element against fp64
+at every instantiation (with random tables, skips and accumulation) and bitwise against the plain form under the identity table,
 vdb_xattn_word_map_f32 against fp64, vdb_local_blend_f32 bitwise against its fp32 restatement; on the mini UNet the edited DDIM
 and DPM-Solver++ walks against oracle/prompt_edit_oracle.py; and the invariants: the source row and a zero-window edit equal
 the unedited batch bit for bit, the graph equals eager, a second call replays the cached graph, and the launches per step."""
@@ -45,7 +45,7 @@ def _ref(q, k, v, bq, bk, bv, Nq, Nk, kvb, scale):
 
 
 @pytest.mark.parametrize("d", [8, 16, 32, 40, 64, 80, 160])
-def test_indexed_attention_per_element(d):
+def test_attention_with_items_per_element(d):
     from vdb200 import ops
     g = np.random.default_rng(d)
     B, Bq, Bkv, H, Nq, Nk, kvb = 4, 5, 7, 2, 200, 77, 80
@@ -58,8 +58,8 @@ def test_indexed_attention_per_element(d):
         prev = g.standard_normal((B * Nq, H * d)).astype(np.float32)
         out = _bf(prev)
         prev64 = out.float().cpu().double().numpy()
-        ops.attention_indexed(tq, tk, tv, out, B, H, Nq, Nk, d, Bq, Bkv, ti, torch.tensor([1], dtype=torch.int32, device=DEV),
-                              kv_bstride=kvb, accumulate=acc)
+        ops.attention(tq, tk, tv, out, B, H, Nq, Nk, d, kv_bstride=kvb, items=ti,
+                      step_idx=torch.tensor([1], dtype=torch.int32, device=DEV), Bq=Bq, Bkv=Bkv, accumulate=acc)
         got = out.float().cpu().double().numpy()
         for b in range(B):
             rows = slice(b * Nq, (b + 1) * Nq)
@@ -73,7 +73,7 @@ def test_indexed_attention_per_element(d):
 
 
 @pytest.mark.parametrize("d", [8, 40, 64, 80, 160])
-def test_identity_table_equals_plain_attention(d):
+def test_identity_items_table_equals_plain_attention(d):
     from vdb200 import ops
     g = np.random.default_rng(100 + d)
     B, H, Nq, Nk, kvb = 3, 2, 256, 77, 80
@@ -82,8 +82,8 @@ def test_identity_table_equals_plain_attention(d):
     ops.attention(tq, tk, tv, plain, B, H, Nq, Nk, d, kv_bstride=kvb)
     ident = torch.arange(B, dtype=torch.int32, device=DEV).view(1, 1, B).repeat(2, 3, 1).contiguous()
     out = torch.empty_like(plain)
-    ops.attention_indexed(tq, tk, tv, out, B, H, Nq, Nk, d, B, B, ident, torch.tensor([1], dtype=torch.int32, device=DEV),
-                          kv_bstride=kvb)
+    ops.attention(tq, tk, tv, out, B, H, Nq, Nk, d, kv_bstride=kvb, items=ident,
+                  step_idx=torch.tensor([1], dtype=torch.int32, device=DEV))
     assert torch.equal(out, plain)
 
 

@@ -139,23 +139,26 @@ def test_tokenizer_matches_reference():
         assert ours.encode(t) == [cls, sep]
 
 
-def test_varlen_attention_checks_arguments_before_launch():
-    """null / misaligned kv_len, d_head other than 64 and causal masking are refused (the fake addresses are never touched)."""
+def test_kv_len_attention_checks_arguments_before_launch():
+    """vdb_attention_bf16 with kv_len: a misaligned kv_len, d_head other than 64, causal masking and an item table together with
+    kv_len are refused; a NULL kv_len is the plain form, not a kv_len error (the fake addresses are never touched)."""
     from vdb200._lib import lib
-    q, k, vt, out, kvl = 0x10000, 0x20000, 0x30000, 0x40000, 0x50000
+    q, k, vt, out, kvl, items, idx = 0x10000, 0x20000, 0x30000, 0x40000, 0x50000, 0x60000, 0x70000
 
-    def call(kv_len=kvl, d_head=64, causal=0, H=12):
-        return lib.vdb_attention_varlen_bf16(q, 1536, 0, k, 1536, 768, vt, 160, out, 768, 2, H, 80, 80, 80, 80, d_head,
-                                             d_head ** -0.5, causal, kv_len, None)
-    for kw, rc, msg in ((dict(kv_len=None), 1, b"kv_len"), (dict(kv_len=kvl + 2), 1, b"kv_len"), (dict(causal=1), 1, b"causal"),
+    def call(kv_len=kvl, d_head=64, causal=0, H=12, q=q, kv_bstride=80, table=(0, 0, None, None, 0)):
+        return lib.vdb_attention_bf16(q, 1536, 0, k, 1536, 768, vt, 160, out, 768, 2, H, 80, 80, 80, kv_bstride, d_head,
+                                      d_head ** -0.5, causal, kv_len, *table, None)
+    for kw, rc, msg in ((dict(kv_len=kvl + 2), 1, b"kv_len"), (dict(causal=1), 1, b"causal"),
                         (dict(d_head=80), 3, b"d_head 64"), (dict(d_head=40), 3, b"d_head 64"),
-                        (dict(d_head=160), 3, b"d_head 64")):
+                        (dict(d_head=160), 3, b"d_head 64"), (dict(table=(2, 2, items, idx, 0)), 3, b"kv_len"),
+                        (dict(table=(2, 2, items, idx, 1)), 3, b"kv_len")):
         assert call(**kw) == rc and msg in lib.vdb_last_error(), (kw, lib.vdb_last_error())
-    # the checks shared with vdb_attention_bf16 still apply
-    assert lib.vdb_attention_varlen_bf16(None, 1536, 0, k, 1536, 768, vt, 160, out, 768, 2, 12, 80, 80, 80, 80, 64, 0.125, 0,
-                                         kvl, None) == 1
-    assert lib.vdb_attention_varlen_bf16(q, 1536, 0, k, 1536, 768, vt, 160, out, 768, 2, 12, 80, 80, 80, 84, 64, 0.125, 0,
-                                         kvl, None) == 1
+    # the checks shared with the plain form still apply
+    assert call(q=None) == 1 and b"null" in lib.vdb_last_error()
+    assert call(kv_bstride=84) == 1 and b"kv_bstride" in lib.vdb_last_error()
+    # a NULL kv_len selects the plain form: the call reaches the shared null check
+    assert call(kv_len=None, q=None) == 1
+    assert b"null" in lib.vdb_last_error() and b"kv_len" not in lib.vdb_last_error()
 
 
 def test_pooler_tanh_is_accepted_and_gelu_still_refused():

@@ -326,6 +326,19 @@ static int launch_attention(AttnParams& p, const AttnArgs& a, void* stream) {
   return launch(kernel, grid, dim3(attention_threads(TMA_WARP)), smem, stream, p);
 }
 
+// The instantiation for the head pads (DK, DVP) of p.dv, plain or indexed.  d_head <= 80: two CTAs per SM, each within 128
+// registers and half the shared memory (d_head <= 64: 128-key tiles, 3 / 2 stages; d_head 80: 64-key tiles, 3 stages).
+// d_head 160 keeps the TMA warp and one CTA per SM: two CTAs' Q and K / V^T stages do not fit; 64-key tiles keep its S + O + P
+// within the register budget.
+template <bool INDEXED>
+static int launch_for_pads(int DK, int DVP, AttnParams& p, const AttnArgs& a, void* stream) {
+  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false, false, INDEXED>(p, a, stream);
+  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false, false, INDEXED>(p, a, stream);
+  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false, false, INDEXED>(p, a, stream);
+  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true, false, INDEXED>(p, a, stream);
+  return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel for d_head %d", p.dv);
+}
+
 // Prompt-to-Prompt's word maps (lib/model_zoo/prompt_edit.py) from the bf16 operands of a cross-attention call, fp32 math:
 //   map[r, p] += sum over h of sum over j < L of w[r, j] softmax_j(scale q[(row0 + r) N + p, head h] . k[(row0 + r) kv_bs + j, head h])
 // One CTA per (block of kWmapQ queries, r).  K of one head at a time sits in shared memory; warp g owns queries
@@ -424,10 +437,25 @@ int vdb_attention_dv_pad(int d_head) {
   return -1;
 }
 
-// Argument checks and parameter block shared by both entry points; returns VDB_OK or the error status.
-static int attention_prepare(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0, const void* Vt,
-                             long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk, int q_bstride, int kv_bstride,
-                             int d_head, float scale, int causal, AttnParams& p, AttnArgs& a) {
+int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
+                       const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
+                       int q_bstride, int kv_bstride, int d_head, float scale, int causal,
+                       const int* kv_len, int Bq, int Bkv, const int* items, const int* step_idx, int accumulate,
+                       void* stream) {
+  // each form's own checks come first.  Any argument of the item table asks for the indexed form, which needs the table.
+  if (items || step_idx || Bq || Bkv || accumulate) {
+    if (!items || !step_idx || (reinterpret_cast<uintptr_t>(items) & 3) || (reinterpret_cast<uintptr_t>(step_idx) & 3))
+      return set_error(VDB_ERR_INVALID, "attention: items and step_idx must be non-null, 4-byte aligned device int32 "
+                                        "(Bq, Bkv and accumulate belong to them)");
+    if (kv_len) return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel takes both kv_len and items");
+    if (Bq <= 0 || Bkv <= 0) return set_error(VDB_ERR_INVALID, "attention: Bq and Bkv must be > 0 (got %d, %d)", Bq, Bkv);
+  } else if (kv_len) {
+    if (reinterpret_cast<uintptr_t>(kv_len) & 3)
+      return set_error(VDB_ERR_INVALID, "attention: kv_len must be a 4-byte aligned device int32 [B]");
+    if (causal) return set_error(VDB_ERR_INVALID, "attention: causal masking together with kv_len is not supported");
+    if (vdb_attention_dk_pad(d_head) != 64 || vdb_attention_dv_pad(d_head) != 64)
+      return set_error(VDB_ERR_UNSUPPORTED, "attention: with kv_len only d_head 64 (BERT) is instantiated, got %d", d_head);
+  }
   if (!Q || !K || !Vt || !out || B <= 0 || H <= 0 || Nq <= 0 || Nk <= 0)
     return set_error(VDB_ERR_INVALID, "attention: null/empty argument");
   const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
@@ -440,75 +468,20 @@ static int attention_prepare(const void* Q, long long ldq, int q_col0, const voi
   if (q_bstride < Nq || kv_bstride < Nk || (kv_bstride % 8))
     return set_error(VDB_ERR_INVALID, "attention: need q_bstride >= Nq, kv_bstride >= Nk and kv_bstride %% 8 == 0 (got %d, %d)",
                      q_bstride, kv_bstride);
+  AttnParams p;
   memset(&p, 0, sizeof(p));
-  a = AttnArgs{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride, B, B};
   p.Nq = Nq; p.Nk = Nk; p.q_bs = q_bstride; p.kv_bs = kv_bstride; p.q_col0 = q_col0; p.k_col0 = k_col0; p.dv = d_head; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.ldo = ldo;
-  return VDB_OK;
-}
-
-int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                       const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                       int q_bstride, int kv_bstride, int d_head, float scale, int causal, void* stream) {
-  AttnParams p;
-  AttnArgs a{};
-  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
-                                   scale, causal, p, a);
-  if (rc) return rc;
-  const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
-  // d_head <= 80: two CTAs per SM, each within 128 registers and half the shared memory (d_head <= 64: 128-key tiles,
-  // 3 / 2 stages; d_head 80: 64-key tiles, 3 stages).  d_head 160 keeps the TMA warp and one CTA per SM: two CTAs' Q and
-  // K / V^T stages do not fit; 64-key tiles keep its S + O + P within the register budget.
-  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false>(p, a, stream);
-  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false>(p, a, stream);
-  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false>(p, a, stream);
-  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true>(p, a, stream);
-  return set_error(VDB_ERR_UNSUPPORTED, "attention: no kernel for d_head %d", d_head);
-}
-
-int vdb_attention_varlen_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                              const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                              int q_bstride, int kv_bstride, int d_head, float scale, int causal, const int* kv_len,
-                              void* stream) {
-  if (!kv_len || (reinterpret_cast<uintptr_t>(kv_len) & 3))
-    return set_error(VDB_ERR_INVALID, "attention_varlen: kv_len must be a non-null, 4-byte aligned device int32 [B]");
-  if (causal) return set_error(VDB_ERR_INVALID, "attention_varlen: causal masking together with kv_len is not supported");
-  if (vdb_attention_dk_pad(d_head) != 64 || vdb_attention_dv_pad(d_head) != 64)
-    return set_error(VDB_ERR_UNSUPPORTED, "attention_varlen: only d_head 64 (BERT) is instantiated, got %d", d_head);
-  AttnParams p;
-  AttnArgs a{};
-  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
-                                   scale, causal, p, a);
-  if (rc) return rc;
   p.kv_len = kv_len;
-  return launch_attention<64, 64, 128, 2, false, true>(p, a, stream);
-}
-
-int vdb_attention_indexed_bf16(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0,
-                               const void* Vt, long long ldv, void* out, long long ldo, int B, int H, int Nq, int Nk,
-                               int q_bstride, int kv_bstride, int d_head, float scale, int causal, int Bq, int Bkv,
-                               const int* items, const int* step_idx, int accumulate, void* stream) {
-  if (!items || !step_idx || (reinterpret_cast<uintptr_t>(items) & 3) || (reinterpret_cast<uintptr_t>(step_idx) & 3))
-    return set_error(VDB_ERR_INVALID, "attention_indexed: items and step_idx must be non-null, 4-byte aligned device int32");
-  if (Bq <= 0 || Bkv <= 0) return set_error(VDB_ERR_INVALID, "attention_indexed: Bq and Bkv must be > 0 (got %d, %d)", Bq, Bkv);
-  AttnParams p;
-  AttnArgs a{};
-  const int rc = attention_prepare(Q, ldq, q_col0, K, ldk, k_col0, Vt, ldv, out, ldo, B, H, Nq, Nk, q_bstride, kv_bstride, d_head,
-                                   scale, causal, p, a);
-  if (rc) return rc;
-  a.Bq = Bq;
-  a.Bkv = Bkv;
   p.items = items;
   p.step_idx = step_idx;
   p.accumulate = accumulate ? 1 : 0;
-  const int DK = vdb_attention_dk_pad(d_head), DVP = vdb_attention_dv_pad(d_head);
-  if (DK == 64 && DVP == 48) return launch_attention<64, 48, 128, 3, false, false, true>(p, a, stream);
-  if (DK == 64 && DVP == 64) return launch_attention<64, 64, 128, 2, false, false, true>(p, a, stream);
-  if (DK == 128 && DVP == 80) return launch_attention<128, 80, 64, 3, false, false, true>(p, a, stream);
-  if (DK == 192 && DVP == 160) return launch_attention<192, 160, 64, 2, true, false, true>(p, a, stream);
-  return set_error(VDB_ERR_UNSUPPORTED, "attention_indexed: no kernel for d_head %d", d_head);
+  const AttnArgs a{Q, K, Vt, ldq, ldk, ldv, B, H, q_bstride, kv_bstride, items ? Bq : B, items ? Bkv : B};
+  if (!kv_len && !items) return launch_for_pads<false>(DK, DVP, p, a, stream);
+  if (kv_len) return launch_attention<64, 64, 128, 2, false, true>(p, a, stream);
+  return launch_for_pads<true>(DK, DVP, p, a, stream);
 }
 
 int vdb_xattn_word_map_f32(const void* Q, long long ldq, const void* K, long long ldk, const float* w, float* map, int n, int row0,

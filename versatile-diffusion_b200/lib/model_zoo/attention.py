@@ -199,9 +199,9 @@ class CrossAttention(PackedModule):
             ops.attention(q, k, vt, o, B, H, N, Nk, d, **kw)
             return
         Bkv = edit.ctx_batch if cross else B
-        ops.attention_indexed(q, k, vt, o, B, H, N, Nk, d, B, Bkv, items, edit.idx, **kw)
+        ops.attention(q, k, vt, o, B, H, N, Nk, d, items=items, step_idx=edit.idx, Bkv=Bkv, **kw)
         if cross and edit.cross2 is not None:
-            ops.attention_indexed(q, k, vt, o, B, H, N, Nk, d, B, Bkv, edit.cross2, edit.idx, accumulate=True, **kw)
+            ops.attention(q, k, vt, o, B, H, N, Nk, d, items=edit.cross2, step_idx=edit.idx, Bkv=Bkv, accumulate=True, **kw)
         if cross and edit.maps_at(N):
             ops.xattn_word_map(q, k, edit.w, edit.map, edit.c0, H, N, Nk, d, kv_bstride=kv_bstride, scale=self.scale)
 

@@ -5,7 +5,7 @@ over BertForLatentConnector_XX (optimus_models/optimus_bert.py:1348-1437) and GP
 encode(texts) turns sentences into text latents z_mu [n, 768] (`net.vae_encode(texts, which='text')`, `net.ctx_encode(texts,
 which='vae_text')`).  The BERT encoder is built only when the module is given an `encoder` config.  Its 12 post-LN layers (LayerNorm
 eps 1e-12, erf GELU) run on the same kernels as the CLIP towers: ops.gemm, ops.layernorm and the flash attention, here with one key
-count per sentence (vdb_attention_varlen_bf16) in place of the reference's -10000 padding mask.  The pooler (tanh of a dense layer on
+count per sentence (vdb_attention_bf16 with kv_len) in place of the reference's -10000 padding mask.  The pooler (tanh of a dense layer on
 the [CLS] row) and the z_mu half of `linear` run as two weight-streaming GEMVs on the [CLS] rows, 16 sentences at a time.
 The WordPiece tokenizer is written from the behaviour of the reference's: the sentence is lowercased first (optimus.py:731, although
 the vocabulary is cased and do_lower_case is false, so accents are kept), BERT's basic tokenizer drops control characters, spaces out

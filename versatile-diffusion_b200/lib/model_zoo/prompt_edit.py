@@ -29,7 +29,7 @@ Cross-attention (every attn2 of the edited context).  The conditional row of tar
 At other positions it is the row's own attention.  Unconditional rows and the source row are never edited, as in P2P, which
 edits only the conditional half.  VD's to_v has no bias, so in exact arithmetic this equals P2P's edit on the probabilities:
 (attn_src M) * c, or (alpha * attn_src[:, map] + (1 - alpha) * attn_tgt) * c.  One indexed flash-attention launch
-(vdb_attention_indexed_bf16) does it; the refinement's second term is a second launch that accumulates into the output.
+(vdb_attention_bf16 with an items table) does it; the refinement's second term is a second launch that accumulates into the output.
 
 Self-attention (attn1 of the edited context's SpatialTransformers).  Only at layers whose token grid is at most (H/4)(W/4)
 tokens (H/4 and W/4 rounded up as the UNet's stride-2 convolutions round them); that is P2P's 16^2 limit at 512^2.  At

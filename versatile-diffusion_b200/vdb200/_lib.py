@@ -50,9 +50,7 @@ SIGNATURES = {
     "vdb_conv3x3_bf16": (i, [p, i, i, i, i, i, p, i, ll, p, i, p, i, p, ll, p, ll, p, ll, i, i, i, i, p, sz, p]),
     "vdb_attention_dk_pad": (i, [i]),
     "vdb_attention_dv_pad": (i, [i]),
-    "vdb_attention_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p]),
-    "vdb_attention_varlen_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p, p]),
-    "vdb_attention_indexed_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, i, i, p, p, i, p]),
+    "vdb_attention_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p, i, i, p, p, i, p]),
     "vdb_xattn_word_map_f32": (i, [p, ll, p, ll, p, p, i, i, i, i, i, i, i, f, p]),
     "vdb_groupnorm_nsplit": (i, [i, i]),
     "vdb_groupnorm_scratch_floats": (ll, [i, i]),

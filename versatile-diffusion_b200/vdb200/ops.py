@@ -477,40 +477,27 @@ def attention_pads(d_head):
 
 
 def attention(q, k, vt, out, B, H, Nq, Nk, d_head, scale=None, q_col0=0, k_col0=0, causal=False,
-              q_bstride=0, kv_bstride=0, kv_len=None):
-    """Flash attention. q [B*q_bstride, ldq], k [B*kv_bstride, ldk], vt [H*DVP, B*kv_bstride], out [B*q_bstride, H*d_head].
-    kv_bstride (default Nk) must be a multiple of 8: pad ragged contexts per batch item.  kv_len (int32 device [B], d_head 64,
-    not causal): item b attends to its first kv_len[b] keys only (vdb_attention_varlen_bf16)."""
+              q_bstride=0, kv_bstride=0, kv_len=None, items=None, step_idx=None, Bq=None, Bkv=None, accumulate=False):
+    """Flash attention (vdb_attention_bf16). q [B*q_bstride, ldq], k [B*kv_bstride, ldk], vt [H*DVP, B*kv_bstride],
+    out [B*q_bstride, H*d_head].  kv_bstride (default Nk) must be a multiple of 8: pad ragged contexts per batch item.
+    kv_len (int32 device [B], d_head 64, not causal): item b attends to its first kv_len[b] keys only.
+    items (int32 device [rows, 3, B]) with step_idx (int32 device [1]): output item b reads Q / K / V^T from items
+    items[r, 0..2, b], r = step_idx[0], entries in [0, Bq) / [0, Bkv) (both default B), a negative V item skips b
+    (lib/model_zoo/prompt_edit.py); accumulate: out += the attention (bf16)."""
     _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(vt, BF16, "vt", True); _need(out, BF16, "out", True)
-    _need(kv_len, torch.int32, "kv_len")
-    if scale is None:
-        scale = d_head ** -0.5
-    args = (_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt), vt.stride(0), _ptr(out), out.stride(0),
-            B, H, Nq, Nk, int(q_bstride), int(kv_bstride), d_head, float(scale), 1 if causal else 0)
-    with _Span("attention", 4.0 * B * H * Nq * Nk * d_head, 2.0 * B * H * d_head * (2 * Nq + 2 * Nk)):
-        if kv_len is None:
-            check(lib.vdb_attention_bf16(*args, _stream()), "attention_bf16")
-        else:
-            check(lib.vdb_attention_varlen_bf16(*args, _ptr(kv_len), _stream()), "attention_varlen_bf16")
-    return out
-
-
-def attention_indexed(q, k, vt, out, B, H, Nq, Nk, d_head, Bq, Bkv, items, step_idx, scale=None, q_col0=0, k_col0=0,
-                      q_bstride=0, kv_bstride=0, accumulate=False):
-    """Flash attention with the operands of each output item chosen by a device table (vdb_attention_indexed_bf16,
-    lib/model_zoo/prompt_edit.py): output item b reads Q / K / V^T from items items[r, 0..2, b], r = step_idx[0]; items int32
-    [rows, 3, B] with entries in [0, Bq) / [0, Bkv), a negative V item skips b.  accumulate: out += the attention (bf16)."""
-    _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(vt, BF16, "vt", True); _need(out, BF16, "out", True)
-    _need(items, torch.int32, "items"); _need(step_idx, torch.int32, "step_idx")
-    if items.dim() != 3 or items.shape[1] != 3 or items.shape[2] != B:
-        raise ValueError(f"items: expected [rows, 3, {B}], got {tuple(items.shape)}")
+    _need(kv_len, torch.int32, "kv_len"); _need(items, torch.int32, "items"); _need(step_idx, torch.int32, "step_idx")
+    if items is not None:
+        if items.dim() != 3 or items.shape[1] != 3 or items.shape[2] != B:
+            raise ValueError(f"items: expected [rows, 3, {B}], got {tuple(items.shape)}")
+        Bq = B if Bq is None else Bq
+        Bkv = B if Bkv is None else Bkv
     if scale is None:
         scale = d_head ** -0.5
     with _Span("attention", 4.0 * B * H * Nq * Nk * d_head, 2.0 * B * H * d_head * (2 * Nq + 2 * Nk)):
-        check(lib.vdb_attention_indexed_bf16(_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt),
-                                             vt.stride(0), _ptr(out), out.stride(0), B, H, Nq, Nk, int(q_bstride), int(kv_bstride),
-                                             d_head, float(scale), 0, int(Bq), int(Bkv), _ptr(items), _ptr(step_idx),
-                                             1 if accumulate else 0, _stream()), "attention_indexed_bf16")
+        check(lib.vdb_attention_bf16(_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(vt), vt.stride(0),
+                                     _ptr(out), out.stride(0), B, H, Nq, Nk, int(q_bstride), int(kv_bstride), d_head, float(scale),
+                                     1 if causal else 0, _ptr(kv_len), int(Bq or 0), int(Bkv or 0), _ptr(items), _ptr(step_idx),
+                                     1 if accumulate else 0, _stream()), "attention_bf16")
     return out
 
 
