@@ -156,6 +156,21 @@ int vdb_region_noise_f32(const unsigned long long* seed, const int* step_idx, lo
 int vdb_region_merge_f32(const float* eps, int halves, int bs, int H, int W, int C, const int* oy, const int* ox, const int* cover_y,
                          const int* cover_x, int ny, int nx, int h, int w, int first, int k, int R, const float* masks, float* out,
                          void* stream);
+/* ---- self-attention guidance — lib/model_zoo/sag.py (an addition: the reference has no SAG; the semantics are specified in that
+ * module's docstring) ----------------------------------------------------------------------------------------------------------------
+ * vdb_sag_degrade_f32: x, e, out fp32 NHWC [bs, H, W, C]; mass fp32 [bs, hm*wm], the mid block's key mass; table device fp32 rows
+ * {sqrt(a_t), sqrt(1 - a_t)}, row *step_idx (device int, required).  Per element, fp32 with explicit round-to-nearest:
+ *   x0 = (x - s1*e) / sa;  v = M ? blur(x0) : x0;  out = sa*v + s1*e
+ * with M = mass[b, (y*hm/H)*wm + x*wm/W] > 1 (integer division: nearest upsampling) and blur the depthwise 9x9 Gaussian of sigma 1
+ * (taps exp(-k^2/2), k = -4..4, normalised in double) with reflect padding by 4, applied along rows then along columns, each sum
+ * in tap order with fused multiply-adds.  VDB_ERR_INVALID before any launch: a null argument, a size <= 0, H or W < 5, a pointer not
+ * 4-byte aligned, or out overlapping x, e or mass; VDB_ERR_UNSUPPORTED: C > 8, hm > H, wm > W or hm*wm > 4096.
+ * vdb_sag_guide_f32, in place on n elements: d = s*(e_src - e_deg) with e_src = e_u when e_u is non-NULL (CFG), else e_c; then
+ * e_c += d and e_u += d, fp32 with explicit round-to-nearest.  VDB_ERR_INVALID before any launch: a null e_c / e_deg, n <= 0, s not
+ * finite, a pointer not 4-byte aligned, or any two of e_u, e_c, e_deg overlapping. */
+int vdb_sag_degrade_f32(const float* x, const float* e, const float* mass, const float* table, const int* step_idx, int bs, int H,
+                        int W, int C, int hm, int wm, float* out, void* stream);
+int vdb_sag_guide_f32(float* e_u, float* e_c, const float* e_deg, float s, long long n, void* stream);
 /* y = a*x + b*z, fp32 — VD_v2_0.q_sample (vd.py:221-224) for the img2img start (ddim.py:97-103) */
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream);
 int vdb_add_int(int* p, int delta, void* stream); /* device-side step counter update */
@@ -274,6 +289,19 @@ int vdb_attention_bf16(const void* Q, long long ldq, int q_col0, const void* K, 
  * odd or short ldq / ldk, a pointer not 4-byte aligned, or map overlapping w. */
 int vdb_xattn_word_map_f32(const void* Q, long long ldq, const void* K, long long ldk, const float* w, float* map, int n, int row0,
                            int H, int N, int L, int kv_bstride, int d_head, float scale, void* stream);
+/* Self-attention guidance's key mass (lib/model_zoo/sag.py) from the operands of a self-attention call, fp32 math: for r in
+ * [0, n) and key j in [0, N),
+ *   mass[r, j] += w * sum over heads h of sum over queries p < N of softmax_j(scale * q . k)
+ * with q = Q row (row0 + r) * N + p at columns q_col0 + h*DK .., k = K row (row0 + r) * kv_bstride + j at columns k_col0 + h*DK ..
+ * (DK = vdb_attention_dk_pad(d_head)), bf16: the fused q | k buffer of a self-attention layer, or its separate q and padded keys.
+ * Two launches: the softmax max and sum of every (r, h, p) into stats (fp32 scratch of n*H*N*2), then one writer per mass entry
+ * adding the heads in order and the queries in a fixed order: bit-reproducible, no atomics.  N <= 4096 and d_head <= 160 a multiple
+ * of 8, else VDB_ERR_UNSUPPORTED.  VDB_ERR_INVALID before any launch: a null Q / K / stats / mass, a size <= 0, row0 < 0,
+ * kv_bstride < N (0 = N), odd or negative column offsets, odd ldq / ldk or ldq < q_col0 + H*DK (ldk likewise), a pointer not 4-byte
+ * aligned, or mass overlapping stats. */
+int vdb_sattn_key_mass_f32(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0, float* stats,
+                           float w, float* mass, int n, int row0, int H, int N, int kv_bstride, int d_head, float scale,
+                           void* stream);
 
 /* ---- GroupNorm(32) [+SiLU] [+channel concat] on NHWC — normalization()/Normalize():
  *      diffusion_utils.py:168-191 (eps 1e-5), attention.py:76-77 & autokl_modules.py:38-39 (1e-6) ----

@@ -421,6 +421,135 @@ __global__ void __launch_bounds__(kWmapThreads) xattn_word_map_kernel(
   }
 }
 
+// Self-attention guidance's key mass (lib/model_zoo/sag.py) from the bf16 operands of a self-attention call, fp32 math:
+//   mass[r, j] += w * sum over h of sum over p < N of softmax_j(scale q[(row0 + r) N + p, head h] . k[(row0 + r) kv_bs + j, head h])
+// A column sum of a row softmax, in two launches.  sattn_row_stats_kernel: one CTA per (kMassQ queries, head, r) walks the keys in
+// shared-memory tiles of kMassKT; warp g owns queries g*kMassQ/8 .., lane l keys l, l + 32 of each tile, with a running
+// (max, sum) per lane merged by a fixed xor tree -> stats[r, h, p] = {max of the raw dots, sum of exp2((dot - max) scale_log2)}.
+// sattn_key_mass_kernel: one CTA per (32 keys, r); lane l owns key l of the block, warp g queries p = g mod 8, all heads in order;
+// the eight warps' partial sums are added in warp order and each mass entry has one writer: the result is bit-reproducible.
+constexpr int kMassThreads = 256, kMassQ = 32, kMassKT = 64, kMassKeys = 32, kMassMaxD = 160, kMassMaxN = 4096;
+
+__device__ __forceinline__ void merge_stats(float& m, float& l, float mo, float lo, float scale_log2) {
+  const float mn = fmaxf(m, mo);
+  const float a = m == -INFINITY ? 0.f : l * exp2f((m - mn) * scale_log2);
+  const float b = mo == -INFINITY ? 0.f : lo * exp2f((mo - mn) * scale_log2);
+  m = mn;
+  l = a + b;
+}
+
+__global__ void __launch_bounds__(kMassThreads) sattn_row_stats_kernel(
+    const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloat16* __restrict__ K, long long ldk,
+    float* __restrict__ stats, int row0, int H, int N, int kv_bs, int d, int DK, float scale_log2) {
+  constexpr int kPerWarp = kMassQ / (kMassThreads / 32);
+  constexpr int kRowWords = kMassMaxD / 2 + 1;     // odd row stride in 4-byte words: lanes reading 32 rows hit 32 banks
+  __shared__ __nv_bfloat162 sK[kMassKT * kRowWords];
+  __shared__ float sq[kMassThreads / 32][kPerWarp][kMassMaxD];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int h = blockIdx.y, r = blockIdx.z, item = row0 + r;
+  const int rw = d / 2 + 1;
+#pragma unroll
+  for (int qq = 0; qq < kPerWarp; ++qq) {
+    const int p = min(blockIdx.x * kMassQ + warp * kPerWarp + qq, N - 1);
+    const __nv_bfloat16* qrow = Q + (static_cast<long long>(item) * N + p) * ldq + h * DK;
+    for (int c = lane; c < d; c += 32) sq[warp][qq][c] = __bfloat162float(qrow[c]);
+  }
+  float m[kPerWarp], l[kPerWarp];
+#pragma unroll
+  for (int qq = 0; qq < kPerWarp; ++qq) m[qq] = -INFINITY, l[qq] = 0.f;
+  for (int j0 = 0; j0 < N; j0 += kMassKT) {
+    const int nk = min(kMassKT, N - j0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < nk * (d / 2); e += kMassThreads) {
+      const int j = e / (d / 2), c2 = e % (d / 2);
+      sK[j * rw + c2] =
+          *reinterpret_cast<const __nv_bfloat162*>(K + (static_cast<long long>(item) * kv_bs + j0 + j) * ldk + h * DK + 2 * c2);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int t = 0; t < kMassKT / 32; ++t) {
+      const int j = lane + 32 * t;
+      if (j >= nk) break;
+      float dot[kPerWarp];
+#pragma unroll
+      for (int qq = 0; qq < kPerWarp; ++qq) dot[qq] = 0.f;
+      for (int c2 = 0; c2 < d / 2; ++c2) {
+        const float2 kv = __bfloat1622float2(sK[j * rw + c2]);
+#pragma unroll
+        for (int qq = 0; qq < kPerWarp; ++qq) {
+          dot[qq] = fmaf(sq[warp][qq][2 * c2], kv.x, dot[qq]);
+          dot[qq] = fmaf(sq[warp][qq][2 * c2 + 1], kv.y, dot[qq]);
+        }
+      }
+#pragma unroll
+      for (int qq = 0; qq < kPerWarp; ++qq) merge_stats(m[qq], l[qq], dot[qq], 1.f, scale_log2);
+    }
+  }
+#pragma unroll
+  for (int qq = 0; qq < kPerWarp; ++qq) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float mo = __shfl_xor_sync(0xffffffffu, m[qq], o), lo = __shfl_xor_sync(0xffffffffu, l[qq], o);
+      merge_stats(m[qq], l[qq], mo, lo, scale_log2);
+    }
+    const int p = blockIdx.x * kMassQ + warp * kPerWarp + qq;
+    if (lane == 0 && p < N) {
+      float* s = stats + ((static_cast<long long>(r) * H + h) * N + p) * 2;
+      s[0] = m[qq];
+      s[1] = l[qq];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kMassThreads) sattn_key_mass_kernel(
+    const __nv_bfloat16* __restrict__ Q, long long ldq, const __nv_bfloat16* __restrict__ K, long long ldk,
+    const float* __restrict__ stats, float w, float* __restrict__ mass, int row0, int H, int N, int kv_bs, int d, int DK,
+    float scale_log2) {
+  constexpr int kWarps = kMassThreads / 32;
+  constexpr int kRowWords = kMassMaxD / 2 + 1;
+  __shared__ __nv_bfloat162 sK[kMassKeys * kRowWords];
+  __shared__ float sq[kWarps][kMassMaxD];
+  __shared__ float part[kWarps][kMassKeys];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.y, item = row0 + r;
+  const int j0 = blockIdx.x * kMassKeys, nk = min(kMassKeys, N - j0);
+  const int rw = d / 2 + 1;
+  float acc = 0.f;
+  for (int h = 0; h < H; ++h) {
+    __syncthreads();
+    for (int e = threadIdx.x; e < nk * (d / 2); e += kMassThreads) {
+      const int j = e / (d / 2), c2 = e % (d / 2);
+      sK[j * rw + c2] =
+          *reinterpret_cast<const __nv_bfloat162*>(K + (static_cast<long long>(item) * kv_bs + j0 + j) * ldk + h * DK + 2 * c2);
+    }
+    __syncthreads();
+    const float* st = stats + (static_cast<long long>(r) * H + h) * N * 2;
+    for (int p = warp; p < N; p += kWarps) {
+      const __nv_bfloat16* qrow = Q + (static_cast<long long>(item) * N + p) * ldq + h * DK;
+      for (int c = lane; c < d; c += 32) sq[warp][c] = __bfloat162float(qrow[c]);
+      __syncwarp();
+      if (lane < nk) {
+        float dot = 0.f;
+        for (int c2 = 0; c2 < d / 2; ++c2) {
+          const float2 kv = __bfloat1622float2(sK[lane * rw + c2]);
+          dot = fmaf(sq[warp][2 * c2], kv.x, dot);
+          dot = fmaf(sq[warp][2 * c2 + 1], kv.y, dot);
+        }
+        acc += exp2f((dot - st[2 * p]) * scale_log2) / st[2 * p + 1];
+      }
+      __syncwarp();
+    }
+  }
+  part[warp][lane] = acc;
+  __syncthreads();
+  if (warp == 0 && lane < nk) {
+    float s = 0.f;
+#pragma unroll
+    for (int g = 0; g < kWarps; ++g) s += part[g][lane];
+    mass[static_cast<long long>(r) * N + j0 + lane] += w * s;
+  }
+}
+
 }  // namespace vdb
 
 using namespace vdb;
@@ -505,6 +634,37 @@ int vdb_xattn_word_map_f32(const void* Q, long long ldq, const void* K, long lon
   return launch(xattn_word_map_kernel, grid, dim3(kWmapThreads), 0, stream, reinterpret_cast<const __nv_bfloat16*>(Q), ldq,
                 reinterpret_cast<const __nv_bfloat16*>(K), ldk, w, map, row0, H, N, L, kv_bstride, d_head, DK,
                 scale * 1.4426950408889634f);
+}
+
+int vdb_sattn_key_mass_f32(const void* Q, long long ldq, int q_col0, const void* K, long long ldk, int k_col0, float* stats,
+                           float w, float* mass, int n, int row0, int H, int N, int kv_bstride, int d_head, float scale,
+                           void* stream) {
+  if (!Q || !K || !stats || !mass || n <= 0 || row0 < 0 || H <= 0 || N <= 0)
+    return set_error(VDB_ERR_INVALID, "sattn_key_mass: null/empty argument");
+  if (N > kMassMaxN) return set_error(VDB_ERR_UNSUPPORTED, "sattn_key_mass: at most %d tokens, got %d", kMassMaxN, N);
+  const int DK = vdb_attention_dk_pad(d_head);
+  if (DK < 0 || d_head <= 0 || d_head > kMassMaxD || d_head % 8)
+    return set_error(VDB_ERR_UNSUPPORTED, "sattn_key_mass: d_head %d not supported (a multiple of 8, <= %d)", d_head, kMassMaxD);
+  if (kv_bstride <= 0) kv_bstride = N;
+  const long long cols = static_cast<long long>(H) * DK;
+  if (kv_bstride < N || q_col0 < 0 || k_col0 < 0 || (q_col0 & 1) || (k_col0 & 1) || (ldq & 1) || (ldk & 1) ||
+      ldq < q_col0 + cols || ldk < k_col0 + cols)
+    return set_error(VDB_ERR_INVALID, "sattn_key_mass: need kv_bstride >= N, even column offsets and even ldq, ldk >= col0 + H * %d",
+                     DK);
+  if ((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(K) | reinterpret_cast<uintptr_t>(stats) |
+       reinterpret_cast<uintptr_t>(mass)) & 3)
+    return set_error(VDB_ERR_INVALID, "sattn_key_mass: pointers must be 4-byte aligned");
+  const char *m0 = reinterpret_cast<const char*>(mass), *m1 = m0 + static_cast<long long>(n) * N * 4;
+  const char *s0 = reinterpret_cast<const char*>(stats), *s1 = s0 + static_cast<long long>(n) * H * N * 2 * 4;
+  if (m0 < s1 && s0 < m1) return set_error(VDB_ERR_INVALID, "sattn_key_mass: mass overlaps stats");
+  const __nv_bfloat16* q = reinterpret_cast<const __nv_bfloat16*>(Q) + q_col0;
+  const __nv_bfloat16* k = reinterpret_cast<const __nv_bfloat16*>(K) + k_col0;
+  const float scale_log2 = scale * 1.4426950408889634f;
+  int st = launch(sattn_row_stats_kernel, dim3((N + kMassQ - 1) / kMassQ, H, n), dim3(kMassThreads), 0, stream, q, ldq, k, ldk,
+                  stats, row0, H, N, kv_bstride, d_head, DK, scale_log2);
+  if (st) return st;
+  return launch(sattn_key_mass_kernel, dim3((N + kMassKeys - 1) / kMassKeys, n), dim3(kMassThreads), 0, stream, q, ldq, k, ldk,
+                static_cast<const float*>(stats), w, mass, row0, H, N, kv_bstride, d_head, DK, scale_log2);
 }
 
 }  // extern "C"

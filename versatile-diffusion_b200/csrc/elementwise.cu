@@ -632,6 +632,77 @@ __global__ void region_merge_kernel(const float* __restrict__ eps, int bs, int H
   }
 }
 
+// Self-attention guidance (lib/model_zoo/sag.py).  sag_degrade_kernel: one CTA per (kSagTile x kSagTile pixels, image b).  The
+// tile's x0 with its 4-wide reflected halo sits in shared memory; the 9-tap Gaussian runs along rows into a second buffer, then
+// along columns, each sum in tap order.  The mask cell of pixel (y, x) is mass[b, (y hm / H) wm + x wm / W] > 1.
+constexpr int kSagTile = 16, kSagHalo = 4, kSagTaps = 2 * kSagHalo + 1, kSagMaxC = 8, kSagMaxMap = 4096;
+
+struct SagTaps {
+  float g[kSagTaps];
+};
+
+__device__ __forceinline__ int reflect_index(int i, int n) {
+  i = i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i);
+  return min(max(i, 0), n - 1);        // rows past the reflected range feed no pixel of the image
+}
+
+__global__ void __launch_bounds__(kSagTile * kSagTile) sag_degrade_kernel(
+    const float* __restrict__ x, const float* __restrict__ e, const float* __restrict__ mass, const float* __restrict__ table,
+    const int* __restrict__ step_idx, SagTaps taps, int H, int W, int C, int hm, int wm, float* __restrict__ out) {
+  constexpr int S = kSagTile + 2 * kSagHalo;
+  __shared__ float sx[S * S * kSagMaxC];
+  __shared__ float sh[S * kSagTile * kSagMaxC];
+  const int idx = *step_idx;
+  const float sa = table[2 * idx], s1 = table[2 * idx + 1];
+  const int b = blockIdx.z, y0 = blockIdx.y * kSagTile, x0 = blockIdx.x * kSagTile;
+  const long long img = static_cast<long long>(b) * H * W * C;
+  for (int i = threadIdx.x; i < S * S * C; i += blockDim.x) {
+    const int c = i % C, lx = (i / C) % S, ly = i / (C * S);
+    const long long g = img + (static_cast<long long>(reflect_index(y0 + ly - kSagHalo, H)) * W +
+                               reflect_index(x0 + lx - kSagHalo, W)) * C + c;
+    sx[i] = __fdiv_rn(__fsub_rn(x[g], __fmul_rn(s1, e[g])), sa);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < S * kSagTile * C; i += blockDim.x) {
+    const int c = i % C, tx = (i / C) % kSagTile, ly = i / (C * kSagTile);
+    float acc = 0.f;
+#pragma unroll
+    for (int k = 0; k < kSagTaps; ++k) acc = fmaf(taps.g[k], sx[(ly * S + tx + k) * C + c], acc);
+    sh[i] = acc;
+  }
+  __syncthreads();
+  const int ty = threadIdx.x / kSagTile, tx = threadIdx.x % kSagTile, y = y0 + ty, xx = x0 + tx;
+  if (y >= H || xx >= W) return;
+  const bool m = mass[static_cast<long long>(b) * hm * wm + (y * hm / H) * wm + xx * wm / W] > 1.f;
+  for (int c = 0; c < C; ++c) {
+    float v = sx[((ty + kSagHalo) * S + tx + kSagHalo) * C + c];
+    if (m) {
+      float acc = 0.f;
+#pragma unroll
+      for (int k = 0; k < kSagTaps; ++k) acc = fmaf(taps.g[k], sh[((ty + k) * kSagTile + tx) * C + c], acc);
+      v = acc;
+    }
+    const long long g = img + (static_cast<long long>(y) * W + xx) * C + c;
+    out[g] = __fadd_rn(__fmul_rn(sa, v), __fmul_rn(s1, e[g]));
+  }
+}
+
+// d = s (e_src - e_deg), e_src = e_u when given (CFG), else e_c; added to e_c and e_u in place
+__global__ void sag_guide_kernel(float* e_u, float* e_c, const float* __restrict__ e_deg, float s, long long n) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float ec = e_c[i];
+    if (e_u) {
+      const float eu = e_u[i];
+      const float d = __fmul_rn(s, __fsub_rn(eu, e_deg[i]));
+      e_u[i] = __fadd_rn(eu, d);
+      e_c[i] = __fadd_rn(ec, d);
+    } else {
+      e_c[i] = __fadd_rn(ec, __fmul_rn(s, __fsub_rn(ec, e_deg[i])));
+    }
+  }
+}
+
 __global__ void add_int_kernel(int* p, int delta) { *p += delta; }
 
 // y = c0*x0 + c1*x1 + c2*x2 + c3*x3 (null pointers skipped) — the Adams-Bashforth eps combination of the PLMS
@@ -2113,6 +2184,41 @@ int vdb_diffedit_mask_f32(const float* e_src_u, const float* e_src_c, float s_sr
       return set_error(VDB_ERR_INVALID, "diffedit_mask: out overlaps an eps input");
   return launch(diffedit_mask_kernel, bs, kDiffEditThreads, 0, stream, e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, bs,
                 hw, c, ratio, out);
+}
+
+int vdb_sag_degrade_f32(const float* x, const float* e, const float* mass, const float* table, const int* step_idx, int bs, int H,
+                        int W, int C, int hm, int wm, float* out, void* stream) {
+  if (!x || !e || !mass || !table || !step_idx || !out || bs <= 0 || H <= 0 || W <= 0 || C <= 0 || hm <= 0 || wm <= 0)
+    return set_error(VDB_ERR_INVALID, "sag_degrade: null/empty argument");
+  if (H <= kSagHalo || W <= kSagHalo)
+    return set_error(VDB_ERR_INVALID, "sag_degrade: reflect padding by %d needs sides >= %d, got %d x %d", kSagHalo, kSagHalo + 1, H, W);
+  if (C > kSagMaxC || hm > H || wm > W || hm * wm > kSagMaxMap)
+    return set_error(VDB_ERR_UNSUPPORTED, "sag_degrade: need C <= %d and a map of hm <= H, wm <= W, hm * wm <= %d (got C %d, %d x %d)",
+                     kSagMaxC, kSagMaxMap, C, hm, wm);
+  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(mass) |
+       reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(step_idx) | reinterpret_cast<uintptr_t>(out)) & 3)
+    return set_error(VDB_ERR_INVALID, "sag_degrade: pointers must be 4-byte aligned");
+  const long long n = static_cast<long long>(bs) * H * W * C;
+  if (overlaps(out, n, x, n) || overlaps(out, n, e, n) || overlaps(out, n, mass, static_cast<long long>(bs) * hm * wm))
+    return set_error(VDB_ERR_INVALID, "sag_degrade: out overlaps x, e or mass");
+  // the Gaussian of sigma 1: exp(-k^2 / 2) for k = -4 .. 4, normalised to sum 1 in double
+  SagTaps taps;
+  double g[kSagTaps], sum = 0.0;
+  for (int k = 0; k < kSagTaps; ++k) sum += g[k] = exp(-0.5 * (k - kSagHalo) * (k - kSagHalo));
+  for (int k = 0; k < kSagTaps; ++k) taps.g[k] = static_cast<float>(g[k] / sum);
+  return launch(sag_degrade_kernel, dim3((W + kSagTile - 1) / kSagTile, (H + kSagTile - 1) / kSagTile, bs),
+                dim3(kSagTile * kSagTile), 0, stream, x, e, mass, table, step_idx, taps, H, W, C, hm, wm, out);
+}
+
+int vdb_sag_guide_f32(float* e_u, float* e_c, const float* e_deg, float s, long long n, void* stream) {
+  if (!e_c || !e_deg || n <= 0) return set_error(VDB_ERR_INVALID, "sag_guide: null/empty argument");
+  if (!std::isfinite(s)) return set_error(VDB_ERR_INVALID, "sag_guide: scale must be finite");
+  if ((reinterpret_cast<uintptr_t>(e_u) | reinterpret_cast<uintptr_t>(e_c) | reinterpret_cast<uintptr_t>(e_deg)) & 3)
+    return set_error(VDB_ERR_INVALID, "sag_guide: pointers must be 4-byte aligned");
+  if (overlaps(e_c, n, e_deg, n) || overlaps(e_u, n, e_deg, n) || overlaps(e_u, n, e_c, n))
+    return set_error(VDB_ERR_INVALID, "sag_guide: e_u, e_c and e_deg must not overlap");
+  const int threads = 256;
+  return launch(sag_guide_kernel, ew_blocks(n, threads), threads, 0, stream, e_u, e_c, e_deg, s, n);
 }
 
 int vdb_axpby_f32(const float* x, const float* z, float a, float b, float* y, long long n, void* stream) {

@@ -31,6 +31,17 @@ class PaddedContext(object):
         self.data, self.length, self.edit = data, length, edit
 
 
+class KeyMass(object):
+    """Where the mid block's self-attention adds its per-key attention mass for self-attention guidance (lib/model_zoo/sag.py):
+    mass fp32 [n, N] for batch items row0 .. row0 + n - 1, each head's column sums weighted by ratio / heads."""
+
+    def __init__(self, mass, row0=0, ratio=1.0):
+        self.mass, self.row0, self.ratio = mass, row0, ratio
+
+    def weighted(self, ratio):
+        return KeyMass(self.mass, self.row0, ratio)
+
+
 def ln_fold_fits(inner, B, H, W):
     """LayerNorms folded into the neighbouring GEMMs need their TMA-store epilogues: inner % 32 == 0, and the B * H * W tokens
     are the N of the V^T projection.  Other token grids run the LayerNorm kernels."""
@@ -188,15 +199,18 @@ class CrossAttention(PackedModule):
         self._kv_put((key, val, context))
         return val
 
-    def _attend(self, q, k, vt, o, B, N, Nk, edit, cross, q_col0=0, k_col0=0, kv_bstride=0):
+    def _attend(self, q, k, vt, o, B, N, Nk, edit, cross, q_col0=0, k_col0=0, kv_bstride=0, key_mass=None):
         """The layer's flash attention.  Under a prompt edit (lib/model_zoo/prompt_edit.py) the indexed form with the edit's
-        table for this layer, the refinement's accumulating second term, and the word maps at the 1/4-side cross layers."""
+        table for this layer, the refinement's accumulating second term, and the word maps at the 1/4-side cross layers.
+        key_mass: a KeyMass of a self-attention layer, which also receives its key mass from the same q and k."""
         ops = _ops()
         H, d = self.heads, self.dim_head
         items = None if edit is None else edit.items(cross, N)
         kw = dict(scale=self.scale, q_col0=q_col0, k_col0=k_col0, kv_bstride=kv_bstride)
         if items is None:
             ops.attention(q, k, vt, o, B, H, N, Nk, d, **kw)
+            if key_mass is not None:
+                ops.sattn_key_mass(q, k, key_mass.mass, key_mass.row0, H, N, d, w=key_mass.ratio / H, **kw)
             return
         Bkv = edit.ctx_batch if cross else B
         ops.attention(q, k, vt, o, B, H, N, Nk, d, items=items, step_idx=edit.idx, Bkv=Bkv, **kw)
@@ -205,9 +219,9 @@ class CrossAttention(PackedModule):
         if cross and edit.maps_at(N):
             ops.xattn_word_map(q, k, edit.w, edit.map, edit.c0, H, N, Nk, d, kv_bstride=kv_bstride, scale=self.scale)
 
-    def forward(self, x, context=None, resid=None, B=1, edit=None):
+    def forward(self, x, context=None, resid=None, B=1, edit=None, key_mass=None):
         """x: [B*N, C] bf16 (already layer-normed); returns to_out(attn) + resid as [B*N, C] bf16.  edit: the prompt edit of a
-        self-attention layer (a cross-attention layer reads it from its context)."""
+        self-attention layer (a cross-attention layer reads it from its context).  key_mass: see _attend."""
         ops = _ops()
         p = self.packed()
         H, d, dk = self.heads, self.dim_head, p["dk"]
@@ -216,7 +230,7 @@ class CrossAttention(PackedModule):
         if context is None and N % 8 == 0:
             qk = ops.gemm(x, p["wqk"])                    # [B*N, 2*H*dk]: q | k
             vt = ops.gemm(p["wv"], x)                     # [H*dvp, B*N]
-            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk)
+            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk, key_mass=key_mass)
         elif context is None:
             # ragged token count (latent sides not a multiple of 8 at this level): keys/values from a copy of
             # the tokens padded to a multiple of 8 per batch item (TMA alignment of the V^T columns)
@@ -227,14 +241,14 @@ class CrossAttention(PackedModule):
             q = ops.gemm(x, p["wq"])
             k = ops.gemm(xp, p["wk"])
             vt = ops.gemm(p["wv"], xp)
-            self._attend(q, k, vt, o, B, N, N, edit, False, kv_bstride=Np)
+            self._attend(q, k, vt, o, B, N, N, edit, False, kv_bstride=Np, key_mass=key_mass)
         else:
             q = ops.gemm(x, p["wq"])
             k, vt, L, Lp = self.context_kv(context)
             self._attend(q, k, vt, o, B, N, L, getattr(context, "edit", None), True, kv_bstride=Lp)
         return ops.gemm(o, p["wo"], bias=p["bo"], resid=resid)
 
-    def forward_folded(self, x, ln, fp, context=None, resid=None, B=1, stats_out=None, edit=None):
+    def forward_folded(self, x, ln, fp, context=None, resid=None, B=1, stats_out=None, edit=None, key_mass=None):
         """x: [B*N, C] bf16 RAW tokens, ln: ops.LnFold with their LayerNorm statistics, fp: pack_folded(); to_out writes the
         statistics of ITS output rows into stats_out (the next LayerNorm's input).  Self-attention needs N % 8 == 0."""
         ops = _ops()
@@ -245,7 +259,7 @@ class CrossAttention(PackedModule):
         if context is None:
             qk = ops.gemm_ln(x, fp["wqk"], bias=fp["cqk"], ln=ln, colsum=fp["sqk"])                       # [B*N, 2*H*dk]: q | k
             vt = ops.gemm_ln(fp["wv"], x, ln=ln, colsum=fp["sv"], on_cols=True, rowbias=fp["cv"])       # [H*dvp, B*N]
-            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk)
+            self._attend(qk, qk, vt, o, B, N, N, edit, False, q_col0=0, k_col0=H * dk, key_mass=key_mass)
         else:
             q = ops.gemm_ln(x, fp["wq"], bias=fp["cq"], ln=ln, colsum=fp["sq"])
             k, vt, L, Lp = self.context_kv(context)
@@ -282,7 +296,7 @@ class BasicTransformerBlock(PackedModule):
                            "ffw": wf[idx].contiguous(), "ffs": sf[idx].contiguous(), "ffc": cf[idx].contiguous()}
         return out
 
-    def forward(self, x, context=None, B=1, stats=None):
+    def forward(self, x, context=None, B=1, stats=None, key_mass=None):
         """x: [B*N, C] bf16 tokens (reference _forward, attention.py:214-218).  stats: (table, partials per row) — the LayerNorm
         partial sums of x's rows written by the GEMM that produced x -> the three LayerNorms run inside the GEMM epilogues."""
         ops = _ops()
@@ -294,11 +308,11 @@ class BasicTransformerBlock(PackedModule):
             st1, parts1 = stats
             st2, st3 = ops.ln_stats_buffer(x.shape[0], C, x.device), ops.ln_stats_buffer(x.shape[0], C, x.device)
             x, parts2 = self.attn1.forward_folded(x, ops.LnFold(st1, parts1, C, self.norm1.eps), f["a1"], None, resid=x, B=B, stats_out=st2,
-                                                 edit=edit)
+                                                 edit=edit, key_mass=key_mass)
             x, parts3 = self.attn2.forward_folded(x, ops.LnFold(st2, parts2, C, self.norm2.eps), f["a2"], context, resid=x, B=B, stats_out=st3)
             h = ops.gemm_ln(x, f["ffw"], bias=f["ffc"], act=ops.ACT_GEGLU, ln=ops.LnFold(st3, parts3, C, self.norm3.eps), colsum=f["ffs"])
             return ops.gemm(h, p["w2"], bias=p["b2"], resid=x)
-        x = self.attn1(ops.layernorm(x, *p["norm1"], eps=self.norm1.eps), None, resid=x, B=B, edit=edit)
+        x = self.attn1(ops.layernorm(x, *p["norm1"], eps=self.norm1.eps), None, resid=x, B=B, edit=edit, key_mass=key_mass)
         x = self.attn2(ops.layernorm(x, *p["norm2"], eps=self.norm2.eps), context, resid=x, B=B)
         h = self.ff.net[0](ops.layernorm(x, *p["norm3"], eps=self.norm3.eps))
         return ops.gemm(h, p["w2"], bias=p["b2"], resid=x)
@@ -320,10 +334,11 @@ class SpatialTransformer(PackedModule):
         return {"g": f32(self.norm.weight), "b": f32(self.norm.bias), "win": pack_conv1x1(self.proj_in.weight),
                 "bin": f32(self.proj_in.bias), "wout": pack_conv1x1(self.proj_out.weight), "bout": f32(self.proj_out.bias)}
 
-    def forward(self, x, context=None, ratio=1.0, acc=None):
+    def forward(self, x, context=None, ratio=1.0, acc=None, key_mass=None):
         """x: NHWC bf16 [B,H,W,C].  Returns ratio * proj_out(blocks(...)) + (acc if given else x):
         with acc=None, ratio=1 this is the reference forward (x + x_in, attention.py:255-266); with the
-        running `acc` it is one term of VD_v2_0.context_mixing (vd.py:391-396) accumulated in the epilogue."""
+        running `acc` it is one term of VD_v2_0.context_mixing (vd.py:391-396) accumulated in the epilogue.
+        key_mass: a KeyMass that the blocks' self-attention adds its key mass to (self-attention guidance)."""
         require_cuda(x, "SpatialTransformer")
         ops = _ops()
         p = self.packed()
@@ -339,7 +354,7 @@ class SpatialTransformer(PackedModule):
             stats = None
             t = ops.gemm(xn.view(B * H * W, C), p["win"], bias=p["bin"])
         for i, blk in enumerate(self.transformer_blocks):
-            t = blk(t, context, B=B, stats=stats if i == 0 else None)
+            t = blk(t, context, B=B, stats=stats if i == 0 else None, key_mass=key_mass)
         base = x if acc is None else acc
         out = ops.gemm(t, p["wout"], bias=p["bout"], resid=base.view(B * H * W, -1), alpha=float(ratio))
         return out.view(B, H, W, -1)

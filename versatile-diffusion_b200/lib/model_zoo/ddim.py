@@ -23,9 +23,9 @@ def _ops():
 
 
 # ------------------------------------------------------------------ sampling modes and how they combine
-# A mode is selected by an optional input: x_info['regions'] (lib/model_zoo/regions.py), x_info['windows'] (lib/model_zoo/
-# panorama.py: the region walk with no regions), a context's 'prompt_edit'
-# (prompt_edit.py), x_info['inversion'] (edit.py) and x_info['inpaint_mask'] (inpaint.py).  The start inputs x_info['x0'] (with
+# A mode is selected by an optional input: x_info['sag'] (lib/model_zoo/sag.py), x_info['regions'] (regions.py), x_info['windows']
+# (panorama.py: the region walk with no regions), a context's 'prompt_edit' (prompt_edit.py), x_info['inversion'] (edit.py) and
+# x_info['inpaint_mask'] (inpaint.py).  The start inputs x_info['x0'] (with
 # 'x0_forward_timesteps') and x_info['xt'] select no mode, but some modes refuse them.
 #
 # REFUSES: who -> {input given: (exception type, message)}, checked in this order.
@@ -41,14 +41,22 @@ REFUSES = {
         ('windows', "PLMSSampler has no window fusion: use DDIMSampler or DPMSolverSampler (lib/model_zoo/panorama.py)"),
         ('regions', "PLMSSampler has no region prompts: use DDIMSampler or DPMSolverSampler (lib/model_zoo/regions.py)"),
         ('inversion', "PLMSSampler cannot sample from an inversion: use DDIMSampler or DPMSolverSampler "
-                      "(lib/model_zoo/edit.py)"))},
+                      "(lib/model_zoo/edit.py)"),
+        ('sag', "PLMSSampler has no self-attention guidance: use DDIMSampler or DPMSolverSampler (lib/model_zoo/sag.py)"))},
     'p_sample': {
         'prompt_edit': (NotImplementedError, "a prompt edit spans the walk (its windows and word maps): use sample / "
                                              "sample_multicontext (lib/model_zoo/prompt_edit.py)"),
         'windows': (NotImplementedError, "window fusion runs inside the sampler's walk: use sample / sample_multicontext "
                                          "(lib/model_zoo/panorama.py)"),
         'regions': (NotImplementedError, "region prompts run inside the sampler's walk: use sample / sample_multicontext "
-                                         "(lib/model_zoo/regions.py)")},
+                                         "(lib/model_zoo/regions.py)"),
+        'sag': (NotImplementedError, "self-attention guidance runs inside the sampler's walk: use sample / sample_multicontext "
+                                     "(lib/model_zoo/sag.py)")},
+    'sag': {
+        'windows': (NotImplementedError, "SAG with windows: window fusion replaces the UNet call (lib/model_zoo/sag.py)"),
+        'regions': (NotImplementedError, "SAG with regions: region prompts replace the UNet call (lib/model_zoo/sag.py)"),
+        'prompt_edit': (NotImplementedError, "SAG with prompt_edit: the edit's item tables index the CFG batch and know nothing of "
+                                             "SAG's second pass (lib/model_zoo/sag.py)")},
     'regions': {
         'prompt_edit': (NotImplementedError, "regions with prompt_edit: the edit's item tables index prompts, not regions "
                                              "(lib/model_zoo/regions.py)"),
@@ -70,7 +78,7 @@ TAKES = {'inversion': ('inpaint_mask',), 'regions': ('windows',)}
 
 def given_inputs(x_info, c_infos):
     """The optional inputs given (not None) to a call."""
-    given = {k for k in ('x0', 'xt', 'x0_forward_timesteps', 'inpaint_mask', 'inversion', 'windows', 'regions')
+    given = {k for k in ('x0', 'xt', 'x0_forward_timesteps', 'inpaint_mask', 'inversion', 'windows', 'regions', 'sag')
              if x_info.get(k, None) is not None}
     if any(ci.get('prompt_edit', None) is not None for ci in c_infos):
         given.add('prompt_edit')
@@ -222,10 +230,12 @@ class DDIMSampler(object):
         from .inpaint import Inpainting
         from .prompt_edit import PromptEditing
         from .regions import RegionPrompts
+        from .sag import SelfAttention
         refuse(entry, x_info, c_infos)
         given = given_inputs(x_info, c_infos)
         taken = {k for m in given for k in TAKES.get(m, ())}
-        return [cls(self, x_info, shape, c_infos) for name, cls in (('regions', RegionPrompts), ('windows', RegionPrompts),
+        return [cls(self, x_info, shape, c_infos) for name, cls in (('sag', SelfAttention), ('regions', RegionPrompts),
+                                                                      ('windows', RegionPrompts),
                                                                       ('prompt_edit', PromptEditing), ('inversion', FromInversion),
                                                                       ('inpaint_mask', Inpainting))
                 if name in given and name not in taken]

@@ -428,31 +428,33 @@ class UNetModel2D_Next(nn.Module):
         return ops.nhwc_to_nchw(h).to(x.dtype)
 
 
-def unet_walk(data_unet, ctx_unets, h, emb, contexts, ratios):
+def unet_walk(data_unet, ctx_unets, h, emb, contexts, ratios, key_mass=None):
     """The i/m/o_order walk of VD_v2_0.apply_model / apply_model_multicontext (vd.py:344-381, 404-455):
-    'd' blocks from data_unet.data_blocks, 'c' blocks from each ctx_unet.context_blocks mixed by ratio."""
+    'd' blocks from data_unet.data_blocks, 'c' blocks from each ctx_unet.context_blocks mixed by ratio.  key_mass: an
+    attention.KeyMass that the mid block's self-attention (the 'c' of m_order) adds its key mass to, each context's at its ratio."""
     hs = []
     d_iter = iter(data_unet.data_blocks)
     c_iters = [iter(u.context_blocks) for u in ctx_unets]
     tot = float(sum(ratios))
     rs = [float(r) / tot for r in ratios]
 
-    def run_c(h):
+    def run_c(h, rec=None):
         mods = [next(ci) for ci in c_iters]
-        if len(mods) == 1:
+        if len(mods) == 1 and rec is None:
             return mods[0](h, emb, contexts[0])
         # context_mixing 'attention' (vd.py:391-396): sum_i r_i*ST_i(h) with sum r_i = 1 == h + sum_i r_i*delta_i,
         # accumulated in the proj_out epilogues (term 1 starts from h, later terms from the running sum)
         acc = None
         for m, c, r in zip(mods, contexts, rs):
-            acc = m[0](h, c, ratio=r, acc=acc)
+            acc = m[0](h, c, ratio=r, acc=acc, key_mass=None if rec is None else rec.weighted(r))
         return acc
 
-    for ltype in data_unet.i_order + data_unet.m_order:
+    mid = len(data_unet.i_order)
+    for n, ltype in enumerate(data_unet.i_order + data_unet.m_order):
         if ltype == 'd':
             h = next(d_iter)(h, emb, None)
         elif ltype == 'c':
-            h = run_c(h)
+            h = run_c(h, key_mass if n >= mid else None)
         elif ltype == 'save_hidden_feature':
             hs.append(h)
     for ltype in data_unet.o_order:

@@ -158,10 +158,11 @@ class VD_v2_0(nn.Module):
             return x_type
         return self.global_layer_ptr
 
-    def eps_nhwc(self, x_nhwc, x_type, t_emb, c_types, contexts, ratios, time_from):
-        """Core of apply_model*: fp32 NHWC latent [B,H,W,4] + fp32 sinusoid [B,model_channels] -> fp32 NHWC eps."""
+    def eps_nhwc(self, x_nhwc, x_type, t_emb, c_types, contexts, ratios, time_from, key_mass=None):
+        """Core of apply_model*: fp32 NHWC latent [B,H,W,4] + fp32 sinusoid [B,model_channels] -> fp32 NHWC eps.  key_mass: an
+        attention.KeyMass that receives the mid block's self-attention key mass (lib/model_zoo/sag.py)."""
         table = self.diffuser[x_type].embed_table(t_emb, time_owner=self.diffuser[time_from])
-        return unet_walk(self.diffuser[x_type], [self.diffuser[ct] for ct in c_types], x_nhwc, table, contexts, ratios)
+        return unet_walk(self.diffuser[x_type], [self.diffuser[ct] for ct in c_types], x_nhwc, table, contexts, ratios, key_mass)
 
     def context_kv_signature(self, c_types, contexts):
         """Projects every context through the K / V^T weights of the cross-attention layers that will read it (a

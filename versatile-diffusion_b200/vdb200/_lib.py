@@ -39,6 +39,8 @@ SIGNATURES = {
     "vdb_region_gather_f32": (i, [p, i, i, i, i, p, p, i, i, i, i, i, i, i, i, p, p, p, p, p, i, p, p, p]),
     "vdb_region_noise_f32": (i, [p, p, ll, i, i, i, p, p, p]),
     "vdb_region_merge_f32": (i, [p, i, i, i, i, i, p, p, p, p, i, i, i, i, i, i, i, p, p, p]),
+    "vdb_sag_degrade_f32": (i, [p, p, p, p, p, i, i, i, i, i, i, p, p]),
+    "vdb_sag_guide_f32": (i, [p, p, p, f, ll, p]),
     "vdb_axpby_f32": (i, [p, p, f, f, p, ll, p]),
     "vdb_add_int": (i, [p, i, p]),
     "vdb_lincomb4_f32": (i, [p, p, p, p, f, f, f, f, p, ll, p]),
@@ -52,6 +54,7 @@ SIGNATURES = {
     "vdb_attention_dv_pad": (i, [i]),
     "vdb_attention_bf16": (i, [p, ll, i, p, ll, i, p, ll, p, ll, i, i, i, i, i, i, i, f, i, p, i, i, p, p, i, p]),
     "vdb_xattn_word_map_f32": (i, [p, ll, p, ll, p, p, i, i, i, i, i, i, i, f, p]),
+    "vdb_sattn_key_mass_f32": (i, [p, ll, i, p, ll, i, p, f, p, i, i, i, i, i, i, f, p]),
     "vdb_groupnorm_nsplit": (i, [i, i]),
     "vdb_groupnorm_scratch_floats": (ll, [i, i]),
     "vdb_groupnorm_nhwc": (i, [p, i, p, i, i, i, i, p, p, f, i, p, p, p]),

@@ -517,6 +517,56 @@ def xattn_word_map(q, k, w, out, row0, H, N, L, d_head, kv_bstride=0, scale=None
     return out
 
 
+def sattn_key_mass(q, k, mass, row0, H, N, d_head, w=1.0, q_col0=0, k_col0=0, kv_bstride=0, scale=None):
+    """Self-attention guidance's key mass (vdb_sattn_key_mass_f32): mass[r, j] += w sum_h sum_p softmax(scale q k^T)[h, p, j] for
+    the n = mass.shape[0] items row0 .. row0 + n - 1 of a self-attention call's q [B*N, >= q_col0 + H*dk] and k
+    [B*kv_bstride, >= k_col0 + H*dk] (the fused q | k buffer passes the same tensor twice)."""
+    _need(q, BF16, "q", True); _need(k, BF16, "k", True); _need(mass, torch.float32, "mass")
+    if mass.dim() != 2 or mass.shape[1] != N:
+        raise ValueError(f"mass: expected [n, {N}], got {tuple(mass.shape)}")
+    n = mass.shape[0]
+    if scale is None:
+        scale = d_head ** -0.5
+    stats = torch.empty(n * H * N * 2, dtype=torch.float32, device=mass.device)
+    check(lib.vdb_sattn_key_mass_f32(_ptr(q), q.stride(0), int(q_col0), _ptr(k), k.stride(0), int(k_col0), _ptr(stats), float(w),
+                                     _ptr(mass), n, int(row0), H, N, int(kv_bstride), d_head, float(scale), _stream()),
+          "sattn_key_mass")
+    return mass
+
+
+def sag_degrade(x, e, mass, table, step_idx, hm, wm, out=None):
+    """Self-attention guidance's degraded latent (vdb_sag_degrade_f32): x, e fp32 NHWC [bs, H, W, C]; mass fp32 [bs, hm*wm]; table
+    fp32 [rows, 2] device rows {sqrt(a_t), sqrt(1 - a_t)}, row step_idx[0] (int32 device tensor) -> out [bs, H, W, C]."""
+    for name, t in (("x", x), ("e", e), ("mass", mass), ("table", table), ("out", out)):
+        _need(t, torch.float32, name)
+    _need(step_idx, torch.int32, "step_idx")
+    bs, H, W, C = x.shape
+    if e.shape != x.shape:
+        raise ValueError(f"e: expected {tuple(x.shape)}, got {tuple(e.shape)}")
+    if mass.numel() != bs * hm * wm:
+        raise ValueError(f"mass: expected [{bs}, {hm * wm}], got {tuple(mass.shape)}")
+    if table.dim() != 2 or table.shape[1] != 2:
+        raise ValueError(f"table: expected [rows, 2], got {tuple(table.shape)}")
+    if out is None:
+        out = torch.empty_like(x)
+    elif out.shape != x.shape:
+        raise ValueError(f"out: expected {tuple(x.shape)}, got {tuple(out.shape)}")
+    check(lib.vdb_sag_degrade_f32(_ptr(x), _ptr(e), _ptr(mass), _ptr(table), _ptr(step_idx), bs, H, W, C, int(hm), int(wm),
+                                  _ptr(out), _stream()), "sag_degrade")
+    return out
+
+
+def sag_guide(e_u, e_c, e_deg, s):
+    """Self-attention guidance (vdb_sag_guide_f32), in place: d = s (e_src - e_deg), e_src = e_u when given (CFG) else e_c, is added
+    to e_c and e_u.  All fp32 of one shape."""
+    for name, t in (("e_u", e_u), ("e_c", e_c), ("e_deg", e_deg)):
+        _need(t, torch.float32, name)
+    for name, t in (("e_u", e_u), ("e_deg", e_deg)):
+        if t is not None and t.shape != e_c.shape:
+            raise ValueError(f"{name}: expected {tuple(e_c.shape)}, got {tuple(t.shape)}")
+    check(lib.vdb_sag_guide_f32(_ptr(e_u), _ptr(e_c), _ptr(e_deg), float(s), e_c.numel(), _stream()), "sag_guide")
+
+
 def local_blend(x, wmap, flags, step_idx, h, w, threshold, x_dup=None):
     """Prompt-to-Prompt's local blend after a step (vdb_local_blend_f32), in place on x fp32 NHWC [n, H, W, C] (row 0 the
     source): wmap fp32 [n, h*w] word maps, flags int32 device table read at step_idx[0]."""
