@@ -39,3 +39,13 @@ def test_product_coefficient_tables_equal_the_oracle_restatement(n_in, n_out):
     ob, ok = coefficients(n_in, n_out)
     assert np.array_equal(pb, ob) and np.array_equal(pk, ok)
     assert pk.dtype == np.int32 and abs(int(pk.sum(axis=1).max()) - (1 << 22)) <= pk.shape[1]      # weights sum to one
+
+
+@pytest.mark.parametrize("n_in,n_out", [(2048, 896), (512, 224), (1024, 224), (50, 224), (60, 268), (130, 291), (100, 224)])
+def test_resample_accumulator_cannot_overflow_int32(n_in, n_out):
+    """vdb_resample_h_u8 / vdb_resample_v_crop_norm accumulate 1 << 21 + sum_t u8 * kk in int32: for the tables of the shapes the
+    device preprocessing is tested at (strong downscales with 11 and 21 taps, upscales), 255 * sum |kk| + 2^21 stays below 2^31."""
+    from lib.model_zoo.clip import CLIPImageContextEncoder
+    _, kk = CLIPImageContextEncoder.pil_bicubic_coeffs(n_in, n_out)
+    worst = 255 * int(np.abs(kk.astype(np.int64)).sum(axis=1).max()) + (1 << 21)
+    assert worst < 2 ** 31, f"{n_in} -> {n_out}: {worst} >= 2^31"

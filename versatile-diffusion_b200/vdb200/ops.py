@@ -322,8 +322,15 @@ def diffedit_mask(e_src_u, e_src_c, s_src, e_tgt_u, e_tgt_c, s_tgt, D, ratio, ou
     return out
 
 
+def _same_shape(ref, t, name):
+    if t is not None and t.shape != ref.shape:
+        raise ValueError(f"{name}: expected {tuple(ref.shape)}, got {tuple(t.shape)}")
+
+
 def axpby(x, z, a, b, out=None):
-    _need(x, torch.float32, "x"); _need(z, torch.float32, "z")
+    _need(x, torch.float32, "x"); _need(z, torch.float32, "z"); _need(out, torch.float32, "out")
+    _same_shape(x, z, "z")
+    _same_shape(x, out, "out")
     if out is None:
         out = torch.empty_like(x)
     check(lib.vdb_axpby_f32(_ptr(x), _ptr(z), float(a), float(b), _ptr(out), x.numel(), _stream()), "axpby")
@@ -332,9 +339,13 @@ def axpby(x, z, a, b, out=None):
 
 def lincomb4(xs, cs, out=None):
     """sum_i cs[i] * xs[i] for 1..4 fp32 tensors of one shape."""
-    assert 1 <= len(xs) <= 4 and len(xs) == len(cs)
-    for t in xs:
-        _need(t, torch.float32, "x")
+    if not 1 <= len(xs) <= 4 or len(xs) != len(cs):
+        raise ValueError(f"lincomb4: need 1 to 4 tensors and as many coefficients, got {len(xs)} and {len(cs)}")
+    for i, t in enumerate(xs):
+        _need(t, torch.float32, f"xs[{i}]")
+        _same_shape(xs[0], t, f"xs[{i}]")
+    _need(out, torch.float32, "out")
+    _same_shape(xs[0], out, "out")
     if out is None:
         out = torch.empty_like(xs[0])
     ptrs = [_ptr(t) for t in xs] + [0] * (4 - len(xs))
@@ -799,7 +810,8 @@ def nhwc_to_nchw(x, mul=1.0, add=0.0, clamp01=False, out=None):
 
 
 def to_bf16(x, out=None):
-    _need(x, torch.float32, "x")
+    _need(x, torch.float32, "x"); _need(out, BF16, "out")
+    _same_shape(x, out, "out")
     if out is None:
         out = torch.empty(x.shape, dtype=BF16, device=x.device)
     check(lib.vdb_cast_f32_bf16(_ptr(x), _ptr(out), x.numel(), _stream()), "cast")
@@ -807,7 +819,8 @@ def to_bf16(x, out=None):
 
 
 def to_f32(x, out=None):
-    _need(x, BF16, "x")
+    _need(x, BF16, "x"); _need(out, torch.float32, "out")
+    _same_shape(x, out, "out")
     if out is None:
         out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
     check(lib.vdb_cast_bf16_f32(_ptr(x), _ptr(out), x.numel(), _stream()), "cast")
@@ -817,10 +830,19 @@ def to_f32(x, out=None):
 def pointwise_small(x, w, bias=None, pre_mul=1.0, out=None):
     """x fp32 [..., Cin<=8] NHWC, w fp32 [Cout, Cin] -> fp32 [..., Cout]."""
     _need(x, torch.float32, "x"); _need(w, torch.float32, "w"); _need(bias, torch.float32, "bias")
+    _need(out, torch.float32, "out")
+    if w.dim() != 2:
+        raise ValueError(f"w: expected [Cout, Cin], got {tuple(w.shape)}")
     cout, cin = w.shape
+    if x.dim() < 1 or x.shape[-1] != cin:
+        raise ValueError(f"x: expected [..., {cin}] for w {tuple(w.shape)}, got {tuple(x.shape)}")
+    if bias is not None and bias.numel() != cout:
+        raise ValueError(f"bias: expected {cout} elements, got {bias.numel()}")
     npix = x.numel() // cin
     if out is None:
         out = torch.empty(x.shape[:-1] + (cout,), dtype=torch.float32, device=x.device)
+    if out.numel() != npix * cout:
+        raise ValueError(f"out: expected {npix * cout} elements ({tuple(x.shape[:-1]) + (cout,)}), got {tuple(out.shape)}")
     check(lib.vdb_pointwise_small(_ptr(x), npix, cin, cout, _ptr(w), _ptr(bias), float(pre_mul), _ptr(out), _stream()),
           "pointwise_small")
     return out
@@ -828,11 +850,18 @@ def pointwise_small(x, w, bias=None, pre_mul=1.0, out=None):
 
 def gaussian_sample(moments, noise=None, post_mul=1.0, out=None):
     """moments fp32 NHWC [..., 2C]; noise fp32 NHWC [..., C] or None (posterior mean)."""
-    _need(moments, torch.float32, "moments"); _need(noise, torch.float32, "noise")
+    _need(moments, torch.float32, "moments"); _need(noise, torch.float32, "noise"); _need(out, torch.float32, "out")
+    if moments.dim() < 1 or moments.shape[-1] < 2 or moments.shape[-1] % 2:
+        raise ValueError(f"moments: expected [..., 2C] (mean | logvar), got {tuple(moments.shape)}")
     C = moments.shape[-1] // 2
     npix = moments.numel() // (2 * C)
+    shape = moments.shape[:-1] + (C,)
+    if noise is not None and noise.shape != shape:
+        raise ValueError(f"noise: expected {tuple(shape)}, got {tuple(noise.shape)}")
     if out is None:
-        out = torch.empty(moments.shape[:-1] + (C,), dtype=torch.float32, device=moments.device)
+        out = torch.empty(shape, dtype=torch.float32, device=moments.device)
+    if out.numel() != npix * C:
+        raise ValueError(f"out: expected {tuple(shape)}, got {tuple(out.shape)}")
     check(lib.vdb_gaussian_sample(_ptr(moments), _ptr(noise), C, npix, float(post_mul), _ptr(out), _stream()),
           "gaussian_sample")
     return out
@@ -840,10 +869,12 @@ def gaussian_sample(moments, noise=None, post_mul=1.0, out=None):
 
 def timestep_embedding(ts, dim, max_period=10000, step_idx=None, batch=None, out=None):
     """ts int64 device tensor [B] (or a table + step_idx int32 device scalar, broadcast to `batch` rows)."""
-    _need(ts, torch.int64, "timesteps")
+    _need(ts, torch.int64, "timesteps"); _need(step_idx, torch.int32, "step_idx"); _need(out, torch.float32, "out")
     B = batch if step_idx is not None else ts.shape[0]
     if out is None:
         out = torch.empty((B, dim), dtype=torch.float32, device=ts.device)
+    if out.numel() != B * dim:
+        raise ValueError(f"out: expected ({B}, {dim}), got {tuple(out.shape)}")
     nlp = torch.tensor(-math.log(max_period), dtype=torch.float32).item()
     check(lib.vdb_timestep_embedding(_ptr(ts), _ptr(step_idx), B, dim, nlp, _ptr(out), _stream()), "timestep_embedding")
     return out
@@ -851,22 +882,31 @@ def timestep_embedding(ts, dim, max_period=10000, step_idx=None, batch=None, out
 
 def linear_small(x, w, bias=None, act_in=ACT_NONE, act_out=ACT_NONE, out=None):
     """x fp32 [M<=16,K], w bf16 [N,K] -> fp32 [M,N]."""
-    _need(x, torch.float32, "x"); _need(w, BF16, "w"); _need(bias, torch.float32, "bias")
+    _need(x, torch.float32, "x"); _need(w, BF16, "w"); _need(bias, torch.float32, "bias"); _need(out, torch.float32, "out")
+    if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1]:
+        raise ValueError(f"w: expected [N, {x.shape[-1]}] for x {tuple(x.shape)}, got {tuple(w.shape)}")
     M, K = x.shape
     N = w.shape[0]
+    if bias is not None and bias.numel() != N:
+        raise ValueError(f"bias: expected {N} elements, got {bias.numel()}")
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    if out.shape != (M, N):
+        raise ValueError(f"out: expected ({M}, {N}), got {tuple(out.shape)}")
     check(lib.vdb_linear_small(_ptr(x), M, K, _ptr(w), N, _ptr(bias), int(act_in), int(act_out), _ptr(out), _stream()),
           "linear_small")
     return out
 
 
 def softmax_rows(x, scale=1.0, out=None):
-    _need(x, BF16, "x")
+    """Row softmax of bf16 [..., n] (x * scale) -> bf16 of the same shape and strides (the kernel walks both with x's row stride)."""
+    _need(x, BF16, "x"); _need(out, BF16, "out")
     n = x.shape[-1]
     rows = x.numel() // n
     if out is None:
         out = torch.empty_like(x)
+    if out.shape != x.shape or out.stride() != x.stride():
+        raise ValueError(f"out: expected shape {tuple(x.shape)} with strides {x.stride()}, got {tuple(out.shape)} with {out.stride()}")
     check(lib.vdb_softmax_rows(_ptr(x), rows, n, x.stride(-2) if x.dim() > 1 else n, float(scale), _ptr(out), _stream()),
           "softmax_rows")
     return out
@@ -912,6 +952,8 @@ def clip_text_embed(tokens, tok_emb, pos_emb, Lp):
     _need(tokens, torch.int64, "tokens"); _need(tok_emb, torch.float32, "tok_emb"); _need(pos_emb, torch.float32, "pos_emb")
     B, L = tokens.shape
     C = tok_emb.shape[1]
+    if pos_emb.dim() != 2 or pos_emb.shape[0] < L or pos_emb.shape[1] != C:
+        raise ValueError(f"pos_emb: expected [>= {L}, {C}], got {tuple(pos_emb.shape)}")
     x = torch.empty((B, Lp, C), dtype=BF16, device=tokens.device)
     check(lib.vdb_clip_text_embed(_ptr(tokens), _ptr(tok_emb), _ptr(pos_emb), B, L, Lp, C, _ptr(x), _stream()), "clip_text_embed")
     return x
@@ -931,6 +973,14 @@ def vit_assemble(patches, cls, pos, B, L, Lp, tok_scale=None):
     _need(patches, BF16, "patches"); _need(cls, torch.float32, "cls"); _need(pos, torch.float32, "pos")
     _need(tok_scale, torch.float32, "tok_scale")
     C = patches.shape[1]
+    if patches.dim() != 2 or patches.shape[0] != B * (L - 1):
+        raise ValueError(f"patches: expected [{B * (L - 1)}, C] (B * (L - 1) rows), got {tuple(patches.shape)}")
+    if cls.numel() != C:
+        raise ValueError(f"cls: expected {C} elements, got {cls.numel()}")
+    if pos.dim() != 2 or pos.shape[0] < L or pos.shape[1] != C:
+        raise ValueError(f"pos: expected [>= {L}, {C}], got {tuple(pos.shape)}")
+    if tok_scale is not None and tok_scale.numel() != B * L:
+        raise ValueError(f"tok_scale: expected {B * L} elements ([{B}, {L}]), got {tuple(tok_scale.shape)}")
     x = torch.empty((B, Lp, C), dtype=BF16, device=patches.device)
     check(lib.vdb_vit_assemble(_ptr(patches), _ptr(cls), _ptr(pos), _ptr(tok_scale), B, L, Lp, C, _ptr(x), _stream()), "vit_assemble")
     return x
@@ -940,6 +990,10 @@ def scale_by_row_norm(z, L, idx=None, row_scale=None):
     """z bf16 [B, Lp, C] -> fp32 [B, L, C] divided by the norm of row idx[b] (token 0 when idx is None)."""
     _need(z, BF16, "z"); _need(idx, torch.int32, "idx"); _need(row_scale, torch.float32, "row_scale")
     B, Lp, C = z.shape
+    if idx is not None and idx.numel() != B:
+        raise ValueError(f"idx: expected {B} elements, got {idx.numel()}")
+    if row_scale is not None and row_scale.numel() != B * L:
+        raise ValueError(f"row_scale: expected {B * L} elements ([{B}, {L}]), got {tuple(row_scale.shape)}")
     out = torch.empty((B, L, C), dtype=torch.float32, device=z.device)
     check(lib.vdb_scale_by_row_norm(_ptr(z), _ptr(idx), _ptr(row_scale), B, L, Lp, C, _ptr(out), _stream()), "scale_by_row_norm")
     return out
