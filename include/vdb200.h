@@ -511,6 +511,8 @@ int vdb_textdec_repetition(float* logits, int R, int V, long long ldl, const int
  * X ~= U diag(S) V^T;  x_new = U diag(S * factors) V^T + rowmean(x) [+ X - U diag(S) V^T when keep_remainder != 0];
  * out = x_new / std(x_new) * std(x) (unbiased, over all m * n elements of the item).  factors: device fp32 [q].  s_out (may be NULL):
  * device fp32 [n_items, q], the unscaled S, descending; u_out [n_items, m, q] and v_out [n_items, n, q] (may be NULL): U and V.
+ * U = X V diag(1 / S) is undefined where S = 0: such a column of u_out is written as zeros (an item whose rows are each constant,
+ * X = 0, has S = 0, U = 0 and V = 0, so U diag(S) V^T = 0 = X as for torch.pca_lowrank).
  * One launch (one 8-CTA cluster per item, X resident in shared memory); the QRs are CholeskyQR2 in fp64, so U and V differ from
  * torch's by column signs only.  Deterministic for a given R.
  * NULL x / R / factors / out, n_items < 1, niter < 0 or a misaligned x / out return VDB_ERR_INVALID; shapes other than n = 768,

@@ -42,6 +42,12 @@ def lowrank(X, R, niter):
 
 def rank_adjust(x, R, factors, keep_remainder, niter=100, dtype=torch.float64):
     """x [n, m, d] -> (x_new, S before scaling) in `dtype`; factors [q] scale S (app.py's s[:, xi] *= yi)."""
+    x_new, _, S, _ = rank_adjust_factors(x, R, factors, keep_remainder, niter, dtype)
+    return x_new, S
+
+
+def rank_adjust_factors(x, R, factors, keep_remainder, niter=100, dtype=torch.float64):
+    """rank_adjust that also returns the factors of the PCA: (x_new, U [n, m, q], S [n, q], V [n, d, q]) in `dtype`."""
     x = x.to(dtype)
     R = R.to(dtype)
     std_save = x.std(dim=(-2, -1), keepdim=True)
@@ -53,4 +59,4 @@ def rank_adjust(x, R, factors, keep_remainder, niter=100, dtype=torch.float64):
     Sf = S * torch.as_tensor(factors, dtype=dtype, device=x.device)
     x_new = torch.bmm(torch.bmm(U, torch.diag_embed(Sf)), V.permute(0, 2, 1)) + x_mean + x_remain
     x_new = x_new / x_new.std(dim=(-2, -1), keepdim=True) * std_save
-    return x_new, S
+    return x_new, U, S, V

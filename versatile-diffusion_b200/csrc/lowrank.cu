@@ -409,12 +409,13 @@ rank_adjust_kernel(const float* __restrict__ xg, int m, const float* __restrict_
       for (int c = 0; c < kQ; ++c) acc = fma(static_cast<double>(s.pq[j * kQ + c]), s.l[c * kQ + perm[k]], acc);
       v_out[(static_cast<long long>(item) * kN + j) * kQ + k] = static_cast<float>(acc);
     }
-  if (u_out != nullptr)                                  // U = Vb = C Ub diag(1 / S): this CTA's rows
+  if (u_out != nullptr)                                  // U = Vb = C Ub diag(1 / S): this CTA's rows; a column with S = 0 is 0
     for (int e = t; e < nr * kQ; e += kThreads) {
       const int i = e / kQ, k = e % kQ;
+      const double lam = s.g[perm[k] * kQ + perm[k]];
       double acc = 0.0;
       for (int c = 0; c < kQ; ++c) acc = fma(static_cast<double>(s.qm[i * kQ + c]), s.l[c * kQ + perm[k]], acc);
-      u_out[(static_cast<long long>(item) * m + row0 + i) * kQ + k] = static_cast<float>(acc / sqrt(s.g[perm[k] * kQ + perm[k]]));
+      u_out[(static_cast<long long>(item) * m + row0 + i) * kQ + k] = lam > 0.0 ? static_cast<float>(acc / sqrt(lam)) : 0.f;
     }
   for (int e = t; e < kQQ; e += kThreads) {
     const int a = e / kQ, b = e % kQ;

@@ -1108,6 +1108,11 @@ def rank_adjust(x, factors, keep_remainder, R, niter=100, out=None, s_out=None, 
     if out is None:
         out = torch.empty_like(x)
     _need(out, torch.float32, "out")
+    if out.shape != x.shape:
+        raise ValueError(f"rank_adjust: out must be {list(x.shape)}, got {list(out.shape)}")
+    x0, o0, nbytes = x.data_ptr(), out.data_ptr(), x.numel() * 4    # both contiguous fp32 of the same size
+    if o0 < x0 + nbytes and x0 < o0 + nbytes:
+        raise ValueError("rank_adjust: out must not overlap x (an out shifted against x writes rows another item has yet to read)")
     for name, t, shape in (("s_out", s_out, (n, q)), ("u_out", u_out, (n, m, q)), ("v_out", v_out, (n, d, q))):
         if t is not None and tuple(t.shape) != shape:
             raise ValueError(f"rank_adjust: {name} must be {list(shape)}, got {list(t.shape)}")
