@@ -88,50 +88,118 @@ def _gn(x, sd, p, eps):
     return F.group_norm(x, 32, sd[p + ".weight"], sd[p + ".bias"], eps)
 
 
-def resblock(sd, p, x, emb):
+def _identity(name, t):
+    return t
+
+
+# Rounding hook.  Every block function below takes rnd(name, tensor) -> tensor, applied to the named intermediate where the
+# reference's evaluation passes it on; the default is the identity, so the functions compute the reference unchanged.  A test
+# passes a hook that rounds the activations a lower-precision implementation stores (tests/test_module_coverage_gpu.py).  Names:
+#   resblock / vae_resnet:  "gn1" (SiLU(GroupNorm(x))), "emb_act" (SiLU(emb)), "conv1" (conv1 + emb), "gn2", "out"
+#   cross_attention:        "q", "k", "v", "p" (the softmax numerator weights exp(s - max), see below), "o" (heads merged)
+#   spatial_transformer:    "gn", "proj_in", "ln1" / "ln2" / "ln3", "attn1" / "attn2" (tokens after each residual),
+#                           "ff_hidden" (GEGLU output), "ff" (tokens after the feed-forward residual), "out"
+#   fcblock:                "gn1_hat" / "gn2_hat" (GroupNorm before its affine), "gn1" / "gn2", "conv1", "out"
+#   vae_attn:               "gn", "q", "k", "s" (q k^T), "p" (softmax), "v" (without its bias), "o" (P v + b_v), "out"
+#   time_embed:             "t_emb", "h" (SiLU of the first linear), "out"
+# cross_attention and vae_attn evaluate the softmax as exp(s - max) / sum exp(s - max) when a hook is given, so that "p" can
+# round the numerator's weights alone; fcblock then applies the GroupNorm affine after normalising.  Both equal the default
+# path up to fp64 reordering.
+def resblock(sd, p, x, emb, rnd=None):
     """ResBlock._forward (non-updown, use_scale_shift_norm=False), openaimodel.py:254-274; GN eps 1e-5."""
-    h = F.conv2d(F.silu(_gn(x, sd, p + ".in_layers.0", 1e-5)), sd[p + ".in_layers.2.weight"], sd[p + ".in_layers.2.bias"], padding=1)
-    e = F.linear(F.silu(emb), sd[p + ".emb_layers.1.weight"], sd[p + ".emb_layers.1.bias"])
-    h = h + e[:, :, None, None]
-    h = F.conv2d(F.silu(_gn(h, sd, p + ".out_layers.0", 1e-5)), sd[p + ".out_layers.3.weight"], sd[p + ".out_layers.3.bias"], padding=1)
+    r = rnd or _identity
+    h = F.conv2d(r("gn1", F.silu(_gn(x, sd, p + ".in_layers.0", 1e-5))), sd[p + ".in_layers.2.weight"], sd[p + ".in_layers.2.bias"],
+                 padding=1)
+    e = F.linear(r("emb_act", F.silu(emb)), sd[p + ".emb_layers.1.weight"], sd[p + ".emb_layers.1.bias"])
+    h = r("conv1", h + e[:, :, None, None])
+    h = F.conv2d(r("gn2", F.silu(_gn(h, sd, p + ".out_layers.0", 1e-5))), sd[p + ".out_layers.3.weight"], sd[p + ".out_layers.3.bias"],
+                 padding=1)
     if (p + ".skip_connection.weight") in sd:
         x = F.conv2d(x, sd[p + ".skip_connection.weight"], sd[p + ".skip_connection.bias"])
-    return x + h
+    return r("out", x + h)
 
 
-def cross_attention(sd, p, x, context, heads):
+def cross_attention(sd, p, x, context, heads, rnd=None):
     """CrossAttention.forward, attention.py:170-193 (no mask on this path)."""
+    r = rnd or _identity
     context = x if context is None else context
-    q = F.linear(x, sd[p + ".to_q.weight"])
-    k = F.linear(context, sd[p + ".to_k.weight"])
-    v = F.linear(context, sd[p + ".to_v.weight"])
+    q = r("q", F.linear(x, sd[p + ".to_q.weight"]))
+    k = r("k", F.linear(context, sd[p + ".to_k.weight"]))
+    v = r("v", F.linear(context, sd[p + ".to_v.weight"]))
     b, n, c = q.shape
     d = c // heads
-    split = lambda t: t.view(b, t.shape[1], heads, d).permute(0, 2, 1, 3)
+    split = lambda t: t.reshape(b, t.shape[1], heads, d).permute(0, 2, 1, 3)
     q, k, v = split(q), split(k), split(v)
     sim = torch.einsum("bhid,bhjd->bhij", q, k) * d ** -0.5
-    out = torch.einsum("bhij,bhjd->bhid", sim.softmax(dim=-1), v)
-    out = out.permute(0, 2, 1, 3).reshape(b, n, c)
+    if rnd is None:
+        out = torch.einsum("bhij,bhjd->bhid", sim.softmax(dim=-1), v)
+    else:
+        w = (sim - sim.amax(-1, keepdim=True)).exp()
+        out = torch.einsum("bhij,bhjd->bhid", r("p", w), v) / w.sum(-1, keepdim=True)
+    out = r("o", out.permute(0, 2, 1, 3).reshape(b, n, c))
     return F.linear(out, sd[p + ".to_out.0.weight"], sd[p + ".to_out.0.bias"])
 
 
-def spatial_transformer(sd, p, x, context, heads):
+def spatial_transformer(sd, p, x, context, heads, rnd=None):
     """SpatialTransformer.forward -> BasicTransformerBlock._forward (depth 1), attention.py:214-218,255-266."""
+    r = rnd or _identity
     b, c, h, w = x.shape
     x_in = x
-    x = _gn(x, sd, p + ".norm", 1e-6)
-    x = F.conv2d(x, sd[p + ".proj_in.weight"], sd[p + ".proj_in.bias"])
+    x = r("gn", _gn(x, sd, p + ".norm", 1e-6))
+    x = r("proj_in", F.conv2d(x, sd[p + ".proj_in.weight"], sd[p + ".proj_in.bias"]))
     x = x.permute(0, 2, 3, 1).reshape(b, h * w, c)
     t = p + ".transformer_blocks.0"
-    ln = lambda y, n: F.layer_norm(y, (c,), sd[f"{t}.{n}.weight"], sd[f"{t}.{n}.bias"], 1e-5)
-    x = cross_attention(sd, t + ".attn1", ln(x, "norm1"), None, heads) + x
-    x = cross_attention(sd, t + ".attn2", ln(x, "norm2"), context, heads) + x
+    ln = lambda y, n: r("ln" + n[-1], F.layer_norm(y, (c,), sd[f"{t}.{n}.weight"], sd[f"{t}.{n}.bias"], 1e-5))
+    x = r("attn1", cross_attention(sd, t + ".attn1", ln(x, "norm1"), None, heads, rnd) + x)
+    x = r("attn2", cross_attention(sd, t + ".attn2", ln(x, "norm2"), context, heads, rnd) + x)
     hdn = F.linear(ln(x, "norm3"), sd[t + ".ff.net.0.proj.weight"], sd[t + ".ff.net.0.proj.bias"])
     val, gate = hdn.chunk(2, dim=-1)                       # GEGLU, attention.py:42-44 (erf gelu)
-    x = F.linear(val * F.gelu(gate), sd[t + ".ff.net.2.weight"], sd[t + ".ff.net.2.bias"]) + x
+    x = r("ff", F.linear(r("ff_hidden", val * F.gelu(gate)), sd[t + ".ff.net.2.weight"], sd[t + ".ff.net.2.bias"]) + x)
     x = x.reshape(b, h, w, c).permute(0, 3, 1, 2)
     x = F.conv2d(x, sd[p + ".proj_out.weight"], sd[p + ".proj_out.bias"])
-    return x + x_in
+    return r("out", x + x_in)
+
+
+def time_embed(sd, p, t_emb, rnd=None):
+    """The time_embed MLP, openaimodel.py:2629-2633: Linear -> SiLU -> Linear on the sinusoid."""
+    r = rnd or _identity
+    h = r("h", F.silu(F.linear(r("t_emb", t_emb), sd[p + ".time_embed.0.weight"], sd[p + ".time_embed.0.bias"])))
+    return r("out", F.linear(h, sd[p + ".time_embed.2.weight"], sd[p + ".time_embed.2.bias"]))
+
+
+def conv_in(sd, p, x):
+    """data_blocks.0: conv3x3 pad 1 on the latent, openaimodel.py:2664."""
+    return F.conv2d(x, sd[p + ".weight"], sd[p + ".bias"], padding=1)
+
+
+def downsample(sd, p, x):
+    """Downsample.op: conv3x3 stride 2 pad 1, openaimodel.py:150-159."""
+    return F.conv2d(x, sd[p + ".op.weight"], sd[p + ".op.bias"], stride=2, padding=1)
+
+
+def upsample(sd, p, x):
+    """Upsample (openaimodel.py:107-117) and the VAE's (autokl_modules.py:38-47): nearest x2 then conv3x3 pad 1."""
+    x = F.interpolate(x, scale_factor=2, mode="nearest")
+    return F.conv2d(x, sd[p + ".conv.weight"], sd[p + ".conv.bias"], padding=1)
+
+
+def out_head(sd, p, x, rnd=None):
+    """GN -> SiLU -> conv3x3, openaimodel.py:2732-2737."""
+    r = rnd or _identity
+    return F.conv2d(r("gn", F.silu(_gn(x, sd, p + ".0", 1e-5))), sd[p + ".2.weight"], sd[p + ".2.bias"], padding=1)
+
+
+def linear_md(sd, p, x, second_dim=4):
+    """Linear_MultiDim (openaimodel.py:2275-2293): nn.Linear over the flattened feature, viewed back as [B, C, second_dim, 1]."""
+    b = x.shape[0]
+    return F.linear(x.reshape(b, -1), sd[p + ".weight"], sd[p + ".bias"]).view(b, -1, second_dim, 1)
+
+
+def out_head0d(sd, p, x, rnd=None):
+    """GroupNorm32(C) -> SiLU -> Linear_MultiDim([C, s, 1] -> [768]), openaimodel.py:2957-2962."""
+    r = rnd or _identity
+    h = r("gn", F.silu(_gn(x, sd, p + ".0", 1e-5)))
+    return F.linear(h.reshape(x.shape[0], -1), sd[p + ".2.weight"], sd[p + ".2.bias"])
 
 
 def unet_layout(model_channels=320, channel_mult=(1, 2, 4, 4), num_res_blocks=(2, 2, 2, 2),
@@ -168,19 +236,26 @@ def unet_layout(model_channels=320, channel_mult=(1, 2, 4, 4), num_res_blocks=(2
     return ops
 
 
-def fcblock(sd, p, x, emb):
+def fcblock(sd, p, x, emb, rnd=None):
     """FCBlock_MultiDim.forward -> FCBlock._forward, openaimodel.py:2134-2141, 2344-2354: the [B, C, s, 1] feature is flattened
     to C*s*1 channels of a 1x1 "image" (index c*s + si), GroupNorm32 (eps 1e-5) -> SiLU -> 1x1 conv, + SiLU->Linear(emb),
     GroupNorm32 -> SiLU -> 1x1 conv, + skip (identity or 1x1 conv); the result is viewed back as [B, Cout, s, 1]."""
+    r = rnd or _identity
     b, _, sdim, _ = x.shape
     xf = x.reshape(b, -1, 1, 1)
-    h = F.conv2d(F.silu(_gn(xf, sd, p + ".in_layers.0", 1e-5)), sd[p + ".in_layers.2.weight"], sd[p + ".in_layers.2.bias"])
-    e = F.linear(F.silu(emb), sd[p + ".emb_layers.1.weight"], sd[p + ".emb_layers.1.bias"])
-    h = h + e[:, :, None, None]
-    h = F.conv2d(F.silu(_gn(h, sd, p + ".out_layers.0", 1e-5)), sd[p + ".out_layers.3.weight"], sd[p + ".out_layers.3.bias"])
+
+    def gn_silu(y, q, n):
+        if rnd is None:
+            return F.silu(_gn(y, sd, q, 1e-5))
+        y = r(n + "_hat", F.group_norm(y, 32, None, None, 1e-5))
+        return r(n, F.silu(y * sd[q + ".weight"][:, None, None] + sd[q + ".bias"][:, None, None]))
+    h = F.conv2d(gn_silu(xf, p + ".in_layers.0", "gn1"), sd[p + ".in_layers.2.weight"], sd[p + ".in_layers.2.bias"])
+    e = F.linear(r("emb_act", F.silu(emb)), sd[p + ".emb_layers.1.weight"], sd[p + ".emb_layers.1.bias"])
+    h = r("conv1", h + e[:, :, None, None])
+    h = F.conv2d(gn_silu(h, p + ".out_layers.0", "gn2"), sd[p + ".out_layers.3.weight"], sd[p + ".out_layers.3.bias"])
     if (p + ".skip_connection.weight") in sd:
         xf = F.conv2d(xf, sd[p + ".skip_connection.weight"], sd[p + ".skip_connection.bias"])
-    y = xf + h
+    y = r("out", xf + h)
     return y.reshape(b, y.shape[1] // sdim, sdim, 1)
 
 
@@ -223,26 +298,20 @@ def apply_model_text(sd, x, timesteps, contexts, ratios=None, c_types=("text",),
     layout = layout or unet0d_layout()
     D = "diffuser.text"
     T = f"diffuser.{time_from}"
-    t_emb = timestep_embedding(timesteps, model_channels)
-    emb = F.linear(F.silu(F.linear(t_emb, sd[T + ".time_embed.0.weight"], sd[T + ".time_embed.0.bias"])),
-                   sd[T + ".time_embed.2.weight"], sd[T + ".time_embed.2.bias"])
+    emb = time_embed(sd, T, timestep_embedding(timesteps, model_channels))
     if ratios is None:
         ratios = [1.0] * len(contexts)
     r = np.array(ratios, dtype=np.float64)
     r = r / r.sum()
-    b = x.shape[0]
     hs, h = [], x
     for kind, idx in layout:
         p = f"{D}.data_blocks.{idx}.0"
-        if kind == "lin_in":       # Linear_MultiDim([768] -> [C, s, 1])
-            h = F.linear(h, sd[p + ".weight"], sd[p + ".bias"]).view(b, -1, second_dim, 1)
-        elif kind == "lin":        # Linear_MultiDim([C, s, 1] -> [C, s, 1])
-            h = F.linear(h.reshape(b, -1), sd[p + ".weight"], sd[p + ".bias"]).view(b, -1, second_dim, 1)
+        if kind in ("lin_in", "lin"):      # Linear_MultiDim([768] or [C, s, 1] -> [C, s, 1])
+            h = linear_md(sd, p, h, second_dim)
         elif kind == "fc":
             h = fcblock(sd, p, h, emb)
-        elif kind == "out":        # GroupNorm32(C) -> SiLU -> Linear_MultiDim([C, s, 1] -> [768])
-            h = F.silu(_gn(h, sd, p + ".0", 1e-5))
-            h = F.linear(h.reshape(b, -1), sd[p + ".2.weight"], sd[p + ".2.bias"])
+        elif kind == "out":
+            h = out_head0d(sd, p, h)
         elif kind == "ctx":
             if len(contexts) == 1:
                 h = spatial_transformer(sd, f"diffuser.{c_types[0]}.context_blocks.{idx}.0", h, contexts[0], num_heads)
@@ -266,27 +335,24 @@ def apply_model(sd, x, timesteps, contexts, ratios=None, x_type="image", c_types
     embedding comes from diffuser.<x_type> (global_layer_ptr='image' == x_type on this path)."""
     layout = layout or unet_layout(model_channels=model_channels, num_heads=num_heads)
     D = f"diffuser.{x_type}"
-    t_emb = timestep_embedding(timesteps, model_channels)
-    emb = F.linear(F.silu(F.linear(t_emb, sd[D + ".time_embed.0.weight"], sd[D + ".time_embed.0.bias"])),
-                   sd[D + ".time_embed.2.weight"], sd[D + ".time_embed.2.bias"])
+    emb = time_embed(sd, D, timestep_embedding(timesteps, model_channels))
     if ratios is None:
         ratios = [1.0] * len(contexts)
     r = np.array(ratios, dtype=np.float64)
     r = r / r.sum()
     hs, h = [], x
     for kind, idx, _ in layout:
+        p = f"{D}.data_blocks.{idx}.0"
         if kind == "conv_in":
-            h = F.conv2d(h, sd[f"{D}.data_blocks.{idx}.0.weight"], sd[f"{D}.data_blocks.{idx}.0.bias"], padding=1)
+            h = conv_in(sd, p, h)
         elif kind == "res":
-            h = resblock(sd, f"{D}.data_blocks.{idx}.0", h, emb)
-        elif kind == "down":   # Downsample.op conv3x3 s2 p1, openaimodel.py:150-159
-            h = F.conv2d(h, sd[f"{D}.data_blocks.{idx}.0.op.weight"], sd[f"{D}.data_blocks.{idx}.0.op.bias"], stride=2, padding=1)
-        elif kind == "up":     # Upsample: nearest x2 then conv3x3, openaimodel.py:107-117
-            h = F.interpolate(h, scale_factor=2, mode="nearest")
-            h = F.conv2d(h, sd[f"{D}.data_blocks.{idx}.0.conv.weight"], sd[f"{D}.data_blocks.{idx}.0.conv.bias"], padding=1)
-        elif kind == "out":    # GN -> SiLU -> conv3x3, openaimodel.py:2732-2737
-            p = f"{D}.data_blocks.{idx}.0"
-            h = F.conv2d(F.silu(_gn(h, sd, p + ".0", 1e-5)), sd[p + ".2.weight"], sd[p + ".2.bias"], padding=1)
+            h = resblock(sd, p, h, emb)
+        elif kind == "down":
+            h = downsample(sd, p, h)
+        elif kind == "up":
+            h = upsample(sd, p, h)
+        elif kind == "out":
+            h = out_head(sd, p, h)
         elif kind == "ctx":
             if len(contexts) == 1:
                 h = spatial_transformer(sd, f"diffuser.{c_types[0]}.context_blocks.{idx}.0", h, contexts[0], num_heads)
@@ -422,29 +488,43 @@ def _swish(x):
     return x * torch.sigmoid(x)
 
 
-def vae_resnet(sd, p, x):
+def vae_resnet(sd, p, x, rnd=None):
     """ResnetBlock.forward with temb=None, autokl_modules.py:119-141; GN eps 1e-6."""
-    h = F.conv2d(_swish(_gn(x, sd, p + ".norm1", 1e-6)), sd[p + ".conv1.weight"], sd[p + ".conv1.bias"], padding=1)
-    h = F.conv2d(_swish(_gn(h, sd, p + ".norm2", 1e-6)), sd[p + ".conv2.weight"], sd[p + ".conv2.bias"], padding=1)
+    r = rnd or _identity
+    h = r("conv1", F.conv2d(r("gn1", _swish(_gn(x, sd, p + ".norm1", 1e-6))), sd[p + ".conv1.weight"], sd[p + ".conv1.bias"], padding=1))
+    h = F.conv2d(r("gn2", _swish(_gn(h, sd, p + ".norm2", 1e-6))), sd[p + ".conv2.weight"], sd[p + ".conv2.bias"], padding=1)
     if (p + ".nin_shortcut.weight") in sd:
         x = F.conv2d(x, sd[p + ".nin_shortcut.weight"], sd[p + ".nin_shortcut.bias"])
-    return x + h
+    return r("out", x + h)
 
 
-def vae_attn(sd, p, x):
-    """AttnBlock.forward, autokl_modules.py:178-202 (single head, d = C)."""
-    h_ = _gn(x, sd, p + ".norm", 1e-6)
-    q = F.conv2d(h_, sd[p + ".q.weight"], sd[p + ".q.bias"])
-    k = F.conv2d(h_, sd[p + ".k.weight"], sd[p + ".k.bias"])
-    v = F.conv2d(h_, sd[p + ".v.weight"], sd[p + ".v.bias"])
+def vae_attn(sd, p, x, rnd=None):
+    """AttnBlock.forward, autokl_modules.py:178-202 (single head, d = C).  With a rounding hook, v is rounded without its bias
+    and b_v is added after P v (the softmax rows sum to 1)."""
+    r = rnd or _identity
+    h_ = r("gn", _gn(x, sd, p + ".norm", 1e-6))
+    q = r("q", F.conv2d(h_, sd[p + ".q.weight"], sd[p + ".q.bias"]))
+    k = r("k", F.conv2d(h_, sd[p + ".k.weight"], sd[p + ".k.bias"]))
     b, c, h, w = q.shape
     q = q.reshape(b, c, h * w).permute(0, 2, 1)
     k = k.reshape(b, c, h * w)
-    w_ = torch.bmm(q, k) * (int(c) ** (-0.5))
-    w_ = F.softmax(w_, dim=2)
-    v = v.reshape(b, c, h * w)
-    h_ = torch.bmm(v, w_.permute(0, 2, 1)).reshape(b, c, h, w)
-    return x + F.conv2d(h_, sd[p + ".proj_out.weight"], sd[p + ".proj_out.bias"])
+    if rnd is None:
+        v = F.conv2d(h_, sd[p + ".v.weight"], sd[p + ".v.bias"])
+        w_ = torch.bmm(q, k) * (int(c) ** (-0.5))
+        w_ = F.softmax(w_, dim=2)
+        v = v.reshape(b, c, h * w)
+        h_ = torch.bmm(v, w_.permute(0, 2, 1)).reshape(b, c, h, w)
+    else:
+        v = r("v", F.conv2d(h_, sd[p + ".v.weight"])).reshape(b, c, h * w)
+        w_ = r("p", F.softmax(r("s", torch.bmm(q, k)) * (int(c) ** (-0.5)), dim=2))
+        h_ = r("o", torch.bmm(v, w_.permute(0, 2, 1)) + sd[p + ".v.bias"][None, :, None]).reshape(b, c, h, w)
+    return r("out", x + F.conv2d(h_, sd[p + ".proj_out.weight"], sd[p + ".proj_out.bias"]))
+
+
+def vae_downsample(sd, p, x):
+    """Downsample with conv, autokl_modules.py:60-79: pad (0, 1, 0, 1), then conv3x3 stride 2."""
+    x = F.pad(x, (0, 1, 0, 1), mode="constant", value=0)
+    return F.conv2d(x, sd[p + ".conv.weight"], sd[p + ".conv.bias"], stride=2)
 
 
 def vae_decode(sd, z, scale_factor=0.18215, ch_mult=(1, 2, 4, 4), num_res_blocks=2, prefix="vae.image"):
@@ -461,8 +541,7 @@ def vae_decode(sd, z, scale_factor=0.18215, ch_mult=(1, 2, 4, 4), num_res_blocks
         for blk in range(num_res_blocks + 1):
             h = vae_resnet(sd, f"{D}.up.{lvl}.block.{blk}", h)
         if lvl != 0:
-            h = F.interpolate(h, scale_factor=2.0, mode="nearest")
-            h = F.conv2d(h, sd[f"{D}.up.{lvl}.upsample.conv.weight"], sd[f"{D}.up.{lvl}.upsample.conv.bias"], padding=1)
+            h = upsample(sd, f"{D}.up.{lvl}.upsample", h)
     h = F.conv2d(_swish(_gn(h, sd, D + ".norm_out", 1e-6)), sd[D + ".conv_out.weight"], sd[D + ".conv_out.bias"], padding=1)
     return torch.clamp((h + 1) / 2, 0, 1)
 
@@ -478,8 +557,7 @@ def vae_encode(sd, x, noise=None, scale_factor=0.18215, ch_mult=(1, 2, 4, 4), nu
         for blk in range(num_res_blocks):
             h = vae_resnet(sd, f"{E}.down.{lvl}.block.{blk}", h)
         if lvl != len(ch_mult) - 1:
-            h = F.pad(h, (0, 1, 0, 1), mode="constant", value=0)     # autokl_modules.py:72-76
-            h = F.conv2d(h, sd[f"{E}.down.{lvl}.downsample.conv.weight"], sd[f"{E}.down.{lvl}.downsample.conv.bias"], stride=2)
+            h = vae_downsample(sd, f"{E}.down.{lvl}.downsample", h)
     h = vae_resnet(sd, E + ".mid.block_1", h)
     h = vae_attn(sd, E + ".mid.attn_1", h)
     h = vae_resnet(sd, E + ".mid.block_2", h)

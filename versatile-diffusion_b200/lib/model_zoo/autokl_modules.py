@@ -104,9 +104,9 @@ class ResnetBlock(PackedModule):
 
 
 class AttnBlock(PackedModule):
-    """Single-head spatial self-attention with d = C = 512 (reference :150-202).  d exceeds what the flash
-    kernel keeps in TMEM, and it runs once per decode, so it is three tcgen05 GEMMs around a row softmax:
-    S = q k^T (bf16), P = softmax(S * C^-1/2), O = P v (+ b_v: rows of P sum to 1), proj_out + x."""
+    """Single-head spatial self-attention with d = C = 512 (reference :150-202).  d exceeds the flash attention
+    kernel's d_head limit (160), and it runs once per decode, so it is three wgmma GEMMs around a row softmax:
+    S = q k^T (bf16), P = softmax(S * C^-1/2) (bf16), O = P v (+ b_v: rows of P sum to 1), proj_out + x."""
 
     def __init__(self, in_channels):
         super().__init__()
