@@ -35,9 +35,10 @@ def step_order(order, k, i, walk_len):
     return o
 
 
-def walk(x, eps_fn, alphas_cumprod, timesteps, order, trace=None):
+def walk(x, eps_fn, alphas_cumprod, timesteps, order, trace=None, after=None):
     """fp64 multistep DPM-Solver++ from x (at t_{len-1}) down to ac[0].  eps_fn(x, i) -> the model's (CFG-mixed) eps at grid
-    index i.  trace, when a list, receives (order, x0_i, x') per step."""
+    index i.  after(i, x') -> the state the next step starts from (a blend after step i; default x').  trace, when a list,
+    receives (order, x0_i, x') per step, x' before after."""
     alpha, sigma, lam, alpha_to, sigma_to = coefficients(alphas_cumprod, timesteps)
     n = len(timesteps)
     x = np.asarray(x, dtype=np.float64)
@@ -64,7 +65,7 @@ def walk(x, eps_fn, alphas_cumprod, timesteps, order, trace=None):
             trace.append((o, x0, xn))
         x0s.append(x0)
         lams.append(lam[i])
-        x = xn
+        x = xn if after is None else after(i, xn)
     return x
 
 
@@ -90,19 +91,13 @@ def sample(sd, x_T, conds, unconds, steps, order, scale=7.5, c_types=("text",), 
     ts = O.make_ddim_timesteps(steps, num_ddpm)
     x = x_T
     if x0 is not None:
-        t0 = torch.full((x0.shape[0],), int(ts[x0_forward_timesteps]), dtype=torch.long)
-        ts = ts[:x0_forward_timesteps]
-        x = O.q_sample(x0, t0, x0_noise, num_ddpm)
+        x, ts = O.img2img_start(x0, x0_noise, ts, x0_forward_timesteps, num_ddpm)
     model = O.apply_model_text if text else O.apply_model
 
     def eps_fn(xv, i):
-        xt = torch.from_numpy(np.asarray(xv)).float()
-        t = torch.full((xt.shape[0],), int(ts[i]), dtype=torch.long)
-        if scale == 1.0:
-            return model(sd, xt, t, conds, ratios, c_types=c_types, **kw).double().numpy()
-        c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
-        e_u, e_c = model(sd, torch.cat([xt] * 2), torch.cat([t] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
-        return (e_u + scale * (e_c - e_u)).double().numpy()
+        t = torch.full((xv.shape[0],), int(ts[i]), dtype=torch.long)
+        e_u, e_c = O.cfg_pass(model, sd, torch.from_numpy(xv).float(), t, conds, unconds, scale != 1.0, ratios, c_types, **kw)
+        return (e_c if e_u is None else e_u + scale * (e_c - e_u)).double().numpy()
 
     out = walk(x.double().numpy(), eps_fn, sch["alphas_cumprod"].numpy(), ts, order)
     return torch.from_numpy(out).float()

@@ -1,13 +1,14 @@
 """Editing oracle — TEST INFRASTRUCTURE ONLY (never imported by the product path).
 
 An fp64 restatement of lib/model_zoo/edit.py: the inversion rows, the DDIM inversion walk (eps from vd_oracle.apply_model, the fp32
-UNet restatement), the walk from an inversion with the trajectory blend after every step (DDIM, and DPM-Solver++ with the
-steps of inpaint_oracle.dpm_walk and the trajectory in place of the re-noised x0), and DiffEdit's mask rule.
+UNet restatement), the walk from an inversion with the trajectory blend after every step (DDIM, and dpm_solver_oracle.walk with
+the blend against the trajectory as its `after`), and DiffEdit's mask rule.
 """
 import numpy as np
 import torch
 
 from . import dpm_solver_oracle as D
+from . import panorama_oracle as P
 from . import vd_oracle as O
 
 
@@ -21,12 +22,8 @@ def inversion_rows(ddim_alphas, ddim_alphas_prev, k):
 def _eps_fn(sd, conds, unconds, scale, c_types, ratios, kw):
     def eps(x, t):
         tt = torch.full((x.shape[0],), int(t), dtype=torch.long)
-        xf = x.float()
-        if scale == 1.0:
-            return O.apply_model(sd, xf, tt, conds, ratios, c_types=c_types, **kw).double()
-        c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
-        e_u, e_c = O.apply_model(sd, torch.cat([xf] * 2), torch.cat([tt] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
-        return (e_u.double() + scale * (e_c.double() - e_u.double()))
+        e_u, e_c = O.cfg_pass(O.apply_model, sd, x.float(), tt, conds, unconds, scale != 1.0, ratios, c_types, **kw)
+        return e_c.double() if e_u is None else e_u.double() + scale * (e_c.double() - e_u.double())
     return eps
 
 
@@ -40,9 +37,7 @@ def invert(sd, x0, conds, unconds, steps, k=None, scale=1.0, c_types=("text",), 
     x = x0.double()
     traj = [x]
     for i in range(k):
-        ap, a = rows[i, 0], rows[i, 1]
-        e = eps(x, ts[i])
-        x = np.sqrt(a) * (x - np.sqrt(1.0 - ap) * e) / np.sqrt(ap) + np.sqrt(1.0 - a) * e
+        x = P.ddim_update(x, eps(x, ts[i]), rows[i, 0], rows[i, 1])
         traj.append(x)
     return torch.stack(traj)
 
@@ -60,40 +55,14 @@ def sample(sd, traj, conds, unconds, steps, mask=None, sampler="ddim", order=2, 
     x = traj[k].double()
     if sampler == "ddim":
         for i in range(k - 1, -1, -1):
-            a, ap = float(sched["alphas"][i]), float(sched["alphas_prev"][i])
-            e = eps(x, ts[i])
-            x = np.sqrt(ap) * (x - np.sqrt(1.0 - a) * e) / np.sqrt(a) + np.sqrt(1.0 - ap) * e
+            x = P.ddim_update(x, eps(x, ts[i]), float(sched["alphas"][i]), float(sched["alphas_prev"][i]))
             if m is not None:
                 x = m * x + (1 - m) * traj[i].double()
         return x
-    # DPM-Solver++: the steps of inpaint_oracle.dpm_walk, blended against slot i in place of x0 re-noised
-    shape = x.shape
-    mm = np.ones(shape) if m is None else m.expand(shape).numpy()
-    slots = traj.double().numpy()
-    alpha, sigma, lam, alpha_to, sigma_to = D.coefficients(ac.numpy(), ts)
-    xv = x.numpy()
-    x0s, lams = [], []
-    for kk, i in enumerate(range(k - 1, -1, -1)):
-        xp = (xv - sigma[i] * eps(torch.from_numpy(xv), ts[i]).numpy()) / alpha[i]
-        h = np.log(alpha_to[i]) - np.log(sigma_to[i]) - lam[i]
-        phi1 = np.expm1(-h)
-        o = D.step_order(order, kk, i, k)
-        xn = sigma_to[i] / sigma[i] * xv - alpha_to[i] * phi1 * xp
-        if o == 2:
-            r0 = (lam[i] - lams[-1]) / h
-            xn = xn - 0.5 * alpha_to[i] * phi1 * (xp - x0s[-1]) / r0
-        elif o == 3:
-            r0, r1 = (lam[i] - lams[-1]) / h, (lams[-1] - lams[-2]) / h
-            d1_0, d1_1 = (xp - x0s[-1]) / r0, (x0s[-1] - x0s[-2]) / r1
-            d1 = d1_0 + r0 / (r0 + r1) * (d1_0 - d1_1)
-            d2 = (d1_0 - d1_1) / (r0 + r1)
-            phi2 = phi1 / h + 1.0
-            phi3 = phi2 / h - 0.5
-            xn = xn + alpha_to[i] * phi2 * d1 - alpha_to[i] * phi3 * d2
-        xv = mm * xn + (1 - mm) * slots[i]
-        x0s.append(xp)
-        lams.append(lam[i])
-    return torch.from_numpy(xv)
+    mm, slots = None if m is None else m.numpy(), traj.double().numpy()
+    after = None if mm is None else lambda i, xn: mm * xn + (1 - mm) * slots[i]
+    out = D.walk(x.numpy(), lambda xv, i: eps(torch.from_numpy(xv), ts[i]), ac.numpy(), ts, order, after=after)
+    return torch.from_numpy(out)
 
 
 def diffedit_mask(e_src, e_tgt, ratio=3.0):

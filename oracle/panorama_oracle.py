@@ -4,8 +4,9 @@ A CPU restatement of the windowed walk of lib/model_zoo/panorama.py in the paper
 each window of the canvas, takes one step on the crop, and averages the windows' x_{t-1} per element.  DDIM runs through
 vd_oracle.p_sample_ddim (the fp32 UNet restatement), with the windows' crops as one batch, and the average is taken in fp64.
 DPM-Solver++ is a multistep method, so its paper form has no per-window state to average; it is the canvas walk of
-inpaint_oracle.dpm_walk with an eps function that averages the windows' (CFG-mixed) eps.  The product averages eps in every case;
-the CPU test of the paper-form DDIM average against the eps average is what checks that the two agree.
+dpm_solver_oracle.walk (with inpaint_oracle's blend as its `after` under a mask) with an eps function that averages the windows'
+(CFG-mixed) eps.  The product averages eps in every case; the CPU test of the paper-form DDIM average against the eps average is
+what checks that the two agree.
 
 The layout is restated here independently of the product: sides min(size, L), origins 0, s, 2s, ... plus a final window flush
 with the far edge (non-circular), or 0, s, ..., W - s with columns read mod W (circular, along W only).
@@ -78,12 +79,8 @@ def _windowed_eps(sd, x, t, conds, unconds, wins, h, w, scale, c_types, ratios, 
     xc = torch.cat([torch.from_numpy(crop(x.numpy(), oy, ox, h, w).copy()) for oy, ox in wins])      # row g*bs + b
     tt = torch.full((n * bs,), int(t), dtype=torch.long)
     rep = lambda cs: [c.repeat(n, 1, 1) for c in cs]
-    if scale == 1.0:
-        e = O.apply_model(sd, xc, tt, rep(conds), ratios, c_types=c_types, **kw)
-    else:
-        c_in = [torch.cat([u, c]) for u, c in zip(rep(unconds), rep(conds))]
-        e_u, e_c = O.apply_model(sd, torch.cat([xc] * 2), torch.cat([tt] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
-        e = e_u + scale * (e_c - e_u)
+    e_u, e_c = O.cfg_pass(O.apply_model, sd, xc, tt, rep(conds), rep(unconds), scale != 1.0, ratios, c_types, **kw)
+    e = e_c if e_u is None else e_u + scale * (e_c - e_u)
     e = e.double().numpy().reshape(n, bs, *e.shape[1:])
     return average(list(e), wins, h, w, x.shape)
 
@@ -99,9 +96,7 @@ def sample(sd, x_T, conds, unconds, steps, size, stride, circular=False, sampler
     H, W = x_T.shape[-2:]
     h, w, wins = windows(H, W, size, stride, circular)
     if x0_forward_timesteps is not None:
-        t0 = torch.full((x0.shape[0],), int(ts[x0_forward_timesteps]), dtype=torch.long)
-        ts = ts[:x0_forward_timesteps]
-        x = O.q_sample(x0.float(), t0, x0_noise, num_ddpm)
+        x, ts = O.img2img_start(x0.float(), x0_noise, ts, x0_forward_timesteps, num_ddpm)
     elif mask is not None:
         x = I.start(x_T.float(), x0.float(), mask.float(), ac.numpy(), int(ts[-1])).float()
     else:
@@ -124,9 +119,6 @@ def sample(sd, x_T, conds, unconds, steps, size, stride, circular=False, sampler
         return _windowed_eps(sd, torch.from_numpy(np.asarray(xv)).float(), ts[i], conds, unconds, wins, h, w, scale, c_types,
                              ratios, kw)
 
-    if mask is None:
-        out = D.walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order)
-    else:
-        out = I.dpm_walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, x0.double().numpy(), mask.double().numpy(),
-                         lambda i: noise_fn(i).double().numpy())
+    after = None if mask is None else I.blend_after(ac.numpy(), ts, x0, mask, noise_fn)
+    out = D.walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, after=after)
     return torch.from_numpy(out).float()

@@ -4,9 +4,10 @@ A CPU restatement of the region walk of lib/model_zoo/regions.py in the paper's 
 every step crops each window of every region's input (the canvas, or under bootstrapping m_r x + (1 - m_r)(a bg + b z) for region
 r >= 1), runs one guided DDIM step per (window, region) with the region's own unconditional and conditional rows, and takes the
 per-element sum of m_r x_{t-1} over windows and regions divided by n D, with m_0 = max(0, 1 - S) and D = m_0 + S.  DPM-Solver++ is
-multistep, so its paper form has no per-view state; it is the canvas walk of dpm_solver_oracle / inpaint_oracle with the
-mask-weighted average of the views' guided eps.  The product averages eps in every case; the CPU tests check that the paper-form
-DDIM step equals the eps average for binary masks, and that all-zero masks reduce to the plain (windowed) walk.
+multistep, so its paper form has no per-view state; it is the canvas walk of dpm_solver_oracle.walk (with inpaint_oracle's blend
+as its `after` under an inpainting mask) with the mask-weighted average of the views' guided eps.  The product averages eps in
+every case; the CPU tests check that the paper-form DDIM step equals the eps average for binary masks, and that all-zero masks
+reduce to the plain (windowed) walk.
 """
 import numpy as np
 import torch
@@ -79,12 +80,8 @@ def _views_eps(sd, xs, t, conds, unconds, region_conds, wins, h, w, scale, c_typ
         xc = torch.cat([torch.from_numpy(P.crop(xr, oy, ox, h, w).copy()).float() for oy, ox in wins])     # row g*bs + b
         tt = torch.full((n * bs,), int(t), dtype=torch.long)
         cs = conds if r == 0 else region_conds[r - 1]
-        if scale == 1.0:
-            e = O.apply_model(sd, xc, tt, rep(cs), ratios, c_types=c_types, **kw)
-        else:
-            c_in = [torch.cat([u, c]) for u, c in zip(rep(unconds), rep(cs))]
-            e_u, e_c = O.apply_model(sd, torch.cat([xc] * 2), torch.cat([tt] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
-            e = e_u + scale * (e_c - e_u)
+        e_u, e_c = O.cfg_pass(O.apply_model, sd, xc, tt, rep(cs), rep(unconds), scale != 1.0, ratios, c_types, **kw)
+        e = e_c if e_u is None else e_u + scale * (e_c - e_u)
         e = e.double().numpy().reshape(n, bs, *e.shape[1:])
         for g in range(n):
             out[g, r] = e[g]
@@ -139,9 +136,6 @@ def sample(sd, x_T, conds, unconds, region_conds, masks, steps, size=None, strid
         ev = views(np.asarray(xv, dtype=np.float64), i, boot)
         return eps_average(np.asarray(xv, dtype=np.float64), lambda xc, g, r: ev[g, r], masks, wins, h, w, boot)
 
-    if mask is None:
-        out = D.walk(x, eps_fn, ac.numpy(), ts, order)
-    else:
-        out = I.dpm_walk(x, eps_fn, ac.numpy(), ts, order, x0.double().numpy(), mask.double().numpy(),
-                         lambda i: noise_fn(i).double().numpy())
+    after = None if mask is None else I.blend_after(ac.numpy(), ts, x0, mask, noise_fn)
+    out = D.walk(x, eps_fn, ac.numpy(), ts, order, after=after)
     return torch.from_numpy(out).float()

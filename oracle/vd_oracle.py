@@ -119,9 +119,12 @@ def resblock(sd, p, x, emb, rnd=None):
     return r("out", x + h)
 
 
-def cross_attention(sd, p, x, context, heads, rnd=None):
-    """CrossAttention.forward, attention.py:170-193 (no mask on this path)."""
+def cross_attention(sd, p, x, context, heads, rnd=None, hook=None):
+    """CrossAttention.forward, attention.py:170-193 (no mask on this path).  hook(probs [b, heads, n, L], is_cross) -> the
+    softmax probabilities that weight V, for the oracles that read or edit the attention maps (SAG, Prompt-to-Prompt)."""
+    assert rnd is None or hook is None
     r = rnd or _identity
+    cross = context is not None
     context = x if context is None else context
     q = r("q", F.linear(x, sd[p + ".to_q.weight"]))
     k = r("k", F.linear(context, sd[p + ".to_k.weight"]))
@@ -132,7 +135,10 @@ def cross_attention(sd, p, x, context, heads, rnd=None):
     q, k, v = split(q), split(k), split(v)
     sim = torch.einsum("bhid,bhjd->bhij", q, k) * d ** -0.5
     if rnd is None:
-        out = torch.einsum("bhij,bhjd->bhid", sim.softmax(dim=-1), v)
+        probs = sim.softmax(dim=-1)
+        if hook is not None:
+            probs = hook(probs, cross)
+        out = torch.einsum("bhij,bhjd->bhid", probs, v)
     else:
         w = (sim - sim.amax(-1, keepdim=True)).exp()
         out = torch.einsum("bhij,bhjd->bhid", r("p", w), v) / w.sum(-1, keepdim=True)
@@ -140,7 +146,7 @@ def cross_attention(sd, p, x, context, heads, rnd=None):
     return F.linear(out, sd[p + ".to_out.0.weight"], sd[p + ".to_out.0.bias"])
 
 
-def spatial_transformer(sd, p, x, context, heads, rnd=None):
+def spatial_transformer(sd, p, x, context, heads, rnd=None, hook=None):
     """SpatialTransformer.forward -> BasicTransformerBlock._forward (depth 1), attention.py:214-218,255-266."""
     r = rnd or _identity
     b, c, h, w = x.shape
@@ -150,8 +156,8 @@ def spatial_transformer(sd, p, x, context, heads, rnd=None):
     x = x.permute(0, 2, 3, 1).reshape(b, h * w, c)
     t = p + ".transformer_blocks.0"
     ln = lambda y, n: r("ln" + n[-1], F.layer_norm(y, (c,), sd[f"{t}.{n}.weight"], sd[f"{t}.{n}.bias"], 1e-5))
-    x = r("attn1", cross_attention(sd, t + ".attn1", ln(x, "norm1"), None, heads, rnd) + x)
-    x = r("attn2", cross_attention(sd, t + ".attn2", ln(x, "norm2"), context, heads, rnd) + x)
+    x = r("attn1", cross_attention(sd, t + ".attn1", ln(x, "norm1"), None, heads, rnd, hook) + x)
+    x = r("attn2", cross_attention(sd, t + ".attn2", ln(x, "norm2"), context, heads, rnd, hook) + x)
     hdn = F.linear(ln(x, "norm3"), sd[t + ".ff.net.0.proj.weight"], sd[t + ".ff.net.0.proj.bias"])
     val, gate = hdn.chunk(2, dim=-1)                       # GEGLU, attention.py:42-44 (erf gelu)
     x = r("ff", F.linear(r("ff_hidden", val * F.gelu(gate)), sd[t + ".ff.net.2.weight"], sd[t + ".ff.net.2.bias"]) + x)
@@ -289,6 +295,26 @@ def unet0d_layout(channel_mult=(1, 2, 4, 4), num_noattn_blocks=(2, 2, 2, 2), wit
     return ops
 
 
+def context_weights(ratios, n):
+    """the mixing weights of n contexts: their ratios (None: equal) normalised to sum 1, fp64"""
+    r = np.array([1.0] * n if ratios is None else ratios, dtype=np.float64)
+    return r / r.sum()
+
+
+def context_block(sd, idx, h, contexts, ratios, c_types, num_heads, hook_for=None):
+    """context block idx of diffuser.<c_type> on h for every context; several contexts are mixed by context_weights
+    (context_mixing 'attention', vd.py:383-395).  hook_for(j, idx) -> the attention hook of context j (cross_attention), or None."""
+    r = context_weights(ratios, len(contexts))
+    acc = None
+    for j, (ct, c) in enumerate(zip(c_types, contexts)):
+        hook = None if hook_for is None else hook_for(j, idx)
+        hj = spatial_transformer(sd, f"diffuser.{ct}.context_blocks.{idx}.0", h, c, num_heads, hook=hook)
+        if len(contexts) > 1:
+            hj = hj * r[j]
+        acc = hj if acc is None else acc + hj
+    return acc
+
+
 def apply_model_text(sd, x, timesteps, contexts, ratios=None, c_types=("text",), layout=None, model_channels=320,
                      second_dim=4, num_heads=8, time_from="image"):
     """VD_v2_0.apply_model / apply_model_multicontext (vd.py:330-455) for x_type = 'text': the 0-D diffuser's data blocks
@@ -299,10 +325,6 @@ def apply_model_text(sd, x, timesteps, contexts, ratios=None, c_types=("text",),
     D = "diffuser.text"
     T = f"diffuser.{time_from}"
     emb = time_embed(sd, T, timestep_embedding(timesteps, model_channels))
-    if ratios is None:
-        ratios = [1.0] * len(contexts)
-    r = np.array(ratios, dtype=np.float64)
-    r = r / r.sum()
     hs, h = [], x
     for kind, idx in layout:
         p = f"{D}.data_blocks.{idx}.0"
@@ -313,14 +335,7 @@ def apply_model_text(sd, x, timesteps, contexts, ratios=None, c_types=("text",),
         elif kind == "out":
             h = out_head0d(sd, p, h)
         elif kind == "ctx":
-            if len(contexts) == 1:
-                h = spatial_transformer(sd, f"diffuser.{c_types[0]}.context_blocks.{idx}.0", h, contexts[0], num_heads)
-            else:
-                acc = None
-                for ct, c, ri in zip(c_types, contexts, r):
-                    hi = spatial_transformer(sd, f"diffuser.{ct}.context_blocks.{idx}.0", h, c, num_heads) * ri
-                    acc = hi if acc is None else acc + hi
-                h = acc
+            h = context_block(sd, idx, h, contexts, ratios, c_types, num_heads)
         elif kind == "save":
             hs.append(h)
         elif kind == "load":
@@ -329,17 +344,14 @@ def apply_model_text(sd, x, timesteps, contexts, ratios=None, c_types=("text",),
 
 
 def apply_model(sd, x, timesteps, contexts, ratios=None, x_type="image", c_types=("text",), layout=None,
-                model_channels=320, num_heads=8):
+                model_channels=320, num_heads=8, hook_for=None):
     """VD_v2_0.apply_model (vd.py:330-381) when len(contexts)==1 and apply_model_multicontext +
     context_mixing 'attention' (vd.py:383-455) otherwise.  sd keys: diffuser.<type>.… ; the time
-    embedding comes from diffuser.<x_type> (global_layer_ptr='image' == x_type on this path)."""
+    embedding comes from diffuser.<x_type> (global_layer_ptr='image' == x_type on this path).
+    hook_for(j, idx) -> the attention hook of context j in context block idx (see context_block)."""
     layout = layout or unet_layout(model_channels=model_channels, num_heads=num_heads)
     D = f"diffuser.{x_type}"
     emb = time_embed(sd, D, timestep_embedding(timesteps, model_channels))
-    if ratios is None:
-        ratios = [1.0] * len(contexts)
-    r = np.array(ratios, dtype=np.float64)
-    r = r / r.sum()
     hs, h = [], x
     for kind, idx, _ in layout:
         p = f"{D}.data_blocks.{idx}.0"
@@ -354,14 +366,7 @@ def apply_model(sd, x, timesteps, contexts, ratios=None, x_type="image", c_types
         elif kind == "out":
             h = out_head(sd, p, h)
         elif kind == "ctx":
-            if len(contexts) == 1:
-                h = spatial_transformer(sd, f"diffuser.{c_types[0]}.context_blocks.{idx}.0", h, contexts[0], num_heads)
-            else:
-                acc = None
-                for ct, c, ri in zip(c_types, contexts, r):
-                    hi = spatial_transformer(sd, f"diffuser.{ct}.context_blocks.{idx}.0", h, c, num_heads) * ri
-                    acc = hi if acc is None else acc + hi
-                h = acc
+            h = context_block(sd, idx, h, contexts, ratios, c_types, num_heads, hook_for)
         elif kind == "save":
             hs.append(h)
         elif kind == "load":
@@ -369,17 +374,21 @@ def apply_model(sd, x, timesteps, contexts, ratios=None, x_type="image", c_types
     return h
 
 
+def cfg_pass(model, sd, x, t, conds, unconds, pair, ratios=None, c_types=("text",), **kw):
+    """model (apply_model or apply_model_text) on x alone -> (None, e_c), or on the CFG batch [x; x] with the contexts
+    [uncond; cond] -> (e_u, e_c); fp32, unmixed (ddim.py:150-158)."""
+    if not pair:
+        return None, model(sd, x, t, conds, ratios, c_types=c_types, **kw)
+    c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
+    e_u, e_c = model(sd, torch.cat([x] * 2), torch.cat([t] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
+    return e_u, e_c
+
+
 def p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types=("text",), ratios=None, **kw):
     """DDIMSampler.p_sample_ddim / _multicontext, ddim.py:129-171, 244-298 (eta noise term omitted: sigma*randn)."""
     b = x.shape[0]
-    if scale == 1.0:
-        e_t = apply_model(sd, x, t, conds, ratios, c_types=c_types, **kw)
-    else:
-        x_in = torch.cat([x] * 2)
-        t_in = torch.cat([t] * 2)
-        c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
-        e_u, e_c = apply_model(sd, x_in, t_in, c_in, ratios, c_types=c_types, **kw).chunk(2)
-        e_t = e_u + scale * (e_c - e_u)
+    e_u, e_c = cfg_pass(apply_model, sd, x, t, conds, unconds, scale != 1.0, ratios, c_types, **kw)
+    e_t = e_c if e_u is None else e_u + scale * (e_c - e_u)
     shape = [b, 1, 1, 1]
     a_t = torch.full(shape, float(sched["alphas"][index]))
     a_prev = torch.full(shape, float(sched["alphas_prev"][index]))
@@ -400,9 +409,7 @@ def ddim_sample_text(sd, x_T, conds, unconds, steps, scale=7.5, c_types=("text",
     for i in range(steps):
         index = steps - i - 1
         t = torch.full((b,), int(sched["timesteps"][index]), dtype=torch.long)
-        x_in, t_in = torch.cat([x] * 2), torch.cat([t] * 2)
-        c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
-        e_u, e_c = apply_model_text(sd, x_in, t_in, c_in, c_types=c_types, **kw).chunk(2)
+        e_u, e_c = cfg_pass(apply_model_text, sd, x, t, conds, unconds, True, c_types=c_types, **kw)
         e_t = e_u + scale * (e_c - e_u)
         a_t, a_prev = float(sched["alphas"][index]), float(sched["alphas_prev"][index])
         s1m = float(sched["sqrt_one_minus_alphas"][index])
@@ -419,19 +426,22 @@ def q_sample(x_start, t, noise, num_ddpm=1000):
             sch["sqrt_one_minus_alphas_cumprod"][t].reshape(shape) * noise)
 
 
+def img2img_start(x0, noise, timesteps, k, num_ddpm=1000):
+    """The img2img start, ddim.py:97-103: (x0 noised to timesteps[k] with q_sample, the first k timesteps to walk)."""
+    t0 = torch.full((x0.shape[0],), int(timesteps[k]), dtype=torch.long)
+    return q_sample(x0, t0, noise, num_ddpm), timesteps[:k]
+
+
 def ddim_sample(sd, x_T, conds, unconds, steps, scale=7.5, c_types=("text",), ratios=None, eta=0.0,
                 num_ddpm=1000, collect=False, x0=None, x0_forward_timesteps=None, x0_noise=None, **kw):
-    """DDIMSampler.sample / ddim_sampling, ddim.py:58-127 with x_T injected (eta must be 0 here).
-    img2img start (ddim.py:97-103): x0 is noised to ddim_timesteps[x0_forward_timesteps] with q_sample and only the
-    first x0_forward_timesteps DDIM timesteps are walked (x_T is ignored)."""
+    """DDIMSampler.sample / ddim_sampling, ddim.py:58-127 with x_T injected (eta must be 0 here).  With x0 the img2img
+    start from x0 and x0_noise (x_T is ignored)."""
     assert eta == 0.0
     sched = ddim_schedule(ddpm_schedule(num_ddpm)["alphas_cumprod"], steps, eta)
     ts = sched["timesteps"]
     x = x_T
     if x0 is not None:
-        t0 = torch.full((x0.shape[0],), int(ts[x0_forward_timesteps]), dtype=torch.long)
-        ts = ts[:x0_forward_timesteps]
-        x = q_sample(x0, t0, x0_noise, num_ddpm)
+        x, ts = img2img_start(x0, x0_noise, ts, x0_forward_timesteps, num_ddpm)
     trace = []
     for i, step in enumerate(np.flip(ts)):
         index = len(ts) - i - 1
@@ -452,11 +462,8 @@ def plms_sample(sd, x_T, conds, unconds, steps, scale=7.5, c_types=("text",), ra
 
     def eps(x, step):
         t = torch.full((b,), int(step), dtype=torch.long)
-        if scale == 1.0:
-            return apply_model(sd, x, t, conds, ratios, c_types=c_types, **kw)
-        c_in = [torch.cat([u, c]) for u, c in zip(unconds, conds)]
-        e_u, e_c = apply_model(sd, torch.cat([x] * 2), torch.cat([t] * 2), c_in, ratios, c_types=c_types, **kw).chunk(2)
-        return e_u + scale * (e_c - e_u)
+        e_u, e_c = cfg_pass(apply_model, sd, x, t, conds, unconds, scale != 1.0, ratios, c_types, **kw)
+        return e_c if e_u is None else e_u + scale * (e_c - e_u)
 
     def update(x, e, index):
         a_t, a_prev, s1m = float(sched["alphas"][index]), float(sched["alphas_prev"][index]), float(sched["sqrt_one_minus_alphas"][index])

@@ -182,8 +182,20 @@ def _setup(steps, n=4000, seed=0):
     return ts, x_T, x0, zs, eps
 
 
+def _masked_walk(x, eps, ts, order, x0, m, zs, trace=None):
+    """D.walk with the inpainting blend as its `after`; trace, when a list, receives x' after each blend"""
+    blend = I.blend_after(AC.numpy(), ts, x0, m, lambda i: zs[i])
+
+    def after(i, xn):
+        xn = blend(i, xn)
+        if trace is not None:
+            trace.append(xn)
+        return xn
+    return D.walk(x, eps, AC.numpy(), ts, order, after=after)
+
+
 @pytest.mark.parametrize("order", [1, 2, 3])
-def test_oracle_walk_on_the_analytic_model(order):
+def test_oracle_walk_with_the_blend_after_on_the_analytic_model(order):
     steps = 50
     ts, x_T, x0, zs, eps = _setup(steps)
     n = x_T.shape[0]
@@ -192,7 +204,7 @@ def test_oracle_walk_on_the_analytic_model(order):
     exact = D.gaussian_exact(x_T, alpha[-1], sigma[-1], np.sqrt(a0), np.sqrt(1 - a0), MU, S)
     unmasked = D.walk(x_T, eps, AC.numpy(), ts, order)
     # all generated: the unmasked walk, bit for bit, and the probability-flow solution within the solver's error
-    ones = I.dpm_walk(x_T, eps, AC.numpy(), ts, order, x0, np.ones(n), lambda i: zs[i])
+    ones = _masked_walk(x_T, eps, ts, order, x0, np.ones(n), zs)
     assert np.array_equal(ones, unmasked)
     assert np.abs(ones - exact).max() <= {1: 0.11, 2: 0.05, 3: 0.03}[order]
     # a hard mask: the elements are independent under this model, so the generated ones follow the unmasked walk exactly and
@@ -202,7 +214,7 @@ def test_oracle_walk_on_the_analytic_model(order):
     x_start = I.start(x_T, x0, m, AC.numpy(), int(ts[-1]))
     a_top = float(AC[int(ts[-1])])
     assert np.array_equal(x_start[m == 0], np.sqrt(a_top) * x0[m == 0] + np.sqrt(1 - a_top) * x_T[m == 0])
-    out = I.dpm_walk(x_start, eps, AC.numpy(), ts, order, x0, m, lambda i: zs[i], trace=trace)
+    out = _masked_walk(x_start, eps, ts, order, x0, m, zs, trace=trace)
     assert np.array_equal(out[m == 1], unmasked[m == 1])
     assert np.array_equal(out[m == 0], x0[m == 0])
     rows = I.blend_rows(AC, ts)
@@ -217,13 +229,13 @@ def test_oracle_walk_on_the_analytic_model(order):
         assert abs(kept.var() / var - 1) <= 5 * np.sqrt(2.0 / kept.size)
 
 
-def test_oracle_soft_mask_is_the_convex_mix_at_every_step():
+def test_oracle_soft_mask_blend_after_is_the_convex_mix_at_every_step():
     """A uniform soft mask m: each step's result is m x' + (1 - m) k of the unblended step from the same x."""
     steps = 20
     ts, x_T, x0, zs, eps = _setup(steps, n=500, seed=3)
     m = np.full(x_T.shape, 0.25)
     trace = []
-    I.dpm_walk(x_T, eps, AC.numpy(), ts, 1, x0, m, lambda i: zs[i], trace=trace)
+    _masked_walk(x_T, eps, ts, 1, x0, m, zs, trace=trace)
     rows = I.blend_rows(AC, ts)
     x = x_T
     for k, i in enumerate(range(len(ts) - 1, -1, -1)):
