@@ -59,6 +59,18 @@ int vdb_ddim_cfg_step(const float* e_uncond, const float* e_cond, const float* x
  * hist / x_next, n <= 0, a pointer not 16-byte aligned, or hist overlapping x, x_next, x_next_dup or pred_x0. */
 int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
                        float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n, void* stream);
+/* ---- CFG mix + one stochastic DPM-Solver++ (SDE) update — DPMSolverSDESampler, lib/model_zoo/dpm_solver.py ---------------------
+ * vdb_dpmpp_cfg_step with the noise column of the row: coef rows of 8 {P, Q, A, B, C, D, N, 0} and, in this op order,
+ *   x_next = (((A*x + B*x0) + C*h1) + D*h2) + N*z,
+ * fp32 with explicit round-to-nearest.  z = noise (fp32, n elements) when non-NULL, else four normals per element quad from
+ * Philox4x32-10 at counter (quad, *step_idx, 0x73646573 "sdes", 0) under the 64-bit key *seed (two Box-Muller pairs,
+ * u = (b + 0.5) 2^-32, as vdb_inpaint_blend_f32).  A C, D or N term whose coefficient is exactly 0 is skipped: at N == 0 nothing
+ * is drawn or read and the result is vdb_dpmpp_cfg_step's bit for bit.  VDB_ERR_INVALID before any launch: the refusals of
+ * vdb_dpmpp_cfg_step, neither seed nor noise, a seed not 8-byte aligned, noise not 16-byte aligned, or noise overlapping hist,
+ * x_next, x_next_dup or pred_x0. */
+int vdb_dpmpp_sde_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
+                           float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n,
+                           const unsigned long long* seed, const float* noise, void* stream);
 /* ---- inpainting: blended latent diffusion — lib/model_zoo/inpaint.py (an addition: the reference has no inpainting; the
  * semantics are specified in that module's docstring) ------------------------------------------------------------------------------
  * vdb_inpaint_blend_f32, after each sampler step: x, x0, noise fp32 NHWC [bs, hw, c]; mask fp32 [bs, hw] (mask_per_item != 0) or

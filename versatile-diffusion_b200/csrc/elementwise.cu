@@ -79,14 +79,33 @@ __global__ void ddim_cfg_step_kernel(const float* __restrict__ e_uncond, const f
 //   x'  = ((A*x + B*x0) [+ C*h1]) [+ D*h2]           h1 = hist slot (idx+1) % 3, h2 = slot (idx+2) % 3
 // A bracketed term is skipped (and its slot not read) when its coefficient is exactly 0: the ring holds no data yet at the
 // first steps.  The slot pointers are 16-byte aligned only when n % 4 == 0, so the ring is accessed by vectors only then.
+//
+// The stochastic form (DPMSolverSDESampler) adds column 6 of the row, N, and one Gaussian term:
+//   x'  = (((A*x + B*x0) [+ C*h1]) [+ D*h2]) [+ N*z]
+// z is the explicit noise when given, else four normals per element quad from philox_normals at counter (quad, idx, "sdes", 0)
+// under the 64-bit key *seed.  At N == 0 the term is skipped and nothing is drawn or read, so such a row gives the bits of the
+// deterministic kernel, which is the same body without the noise term.
 // ---------------------------------------------------------------------------------------------
-__global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const float* __restrict__ e_cond,
-                                      const float* x, const float* __restrict__ coef, const int* __restrict__ step_idx,
-                                      float scale, float* __restrict__ hist, float* x_next, float* __restrict__ x_next_dup,
-                                      float* __restrict__ pred_x0, long long n) {
+constexpr unsigned kSdeTag = 0x73646573u;       // "sdes": distinct from "inpt", "rgns" and "text"
+
+__device__ __forceinline__ void philox_normals(unsigned long long key, unsigned quad, int step, unsigned tag, float z[4]);
+
+template <bool kNoise>
+__device__ __forceinline__ void dpmpp_cfg_step_body(const float* __restrict__ e_uncond, const float* __restrict__ e_cond,
+                                                    const float* x, const float* __restrict__ coef,
+                                                    const int* __restrict__ step_idx, float scale, float* __restrict__ hist,
+                                                    float* x_next, float* __restrict__ x_next_dup, float* __restrict__ pred_x0,
+                                                    long long n, const unsigned long long* __restrict__ seed,
+                                                    const float* __restrict__ noise) {
   const int idx = *step_idx;
   const float* c = coef + 8 * idx;
   const float P = c[0], Q = c[1], A = c[2], B = c[3], C = c[4], D = c[5];
+  float N = 0.f;
+  unsigned long long key = 0ull;
+  if (kNoise) {
+    N = c[6];
+    if (N != 0.f && !noise) key = *seed;
+  }
   float* h0 = hist + static_cast<long long>(idx % 3) * n;
   const float* h1 = hist + static_cast<long long>((idx + 1) % 3) * n;
   const float* h2 = hist + static_cast<long long>((idx + 2) % 3) * n;
@@ -117,6 +136,17 @@ __global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const 
           if (D != 0.f) a2[q] = h2[i + q];
         }
     }
+    float zv[4] = {0.f, 0.f, 0.f, 0.f};
+    if (kNoise && N != 0.f) {
+      if (!noise) {
+        philox_normals(key, static_cast<unsigned>(i >> 2), idx, kSdeTag, zv);
+      } else if (full) {
+        *reinterpret_cast<float4*>(zv) = __ldg(reinterpret_cast<const float4*>(noise + i));
+      } else {
+        for (int q = 0; q < 4; ++q)
+          if (i + q < n) zv[q] = noise[i + q];
+      }
+    }
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       float e = ec[q];
@@ -125,6 +155,7 @@ __global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const 
       float v = __fadd_rn(__fmul_rn(A, xv[q]), __fmul_rn(B, px0));
       if (C != 0.f) v = __fadd_rn(v, __fmul_rn(C, a1[q]));
       if (D != 0.f) v = __fadd_rn(v, __fmul_rn(D, a2[q]));
+      if (kNoise && N != 0.f) v = __fadd_rn(v, __fmul_rn(N, zv[q]));
       xn[q] = v;
       p0[q] = px0;
     }
@@ -147,6 +178,21 @@ __global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const 
         if (i + q < n) h0[i + q] = p0[q];
     }
   }
+}
+
+__global__ void dpmpp_cfg_step_kernel(const float* __restrict__ e_uncond, const float* __restrict__ e_cond,
+                                      const float* x, const float* __restrict__ coef, const int* __restrict__ step_idx,
+                                      float scale, float* __restrict__ hist, float* x_next, float* __restrict__ x_next_dup,
+                                      float* __restrict__ pred_x0, long long n) {
+  dpmpp_cfg_step_body<false>(e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n, nullptr, nullptr);
+}
+
+__global__ void dpmpp_sde_cfg_step_kernel(const float* __restrict__ e_uncond, const float* __restrict__ e_cond,
+                                          const float* x, const float* __restrict__ coef, const int* __restrict__ step_idx,
+                                          float scale, float* __restrict__ hist, float* x_next, float* __restrict__ x_next_dup,
+                                          float* __restrict__ pred_x0, long long n, const unsigned long long* __restrict__ seed,
+                                          const float* __restrict__ noise) {
+  dpmpp_cfg_step_body<true>(e_uncond, e_cond, x, coef, step_idx, scale, hist, x_next, x_next_dup, pred_x0, n, seed, noise);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2015,6 +2061,30 @@ int vdb_dpmpp_cfg_step(const float* e_uncond, const float* e_cond, const float* 
   const int threads = 256;
   return launch(dpmpp_cfg_step_kernel, ew_blocks((n + 3) / 4, threads), threads, 0, stream, e_uncond, e_cond, x, coef, step_idx,
                 scale, hist, x_next, x_next_dup, pred_x0, n);
+}
+
+int vdb_dpmpp_sde_cfg_step(const float* e_uncond, const float* e_cond, const float* x, const float* coef, const int* step_idx,
+                           float scale, float* hist, float* x_next, float* x_next_dup, float* pred_x0, long long n,
+                           const unsigned long long* seed, const float* noise, void* stream) {
+  if (!e_cond || !x || !coef || !step_idx || !hist || !x_next || n <= 0)
+    return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: null/empty argument");
+  if (!seed && !noise) return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: null seed and noise (one is needed)");
+  if ((reinterpret_cast<uintptr_t>(e_cond) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(x_next) |
+       reinterpret_cast<uintptr_t>(e_uncond) | reinterpret_cast<uintptr_t>(hist) | reinterpret_cast<uintptr_t>(pred_x0) |
+       reinterpret_cast<uintptr_t>(x_next_dup) | reinterpret_cast<uintptr_t>(noise)) & 15)
+    return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: pointers must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(seed) & 7) return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: seed must be 8-byte aligned");
+  for (const float* p : {x, static_cast<const float*>(x_next), static_cast<const float*>(x_next_dup),
+                         static_cast<const float*>(pred_x0)})
+    if (overlaps(hist, 3 * n, p, n))
+      return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: hist overlaps x, x_next, x_next_dup or pred_x0");
+  // the noise is read through the read-only path while the outputs are written: it must not share a byte with them
+  if (overlaps(noise, n, hist, 3 * n) || overlaps(noise, n, x_next, n) || overlaps(noise, n, x_next_dup, n) ||
+      overlaps(noise, n, pred_x0, n))
+    return set_error(VDB_ERR_INVALID, "dpmpp_sde_cfg_step: noise overlaps hist, x_next, x_next_dup or pred_x0");
+  const int threads = 256;
+  return launch(dpmpp_sde_cfg_step_kernel, ew_blocks((n + 3) / 4, threads), threads, 0, stream, e_uncond, e_cond, x, coef,
+                step_idx, scale, hist, x_next, x_next_dup, pred_x0, n, seed, noise);
 }
 
 int vdb_inpaint_blend_f32(float* x, float* x_dup, const float* x0, const float* mask, int mask_per_item, const float* table,

@@ -13,8 +13,8 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-from .diffusion_utils import (make_ddim_sampling_parameters, make_ddim_timesteps, noise_like, pack_epoch, require_cuda,
-                              to_numpy)
+from .diffusion_utils import (GRIDS, make_ddim_sampling_parameters, make_ddim_timesteps, noise_like, pack_epoch,
+                              require_cuda, to_numpy)
 
 
 def _ops():
@@ -141,6 +141,10 @@ class DDIMSampler(object):
         self.ddpm_num_timesteps = model.num_timesteps
         self.schedule = schedule
         self.use_cuda_graph = kwargs.get("use_cuda_graph", True)
+        # the time grid every walk of this sampler takes (make_ddim_timesteps): 'uniform' (DDIM's), 'trailing' or 'karras'
+        self.grid = kwargs.get("grid", "uniform")
+        if self.grid not in GRIDS:
+            raise ValueError(f"grid must be one of {GRIDS}, got {self.grid!r}")
 
     def register_buffer(self, name, attr):
         # the reference forces .to('cuda') here (ddim.py:17-21); follow the model's device instead
@@ -148,10 +152,11 @@ class DDIMSampler(object):
             attr = attr.to(torch.device(self.model.device))
         setattr(self, name, attr)
 
-    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=True):
-        """reference ddim.py:23-56 (same fp64/fp32 dtype walk)."""
-        self.ddim_timesteps = make_ddim_timesteps(ddim_discr_method=ddim_discretize, num_ddim_timesteps=ddim_num_steps,
-                                                  num_ddpm_timesteps=self.ddpm_num_timesteps, verbose=verbose)
+    def make_schedule(self, ddim_num_steps, ddim_discretize=None, ddim_eta=0., verbose=True):
+        """reference ddim.py:23-56 (same fp64/fp32 dtype walk).  ddim_discretize defaults to the sampler's grid."""
+        self.ddim_timesteps = make_ddim_timesteps(ddim_discr_method=ddim_discretize or self.grid,
+                                                  num_ddim_timesteps=ddim_num_steps, num_ddpm_timesteps=self.ddpm_num_timesteps,
+                                                  verbose=verbose, alphas_cumprod=self.model.alphas_cumprod)
         alphas_cumprod = self.model.alphas_cumprod
         assert alphas_cumprod.shape[0] == self.ddpm_num_timesteps, 'alphas have to be defined for each timestep'
         to_torch = lambda x: x.clone().detach().to(torch.float32).to(self.model.device)

@@ -26,16 +26,43 @@ def make_beta_schedule(schedule, n_timestep, linear_start=1e-4, linear_end=2e-2,
     return betas.numpy() if isinstance(betas, torch.Tensor) else np.asarray(betas)
 
 
-def make_ddim_timesteps(ddim_discr_method, num_ddim_timesteps, num_ddpm_timesteps, verbose=True):
-    """reference :32-46 — uniform: range(0, T, T // S) + 1."""
+GRIDS = ("uniform", "trailing", "karras")     # the samplers' `grid` option
+
+
+def make_ddim_timesteps(ddim_discr_method, num_ddim_timesteps, num_ddpm_timesteps, verbose=True, alphas_cumprod=None):
+    """Ascending integer timesteps of the walk (T = num_ddpm_timesteps, S = num_ddim_timesteps); step i goes from t_i to
+    t_{i-1}, step 0 to ac[0].
+      - uniform (reference :32-46): range(0, T, T // S) + 1.  The walk starts below T - 1: at 951 for 20 steps.
+      - quad (reference): linspace(0, sqrt(0.8 T), S)^2 + 1.
+      - trailing (diffusers' timestep_spacing="trailing"): round(arange(T, 0, -T / S)) - 1, S points, so the walk starts at T - 1.
+      - karras (Karras et al. 2022, rho = 7): S sigmas from sigma(T - 1) down to sigma(1), sigma(t) = sqrt((1 - ac[t]) / ac[t])
+        in fp64 from the fp32 alphas_cumprod (so it needs them), evenly spaced in sigma^(1/7); each is mapped to t by linear
+        interpolation of t over log sigma(t) (diffusers' _sigma_to_t), rounded to the nearest integer, repeats dropped.  The
+        grid ends at t = 1 as uniform does, so step 0 never has a zero step.  Where the low sigmas lie closer than one timestep
+        the grid has fewer than S points and the walk takes fewer steps: 98 at S = 100 on the linear schedule."""
     if ddim_discr_method == "uniform":
         c = num_ddpm_timesteps // num_ddim_timesteps
-        ddim_timesteps = np.asarray(list(range(0, num_ddpm_timesteps, c)))
+        steps_out = np.asarray(list(range(0, num_ddpm_timesteps, c))) + 1
     elif ddim_discr_method == "quad":
-        ddim_timesteps = ((np.linspace(0, np.sqrt(num_ddpm_timesteps * .8), num_ddim_timesteps)) ** 2).astype(int)
+        steps_out = ((np.linspace(0, np.sqrt(num_ddpm_timesteps * .8), num_ddim_timesteps)) ** 2).astype(int) + 1
+    elif ddim_discr_method == "trailing":
+        # np.arange's length is computed in floating point and is S + 1 for some S (61, 103, ...), the extra point at about 0:
+        # the grid is its first S points
+        ts = np.round(np.arange(num_ddpm_timesteps, 0, -num_ddpm_timesteps / num_ddim_timesteps))[:num_ddim_timesteps]
+        steps_out = np.sort(ts.astype(np.int64) - 1)
+    elif ddim_discr_method == "karras":
+        if num_ddim_timesteps < 2:
+            raise ValueError(f"the karras grid needs at least 2 steps, got {num_ddim_timesteps}")
+        if alphas_cumprod is None:
+            raise ValueError("the karras grid needs the model's alphas_cumprod")
+        ac = to_numpy(alphas_cumprod, np.float32).astype(np.float64)
+        sigma = np.sqrt((1.0 - ac) / ac)
+        lo, hi = sigma[1] ** (1 / 7), sigma[num_ddpm_timesteps - 1] ** (1 / 7)
+        j = np.arange(num_ddim_timesteps, dtype=np.float64) / (num_ddim_timesteps - 1)
+        t = np.interp(np.log((hi + j * (lo - hi)) ** 7), np.log(sigma), np.arange(num_ddpm_timesteps, dtype=np.float64))
+        steps_out = np.unique(np.rint(t).astype(np.int64))
     else:
         raise NotImplementedError(f'There is no ddim discretization method called "{ddim_discr_method}"')
-    steps_out = ddim_timesteps + 1
     if verbose:
         print(f"Selected timesteps for ddim sampler: {steps_out}")
     return steps_out

@@ -30,10 +30,11 @@ sample_multicontext and DPMSolverSampler (same methods; its targets are DDIM's a
     trajectory, never re-noised x0, and no noise is drawn.  Slot 0 is x0, so the kept region of the result is x0 bit for bit.
   - Without 'inversion' nothing changes: the same launches, the same bits, the same graph key.
 
-Mask (diffedit_mask(net, x0, src, tgt, steps=50, strength=0.5, n_draws=10, ratio=3.0), the paper's rule as diffusers'
-StableDiffusionDiffEditPipeline.generate_mask applies it).  src / tgt: a context dict, or a list of them (multi-context); every
-context of both sides has the batch bs (ValueError otherwise, before any device work).
-  - k = int(steps * strength), t_m = t_{k-1}: the level of slot k, where edit's walk starts.  D = n_draws draws
+Mask (diffedit_mask(net, x0, src, tgt, steps=50, strength=0.5, n_draws=10, ratio=3.0, grid='uniform'), the paper's rule as
+diffusers' StableDiffusionDiffEditPipeline.generate_mask applies it).  src / tgt: a context dict, or a list of them (multi-context);
+every context of both sides has the batch bs (ValueError otherwise, before any device work).
+  - k = int(steps * strength), t_m = t_{k-1} on the time grid `grid` (edit passes the sampler's): the level of slot k, where
+    edit's walk starts.  D = n_draws draws
     x_d = sqrt(ac[t_m]) x0 + sqrt(1 - ac[t_m]) z_d, z_d from torch.randn (torch.manual_seed fixes the mask).
   - E_src, E_tgt: the CFG-mixed eps of each side at its own scale; one UNet call per side on a batch of D * bs (doubled under
     CFG), draw d of image b at row d * bs + b.
@@ -166,9 +167,11 @@ def _side_contexts(c_infos, scale, D, device):
 
 
 @torch.no_grad()
-def diffedit_mask(net, x0, src, tgt, steps=50, strength=0.5, n_draws=10, ratio=3.0):
-    """DiffEdit's {0, 1} latent mask [bs, 1, H, W] (1 = edit) from the disagreement of the src and tgt noise predictions."""
-    n = len(make_ddim_timesteps('uniform', steps, net.num_timesteps, verbose=False))
+def diffedit_mask(net, x0, src, tgt, steps=50, strength=0.5, n_draws=10, ratio=3.0, grid='uniform'):
+    """DiffEdit's {0, 1} latent mask [bs, 1, H, W] (1 = edit) from the disagreement of the src and tgt noise predictions, at the
+    level of slot k of the inversion over `grid` (the sampler's time grid)."""
+    ts = make_ddim_timesteps(grid, steps, net.num_timesteps, verbose=False, alphas_cumprod=net.alphas_cumprod)
+    n = len(ts)
     k = int(steps * strength)
     if not 1 <= k <= n:
         raise ValueError(f"strength {strength} at {steps} steps gives k = {k}: need 1 <= k <= {n}")
@@ -188,7 +191,7 @@ def diffedit_mask(net, x0, src, tgt, steps=50, strength=0.5, n_draws=10, ratio=3
     ops = _ops()
     device = torch.device(net.device)
     _, C, H, W = x0.shape
-    t_m = int(make_ddim_timesteps('uniform', steps, net.num_timesteps, verbose=False)[k - 1])
+    t_m = int(ts[k - 1])
     ac = float(net.alphas_cumprod[t_m])
     z = torch.randn(D * bs, C, H, W)                      # torch's CPU generator: torch.manual_seed fixes the mask
     x0r = x0.to(device=device, dtype=torch.float32).expand(bs, C, H, W).repeat(D, 1, 1, 1).contiguous()
@@ -226,7 +229,7 @@ def edit(net, sampler, image, src, tgt, steps=50, strength=0.5, mask='auto', n_d
     if isinstance(mask, str):
         if mask != 'auto':
             raise ValueError(f"mask: 'auto', a tensor or None, got {mask!r}")
-        mask = diffedit_mask(net, x0, src, tgt, steps=steps, strength=strength, n_draws=n_draws)
+        mask = diffedit_mask(net, x0, src, tgt, steps=steps, strength=strength, n_draws=n_draws, grid=sampler.grid)
     x_info = {'type': 'image', 'inversion': inv}
     if mask is not None:
         x_info['inpaint_mask'] = mask

@@ -29,7 +29,7 @@ class PLMSSampler(DDIMSampler):
         kwargs.setdefault("use_cuda_graph", False)
         super().__init__(model, schedule=schedule, **kwargs)
 
-    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=True):
+    def make_schedule(self, ddim_num_steps, ddim_discretize=None, ddim_eta=0., verbose=True):
         if ddim_eta != 0:
             raise ValueError('ddim_eta must be 0 for PLMS')
         super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)

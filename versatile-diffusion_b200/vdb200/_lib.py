@@ -28,6 +28,7 @@ SIGNATURES = {
     "vdb_num_sms": (i, []),
     "vdb_ddim_cfg_step": (i, [p, p, p, p, p, p, f, f, p, p, p, ll, p]),
     "vdb_dpmpp_cfg_step": (i, [p, p, p, p, p, f, p, p, p, p, ll, p]),
+    "vdb_dpmpp_sde_cfg_step": (i, [p, p, p, p, p, f, p, p, p, p, ll, p, p, p]),
     "vdb_inpaint_blend_f32": (i, [p, p, p, p, i, p, p, p, p, i, ll, i, p]),
     "vdb_inpaint_noise_f32": (i, [p, p, ll, p, p]),
     "vdb_mask_to_latent": (i, [p, i, i, i, p, p]),
