@@ -7,7 +7,7 @@ the blend against the trajectory as its `after`), and DiffEdit's mask rule.
 import numpy as np
 import torch
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import panorama_oracle as P
 from . import vd_oracle as O
 
@@ -27,9 +27,11 @@ def _eps_fn(sd, conds, unconds, scale, c_types, ratios, kw):
     return eps
 
 
-def invert(sd, x0, conds, unconds, steps, k=None, scale=1.0, c_types=("text",), ratios=None, num_ddpm=1000, **kw):
-    """The inversion walk in fp64 (eps from the fp32 UNet restatement) -> trajectory [k+1, bs, C, H, W] (slot 0 = x0)."""
-    sched = O.ddim_schedule(O.ddpm_schedule(num_ddpm)["alphas_cumprod"], steps)
+def invert(sd, x0, conds, unconds, steps, k=None, scale=1.0, c_types=("text",), ratios=None, num_ddpm=1000, grid_name="uniform",
+           **kw):
+    """The inversion walk in fp64 (eps from the fp32 UNet restatement) on grid grid_name -> trajectory [k+1, bs, C, H, W]
+    (slot 0 = x0)."""
+    sched = G.schedule(grid_name, steps, 0.0, num_ddpm)[1]
     ts = sched["timesteps"]
     k = len(ts) if k is None else k
     rows = inversion_rows(sched["alphas"], sched["alphas_prev"], k)
@@ -43,11 +45,12 @@ def invert(sd, x0, conds, unconds, steps, k=None, scale=1.0, c_types=("text",), 
 
 
 def sample(sd, traj, conds, unconds, steps, mask=None, sampler="ddim", order=2, scale=7.5, c_types=("text",), ratios=None,
-           num_ddpm=1000, **kw):
+           num_ddpm=1000, grid_name="uniform", eta=0.0, noise=None, **kw):
     """The walk from slot k = len(traj) - 1 over grid points k-1 ... 0, with x <- m x + (1 - m) slot_i after step i when a
-    latent mask [bs or 1, 1, H, W] is given (1 = regenerate)."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    sched = O.ddim_schedule(ac, steps)
+    latent mask [bs or 1, 1, H, W] is given (1 = regenerate).  grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature)."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
     k = traj.shape[0] - 1
     ts = sched["timesteps"][:k]
     m = None if mask is None else mask.double()
@@ -55,13 +58,17 @@ def sample(sd, traj, conds, unconds, steps, mask=None, sampler="ddim", order=2, 
     x = traj[k].double()
     if sampler == "ddim":
         for i in range(k - 1, -1, -1):
-            x = P.ddim_update(x, eps(x, ts[i]), float(sched["alphas"][i]), float(sched["alphas_prev"][i]))
+            a_t, a_prev = float(sched["alphas"][i]), float(sched["alphas_prev"][i])
+            if eta == 0:
+                x = P.ddim_update(x, eps(x, ts[i]), a_t, a_prev)
+            else:
+                x = P.ddim_update(x, eps(x, ts[i]), a_t, a_prev, float(sched["sigmas"][i]), torch.as_tensor(noise(i)).double())
             if m is not None:
                 x = m * x + (1 - m) * traj[i].double()
         return x
     mm, slots = None if m is None else m.numpy(), traj.double().numpy()
     after = None if mm is None else lambda i, xn: mm * xn + (1 - mm) * slots[i]
-    out = D.walk(x.numpy(), lambda xv, i: eps(torch.from_numpy(xv), ts[i]), ac.numpy(), ts, order, after=after)
+    out = G.dpm_walk(x.numpy(), lambda xv, i: eps(torch.from_numpy(xv), ts[i]), ac.numpy(), ts, order, eta, noise, after=after)
     return torch.from_numpy(out)
 
 

@@ -11,7 +11,7 @@ device table: the rows come from the schedule here.
 import numpy as np
 import torch
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import vd_oracle as O
 
 
@@ -43,12 +43,13 @@ def blend_after(alphas_cumprod, timesteps, x0, mask, noise_fn):
 
 
 def sample(sd, x_T, conds, unconds, steps, x0, mask, noise_fn, sampler="ddim", order=2, scale=7.5, c_types=("text",),
-           ratios=None, x0_forward_timesteps=None, x0_noise=None, num_ddpm=1000, **kw):
+           ratios=None, x0_forward_timesteps=None, x0_noise=None, num_ddpm=1000, grid_name="uniform", eta=0.0, noise=None, **kw):
     """The masked DDIMSampler / DPMSolverSampler walk on the UNet restatement.  x_T, x0 [bs or 1, C, H, W] and the latent mask
     [bs or 1, 1, H, W] as torch tensors; noise_fn(i) -> z_i, a [bs, C, H, W] tensor.  With x0_forward_timesteps the img2img start
-    (x0 noised with x0_noise), else the full walk from x_T with the masked start."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    sched = O.ddim_schedule(ac, steps)
+    (x0 noised with x0_noise), else the full walk from x_T with the masked start.  grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature)."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
     ts = sched["timesteps"]
     x0, mask = x0.float(), mask.float()
     if x0_forward_timesteps is not None:
@@ -59,7 +60,8 @@ def sample(sd, x_T, conds, unconds, steps, x0, mask, noise_fn, sampler="ddim", o
         rows = torch.from_numpy(blend_rows(ac.numpy(), ts).astype(np.float32))
         for i in range(len(ts) - 1, -1, -1):
             t = torch.full((x.shape[0],), int(ts[i]), dtype=torch.long)
-            x, _, _ = O.p_sample_ddim(sd, x, conds, unconds, t, i, sched, scale, c_types, ratios, **kw)
+            z = None if eta == 0 else torch.as_tensor(noise(i)).float()
+            x, _, _ = O.p_sample_ddim(sd, x, conds, unconds, t, i, sched, scale, c_types, ratios, noise=z, **kw)
             x = blend(x, x0, mask, noise_fn(i).float(), rows[i, 0], rows[i, 1])
         return x
 
@@ -69,5 +71,6 @@ def sample(sd, x_T, conds, unconds, steps, x0, mask, noise_fn, sampler="ddim", o
                               **kw)
         return (e_c if e_u is None else e_u + scale * (e_c - e_u)).double().numpy()
 
-    out = D.walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, after=blend_after(ac.numpy(), ts, x0, mask, noise_fn))
+    out = G.dpm_walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, eta, noise,
+                     after=blend_after(ac.numpy(), ts, x0, mask, noise_fn))
     return torch.from_numpy(out).float()

@@ -14,7 +14,7 @@ with the far edge (non-circular), or 0, s, ..., W - s with columns read mod W (c
 import numpy as np
 import torch
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import inpaint_oracle as I
 from . import vd_oracle as O
 
@@ -53,9 +53,12 @@ def average(parts, wins, h, w, shape):
     return acc / cnt
 
 
-def ddim_update(x, e, a_t, a_prev):
-    """DDIM at eta 0: x' = sqrt(a') (x - sqrt(1 - a) e) / sqrt(a) + sqrt(1 - a') e"""
-    return np.sqrt(a_prev) * (x - np.sqrt(1.0 - a_t) * e) / np.sqrt(a_t) + np.sqrt(1.0 - a_prev) * e
+def ddim_update(x, e, a_t, a_prev, sigma=0.0, z=None):
+    """DDIM at eta 0: x' = sqrt(a') (x - sqrt(1 - a) e) / sqrt(a) + sqrt(1 - a') e.  With z (the step's standard normal times
+    the temperature) the stochastic step of ddim.py:159-171: x' = sqrt(a') x0 + sqrt(1 - a' - sigma^2) e + sigma z."""
+    if z is None:
+        return np.sqrt(a_prev) * (x - np.sqrt(1.0 - a_t) * e) / np.sqrt(a_t) + np.sqrt(1.0 - a_prev) * e
+    return np.sqrt(a_prev) * (x - np.sqrt(1.0 - a_t) * e) / np.sqrt(a_t) + np.sqrt(1.0 - a_prev - sigma ** 2) * e + sigma * z
 
 
 def paper_step(x, eps_fn, wins, h, w, a_t, a_prev):
@@ -86,12 +89,17 @@ def _windowed_eps(sd, x, t, conds, unconds, wins, h, w, scale, c_types, ratios, 
 
 
 def sample(sd, x_T, conds, unconds, steps, size, stride, circular=False, sampler="ddim", order=2, scale=7.5, c_types=("text",),
-           ratios=None, x0=None, mask=None, noise_fn=None, x0_forward_timesteps=None, x0_noise=None, num_ddpm=1000, **kw):
+           ratios=None, x0=None, mask=None, noise_fn=None, x0_forward_timesteps=None, x0_noise=None, num_ddpm=1000,
+           grid_name="uniform", eta=0.0, noise=None, **kw):
     """The windowed DDIMSampler / DPMSolverSampler walk on the UNet restatement.  x_T [bs, C, H, W] torch; with mask (latent,
     [bs or 1, 1, H, W]) the inpainting blend of inpaint_oracle after every step, noise_fn(i) -> z_i [bs, C, H, W]; with
-    x0_forward_timesteps the img2img start (x0 noised with x0_noise), else the full walk from x_T (masked start with a mask)."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    sched = O.ddim_schedule(ac, steps)
+    x0_forward_timesteps the img2img start (x0 noised with x0_noise), else the full walk from x_T (masked start with a mask).
+    grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature).  The noise is the canvas's: DDIM at eta > 0 averages the windows' eps and takes one canvas step
+    (lib/model_zoo/panorama.py and regions.py: the window walk is the region walk, whose step is the unchanged update on the
+    averaged eps)."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
     ts = sched["timesteps"]
     H, W = x_T.shape[-2:]
     h, w, wins = windows(H, W, size, stride, circular)
@@ -104,13 +112,18 @@ def sample(sd, x_T, conds, unconds, steps, size, stride, circular=False, sampler
     if sampler == "ddim":
         rows = torch.from_numpy(I.blend_rows(ac.numpy(), ts).astype(np.float32))
         for i in range(len(ts) - 1, -1, -1):
-            bs = x.shape[0]
-            xc = torch.cat([torch.from_numpy(crop(x.numpy(), oy, ox, h, w).copy()) for oy, ox in wins])
-            t = torch.full((xc.shape[0],), int(ts[i]), dtype=torch.long)
-            rep = lambda cs: [c.repeat(len(wins), 1, 1) for c in cs]
-            xp, _, _ = O.p_sample_ddim(sd, xc, rep(conds), rep(unconds), t, i, sched, scale, c_types, ratios, **kw)
-            xp = xp.double().numpy().reshape(len(wins), bs, *xp.shape[1:])
-            x = torch.from_numpy(average(list(xp), wins, h, w, x.shape)).float()
+            if eta == 0:
+                bs = x.shape[0]
+                xc = torch.cat([torch.from_numpy(crop(x.numpy(), oy, ox, h, w).copy()) for oy, ox in wins])
+                t = torch.full((xc.shape[0],), int(ts[i]), dtype=torch.long)
+                rep = lambda cs: [c.repeat(len(wins), 1, 1) for c in cs]
+                xp, _, _ = O.p_sample_ddim(sd, xc, rep(conds), rep(unconds), t, i, sched, scale, c_types, ratios, **kw)
+                xp = xp.double().numpy().reshape(len(wins), bs, *xp.shape[1:])
+                x = torch.from_numpy(average(list(xp), wins, h, w, x.shape)).float()
+            else:
+                e = _windowed_eps(sd, x, ts[i], conds, unconds, wins, h, w, scale, c_types, ratios, kw)
+                x = torch.from_numpy(ddim_update(x.double().numpy(), e, float(sched["alphas"][i]), float(sched["alphas_prev"][i]),
+                                                 float(sched["sigmas"][i]), np.asarray(noise(i), dtype=np.float64))).float()
             if mask is not None:
                 x = I.blend(x, x0.float(), mask.float(), noise_fn(i).float(), rows[i, 0], rows[i, 1])
         return x
@@ -120,5 +133,5 @@ def sample(sd, x_T, conds, unconds, steps, size, stride, circular=False, sampler
                              ratios, kw)
 
     after = None if mask is None else I.blend_after(ac.numpy(), ts, x0, mask, noise_fn)
-    out = D.walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, after=after)
+    out = G.dpm_walk(x.double().numpy(), eps_fn, ac.numpy(), ts, order, eta, noise, after=after)
     return torch.from_numpy(out).float()

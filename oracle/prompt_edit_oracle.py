@@ -3,7 +3,7 @@
 Restates lib/model_zoo/prompt_edit.py as P2P computes it: on materialised attention probabilities of vd_oracle.apply_model (the
 fp32 UNet, with an attention hook on the text context's SpatialTransformers), with the mapper einsum, the equalizer
 product, the alpha mix, the self-map replacement, and LocalBlend with max_pool2d / nearest interpolate.  It never forms the
-factored A * ctx contexts, so comparing against it checks the factoring too.  The walk is DDIM or DPM-Solver++ (orders 1 and 2,
+factored A * ctx contexts, so comparing against it checks the factoring too.  The walk is DDIM or DPM-Solver++ (orders 1 to 3,
 dpm_solver_oracle.walk with the local blend as its `after`) in fp64.
 """
 import math
@@ -11,7 +11,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import panorama_oracle as P
 from . import vd_oracle as O
 
@@ -81,25 +81,32 @@ def _eps_fn(sd, ctl, conds, unconds, scale, c_types, ratios, kw):
 
 
 def sample(sd, ctl, x_T, conds, unconds, steps, sampler="ddim", order=2, scale=7.5, c_types=("text",), ratios=None,
-           num_ddpm=1000, **kw):
-    """The edited walk from x_T [n, C, H, W] (fp64 state, fp32 UNet) with the local blend after every step."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    sched = O.ddim_schedule(ac, steps)
-    ts = sched["timesteps"][:steps]         # both walks visit grid points steps-1 ... 0, also when the grid has one more
+           num_ddpm=1000, grid_name="uniform", eta=0.0, noise=None, **kw):
+    """The edited walk from x_T [n, C, H, W] (fp64 state, fp32 UNet) with the local blend after every step, over the first
+    `steps` grid points (so over steps - 1 ... 0 also when a uniform grid has one more; a Karras grid can have fewer).  ctl.T
+    is the walk's length.  grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature)."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
+    ts = sched["timesteps"][:steps]
+    n = len(ts)
     eps = _eps_fn(sd, ctl, conds, unconds, scale, c_types, ratios, kw)
     x = x_T.double()
     if sampler == "ddim":
-        for k, i in enumerate(range(steps - 1, -1, -1)):
+        for k, i in enumerate(range(n - 1, -1, -1)):
             ctl.i = k
-            x = P.ddim_update(x, eps(x, ts[i]), float(sched["alphas"][i]), float(sched["alphas_prev"][i]))
+            a_t, a_prev = float(sched["alphas"][i]), float(sched["alphas_prev"][i])
+            if eta == 0:
+                x = P.ddim_update(x, eps(x, ts[i]), a_t, a_prev)
+            else:
+                x = P.ddim_update(x, eps(x, ts[i]), a_t, a_prev, float(sched["sigmas"][i]), torch.as_tensor(noise(i)).double())
             x = ctl.blend(x)
         return x
-    if order > 2:
-        raise NotImplementedError("order 3 is not restated here")
 
     def eps_fn(xv, i):
-        ctl.i = steps - 1 - i
+        ctl.i = n - 1 - i
         return eps(torch.from_numpy(xv), ts[i])
 
-    out = D.walk(x.numpy(), eps_fn, ac.numpy(), ts, order, after=lambda i, xn: ctl.blend(torch.from_numpy(xn)).numpy())
+    out = G.dpm_walk(x.numpy(), eps_fn, ac.numpy(), ts, order, eta, noise,
+                     after=lambda i, xn: ctl.blend(torch.from_numpy(xn)).numpy())
     return torch.from_numpy(out)

@@ -12,7 +12,7 @@ reduce to the plain (windowed) walk.
 import numpy as np
 import torch
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import inpaint_oracle as I
 from . import panorama_oracle as P
 from . import vd_oracle as O
@@ -90,14 +90,16 @@ def _views_eps(sd, xs, t, conds, unconds, region_conds, wins, h, w, scale, c_typ
 
 def sample(sd, x_T, conds, unconds, region_conds, masks, steps, size=None, stride=8, circular=False, sampler="ddim", order=2,
            scale=7.5, c_types=("text",), ratios=None, bootstrap_steps=0, backgrounds=None, pick_fn=None, z_fn=None, x0=None,
-           mask=None, noise_fn=None, num_ddpm=1000, **kw):
+           mask=None, noise_fn=None, num_ddpm=1000, grid_name="uniform", eta=0.0, noise=None, **kw):
     """The region DDIMSampler / DPMSolverSampler walk on the UNet restatement, from x_T [bs, C, H, W] (torch).  region_conds[r]:
     region r + 1's contexts (one per c_type); masks: latent masks fp64 [R, bs, H, W].  size: window side (None: one window, the
     canvas).  Bootstrapping at the first bootstrap_steps steps: pick_fn(i) -> int [R, bs] rows of backgrounds ([nb, C]),
     z_fn(i) -> z [bs, C, H, W].  With mask (latent, [bs or 1, 1, H, W]) and x0: the inpainting start and blend of inpaint_oracle,
-    noise_fn(i) -> its z_i."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    sched = O.ddim_schedule(ac, steps)
+    noise_fn(i) -> its z_i.  grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature).  The noise is the canvas's, added once per step: regions.py's step
+    is the unchanged update on the mask-weighted eps average, so DDIM at eta > 0 takes that average and one canvas step."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
     ts = sched["timesteps"]
     total = len(ts)
     H, W = x_T.shape[-2:]
@@ -125,7 +127,11 @@ def sample(sd, x_T, conds, unconds, region_conds, masks, steps, size=None, strid
             boot = boot_at(i)
             ev = views(x, i, boot)
             a_t, a_prev = float(sched["alphas"][i]), float(sched["alphas_prev"][i])
-            x = paper_step(x, lambda xc, g, r: ev[g, r], masks, wins, h, w, a_t, a_prev, boot)
+            if eta == 0:
+                x = paper_step(x, lambda xc, g, r: ev[g, r], masks, wins, h, w, a_t, a_prev, boot)
+            else:
+                e = eps_average(x, lambda xc, g, r: ev[g, r], masks, wins, h, w, boot)
+                x = P.ddim_update(x, e, a_t, a_prev, float(sched["sigmas"][i]), np.asarray(noise(i), dtype=np.float64))
             if mask is not None:
                 x = I.blend(torch.from_numpy(x).float(), x0.float(), mask.float(), noise_fn(i).float(), rows[i, 0],
                             rows[i, 1]).double().numpy()
@@ -137,5 +143,5 @@ def sample(sd, x_T, conds, unconds, region_conds, masks, steps, size=None, strid
         return eps_average(np.asarray(xv, dtype=np.float64), lambda xc, g, r: ev[g, r], masks, wins, h, w, boot)
 
     after = None if mask is None else I.blend_after(ac.numpy(), ts, x0, mask, noise_fn)
-    out = D.walk(x, eps_fn, ac.numpy(), ts, order, after=after)
+    out = G.dpm_walk(x, eps_fn, ac.numpy(), ts, order, eta, noise, after=after)
     return torch.from_numpy(out).float()

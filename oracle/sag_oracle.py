@@ -11,8 +11,9 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from . import dpm_solver_oracle as D
+from . import dpm_sde_oracle as G
 from . import inpaint_oracle as I
+from . import panorama_oracle as P
 from . import vd_oracle as O
 
 
@@ -93,13 +94,16 @@ def sag_eps(sd, x, t, conds, unconds, scale, s, a, c_types=("text",), ratios=Non
 
 
 def sample(sd, x_T, conds, unconds, steps, s, sampler="ddim", scale=7.5, c_types=("text",), ratios=None, x0=None, mask=None,
-           noise_fn=None, masses=None, num_ddpm=1000, **kw):
-    """The SAG walk from x_T [bs, C, H, W]: DDIM (order 1) or DPM-Solver++ 2M in fp64, with the inpainting blend when mask (latent
-    [bs or 1, 1, H, W]) and x0 are given (noise_fn(i) -> z_i, the full walk's masked start)."""
-    ac = O.ddpm_schedule(num_ddpm)["alphas_cumprod"]
-    ts = O.make_ddim_timesteps(steps, num_ddpm)
+           noise_fn=None, masses=None, num_ddpm=1000, order=2, grid_name="uniform", eta=0.0, noise=None, **kw):
+    """The SAG walk from x_T [bs, C, H, W]: DDIM (order 1 at eta 0, the stochastic DDIM step at eta > 0) or DPM-Solver++ of
+    `order` in fp64, with the inpainting blend when mask (latent [bs or 1, 1, H, W]) and x0 are given (noise_fn(i) -> z_i, the
+    full walk's masked start).  grid_name: the sampler's time grid ('uniform', 'trailing' or 'karras'); eta: DDIM's eta, or the SDE walk's
+    (dpm_sde_oracle.walk) for DPM-Solver++; noise(i) -> the step's standard normal z at grid index i, read where eta > 0 (for
+    DDIM times the temperature)."""
+    ac, sched = G.schedule(grid_name, steps, eta, num_ddpm)
+    ts = sched["timesteps"]
     acn = ac.numpy()
-    order = 1 if sampler == "ddim" else 2
+    order = 1 if sampler == "ddim" else order
 
     def eps_fn(xv, i):
         a = float(np.float64(acn[ts[i]]))
@@ -110,5 +114,12 @@ def sample(sd, x_T, conds, unconds, steps, s, sampler="ddim", scale=7.5, c_types
     if mask is not None:
         x = I.start(x_T.float(), x0.float(), mask.float(), acn, int(ts[-1]))
         after = I.blend_after(acn, ts, x0, mask, noise_fn)
-    out = D.walk(x.double().numpy(), eps_fn, acn, ts, order, after=after)
+    if sampler == "ddim" and eta != 0:
+        x = x.double().numpy()
+        for i in range(len(ts) - 1, -1, -1):
+            x = P.ddim_update(x, eps_fn(x, i), float(sched["alphas"][i]), float(sched["alphas_prev"][i]), float(sched["sigmas"][i]),
+                              np.asarray(noise(i), dtype=np.float64))
+            x = x if after is None else after(i, x)
+        return torch.from_numpy(x).float()
+    out = G.dpm_walk(x.double().numpy(), eps_fn, acn, ts, order, eta, noise, after=after)
     return torch.from_numpy(out).float()

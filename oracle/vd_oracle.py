@@ -50,12 +50,13 @@ def make_ddim_timesteps(num_ddim, num_ddpm=1000):
     return np.asarray(list(range(0, num_ddpm, c))) + 1
 
 
-def ddim_schedule(alphas_cumprod, num_ddim, eta=0.0):
+def ddim_schedule(alphas_cumprod, num_ddim, eta=0.0, timesteps=None):
     """DDIMSampler.make_schedule + make_ddim_sampling_parameters, ddim.py:23-56, diffusion_utils.py:48-59.
     alphas_cumprod: fp32 tensor (the model buffer). Returns fp32 python lists per DDIM index, with the
     same dtype walk as the reference: alphas fp32 tensor; alphas_prev fp64 ndarray built from fp32
-    values; sigmas = eta*sqrt(...) in fp64; sqrt(1-alphas) on the fp32 tensor."""
-    ts = make_ddim_timesteps(num_ddim, alphas_cumprod.shape[0])
+    values; sigmas = eta*sqrt(...) in fp64; sqrt(1-alphas) on the fp32 tensor.  timesteps: the grid
+    (default DDIM's uniform one of num_ddim steps)."""
+    ts = make_ddim_timesteps(num_ddim, alphas_cumprod.shape[0]) if timesteps is None else np.asarray(timesteps)
     ac = alphas_cumprod.cpu()
     alphas = ac[ts]                                                       # fp32 tensor
     alphas_prev = np.asarray([ac[0]] + ac[ts[:-1]].tolist())              # fp64 ndarray of fp32 values
@@ -384,8 +385,10 @@ def cfg_pass(model, sd, x, t, conds, unconds, pair, ratios=None, c_types=("text"
     return e_u, e_c
 
 
-def p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types=("text",), ratios=None, **kw):
-    """DDIMSampler.p_sample_ddim / _multicontext, ddim.py:129-171, 244-298 (eta noise term omitted: sigma*randn)."""
+def p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types=("text",), ratios=None, noise=None, temperature=1.0,
+                  **kw):
+    """DDIMSampler.p_sample_ddim / _multicontext, ddim.py:129-171, 244-298.  noise: the step's standard normal z (shaped like
+    x), which adds sigma_t * temperature * z; None leaves the term out (eta = 0)."""
     b = x.shape[0]
     e_u, e_c = cfg_pass(apply_model, sd, x, t, conds, unconds, scale != 1.0, ratios, c_types, **kw)
     e_t = e_c if e_u is None else e_u + scale * (e_c - e_u)
@@ -397,6 +400,8 @@ def p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types=("text"
     pred_x0 = (x - s1m * e_t) / a_t.sqrt()
     dir_xt = (1.0 - a_prev - sigma_t ** 2).sqrt() * e_t
     x_prev = a_prev.sqrt() * pred_x0 + dir_xt
+    if noise is not None:
+        x_prev = x_prev + sigma_t * temperature * noise
     return x_prev, pred_x0, e_t
 
 
@@ -433,11 +438,12 @@ def img2img_start(x0, noise, timesteps, k, num_ddpm=1000):
 
 
 def ddim_sample(sd, x_T, conds, unconds, steps, scale=7.5, c_types=("text",), ratios=None, eta=0.0,
-                num_ddpm=1000, collect=False, x0=None, x0_forward_timesteps=None, x0_noise=None, **kw):
-    """DDIMSampler.sample / ddim_sampling, ddim.py:58-127 with x_T injected (eta must be 0 here).  With x0 the img2img
-    start from x0 and x0_noise (x_T is ignored)."""
-    assert eta == 0.0
-    sched = ddim_schedule(ddpm_schedule(num_ddpm)["alphas_cumprod"], steps, eta)
+                num_ddpm=1000, collect=False, x0=None, x0_forward_timesteps=None, x0_noise=None, noise=None, temperature=1.0,
+                timesteps=None, **kw):
+    """DDIMSampler.sample / ddim_sampling, ddim.py:58-127 with x_T injected.  With x0 the img2img start from x0 and x0_noise
+    (x_T is ignored).  eta > 0 needs noise(index) -> the step's z; timesteps: the grid (default DDIM's uniform one)."""
+    assert eta == 0.0 or noise is not None
+    sched = ddim_schedule(ddpm_schedule(num_ddpm)["alphas_cumprod"], steps, eta, timesteps)
     ts = sched["timesteps"]
     x = x_T
     if x0 is not None:
@@ -446,7 +452,8 @@ def ddim_sample(sd, x_T, conds, unconds, steps, scale=7.5, c_types=("text",), ra
     for i, step in enumerate(np.flip(ts)):
         index = len(ts) - i - 1
         t = torch.full((x.shape[0],), int(step), dtype=torch.long)
-        x, pred_x0, e_t = p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types, ratios, **kw)
+        z = None if eta == 0.0 else noise(index)
+        x, pred_x0, e_t = p_sample_ddim(sd, x, conds, unconds, t, index, sched, scale, c_types, ratios, z, temperature, **kw)
         if collect:
             trace.append({"x": x.clone(), "pred_x0": pred_x0.clone(), "e_t": e_t.clone()})
     return (x, trace) if collect else x

@@ -1,5 +1,5 @@
 """Stochastic DPM-Solver++ (DPMSolverSDESampler), CPU side: the table at eta = 0 is the ODE table bit for bit; at eta > 0 its rows
-fold the fp64 direct SDE step (tests/dpm_sde_oracle.py); the last row is deterministic; the sampler's argument checks; the refusals
+fold the fp64 direct SDE step (oracle/dpm_sde_oracle.py); the last row is deterministic; the sampler's argument checks; the refusals
 of vdb_dpmpp_sde_cfg_step; weak convergence of the oracle's SDE walk on the analytic Gaussian model."""
 import types
 
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import dpm_sde_oracle as G
+from oracle import dpm_sde_oracle as G
 from oracle import dpm_solver_oracle as D
 from oracle import vd_oracle as O
 

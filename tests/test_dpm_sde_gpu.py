@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-import dpm_sde_oracle as G
+from oracle import dpm_sde_oracle as G
 from oracle import dpm_solver_oracle as D
 from oracle import vd_oracle as O
 from test_dpm_solver_gpu import _data, _dev, restate

@@ -45,7 +45,7 @@ def _sampler(sampler):
 def test_combination_matrix_with_sag(sampler, entry, text):
     from lib.model_zoo.sag import SelfAttentionGuidance
     states = [_draws_after(n) for n in range(3)]
-    for given in SUBSETS:
+    for given in [s for s in SUBSETS if not {"regions", "sag"} & set(s)]:      # 'sag' is added to each below
         exc, match, draws = expected_with_sag(sampler, entry, given, text)
         shape, x_info, c_infos = _inputs(given, text)
         x_info["sag"] = SelfAttentionGuidance(0.75)

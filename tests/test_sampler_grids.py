@@ -1,5 +1,5 @@
 """The samplers' time grids (make_ddim_timesteps, the `grid` option): 'trailing' and 'karras' against their restatement from
-diffusers / k-diffusion (tests/dpm_sde_oracle.py), their shape, 'uniform' unchanged, the refusals, and the grid reaching every
+diffusers / k-diffusion (oracle/dpm_sde_oracle.py), their shape, 'uniform' unchanged, the refusals, and the grid reaching every
 sampler and DiffEdit's mask level."""
 import types
 
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import dpm_sde_oracle as G
+from oracle import dpm_sde_oracle as G
 from oracle import vd_oracle as O
 
 AC = O.ddpm_schedule(1000)["alphas_cumprod"]

@@ -219,8 +219,13 @@ class DDIMSampler(object):
         if x_info.get('xt', None) is not None:
             x = x_info['xt'].to(dtype).to(device)       # (the reference's `.astype` here is a bug, ddim.py:95)
         elif x_info.get('x0', None) is not None:
+            k = x_info['x0_forward_timesteps']
+            if k >= len(timesteps):
+                # x0 is noised to grid point k, so k must lie on the grid, which can be shorter than the steps asked for (a
+                # Karras grid drops low sigmas that round to one timestep)
+                raise ValueError(f"x0_forward_timesteps must be below the grid's {len(timesteps)} points, got {k}")
             x0 = x_info['x0'].type(dtype).to(device)
-            ts = np.repeat(timesteps[x_info['x0_forward_timesteps']], shape[0])
+            ts = np.repeat(timesteps[k], shape[0])
             ts = torch.Tensor(ts).long().to(device)
             timesteps = timesteps[:x_info['x0_forward_timesteps']]
             x = self.model.q_sample(x0, ts)

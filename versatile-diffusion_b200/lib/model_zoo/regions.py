@@ -66,8 +66,9 @@ backgrounds and key while bootstrapping, the chunk batch and the canvas eps) is 
 on new prompts and masks.
 
 Refusals, before any device work.  ValueError: x_info['regions'] not a Regions; a text latent; a mask or conditioning of the wrong
-type or shape; mask values outside [0, 1] or NaN; R outside [1, 8]; bootstrap_steps outside [0, steps]; bootstrapping without
-backgrounds, or backgrounds not [nb >= 1, C]; x_info['windows'] not a panorama.Windows or a layout panorama refuses.
+type or shape; mask values outside [0, 1] or NaN; R outside [1, 8]; bootstrap_steps outside [0, the walk's grid points];
+bootstrapping without backgrounds, or backgrounds not [nb >= 1, C]; x_info['windows'] not a panorama.Windows or a layout panorama
+refuses.
 NotImplementedError: prompt_edit, sampling from an inversion, PLMSSampler and the single-step p_sample_ddim.  The img2img start,
 inpaint_mask (outpainting with regions) and single or dual contexts combine unchanged.  Without 'regions' nothing changes: the same
 launches, the same bits, the same graph key.
@@ -213,7 +214,8 @@ class RegionPrompts(SamplerMode):
         if regs is not None:
             steps = len(sampler.ddim_timesteps)
             if regs.bootstrap_steps > steps:
-                raise ValueError(f"Regions: bootstrap_steps must lie in [0, {steps}] (the steps), got {regs.bootstrap_steps}")
+                raise ValueError(f"Regions: bootstrap_steps must lie in [0, {steps}] (the walk's grid points), "
+                                 f"got {regs.bootstrap_steps}")
             if regs.backgrounds is not None and regs.backgrounds.shape[1] != C:
                 raise ValueError(f"Regions: backgrounds expected [nb, {C}], got {tuple(regs.backgrounds.shape)}")
         if win is None:
